@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the TAPIR hot path (driver contract: see the task brief / DESIGN.md section 6).
+"""Benchmark of the TAPIR hot path (DESIGN.md section 6).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 A "step" is one full inference pass  get_feature_grids + get_query_features +
 estimate_trajectories (+ the per-level mean of forward)  over one synthetic clip.
@@ -61,7 +61,8 @@ def _peaks():
       d = json.load(fh)
     return dict(hbm=d['hbm_gbs'], tf_burst=d['bf16_tflops'], tf_sustained=d['bf16_tflops_sustained'],
                 source='measured (MEASURED_PEAKS.json)')
-  return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+  return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0,
+              source='H100 SXM data sheet (dense BF16, 700 W card), not a measured peak')
 
 
 # bf16 MMAs issued per fp32-equivalent product term under each precision policy (DESIGN.md 2)
@@ -180,7 +181,7 @@ class Runner:
     self.model = tapir_model.TAPIR(pyramid_level=1, precision=args.precision)
     self.model.load_state_dict(self.sd)
     self.model = self.model.to(self.dev).eval()
-    self.flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=self.dev)  # > 126 MB L2
+    self.flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=self.dev)  # > 50 MB L2
     self.sampler = ClockSampler(self.local_rank)
     if self.rank == 0:
       self.sampler.start()
@@ -193,7 +194,8 @@ class Runner:
 
   def timed(self, fn, steps):
     """K steps inside one barrier+sync bracket; per-step CUDA events; L2 flushed between steps.
-    Returns (ms per step = max over ranks of the per-rank mean, clocks window)."""
+    Returns (ms per step = max over ranks of the per-rank mean, clocks window); what the last
+    step returned is kept in self.last_out."""
     evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True))
            for _ in range(steps)]
     self.barrier()
@@ -201,7 +203,7 @@ class Runner:
     for a, b in evs:
       self.flush.zero_()
       a.record()
-      fn()
+      self.last_out = fn()
       b.record()
     self.barrier()
     t1 = time.time()
@@ -233,18 +235,10 @@ class Runner:
     return prof, breakdown
 
 
-def _traffic(name):
-  tpath = os.path.join(ROOT, 'profiles', 'roofline_traffic.json')
-  if os.path.exists(tpath):
-    with open(tpath) as fh:
-      return json.load(fh).get(name)
-  return None
-
-
 def roofline_tensor(name, v, peaks, terms, note=None):
   ach = v['flops'] / (v['ms'] * 1e-3) / 1e12
   d = dict(kernel=name, bound='tensor', achieved=round(ach, 2), peak=peaks['tf_sustained'],
-           unit='TFLOP/s', frac=round(ach / peaks['tf_sustained'], 4), traffic=_traffic(name),
+           unit='TFLOP/s', frac=round(ach / peaks['tf_sustained'], 4),
            peak_source=peaks['source'] + ', sustained (kernel timed inside a long step)',
            launches=v['launches'], avg_launch_ms=round(v['ms'] / v['launches'], 4),
            mma_terms=terms, issued_mma_tflops=round(ach * terms, 1),
@@ -261,11 +255,36 @@ def roofline_tensor(name, v, peaks, terms, note=None):
 def roofline_hbm(name, v, peaks):
   ach = v['bytes'] / (v['ms'] * 1e-3) / 1e9
   return dict(kernel=name, bound='hbm', achieved=round(ach, 1), peak=peaks['hbm'], unit='GB/s',
-              frac=round(ach / peaks['hbm'], 4), traffic=_traffic(name), peak_source=peaks['source'],
+              frac=round(ach / peaks['hbm'], 4), peak_source=peaks['source'],
               launches=v['launches'], avg_launch_ms=round(v['ms'] / v['launches'], 4))
 
 
-def run_offline_workload(R, name, steps, warmup, with_profile=True, legs=('device', 'e2e', 'e2e_u8')):
+def dump_outputs(out, dump_dir):
+  """The arrays a caller of the timed path receives, as DIR/<name>.npy in float32 (at most 64 MB in
+  all: a larger output is cut to a fixed, seeded sample of its query points).  List entries of the
+  output (`unrefined_*`, one tensor per refinement iteration) become DIR/<name>_<i>.npy.  Under
+  --gpus N the timed path returns each rank its own query shard, and rank 0 writes its shard."""
+  import numpy as np  # pylint: disable=g-import-not-at-top
+  os.makedirs(dump_dir, exist_ok=True)
+  arrays = {}
+  for k, v in out.items():
+    if torch.is_tensor(v):
+      arrays[k] = v.detach().float().cpu()
+    elif isinstance(v, (list, tuple)):
+      arrays.update({f'{k}_{i}': t.detach().float().cpu() for i, t in enumerate(v) if torch.is_tensor(t)})
+  total = sum(a.numel() * 4 for a in arrays.values())
+  budget = 64 * 1024 * 1024
+  if total > budget:  # every output is [B, N, ...]: keep the same query points of each
+    n = next(iter(arrays.values())).shape[1]
+    keep = max(1, int(n * budget // total))
+    idx = torch.randperm(n, generator=torch.Generator().manual_seed(0))[:keep].sort().values
+    arrays = {k: a[:, idx] for k, a in arrays.items()}
+  for k, a in arrays.items():
+    np.save(os.path.join(dump_dir, f'{k}.npy'), a.numpy())
+
+
+def run_offline_workload(R, name, steps, warmup, with_profile=True, legs=('device', 'e2e', 'e2e_u8'),
+                         dump_dir=None):
   """One offline workload (c2 / c4 / c5) -> record dict (rank 0) or None."""
   from tapnet_b200 import distributed as tdist
   wl = WORKLOADS[name]
@@ -306,6 +325,8 @@ def run_offline_workload(R, name, steps, warmup, with_profile=True, legs=('devic
   launches0 = R.lib.tapir_launch_count()
   ms_step, clocks = R.timed(step_device, steps)
   launches = (R.lib.tapir_launch_count() - launches0) // max(steps, 1)
+  if dump_dir is not None and rank == 0:
+    dump_outputs(R.last_out, dump_dir)
   d2h = int(sum(t.numel() * 4 for t in out_pin.values()))
   e2e = e2e_u8 = None
   if 'e2e' in legs and video_pin is not None:
@@ -438,7 +459,7 @@ def run_c3_stream(R):
 def run_ours(args):
   R = Runner(args)
   world, rank = R.world, R.rank
-  main = run_offline_workload(R, args.workload, args.steps, args.warmup)
+  main = run_offline_workload(R, args.workload, args.steps, args.warmup, dump_dir=args.dump_outputs)
   sub = {}
   if not args.no_sub and args.workload == 'c2':
     sub_steps = max(2, min(args.steps, 5))
@@ -522,13 +543,12 @@ def run_ours(args):
 
 
 def _load_reference_module():
-  """The UNMODIFIED reference torch path, if it can be imported on this box: `baseline/_ref`
-  (pip --target install of /root/reference made in the build container, git-ignored, travels
-  with the snapshot) or /root/reference itself (build container only).  Layout-only shims for
-  its two absent dependencies (einshape, dm-tree) come from oracle/shims.  Returns the module
+  """The UNMODIFIED reference torch path, if a copy of it has been placed under `oracle/_ref`
+  (git-ignored; nothing in the repository creates it).  Layout-only shims for its two absent
+  dependencies (einshape, dm-tree) come from oracle/shims.  Returns the module
   `tapnet.torch.tapir_model` or None."""
   shims = os.path.join(ROOT, 'oracle', 'shims')
-  for root in (os.path.join(ROOT, 'baseline', '_ref'), '/root/reference'):
+  for root in (os.path.join(ROOT, 'oracle', '_ref'),):
     if os.path.isfile(os.path.join(root, 'tapnet', 'torch', 'tapir_model.py')):
       for p in (root, shims):
         if p not in sys.path:
@@ -612,7 +632,7 @@ class CpuArm:
 
   def pick_threads(self):
     """torch's CPU kernels do not scale to very wide hosts on these small per-frame problems
-    (128 threads were 40x slower than 8 on the GPU box): give the reference its best case.  The
+    (128 threads were 40x slower than 8 on a 128-core host): give the reference its best case.  The
     thread count is chosen from the median of 3 repetitions of THE SAMPLE ITSELF per candidate."""
     ncpu = os.cpu_count() or 1
     cands = sorted({c for c in (8, 16, 32, 64) if c <= ncpu} or {ncpu})
@@ -697,7 +717,10 @@ def main():
   ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
   ap.add_argument('--no-sub', action='store_true', help='skip the c4 / c3 / c5 sub-records')
   ap.add_argument('--workload', default='c2', choices=['c2', 'c4', 'c5'],
-                  help='headline workload: c2 = driver contract (default)')
+                  help='headline workload (default c2)')
+  ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                  help='after the timed steps, write the outputs of the last timed step as DIR/<name>.npy '
+                       '(rank 0 writes its own query shard under --gpus N)')
   args = ap.parse_args()
   if args.impl == 'reference':
     run_reference(args)

@@ -29,7 +29,6 @@ for t in $TIERS; do
     io)          run io "X=1" tests/test_io_gpu.py ;;
     bulk)        run bulk "X=1" tests/test_bulk_gpu.py ;;
     no_halo)     run no_halo "TAPIR_B200_CONV_HALO=0" tests/test_gemm_gpu.py tests/test_stages_gpu.py tests/test_end_to_end_gpu.py ;;
-    no_tail)     run no_tail "TAPIR_B200_GEMM_TAIL=0" tests/test_gemm_gpu.py tests/test_end_to_end_gpu.py ;;
     no_splitk)   run no_splitk "TAPIR_B200_SPLITK=0" tests/test_stages_gpu.py tests/test_properties_gpu.py ;;
     all)         run all "X=1" tests ;;
   esac

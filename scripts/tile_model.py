@@ -1,54 +1,28 @@
 """Wave model of the GEMM launches of one inference step (no GPU needed).
 
-For every GEMM of the step it replays the tile choice of csrc/gemm_tc.cu (2-SM pair tiles of
-256 x {128,256} over 74 clusters with the last partial round cut along N; 1-SM 128 x {64,128}
-tiles over 148 CTAs for N = 64 and for problems too small to fill the GPU) and reports
-tiles, rounds, the wave-quantisation efficiency tiles / (rounds * workers), and the time the
-issued bf16 MMA work would take at the measured cuBLAS peak.  DESIGN.md section 8 quotes it.
+For every GEMM of the step it replays the tile choice of csrc/gemm_tc.cu (persistent wgmma
+kernel, 128 x {64,128} tiles over 132 CTAs; 64-wide for N = 64 and for problems too small to fill
+the GPU) and reports tiles, rounds, the wave-quantisation efficiency tiles / (rounds * workers),
+and the time the issued bf16 MMA work would take at the given peak (default: the H100 SXM data
+sheet's dense bf16 figure, not a measured rate).
 
-  python scripts/tile_model.py [--frames 48 --queries 256] [--peak 1422.8]
+  python scripts/tile_model.py [--frames 48 --queries 256] [--peak 989]
 """
 import argparse
 import math
 
-SMS = 148
+SMS = 132
 
 
-def _tail_plan(pairs, n, bn, tail=True):
-  """(cost per cluster in quarter-chunk units, tiles) of W tiles on 74 clusters with the last
-  partial round cut along N into k pieces of >= 64 columns (gemm_tc.cu: tail_plan).  A piece of
-  c 32-column chunks costs max(4c, 8 + c): narrow pieces are bound by the A-operand reads."""
-  half = SMS // 2
-  w = pairs * math.ceil(n / bn)
-  c = min(w, half)
-  rem = w % c
-  cost = (w // c) * (bn // 32) * 4
-  if rem:
-    k = min(c // rem, bn // 64) if tail else 1
-    if k >= 2 and w > c:
-      base, extra = (bn // 32) // k, (bn // 32) % k
-      ch = base + (1 if extra else 0)
-      cost += max(4 * ch, 8 + ch)
-    else:
-      cost += (bn // 32) * 4
-  return cost, w
-
-
-def choice(m_rows, n, planes, tail=True):
-  """Replays gemm_tc.cu's dispatch.  Returns (kernel, tiles, workers, rounds) where `rounds` is
-  the schedule length in units of one full tile (fractional when the tail is split)."""
+def choice(m_rows, n, planes):
+  """Replays gemm_tc.cu's dispatch (plain GEMMs, no split-K).  Returns (kernel, tiles, workers,
+  rounds)."""
+  del planes  # the tile choice does not depend on the number of planes
   m_tiles = math.ceil(m_rows / 128)
-  pr = (m_tiles + 1) // 2
-  small = 2 * pr * math.ceil(n / 128) * 10 < SMS * 6
-  if n >= 128 and m_tiles >= 2 and not small:
-    c128, _ = _tail_plan(pr, n, 128, tail)
-    c256, _ = _tail_plan(pr, n, 256, tail)
-    bn = 256 if (n >= 256 and c256 * (10 if planes == 3 else 9) <= c128 * 10) else 128
-    cost, tiles = _tail_plan(pr, n, bn, tail)
-    return f'2SM 256x{bn}', tiles, SMS // 2, cost / (bn // 32 * 4)
+  small = m_tiles * math.ceil(n / 128) * 10 < SMS * 6
   bn = 64 if (n <= 64 or (small and m_tiles * math.ceil(n / 128) * 2 <= SMS)) else 128
   tiles = m_tiles * math.ceil(n / bn)
-  return f'1SM 128x{bn}', tiles, SMS, math.ceil(tiles / SMS)
+  return f'128x{bn}', tiles, SMS, math.ceil(tiles / SMS)
 
 
 def step_gemms(frames, queries):
@@ -88,16 +62,16 @@ def _class_of(name):
   return None
 
 
-def compare(bench_json, frames, queries, peak, chunks=1, tail=True):
+def compare(bench_json, frames, queries, peak, chunks=1):
   """Per GEMM class: measured ms (bench.py kernel_breakdown) against the MMA-bound time at the
-  cuBLAS peak and against that time divided by the wave-quantisation efficiency."""
+  given peak and against that time divided by the wave-quantisation efficiency."""
   import json
   with open(bench_json) as fh:
     line = [l for l in fh if l.startswith('{')][-1]
   kb = json.loads(line)['kernel_breakdown']
   agg = {}
   for name, m, n, k, planes, count in step_gemms(frames, queries):
-    kind, tiles, workers, rounds = choice(m, n, planes, tail)
+    kind, tiles, workers, rounds = choice(m, n, planes)
     eff = tiles / (rounds * workers)
     terms = planes * (planes + 1) // 2
     ms = 2.0 * m * n * k * terms / (peak * 1e12) * 1e3 * count
@@ -124,17 +98,16 @@ def main():
                   help='query chunks per step (--queries is then the chunk size)')
   ap.add_argument('--frames', type=int, default=48)
   ap.add_argument('--queries', type=int, default=256)
-  ap.add_argument('--peak', type=float, default=1422.8, help='bf16 TFLOP/s (MEASURED_PEAKS sustained)')
-  ap.add_argument('--no-tail', action='store_true', help='model the schedule without the N-split tail')
+  ap.add_argument('--peak', type=float, default=989.0, help='bf16 TFLOP/s (H100 SXM data sheet, dense)')
   a = ap.parse_args()
   if a.bench:
-    compare(a.bench, a.frames, a.queries, a.peak, a.chunks, not a.no_tail)
+    compare(a.bench, a.frames, a.queries, a.peak, a.chunks)
     return
   print(f'| GEMM | M x N x K | tile | tiles | rounds | quantisation | launches | MMA-bound ms/step |')
   print('|---|---|---|---|---|---|---|---|')
   total = 0.0
   for name, m, n, k, planes, count in step_gemms(a.frames, a.queries):
-    kind, tiles, workers, rounds = choice(m, n, planes, not a.no_tail)
+    kind, tiles, workers, rounds = choice(m, n, planes)
     eff = tiles / (rounds * workers)
     terms = planes * (planes + 1) // 2
     ms = 2.0 * m * n * k * terms / (a.peak * 1e12) * 1e3 * count

@@ -1,4 +1,4 @@
-"""tapnet_b200: B200-native TAPIR / BootsTAPIR point-tracking inference engine.
+"""tapnet_b200: H100-native TAPIR / BootsTAPIR point-tracking inference engine.
 
 Drop-in for the `tapnet/torch/tapir_model.py` surface of google-deepmind/tapnet:
 

@@ -1,4 +1,4 @@
-"""Builds tapnet_b200/libtapir_b200.so (sm_100a only) with nvcc, in-tree."""
+"""Builds tapnet_b200/libtapir_b200.so (sm_90a only) with nvcc, in-tree."""
 import hashlib
 import os
 import subprocess
@@ -9,7 +9,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libtapir_b200.so')
 SOURCES = ['common.cu', 'gemm_tc.cu', 'gemm_simt.cu', 'backbone.cu', 'stage_a.cu', 'refine.cu',
            'frames_io.cu', 'api.cu']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC']
 
 
@@ -62,7 +62,7 @@ def build(force=False, verbose=False):
       print(out.decode())
   if failed:
     raise RuntimeError('nvcc compilation failed')
-  cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-ldl']
+  cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '-ldl']
   subprocess.check_call(cmd)
   with open(stamp, 'w') as fh:
     fh.write(digest)

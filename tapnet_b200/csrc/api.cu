@@ -71,7 +71,7 @@ int tapir_gemm(const void* a_planes, int32_t lda, int64_t a_plane_stride, const 
   g.stats = stats; g.rows_per_frame = rows_per_frame;
   if (impl == 1) return gemm_simt(g, S(stream));
   if (impl == 0) return gemm_tc(g, S(stream));
-  set_error("tapir_gemm: impl must be 0 (tcgen05) or 1 (simt)");
+  set_error("tapir_gemm: impl must be 0 (wgmma) or 1 (simt)");
   return kBadArgument;
 }
 

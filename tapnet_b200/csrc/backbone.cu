@@ -1,5 +1,5 @@
 // Feature-pyramid backbone (SURVEY.md 8(a3)): ResNet-V2 + InstanceNorm, ExtraConvs, L2 norm.
-// All 3x3 / 1x1 convolutions run as split-bf16 tcgen05 GEMMs (gemm_tc.cu); this file holds the
+// All 3x3 / 1x1 convolutions run as split-bf16 wgmma GEMMs (gemm_tc.cu); this file holds the
 // HBM-bound kernels around them (stem conv, instance/layer norm, im2col for the three
 // stride-2 layers, resize) and the per-frame-chunk orchestration.
 #include "kernels.cuh"

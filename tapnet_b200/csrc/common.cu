@@ -133,7 +133,7 @@ int num_sms() {
   const int dev = current_device();
   if (n[dev] == 0) {
     if (cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n[dev] <= 0)
-      n[dev] = 148;
+      n[dev] = 132;
   }
   return n[dev];
 }

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the tapir_b200 kernels (sm_100a only).
+// Shared device/host helpers for the tapir_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -111,22 +111,33 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   return x * r;
 }
 
-// Two tanh-GELUs at once on packed fp32 (mul/fma.rn.f32x2: one issue slot per pair); the two
-// ex2 and the two reciprocals stay scalar MUFU operations.  Same formula as gelu_tanh.
+// Elementwise fp32 pair arithmetic, each half an IEEE round-to-nearest operation (never
+// contracted or reassociated).  Hopper has no packed fp32 instructions: two scalar ops each.
+__device__ __forceinline__ float2 fma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 mul2_rn(float2 a, float2 b) {
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 add2_rn(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
+}
+
+// Two tanh-GELUs on an fp32 pair.  Same formula and rounding as gelu_tanh.
 __device__ __forceinline__ float2 gelu_tanh2(float2 x) {
   const float2 A = make_float2(-2.3022081983f, -2.3022081983f);
   const float2 B = make_float2(-0.1029432396f, -0.1029432396f);
-  const float2 u = __fmul2_rn(x, __ffma2_rn(__fmul2_rn(x, x), B, A));
+  const float2 u = mul2_rn(x, fma2_rn(mul2_rn(x, x), B, A));
   float2 e;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.x) : "f"(u.x));
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e.y) : "f"(u.y));
-  const float2 d = __fadd2_rn(e, make_float2(1.0f, 1.0f));
+  const float2 d = add2_rn(e, make_float2(1.0f, 1.0f));
   // d is in [1, +inf]: rcp.approx needs none of div.approx's range handling (which costs an
   // FSETP and two FMULs per division); rcp(+inf) = 0 gives gelu(-large) = -0 like the quotient
   float2 r;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r.x) : "f"(d.x));
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r.y) : "f"(d.y));
-  return __fmul2_rn(x, r);
+  return mul2_rn(x, r);
 }
 
 // One step of the bf16 split for two values at once: returns bf16x2(a, b) (a in the low half)
@@ -152,10 +163,8 @@ __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16 (&out)[P]) {
   }
 }
 
-// Same split step with integer-ALU rounding only (round-to-nearest-even on the raw bits).  On
-// sm_100 both F2F and F2FP go through the variable-latency conversion unit; in the GEMM
-// epilogue their scoreboard stalls dominated (ncu: 30 % of samples on the dependent shift), so
-// the hot epilogue rounds with IADD3/LOP3/PRMT instead.  Bit-identical to cvt.rn for finite x.
+// Same split step with integer-ALU rounding only (round-to-nearest-even on the raw bits), which
+// keeps the conversion unit out of the dependency chain.  Bit-identical to cvt.rn for finite x.
 __device__ __forceinline__ uint32_t bf16x2_split_alu(float& a, float& b) {
   uint32_t ua = __float_as_uint(a), ub = __float_as_uint(b);
   ua = (ua + 0x7fffu + ((ua >> 16) & 1u)) & 0xffff0000u;

@@ -1,5 +1,5 @@
 // Split-bf16 GEMM / implicit-GEMM 3x3 convolution: host-side description shared by the
-// tcgen05 kernel (gemm_tc.cu) and the SIMT verification kernel (gemm_simt.cu).
+// wgmma kernel (gemm_tc.cu) and the SIMT verification kernel (gemm_simt.cu).
 //
 //   D[m, n] = sum_{i + j < P} sum_k A_i[m, k] * B_j[n, k]        (fp32 accumulation)
 //   v = D + bias[n];  v = act ? gelu_tanh(v) : v;  v += residual[m, n]
@@ -55,7 +55,7 @@ struct GemmArgs {
 };
 
 int validate_gemm_args(const GemmArgs& g);
-// tcgen05 + TMA implementation (the product path).
+// wgmma + TMA implementation (the product path).
 int gemm_tc(const GemmArgs& g, cudaStream_t stream);
 // Straightforward SIMT implementation of the same arithmetic (verification / bring-up).
 int gemm_simt(const GemmArgs& g, cudaStream_t stream);

@@ -1,5 +1,5 @@
 // SIMT fp32 implementation of the GemmArgs contract (gemm.cuh).  Not the product path: it is
-// the on-device cross-check for the tcgen05 kernel (tests/test_gemm_gpu.py) and a bring-up
+// the on-device cross-check for the wgmma kernel (tests/test_gemm_gpu.py) and a bring-up
 // switch (TAPIR_B200_GEMM=simt).  It reconstructs a = sum_i A_i, b = sum_j B_j in fp32 and
 // runs a shared-memory tiled fp32 GEMM; versus the tensor-core path it additionally contains
 // the dropped (i + j >= P) cross terms, i.e. it differs by <= 2^-16 relative for P=2.

@@ -1,21 +1,23 @@
-// tcgen05 / TMEM / TMA split-bf16 GEMM and implicit-GEMM 3x3 convolution for sm_100a.
+// wgmma / TMA split-bf16 GEMM and implicit-GEMM 3x3 convolution for sm_90a.
 //
-// One persistent CTA per SM, 2 + 4*G warps (G = column groups of the epilogue, 16 epilogue warps for
-// BLOCK_N >= 128):
-//   warp E (one lane)  TMA producer: cp.async.bulk.tensor tiles of A and B planes into a
-//                      multi-stage shared-memory ring (128B-swizzled, K-major)
-//   warp E+1 (1 lane)  MMA issuer: tcgen05.mma.cta_group::1.kind::f16, M=128, N=BLOCK_N, K=16,
-//                      fp32 accumulators in TMEM (double buffered: 2 x BLOCK_N columns)
-//   warps 0..E-1       epilogue: tcgen05.ld the accumulator (one TMEM lane = one output row
-//                      per thread), bias / tanh-GELU / residual, store fp32 and/or bf16 planes
-// Pipelines: full/empty mbarriers between TMA and MMA, tmem_full/tmem_empty between MMA and
-// epilogue, so the epilogue of tile i overlaps the main loop of tile i+1.
+// One persistent CTA per SM, three warpgroups:
+//   warpgroup 0 (one lane)  TMA producer: cp.async.bulk.tensor tiles of A and B planes into a
+//                           multi-stage shared-memory ring (128B-swizzled, K-major)
+//   warpgroups 1, 2         consumers: each owns 64 rows of the 128-row tile, issues
+//                           wgmma.m64nBLOCK_Nk16 (bf16 operands from shared memory, fp32
+//                           accumulators in registers) and then runs the epilogue from its
+//                           registers: bias / tanh-GELU / residual, fp32 and/or bf16-plane stores
+// full/empty mbarriers between producer and consumers; the producer runs ahead into the next
+// tile while the consumers are in the epilogue of the current one.
 //
 // A operand, plain mode: 3-D tensor map {K, M, plane}, box {64, 128, 1}.
 // A operand, conv mode : 5-D tensor map {C, W, H, frame, plane} over the NHWC activation,
 //   box {64, tileW, tileH, 1, 1}; the 3x3 taps are shifted box origins, and TMA's
 //   out-of-bounds zero fill implements the zero padding (nets.py:296-303,40-53 padding=1).
 // B operand: 3-D tensor map {K, N, plane}, box {64, BLOCK_N, 1}.
+//
+// Every output element accumulates its K terms in the same order (k-block, then plane pair
+// (i, j), then 16-wide k step) whatever the tile shape, so results do not depend on BLOCK_N.
 #include <cuda.h>
 
 #include <cstdlib>
@@ -29,22 +31,17 @@ namespace {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;  // 64 bf16 = 128 B = one swizzle row
-constexpr int kUmmaK = 16;
-// Epilogue warps: 4 TMEM lane quadrants x G column groups.  The epilogue is latency bound
-// (conversions, MUFU, TMEM loads), so it needs thread-level parallelism: with the accumulator
-// tile split over 16 warps it hides behind a K=512 main loop; measured on the mixer `up` GEMM
-// (12288 x 2048 x 512): main loop alone 54 us, with 8 epilogue warps 85 us.
-__host__ __device__ constexpr int epi_groups(int block_n) { return block_n >= 128 ? 4 : block_n / 32; }
-__host__ __device__ constexpr int epi_warps(int block_n) { return 4 * epi_groups(block_n); }
-__host__ __device__ constexpr int num_threads(int block_n) { return 64 + 32 * epi_warps(block_n); }
-constexpr int kNumAccStages = 2;
+constexpr int kMmaK = 16;
+constexpr int kConsumers = 2;             // warpgroups, 64 rows each
+constexpr int kThreads = 128 * (1 + kConsumers);
+constexpr int kConsumerArrivals = 4 * kConsumers;  // one arrive per consumer warp
 constexpr int kSmemLimit = 227 * 1024;
 constexpr int kBarrierBytes = 256;
 
 struct TcParams {
   CUtensorMap tmA;
   CUtensorMap tmB;
-  CUtensorMap tmBh;     // cluster mode: half-height B box (BLOCK_N/2 rows), multicast to the CTA pair
+  CUtensorMap tmPatch;  // halo convolution: one patch row {64 ch, 10 px} per load
   int frames;
   int M, N;
   int num_k_blocks;
@@ -66,13 +63,6 @@ struct TcParams {
   int split_k;          // >1: K is split over `split_k` work items; raw fp32 partials go to out_f32
   long long split_stride;  // elements between partial buffers (M * ldo)
   int* err;
-  int debug_mode;       // bring-up only: 1 = epilogue skips TMEM loads and stores
-  // 2-SM kernel, tail of the persistent schedule: the last `tiles - tail_first` tiles are cut
-  // along N into `tail_k` pieces of 32-column chunks (piece j gets tail_base + (j < tail_extra)
-  // chunks) so that the partial last round spreads over all clusters instead of a few.
-  CUtensorMap tmB16;    // B with a 16-row box: pieces load their half-width in 16-row slabs
-  int tail_first, tail_k, tail_base, tail_extra;
-  CUtensorMap tmPatch;  // halo convolution: one patch row {64 ch, 10 px} per load
 };
 
 template <int BLOCK_N, int P>
@@ -80,223 +70,172 @@ struct TcCfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   static constexpr int kStageBytes = P * (kABytes + kBBytes);
-  static constexpr int kEpiWarps = epi_warps(BLOCK_N);
-  static constexpr int kChunks = BLOCK_N / 32 / epi_groups(BLOCK_N);  // 32-column chunks per warp
-  static constexpr int kBiasBytes = kEpiWarps * kChunks * 32 * 4;  // per-warp bias slice
-  static constexpr int kAvail = kSmemLimit - 1024 - kBarrierBytes - kBiasBytes;
+  static constexpr int kAvail = kSmemLimit - 1024 - kBarrierBytes;
   static constexpr int kStagesRaw = kAvail / kStageBytes;
   static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
-  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kBarrierBytes + kBiasBytes;
-  static constexpr int kTmemCols = (kNumAccStages * BLOCK_N <= 128) ? 128
-                                   : (kNumAccStages * BLOCK_N <= 256) ? 256 : 512;
-  static_assert(kStages >= 1, "tile does not fit in shared memory");
-  static_assert(kStages * 2 + 2 * kNumAccStages <= (kBarrierBytes - 16) / 8, "barrier space");
+  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kBarrierBytes;
+  static_assert(kStages >= 2, "tile does not fit in shared memory");
+  static_assert(kStages * 2 <= kBarrierBytes / 8, "barrier space");
 };
 
-// One output row (this thread) x 32 consecutive columns.  `bias_s` points at this chunk's 32
-// bias values in shared memory (staged by the warp before it waited for the accumulator).
-__device__ __forceinline__ void store_row_chunk(const TcParams& p, long long row, int col0,
-                                                const uint32_t (&acc)[32],
-                                                const float* __restrict__ bias_s, bool row_ok,
-                                                int frame, int lane, long long out_off) {
-  const bool full = (col0 + 32 <= p.N);
-  if (p.debug_mode == 3) row &= 127;  // bring-up: all tiles store to the same rows (L2-resident)
-  float v[32];
+template <int BLOCK_N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BLOCK_N / 2], uint64_t adesc, uint64_t bdesc,
+                                           uint32_t accumulate) {
+  if constexpr (BLOCK_N == 64) ptx::wgmma_m64n64k16(d, adesc, bdesc, accumulate);
+  else ptx::wgmma_m64n128k16(d, adesc, bdesc, accumulate);
+}
+
+// Epilogue of one consumer warpgroup from its 64 x BLOCK_N accumulator in the wgmma fragment
+// layout: lane l of warp w holds tile rows 16 w + l / 4 (h = 0) and + 8 (h = 1), columns
+// 8 j + 2 (l % 4) + {0, 1} in acc[4 j + 2 h + {0, 1}].  row[h] / row_ok[h]: the global rows.
+template <int BLOCK_N>
+__device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[BLOCK_N / 2],
+                                         const long long (&row)[2], const bool (&row_ok)[2], int n0,
+                                         int frame, int lane, long long out_off) {
+  const bool vec_r = p.residual != nullptr && (p.ldr & 1) == 0 && (reinterpret_cast<uintptr_t>(p.residual) & 7) == 0;
+  const bool vec_o = p.out_f32 != nullptr && (p.ldo & 1) == 0 && (reinterpret_cast<uintptr_t>(p.out_f32) & 7) == 0;
+  const bool vec_p = p.out_planes != nullptr && (p.ldp & 1) == 0 && (p.out_plane_stride & 1) == 0 &&
+                     (reinterpret_cast<uintptr_t>(p.out_planes) & 3) == 0;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(acc[j]);
-  if (p.bias != nullptr) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      const float4 b = *reinterpret_cast<const float4*>(bias_s + j);  // broadcast LDS.128
-      v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int c = n0 + 8 * j + 2 * (lane & 3);
+    const bool ok0 = c < p.N, ok1 = c + 1 < p.N;
+    float b0 = 0.f, b1 = 0.f;
+    if (p.bias != nullptr) {
+      if (ok0) b0 = __ldg(p.bias + c);
+      if (ok1) b1 = __ldg(p.bias + c + 1);
     }
-  }
-  if (p.act == 1) {
+    float st[4] = {0.f, 0.f, 0.f, 0.f};  // column c, c + 1: sum, then sum of squares
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = gelu_tanh(v[j]);
-  }
-  if (p.residual != nullptr && row_ok) {
-    const float* r = p.residual + row * (long long)p.ldr + col0;
-    if (full && (p.ldr & 7) == 0) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        uint32_t w[8];
-        ptx::ld_global_v8(r + j, w);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) v[j + e] += __uint_as_float(w[e]);
-      }
-    } else if (full && (p.ldr & 3) == 0) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        float4 b = *reinterpret_cast<const float4*>(r + j);
-        v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (col0 + j < p.N) v[j] += r[j];
-    }
-  }
-  if (p.out_f32 != nullptr && row_ok) {
-    float* o = p.out_f32 + out_off + row * (long long)p.ldo + col0;
-    if (full && (p.ldo & 7) == 0) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        uint32_t w[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) w[e] = __float_as_uint(v[j + e]);
-        ptx::st_global_v8(o + j, w);
-      }
-    } else if (full && (p.ldo & 3) == 0) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        *reinterpret_cast<float4*>(o + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (col0 + j < p.N) o[j] = v[j];
-    }
-  }
-  if (p.stats != nullptr) {
-    // InstanceNorm statistics of the tensor this GEMM produces (nets.py:280-286), fused here so
-    // the activation is not re-read: per column, sum and sum of squares over this warp's 32
-    // rows by a warp transpose-reduce (lane l ends up owning column col0 + l), then one fp64
-    // atomic pair per lane.
-    // two passes (sum, then sum of squares) so only one 32-entry scratch array is live
-    float tot[2];
-#pragma unroll
-    for (int pass = 0; pass < 2; ++pass) {
-      float t[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const float x = (row_ok && col0 + j < p.N) ? v[j] : 0.f;
-        t[j] = pass == 0 ? x : x * x;
-      }
-#pragma unroll
-      for (int sft = 16; sft >= 1; sft >>= 1) {
-#pragma unroll
-        for (int j = 0; j < sft; ++j) {
-          const bool up = (lane & sft) != 0;
-          const float send = up ? t[j] : t[j + sft], keep = up ? t[j + sft] : t[j];
-          t[j] = keep + __shfl_xor_sync(0xffffffffu, send, sft);
+    for (int h = 0; h < 2; ++h) {
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if (!row_ok[h] || !ok0) continue;
+      if (p.bias != nullptr) { v0 += b0; v1 += b1; }
+      if (p.act == 1) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
+      const long long r = row[h];
+      if (p.residual != nullptr) {
+        const float* rp = p.residual + r * (long long)p.ldr + c;
+        if (ok1 && vec_r) {
+          const float2 t = *reinterpret_cast<const float2*>(rp);
+          v0 += t.x; v1 += t.y;
+        } else {
+          v0 += rp[0];
+          if (ok1) v1 += rp[1];
         }
       }
-      tot[pass] = t[0];
-    }
-    const int col = col0 + lane;
-    if (col < p.N) {
-      double* dst = p.stats + ((long long)frame * p.N + col) * 2;
-      atomicAdd(dst, (double)tot[0]);
-      atomicAdd(dst + 1, (double)tot[1]);
-    }
-  }
-  if (p.out_planes != nullptr && row_ok) {
-    // successive bf16 terms of v: plane q holds bf16(v - sum_{r<q} plane r)
-    for (int q = 0; q < p.out_P; ++q) {
-      __nv_bfloat16* o = p.out_planes + q * p.out_plane_stride + row * (long long)p.ldp + col0;
-      if (full && (p.ldp & 15) == 0) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 16) {
-          uint32_t w[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) w[e] = bf16x2_split(v[j + 2 * e], v[j + 2 * e + 1]);
-          ptx::st_global_v8(o + j, w);
+      if (p.out_f32 != nullptr) {
+        float* o = p.out_f32 + out_off + r * (long long)p.ldo + c;
+        if (ok1 && vec_o) {
+          *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+        } else {
+          o[0] = v0;
+          if (ok1) o[1] = v1;
         }
-      } else if (full && (p.ldp & 7) == 0) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 8) {
-          uint4 w;
-          w.x = bf16x2_split(v[j], v[j + 1]);
-          w.y = bf16x2_split(v[j + 2], v[j + 3]);
-          w.z = bf16x2_split(v[j + 4], v[j + 5]);
-          w.w = bf16x2_split(v[j + 6], v[j + 7]);
-          *reinterpret_cast<uint4*>(o + j) = w;
+      }
+      if (p.stats != nullptr) {
+        // InstanceNorm statistics of the tensor this GEMM produces (nets.py:280-286), fused here
+        // so the activation is not re-read
+        st[0] += v0; st[2] += v0 * v0;
+        if (ok1) { st[1] += v1; st[3] += v1 * v1; }
+      }
+      if (p.out_planes != nullptr) {
+        // successive bf16 terms of v: plane q holds bf16(v - sum_{s<q} plane s)
+        for (int q = 0; q < p.out_P; ++q) {
+          __nv_bfloat16* o = p.out_planes + q * p.out_plane_stride + r * (long long)p.ldp + c;
+          if (ok1 && vec_p) {
+            *reinterpret_cast<uint32_t*>(o) = bf16x2_split(v0, v1);
+          } else {
+            const __nv_bfloat16 h0 = __float2bfloat16_rn(v0);
+            v0 -= __bfloat162float(h0);
+            o[0] = h0;
+            if (ok1) {
+              const __nv_bfloat16 h1 = __float2bfloat16_rn(v1);
+              v1 -= __bfloat162float(h1);
+              o[1] = h1;
+            }
+          }
         }
-      } else {
+      }
+    }
+    if (p.stats != nullptr) {
+      // sum over the warp's 16 rows: the 8 lanes that share (l % 4) hold the same columns
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          __nv_bfloat16 h = __float2bfloat16_rn(v[j]);
-          v[j] -= __bfloat162float(h);
-          if (col0 + j < p.N) o[j] = h;
+      for (int s = 4; s < 32; s <<= 1)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) st[e] += __shfl_xor_sync(0xffffffffu, st[e], s);
+      if (lane < 4 && ok0) {
+        double* dst = p.stats + ((long long)frame * p.N + c) * 2;
+        atomicAdd(dst, (double)st[0]);
+        atomicAdd(dst + 1, (double)st[2]);
+        if (ok1) {
+          atomicAdd(dst + 2, (double)st[1]);
+          atomicAdd(dst + 3, (double)st[3]);
         }
       }
     }
   }
 }
 
-// CL = 2-CTA cluster: the two CTAs work on vertically adjacent tiles (same columns), each loads
-// half of the shared B tile and multicasts it to both, which removes a quarter of the L2 -> SM
-// operand traffic (the K <= 2048 GEMMs are L2-bound, DESIGN.md 4.1).
-template <int BLOCK_N, int P, bool CL>
-__global__ void __launch_bounds__(num_threads(BLOCK_N), 1)
+// Global row of tile row r (0..127) of output tile `m_tile`, and whether it exists.
+__device__ __forceinline__ void tile_row(const TcParams& p, int m_tile, int r, long long& row, bool& ok) {
+  if (p.mode == kGemmConv3x3) {
+    const int per_frame = p.tiles_x * p.tiles_y;
+    const int frame = m_tile / per_frame;
+    const int rr = m_tile % per_frame;
+    const int y = (rr / p.tiles_x) * p.tileH + r / p.tileW;
+    const int x = (rr % p.tiles_x) * p.tileW + r % p.tileW;
+    ok = (y < p.H) && (x < p.W);
+    row = ((long long)frame * p.H + y) * p.W + x;
+  } else {
+    row = (long long)m_tile * kBlockM + r;
+    ok = row < p.M;
+  }
+}
+
+template <int BLOCK_N, int P>
+__global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ TcParams p) {
   using Cfg = TcCfg<BLOCK_N, P>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = ptx::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + Cfg::kStages;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;
-  uint64_t* tmem_empty_bar = tmem_full_bar + kNumAccStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + kNumAccStages);
-  float* bias_smem = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes + kBarrierBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+  uint64_t* empty_bar = full_bar + Cfg::kStages;
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
+  const int warp = (threadIdx.x >> 5) & 3;  // within the warpgroup
   const int lane = threadIdx.x & 31;
-
-  // Role layout: epilogue warps FIRST (0 .. kEpiWarps-1), then the TMA producer and the MMA issuer.
-  // The warp scheduler favours high warp ids, and a starved single-lane MMA issuer stalls the
-  // tensor pipe: with the issuer as warp 1 every epilogue instruction delayed the main loop.
-  constexpr int kProducerWarp = Cfg::kEpiWarps;
-  constexpr int kMmaWarp = Cfg::kEpiWarps + 1;
   if (threadIdx.x == 0) {
     for (int s = 0; s < Cfg::kStages; ++s) {
       ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], CL ? 2 : 1);  // cluster: both CTAs' MMAs release the slot
-    }
-    for (int a = 0; a < kNumAccStages; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);
-      ptx::mbar_init(&tmem_empty_bar[a], Cfg::kEpiWarps);  // one arrive per epilogue warp
+      ptx::mbar_init(&empty_bar[s], kConsumerArrivals);
     }
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&p.tmA);
     ptx::prefetch_tensormap(&p.tmB);
-    if (CL) ptx::prefetch_tensormap(&p.tmBh);
   }
-  if (warp == kMmaWarp) {
-    ptx::tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
-  if (CL) ptx::cluster_sync(); else __syncthreads();  // barrier inits visible to the peer CTA
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
   const int nkb = p.num_k_blocks;
-  // work items: plain = tiles, cluster = tile pairs (m_tile = 2*pair + rank, same n_tile)
-  const int rank = CL ? (int)ptx::cluster_ctarank() : 0;
-  const int work_first = CL ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int work_stride = CL ? (int)(gridDim.x >> 1) : (int)gridDim.x;
   // split-K (small problems that cannot fill the GPU): work item = (tile, k-slice)
   const int S = p.split_k;
-  const int num_work = (CL ? (p.num_m_tiles + 1) / 2 : p.num_m_tiles) * p.num_n_tiles * S;
+  const int num_work = p.num_m_tiles * p.num_n_tiles * S;
   auto decode = [&](int w, int& m_tile, int& n0, int& kb0, int& kb1) {
     const int split = w % S;
     const int tile = w / S;
-    const int mm = tile / p.num_n_tiles;
-    m_tile = CL ? 2 * mm + rank : mm;
-    n0 = (tile - mm * p.num_n_tiles) * BLOCK_N;
+    m_tile = tile / p.num_n_tiles;
+    n0 = (tile - m_tile * p.num_n_tiles) * BLOCK_N;
     kb0 = (int)((long long)nkb * split / S);
     kb1 = (int)((long long)nkb * (split + 1) / S);
     return split;
   };
 
-  if (warp == kProducerWarp && lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x != 0) return;
     // ------------------------------------------------------------------ TMA producer
     int stage = 0;
     uint32_t phase = 0;
-    for (int w = work_first; w < num_work; w += work_stride) {
+    for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
       int m_tile, n0, kb0, kb1;
       decode(w, m_tile, n0, kb0, kb1);
       int frame = 0, y0 = 0, x0 = 0;
@@ -326,419 +265,80 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
             ptx::tma_load_3d(sa + pl * Cfg::kABytes, &p.tmA, &full_bar[stage], kb * kBlockK,
                              m_tile * kBlockM, pl);
         }
-        if (CL) {
-          // my half of the B tile, delivered to both CTAs (the peer sends me the other half)
 #pragma unroll
-          for (int pl = 0; pl < P; ++pl)
-            ptx::tma_load_3d_multicast(sb + pl * Cfg::kBBytes + rank * (Cfg::kBBytes / 2), &p.tmBh,
-                                       &full_bar[stage], kb * kBlockK, n0 + rank * (BLOCK_N / 2), pl,
-                                       (uint16_t)0x3);
-        } else {
-#pragma unroll
-          for (int pl = 0; pl < P; ++pl)
-            ptx::tma_load_3d(sb + pl * Cfg::kBBytes, &p.tmB, &full_bar[stage], kb * kBlockK, n0, pl);
-        }
+        for (int pl = 0; pl < P; ++pl)
+          ptx::tma_load_3d(sb + pl * Cfg::kBBytes, &p.tmB, &full_bar[stage], kb * kBlockK, n0, pl);
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == kMmaWarp && lane == 0) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = ptx::make_idesc_bf16(kBlockM, BLOCK_N);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int w = work_first; w < num_work; w += work_stride, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      ptx::mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1u, p.err, 102);
-      ptx::tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-      int m_tile_unused, n0_unused, kb0, kb1;
-      decode(w, m_tile_unused, n0_unused, kb0, kb1);
-      for (int kb = kb0; kb < kb1; ++kb) {
-        ptx::mbar_wait(&full_bar[stage], phase, p.err, 103);
-        ptx::tc_fence_after();
-        const uint32_t sa = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint32_t sb = sa + P * Cfg::kABytes;
-        uint32_t accumulate = (kb > kb0) ? 1u : 0u;
-#pragma unroll
-        for (int i = 0; i < P; ++i) {
-#pragma unroll
-          for (int j = 0; j < P - i; ++j) {
-            const uint64_t adesc = ptx::make_smem_desc_sw128(sa + i * Cfg::kABytes);
-            const uint64_t bdesc = ptx::make_smem_desc_sw128(sb + j * Cfg::kBBytes);
-#pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-              // advance 16 bf16 = 32 B inside the 128 B swizzle row: +2 in 16-byte units
-              ptx::umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, accumulate);
-              accumulate = 1u;
-            }
-          }
-        }
-        // smem slot reusable once these MMAs retire (cluster: tell both producers)
-        if (CL) ptx::umma_commit_multicast(&empty_bar[stage], (uint16_t)0x3); else ptx::umma_commit(&empty_bar[stage]);
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
-      }
-      ptx::umma_commit(&tmem_full_bar[acc]);  // accumulator complete -> epilogue
-    }
-  } else if (warp < Cfg::kEpiWarps) {
-    // ------------------------------------------------------------------ epilogue
-    // TMEM lane quadrant q = warp % 4 (hardware restriction: a warp may only touch lanes
-    // [32*(warp%4), +32)), column group = warp / 4.  TMEM loads are software
-    // pipelined: chunk i+1 is in flight while chunk i goes through bias / GELU / stores.
-    constexpr int kChunks = Cfg::kChunks;
-    const int q = warp & 3;
-    const int cbase = (warp >> 2) * kChunks;
-    float* bias_w = bias_smem + warp * (kChunks * 32);  // private to this warp
-    int it = 0;
-    for (int w = work_first; w < num_work; w += work_stride, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      int m_tile, n0, kb0, kb1;
-      const int split = decode(w, m_tile, n0, kb0, kb1);
-      const bool tile_valid = m_tile < p.num_m_tiles;  // cluster: odd tile count leaves a ghost
-      const int r = q * 32 + lane;
-      long long row;
-      bool row_ok;
-      int frame = 0;
-      if (p.mode == kGemmConv3x3) {
-        const int per_frame = p.tiles_x * p.tiles_y;
-        frame = m_tile / per_frame;
-        const int rr = m_tile % per_frame;
-        const int y = (rr / p.tiles_x) * p.tileH + r / p.tileW;
-        const int x = (rr % p.tiles_x) * p.tileW + r % p.tileW;
-        row_ok = (y < p.H) && (x < p.W) && tile_valid;
-        row = ((long long)frame * p.H + y) * p.W + x;
-      } else {
-        row = (long long)m_tile * kBlockM + r;
-        row_ok = row < p.M;
-        if (p.stats != nullptr) frame = (int)(((long long)m_tile * kBlockM) / p.rows_per_frame);
-      }
-      const int colbase = n0 + cbase * 32;
-      if (p.bias != nullptr) {  // stage this warp's bias slice while the main loop runs
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < kChunks; ++j) {
-          const int c = colbase + j * 32 + lane;
-          bias_w[j * 32 + lane] = (c < p.N) ? __ldg(p.bias + c) : 0.f;
-        }
-        __syncwarp();
-      }
-      ptx::mbar_wait(&tmem_full_bar[acc], acc_phase, p.err, 104);
-      ptx::tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BLOCK_N + cbase * 32;
-      uint32_t va[32], vb[32];
-      if (p.debug_mode == 1 || !tile_valid) {
-        ptx::tc_fence_before();
-        __syncwarp();
-        if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc]);
-        continue;
-      }
-      if (colbase < p.N) ptx::tmem_ld_32x32(taddr, va);  // all conditions are warp-uniform
-#pragma unroll
-      for (int i = 0; i < kChunks; i += 2) {
-        const int col0 = colbase + i * 32;
-        if (col0 < p.N) {
-          ptx::tmem_ld_wait();
-          if (i + 1 < kChunks && col0 + 32 < p.N) ptx::tmem_ld_32x32(taddr + (i + 1) * 32, vb);
-          if (row_ok || p.stats != nullptr) store_row_chunk(p, row, col0, va, bias_w + i * 32, row_ok, frame, lane, split * p.split_stride);
-        }
-        if (i + 1 < kChunks) {
-          const int col1 = col0 + 32;
-          if (col1 < p.N) {
-            ptx::tmem_ld_wait();
-            if (i + 2 < kChunks && col1 + 32 < p.N) ptx::tmem_ld_32x32(taddr + (i + 2) * 32, va);
-            if (row_ok || p.stats != nullptr) store_row_chunk(p, row, col1, vb, bias_w + (i + 1) * 32, row_ok, frame, lane, split * p.split_stride);
-          }
-        }
-      }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc]);
-    }
+    return;
   }
 
-  ptx::tc_fence_before();
-  // cluster: nobody may exit while the peer can still multicast into its shared memory / barriers
-  if (CL) ptx::cluster_sync(); else __syncthreads();
-  if (warp == kMmaWarp) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, Cfg::kTmemCols);
+  // -------------------------------------------------------------------- consumers
+  const int cw = wg - 1;                        // rows [64 cw, 64 cw + 64) of the tile
+  const uint32_t a_off = (uint32_t)cw * 64 * 128;  // their A rows: eight whole swizzle atoms
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BLOCK_N / 2];
+  for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+    int m_tile, n0, kb0, kb1;
+    const int split = decode(w, m_tile, n0, kb0, kb1);
+#pragma unroll
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      ptx::mbar_wait(&full_bar[stage], phase, p.err, 103);
+      const uint32_t sa = ptx::smem_u32(smem + stage * Cfg::kStageBytes) + a_off;
+      const uint32_t sb = ptx::smem_u32(smem + stage * Cfg::kStageBytes) + P * Cfg::kABytes;
+      uint32_t accumulate = (kb > kb0) ? 1u : 0u;
+      ptx::wgmma_fence();
+#pragma unroll
+      for (int i = 0; i < P; ++i) {
+#pragma unroll
+        for (int j = 0; j < P - i; ++j) {
+          const uint64_t adesc = ptx::make_smem_desc_sw128(sa + i * Cfg::kABytes);
+          const uint64_t bdesc = ptx::make_smem_desc_sw128(sb + j * Cfg::kBBytes);
+#pragma unroll
+          for (int k = 0; k < kBlockK / kMmaK; ++k) {
+            wgmma_bf16<BLOCK_N>(acc, adesc + 2 * k, bdesc + 2 * k, accumulate);
+            accumulate = 1u;
+          }
+        }
+      }
+      ptx::wgmma_commit();
+      // the previous k-block's MMAs have retired once at most this group is pending
+      ptx::wgmma_wait<1>();
+      ptx::reg_fence(acc);
+      if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
+    }
+    ptx::wgmma_wait<0>();
+    ptx::reg_fence(acc);
+    if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
+
+    const int r0 = cw * 64 + warp * 16 + (lane >> 2);
+    long long row[2];
+    bool row_ok[2];
+    tile_row(p, m_tile, r0, row[0], row_ok[0]);
+    tile_row(p, m_tile, r0 + 8, row[1], row_ok[1]);
+    int frame = 0;
+    if (p.stats != nullptr)
+      frame = (p.mode == kGemmConv3x3) ? m_tile / (p.tiles_x * p.tiles_y)
+                                       : (int)(((long long)m_tile * kBlockM) / p.rows_per_frame);
+    epilogue<BLOCK_N>(p, acc, row, row_ok, n0, frame, lane, split * p.split_stride);
   }
 }
-
-// ------------------------------------------------------------------------------ 2-SM kernel
-// cta_group::2: a cluster of two CTAs (one TPC) computes a 256 x BN tile.  Each CTA loads its own
-// 128 rows of A and HALF of the B tile (BN/2 rows); the pair's tensor cores read both halves, so
-// the L2 -> SM operand requests per FLOP drop by 25 % (BN = 128) / 50 % (BN = 256) and a stage is
-// 48-64 KB.  One thread of the leader CTA (rank 0) issues the MMAs; TMA completions of both CTAs
-// land on the leader's full barrier; tcgen05.commit multicasts slot-free / accumulator-ready to
-// both CTAs; every CTA runs its own epilogue on its 128 TMEM lanes and reports back to the
-// leader's tmem_empty barrier.
-template <int BN, int P>
-struct Tc2Cfg {
-  static constexpr int kABytes = kBlockM * kBlockK * 2;
-  static constexpr int kBhBytes = (BN / 2) * kBlockK * 2;
-  static constexpr int kStageBytes = P * (kABytes + kBhBytes);
-  static constexpr int kEpiWarps = 16;
-  static constexpr int kChunks = BN / 32 / 4;
-  static constexpr int kBiasBytes = kEpiWarps * kChunks * 32 * 4;
-  static constexpr int kAvail = kSmemLimit - 1024 - kBarrierBytes - kBiasBytes;
-  static constexpr int kStagesRaw = kAvail / kStageBytes;
-  static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
-  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kBarrierBytes + kBiasBytes;
-  static constexpr int kTmemCols = kNumAccStages * BN;  // 256 or 512
-  static constexpr int kThreads = 64 + 32 * kEpiWarps;
-  static_assert(kStages >= 2, "tile does not fit in shared memory");
-  static_assert(BN == 128 || BN == 256, "pair tile width");
-};
-
-template <int BN, int P>
-__global__ void __launch_bounds__(Tc2Cfg<BN, P>::kThreads, 1)
-gemm_tc2_kernel(const __grid_constant__ TcParams p) {
-  using Cfg = Tc2Cfg<BN, P>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = ptx::smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + Cfg::kStages;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::kStages;
-  uint64_t* tmem_empty_bar = tmem_full_bar + kNumAccStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + kNumAccStages);
-  float* bias_smem = reinterpret_cast<float*>(smem + Cfg::kStages * Cfg::kStageBytes + kBarrierBytes);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int rank = (int)ptx::cluster_ctarank();
-  const bool leader = rank == 0;
-  constexpr int kProducerWarp = Cfg::kEpiWarps;
-  constexpr int kMmaWarp = Cfg::kEpiWarps + 1;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      ptx::mbar_init(&full_bar[s], 1);   // leader's producer (expect_tx for both CTAs' bytes)
-      ptx::mbar_init(&empty_bar[s], 1);  // pair commit, multicast
-    }
-    for (int a = 0; a < kNumAccStages; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);                    // pair commit, multicast
-      ptx::mbar_init(&tmem_empty_bar[a], 2 * Cfg::kEpiWarps);  // epilogue warps of BOTH CTAs
-    }
-    ptx::fence_barrier_init();
-    ptx::prefetch_tensormap(&p.tmA);
-    ptx::prefetch_tensormap(&p.tmBh);
-  }
-  if (warp == kMmaWarp) {  // both CTAs, same warp id: collective allocation for the pair
-    ptx::tmem_alloc_2sm(tmem_slot, Cfg::kTmemCols);
-    ptx::tmem_relinquish_2sm();
-  }
-  ptx::tc_fence_before();
-  ptx::cluster_sync();
-  __syncthreads();  // redundant after the cluster barrier; lets compute-sanitizer racecheck see the
-                    // ordering between tcgen05.alloc's write of tmem_slot and the reads below
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  const int nkb = p.num_k_blocks;
-  const int n_tiles = (p.N + BN - 1) / BN;
-  const int num_tiles = ((p.num_m_tiles + 1) / 2) * n_tiles;
-  const int num_work = p.tail_first + (num_tiles - p.tail_first) * p.tail_k;
-  const int work_first = (int)(blockIdx.x >> 1), work_stride = (int)(gridDim.x >> 1);
-  // work item -> (row pair tile, first column, width).  Full tiles first, then the tail pieces.
-  // The K-summation order of an output element does not depend on the piece it falls into, so the
-  // result is bit-identical with and without the tail split.
-  auto decode = [&](int w, int& m_tile, int& n0, int& width) {
-    int tile = w, c0 = 0;
-    width = BN;
-    if (w >= p.tail_first) {
-      const int pw = w - p.tail_first;
-      const int t = pw / p.tail_k, part = pw - t * p.tail_k;
-      tile = p.tail_first + t;
-      c0 = part * p.tail_base + (part < p.tail_extra ? part : p.tail_extra);
-      width = 32 * (p.tail_base + (part < p.tail_extra ? 1 : 0));
-    }
-    const int mm = tile / n_tiles;
-    m_tile = 2 * mm + rank;
-    n0 = (tile - mm * n_tiles) * BN + c0 * 32;
-    if (n0 >= p.N) width = 0;  // piece entirely right of the matrix: every role skips it
-  };
-
-  if (warp == kProducerWarp && lane == 0) {
-    // ------------------------------------------------------------------ TMA producer (each CTA)
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int w = work_first; w < num_work; w += work_stride) {
-      int m_tile, n0, width;
-      decode(w, m_tile, n0, width);
-      if (width == 0) continue;
-      int frame = 0, y0 = 0, x0 = 0;
-      if (p.mode == kGemmConv3x3) {
-        const int per_frame = p.tiles_x * p.tiles_y;
-        frame = m_tile / per_frame;
-        const int r = m_tile % per_frame;
-        y0 = (r / p.tiles_x) * p.tileH;
-        x0 = (r % p.tiles_x) * p.tileW;
-      }
-      const int half = width / 2;  // B rows this CTA loads (each row = one 128-byte swizzle row)
-      const uint32_t stage_tx = 2u * P * (uint32_t)(Cfg::kABytes + half * kBlockK * 2);
-      for (int kb = 0; kb < nkb; ++kb) {
-        ptx::mbar_wait(&empty_bar[stage], phase ^ 1u, p.err, 201);
-        if (leader) ptx::mbar_arrive_expect_tx(&full_bar[stage], stage_tx);
-        uint8_t* sa = smem + stage * Cfg::kStageBytes;
-        uint8_t* sb = sa + P * Cfg::kABytes;
-        if (p.mode == kGemmConv3x3) {
-          const int tap = kb / p.cblocks;
-          const int cb = kb - tap * p.cblocks;
-          const int ky = tap / 3, kx = tap - ky * 3;
-#pragma unroll
-          for (int pl = 0; pl < P; ++pl)
-            ptx::tma_load_5d_2sm(sa + pl * Cfg::kABytes, &p.tmA, &full_bar[stage], cb * kBlockK,
-                                 x0 + kx - 1, y0 + ky - 1, frame, pl);
-        } else {
-#pragma unroll
-          for (int pl = 0; pl < P; ++pl)
-            ptx::tma_load_3d_2sm(sa + pl * Cfg::kABytes, &p.tmA, &full_bar[stage], kb * kBlockK,
-                                 m_tile * kBlockM, pl);
-        }
-        if (width == BN) {
-#pragma unroll
-          for (int pl = 0; pl < P; ++pl)
-            ptx::tma_load_3d_2sm(sb + pl * Cfg::kBhBytes, &p.tmBh, &full_bar[stage], kb * kBlockK,
-                                 n0 + rank * (BN / 2), pl);
-        } else {  // tail piece: this CTA's half of the piece in 16-row slabs (2 KB each)
-#pragma unroll
-          for (int pl = 0; pl < P; ++pl)
-            for (int r16 = 0; r16 < half; r16 += 16)
-              ptx::tma_load_3d_2sm(sb + pl * Cfg::kBhBytes + r16 * (kBlockK * 2), &p.tmB16, &full_bar[stage],
-                                   kb * kBlockK, n0 + rank * half + r16, pl);
-        }
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
-      }
-    }
-  } else if (warp == kMmaWarp && lane == 0 && leader) {
-    // ------------------------------------------------------------------ MMA issuer (leader only)
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int w = work_first; w < num_work; w += work_stride) {
-      int m_tile_unused, n0_unused, width;
-      decode(w, m_tile_unused, n0_unused, width);
-      if (width == 0) continue;
-      const uint32_t idesc = ptx::make_idesc_bf16(2 * kBlockM, width);
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      ++it;
-      ptx::mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1u, p.err, 202);
-      ptx::tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < nkb; ++kb) {
-        ptx::mbar_wait(&full_bar[stage], phase, p.err, 203);
-        ptx::tc_fence_after();
-        const uint32_t sa = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint32_t sb = sa + P * Cfg::kABytes;
-        uint32_t accumulate = (kb > 0) ? 1u : 0u;
-#pragma unroll
-        for (int i = 0; i < P; ++i) {
-#pragma unroll
-          for (int j = 0; j < P - i; ++j) {
-            const uint64_t adesc = ptx::make_smem_desc_sw128(sa + i * Cfg::kABytes);
-            const uint64_t bdesc = ptx::make_smem_desc_sw128(sb + j * Cfg::kBhBytes);
-#pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-              ptx::umma_f16_2sm(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, accumulate);
-              accumulate = 1u;
-            }
-          }
-        }
-        ptx::umma_commit_2sm(&empty_bar[stage]);  // both producers may refill the slot
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
-      }
-      ptx::umma_commit_2sm(&tmem_full_bar[acc]);  // both epilogues may read their TMEM half
-    }
-  } else if (warp < Cfg::kEpiWarps) {
-    // ------------------------------------------------------------------ epilogue (each CTA)
-    constexpr int kChunks = Cfg::kChunks;
-    const int q = warp & 3;
-    const int cg = warp >> 2;  // column group: 32-column chunks cg, cg + 4, cg + 8, ...
-    float* bias_w = bias_smem + warp * (kChunks * 32);
-    int it = 0;
-    for (int w = work_first; w < num_work; w += work_stride) {
-      int m_tile, n0, width;
-      decode(w, m_tile, n0, width);
-      if (width == 0) continue;
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      ++it;
-      const bool tile_valid = m_tile < p.num_m_tiles;
-      const int r = q * 32 + lane;
-      long long row;
-      bool row_ok;
-      int frame = 0;
-      if (p.mode == kGemmConv3x3) {
-        const int per_frame = p.tiles_x * p.tiles_y;
-        frame = m_tile / per_frame;
-        const int rr = m_tile % per_frame;
-        const int y = (rr / p.tiles_x) * p.tileH + r / p.tileW;
-        const int x = (rr % p.tiles_x) * p.tileW + r % p.tileW;
-        row_ok = (y < p.H) && (x < p.W) && tile_valid;
-        row = ((long long)frame * p.H + y) * p.W + x;
-      } else {
-        row = (long long)m_tile * kBlockM + r;
-        row_ok = row < p.M;
-        if (p.stats != nullptr) frame = (int)(((long long)m_tile * kBlockM) / p.rows_per_frame);
-      }
-      if (p.bias != nullptr) {
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < kChunks; ++j) {
-          const int c = n0 + (cg + 4 * j) * 32 + lane;
-          bias_w[j * 32 + lane] = (c < p.N) ? __ldg(p.bias + c) : 0.f;
-        }
-        __syncwarp();
-      }
-      ptx::mbar_wait(&tmem_full_bar[acc], acc_phase, p.err, 204);
-      ptx::tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-      if (tile_valid && p.debug_mode != 1) {
-#pragma unroll 1
-        for (int i = 0; i < kChunks; ++i) {
-          const int chunk = cg + 4 * i;
-          const int col0 = n0 + chunk * 32;
-          if (chunk * 32 >= width || col0 >= p.N) break;  // warp-uniform
-          uint32_t v[32];
-          ptx::tmem_ld_32x32(taddr + chunk * 32, v);
-          ptx::tmem_ld_wait();
-          if (row_ok || p.stats != nullptr)
-            store_row_chunk(p, row, col0, v, bias_w + i * 32, row_ok, frame, lane, 0);
-        }
-      }
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (leader) ptx::mbar_arrive(&tmem_empty_bar[acc]);
-        else ptx::mbar_arrive_leader(&tmem_empty_bar[acc]);
-      }
-    }
-  }
-
-  ptx::tc_fence_before();
-  ptx::cluster_sync();  // no CTA may exit while the pair's MMAs / commits can still touch it
-  if (warp == kMmaWarp) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc_2sm(tmem_base, Cfg::kTmemCols);
-  }
-}
-
 
 // ------------------------------------------------------------------------------ halo-patch conv
 // 3x3 convolution, C = 64 -> N = 64 (the first ResNet group, stride 1).  The generic implicit GEMM
-// loads one shifted 128-pixel box per tap: every input element crosses L2 -> SM nine times and
-// these layers ran at the L2 limit (2.7 GB per launch, 300 us against a 109 us MMA bound).  Here a
-// tile of 8 x 16 output pixels stages its 10 x 18 input patch ONCE (18 TMA loads of one patch row
-// each into rows padded to 16 pixels = 2048 B, so that every 8-pixel group of every tap view has the
-// same swizzle phase) and the nine taps are nine shared-memory views of it: start = patch +
-// ky * 2048 + kx * 128, 2048 B between row groups (ptx::make_smem_desc_sw128_view).
-// B (weights, 8 KB per tap and plane) streams through a 4-slot ring.  Epilogue as in gemm_tc_kernel.
+// loads one shifted 128-pixel box per tap, so every input element crosses L2 -> SM nine times.
+// Here a tile of 8 x 16 output pixels stages its 10 x 18 input patch ONCE (18 TMA loads of one
+// patch row each into rows padded to 16 pixels = 2048 B, so that every 8-pixel group of every tap
+// view has the same swizzle phase) and the nine taps are nine shared-memory views of it: consumer
+// c (output rows 8c .. 8c + 7 of the tile) reads start = patch + (8c + ky) * 2048 + kx * 128, with
+// 2048 B between its 8-pixel row groups.  B (weights, 8 KB per tap and plane) streams through a
+// 4-slot ring.  Epilogue as in gemm_tc_kernel.
 constexpr int kHaloTileW = 8, kHaloTileH = 16;
 constexpr int kHaloRowBytes = 2048;                        // 16 pixels x 128 B
 constexpr int kHaloPatchRows = kHaloTileH + 2;
@@ -750,15 +350,12 @@ template <int P>
 struct HaloCfg {
   static constexpr int kPatchStage = P * kHaloPatchBytes;
   static constexpr int kBStage = P * kHaloBBytes;
-  static constexpr int kEpiWarps = epi_warps(64);
-  static constexpr int kBiasBytes = kEpiWarps * 32 * 4;
-  static constexpr int kSmemBytes = 1024 + 2 * kPatchStage + kHaloBStages * kBStage + kBarrierBytes + kBiasBytes;
-  static constexpr int kThreads = num_threads(64);
+  static constexpr int kSmemBytes = 1024 + 2 * kPatchStage + kHaloBStages * kBStage + kBarrierBytes;
   static_assert(kSmemBytes <= kSmemLimit, "halo conv: shared memory");
 };
 
 template <int P>
-__global__ void __launch_bounds__(HaloCfg<P>::kThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
   using Cfg = HaloCfg<P>;
   extern __shared__ uint8_t smem_raw[];
@@ -771,38 +368,23 @@ conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
   uint64_t* pempty = bars + 2;               // [2]
   uint64_t* bfull = bars + 4;                // [4]
   uint64_t* bempty = bars + 8;               // [4]
-  uint64_t* tmem_full_bar = bars + 12;       // [2]
-  uint64_t* tmem_empty_bar = bars + 14;      // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-  float* bias_smem = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + kBarrierBytes);
 
-  const int warp = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7;
+  const int warp = (threadIdx.x >> 5) & 3;
   const int lane = threadIdx.x & 31;
-  constexpr int kProducerWarp = Cfg::kEpiWarps;
-  constexpr int kMmaWarp = Cfg::kEpiWarps + 1;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&pfull[s], 1); ptx::mbar_init(&pempty[s], 1); }
-    for (int s = 0; s < kHaloBStages; ++s) { ptx::mbar_init(&bfull[s], 1); ptx::mbar_init(&bempty[s], 1); }
-    for (int a = 0; a < kNumAccStages; ++a) {
-      ptx::mbar_init(&tmem_full_bar[a], 1);
-      ptx::mbar_init(&tmem_empty_bar[a], Cfg::kEpiWarps);
-    }
+    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&pfull[s], 1); ptx::mbar_init(&pempty[s], kConsumerArrivals); }
+    for (int s = 0; s < kHaloBStages; ++s) { ptx::mbar_init(&bfull[s], 1); ptx::mbar_init(&bempty[s], kConsumerArrivals); }
     ptx::fence_barrier_init();
     ptx::prefetch_tensormap(&p.tmPatch);
     ptx::prefetch_tensormap(&p.tmB);
   }
-  if (warp == kMmaWarp) {
-    ptx::tmem_alloc(tmem_slot, 128);  // two 64-column accumulators
-    ptx::tmem_relinquish();
-  }
-  ptx::tc_fence_before();
   __syncthreads();
-  ptx::tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int num_work = p.num_m_tiles;
   const int per_frame = p.tiles_x * p.tiles_y;
 
-  if (warp == kProducerWarp && lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x != 0) return;
     int ps = 0, bs = 0;
     uint32_t pphase = 0, bphase = 0;
     for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
@@ -825,82 +407,61 @@ conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
         if (++bs == kHaloBStages) { bs = 0; bphase ^= 1u; }
       }
     }
-  } else if (warp == kMmaWarp && lane == 0) {
-    constexpr uint32_t idesc = ptx::make_idesc_bf16(kBlockM, 64);
-    int ps = 0, bs = 0, it = 0;
-    uint32_t pphase = 0, bphase = 0;
-    for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      ptx::mbar_wait(&tmem_empty_bar[acc], acc_phase ^ 1u, p.err, 403);
-      ptx::mbar_wait(&pfull[ps], pphase, p.err, 404);
-      ptx::tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * 64;
-      const uint32_t pbase = ptx::smem_u32(patch + ps * Cfg::kPatchStage);
-      uint32_t accumulate = 0u;
-      for (int tap = 0; tap < 9; ++tap) {
-        const int ky = tap / 3, kx = tap - ky * 3;
-        ptx::mbar_wait(&bfull[bs], bphase, p.err, 405);
-        ptx::tc_fence_after();
-        const uint32_t sb = ptx::smem_u32(bring + bs * Cfg::kBStage);
+    return;
+  }
+
+  const int cw = wg - 1;
+  int ps = 0, bs = 0;
+  uint32_t pphase = 0, bphase = 0;
+  float acc[32];
+  for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
 #pragma unroll
-        for (int i = 0; i < P; ++i) {
+    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+    ptx::mbar_wait(&pfull[ps], pphase, p.err, 404);
+    const uint32_t pbase = ptx::smem_u32(patch + ps * Cfg::kPatchStage) + (uint32_t)cw * 8 * kHaloRowBytes;
+    uint32_t accumulate = 0u;
+    int prev = -1;
+    for (int tap = 0; tap < 9; ++tap) {
+      const int ky = tap / 3, kx = tap - ky * 3;
+      ptx::mbar_wait(&bfull[bs], bphase, p.err, 405);
+      const uint32_t sb = ptx::smem_u32(bring + bs * Cfg::kBStage);
+      ptx::wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < P - i; ++j) {
-            const uint64_t adesc = ptx::make_smem_desc_sw128_view(
-                pbase + i * kHaloPatchBytes + ky * kHaloRowBytes + kx * 128, kHaloRowBytes);
-            const uint64_t bdesc = ptx::make_smem_desc_sw128(sb + j * kHaloBBytes);
+      for (int i = 0; i < P; ++i) {
 #pragma unroll
-            for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-              ptx::umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, accumulate);
-              accumulate = 1u;
-            }
+        for (int j = 0; j < P - i; ++j) {
+          const uint64_t adesc = ptx::make_smem_desc_sw128(
+              pbase + i * kHaloPatchBytes + ky * kHaloRowBytes + kx * 128, kHaloRowBytes);
+          const uint64_t bdesc = ptx::make_smem_desc_sw128(sb + j * kHaloBBytes);
+#pragma unroll
+          for (int k = 0; k < kBlockK / kMmaK; ++k) {
+            ptx::wgmma_m64n64k16(acc, adesc + 2 * k, bdesc + 2 * k, accumulate);
+            accumulate = 1u;
           }
         }
-        ptx::umma_commit(&bempty[bs]);
-        if (++bs == kHaloBStages) { bs = 0; bphase ^= 1u; }
       }
-      ptx::umma_commit(&pempty[ps]);
-      ptx::umma_commit(&tmem_full_bar[acc]);
-      if (++ps == 2) { ps = 0; pphase ^= 1u; }
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<1>();
+      ptx::reg_fence(acc);
+      if (prev >= 0 && lane == 0) ptx::mbar_arrive(&bempty[prev]);
+      prev = bs;
+      if (++bs == kHaloBStages) { bs = 0; bphase ^= 1u; }
     }
-  } else if (warp < Cfg::kEpiWarps) {
-    const int q = warp & 3;
-    const int chunk = warp >> 2;  // 2 column groups x one 32-column chunk
-    float* bias_w = bias_smem + warp * 32;
-    int it = 0;
-    for (int w = blockIdx.x; w < num_work; w += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int frame = w / per_frame;
-      const int rr = w - frame * per_frame;
-      const int r = q * 32 + lane;
-      const int y = (rr / p.tiles_x) * kHaloTileH + r / kHaloTileW;
-      const int x = (rr % p.tiles_x) * kHaloTileW + r % kHaloTileW;
-      const bool row_ok = (y < p.H) && (x < p.W);
-      const long long row = ((long long)frame * p.H + y) * p.W + x;
-      const int col0 = chunk * 32;
-      if (p.bias != nullptr) {
-        __syncwarp();
-        bias_w[lane] = (col0 + lane < p.N) ? __ldg(p.bias + col0 + lane) : 0.f;
-        __syncwarp();
-      }
-      ptx::mbar_wait(&tmem_full_bar[acc], acc_phase, p.err, 406);
-      ptx::tc_fence_after();
-      uint32_t v[32];
-      ptx::tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * 64 + col0, v);
-      ptx::tmem_ld_wait();
-      if (row_ok || p.stats != nullptr) store_row_chunk(p, row, col0, v, bias_w, row_ok, frame, lane, 0);
-      ptx::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) ptx::mbar_arrive(&tmem_empty_bar[acc]);
+    ptx::wgmma_wait<0>();
+    ptx::reg_fence(acc);
+    if (lane == 0) {
+      ptx::mbar_arrive(&bempty[prev]);
+      ptx::mbar_arrive(&pempty[ps]);
     }
-  }
-  ptx::tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    ptx::tc_fence_after();
-    ptx::tmem_dealloc(tmem_base, 128);
+    if (++ps == 2) { ps = 0; pphase ^= 1u; }
+
+    const int frame = w / per_frame;
+    long long row[2];
+    bool row_ok[2];
+    const int r0 = cw * 64 + warp * 16 + (lane >> 2);
+    tile_row(p, w, r0, row[0], row_ok[0]);
+    tile_row(p, w, r0 + 8, row[1], row_ok[1]);
+    epilogue<64>(p, acc, row, row_ok, 0, frame, lane, 0);
   }
 }
 
@@ -1001,26 +562,12 @@ void choose_conv_tile(int H, int W, int* tw, int* th) {
   }
 }
 
-bool use_cluster() {
-  static int v = -1;
-  if (v < 0) {
-    // Opt-in experiment.  Measured (scripts/gemm_bench.py): identical times with and without the
-    // multicast, i.e. a 2-CTA TMA multicast does not reduce L2 request pressure on this part
-    // (consistent with B300_MICROARCH.md "at cluster size <= 4, multicast ~ unicast").
-    const char* e = getenv("TAPIR_B200_GEMM_CLUSTER");
-    v = (e != nullptr && atoi(e) != 0) ? 1 : 0;
-  }
-  return v == 1;
-}
-
 template <int BLOCK_N, int P>
 int launch(const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
   using Cfg = TcCfg<BLOCK_N, P>;
   static PerDeviceOnce configured;
   if (configured.pending()) {
-    TAPIR_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, P, false>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    TAPIR_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, P, true>,
+    TAPIR_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, P>,
                                     cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     configured.mark();
   }
@@ -1030,99 +577,32 @@ int launch(const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
   ProfileScope ps(g.tag ? g.tag : "gemm", stream, 2.0 * g.M * g.N * kl,
                   2.0 * P * (a_elems + (double)g.N * g.K) + out_b * g.M * g.N);
   const int sms = num_sms();
-  // pairs of vertically adjacent tiles share their B operand through a 2-CTA cluster
-  const bool cluster = use_cluster() && p.num_m_tiles >= 2 && (sms % 2 == 0);
-  if (cluster) {
-    const int pairs = ((p.num_m_tiles + 1) / 2) * p.num_n_tiles;
-    const int clusters = pairs < sms / 2 ? pairs : sms / 2;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(2 * clusters);
-    cfg.blockDim = dim3(num_threads(BLOCK_N));
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    TAPIR_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc_kernel<BLOCK_N, P, true>, p));
-  } else {
-    const int tiles = p.num_m_tiles * p.num_n_tiles * (p.split_k > 1 ? p.split_k : 1);  // work items
-    const int grid = tiles < sms ? tiles : sms;
-    gemm_tc_kernel<BLOCK_N, P, false><<<grid, num_threads(BLOCK_N), Cfg::kSmemBytes, stream>>>(p);
-  }
+  const int tiles = p.num_m_tiles * p.num_n_tiles * (p.split_k > 1 ? p.split_k : 1);  // work items
+  const int grid = tiles < sms ? tiles : sms;
+  gemm_tc_kernel<BLOCK_N, P><<<grid, kThreads, Cfg::kSmemBytes, stream>>>(p);
   count_launch();
   TAPIR_LAUNCH_CHECK("gemm_tc_kernel");
   return kOk;
 }
 
-int use_2sm() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TAPIR_B200_GEMM_2SM");
-    v = e != nullptr ? atoi(e) : 1;  // 0 = off, 1 = auto width (default), 128 / 256 = forced width
-  }
-  return v;
-}
-
-template <int BN, int P>
-int launch2(const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
-  using Cfg = Tc2Cfg<BN, P>;
-  static PerDeviceOnce configured;
-  if (configured.pending()) {
-    TAPIR_CUDA(cudaFuncSetAttribute(gemm_tc2_kernel<BN, P>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    Cfg::kSmemBytes));
-    configured.mark();
-  }
-  const double kl = g.k_logical > 0 ? g.k_logical : g.K;
-  const double out_b = (g.out_f32 ? 4.0 : 0.0) + (g.out_planes ? 2.0 * g.out_P : 0.0) + (g.residual ? 4.0 : 0.0);
-  const double a_elems = (g.mode == kGemmConv3x3) ? (double)g.M * g.C : (double)g.M * g.K;
-  ProfileScope ps(g.tag ? g.tag : "gemm", stream, 2.0 * g.M * g.N * kl,
-                  2.0 * P * (a_elems + (double)g.N * g.K) + out_b * g.M * g.N);
-  const int sms = num_sms();
-  const int pairs = ((p.num_m_tiles + 1) / 2) * ceil_div(g.N, BN);
-  const int clusters = pairs < sms / 2 ? pairs : sms / 2;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(Cfg::kThreads);
-  cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  TAPIR_CUDA(cudaLaunchKernelEx(&cfg, gemm_tc2_kernel<BN, P>, p));
-  count_launch();
-  TAPIR_LAUNCH_CHECK("gemm_tc2_kernel");
-  return kOk;
-}
-
-// Small problems (streaming: one frame, ~1000 mixer rows) cannot fill the GPU with 256-row pair
-// tiles: mixer `down` at 1024 rows is 16 pair tiles = 32 of 148 SMs, each walking all of K.  They
-// take the 1-SM kernel with the narrowest tile that still gives every SM one: 4x the CTAs, each
-// with a quarter of the MMA work per k-block.  (The K-summation order of an output element does
-// not depend on the tile shape, so results stay bit-identical across these choices.)
+// Small problems (streaming: one frame, ~1000 mixer rows) cannot fill the GPU with 128 x 128
+// tiles: mixer `down` at 1024 rows is 32 tiles for 132 SMs, each walking all of K.
 bool small_problem(int m_tiles, int N) {
-  const int pairs128 = ((m_tiles + 1) / 2) * ceil_div(N, 128);
-  return 2 * pairs128 * 10 < num_sms() * 6;  // fewer than ~0.6 CTAs per SM as pair tiles
+  return m_tiles * ceil_div(N, 128) * 10 < num_sms() * 6;  // fewer than ~0.6 CTAs per SM
 }
 
-int pick_block_n(int m_tiles, int N, int P) {
+// 64-wide tiles for N <= 64, and for small problems when that gives every SM a tile: twice the
+// CTAs, each with half the MMA work per k-block.  (The K-summation order of an output element does
+// not depend on the tile shape, so results stay bit-identical across these choices.)
+int pick_block_n(int m_tiles, int N) {
   const char* force = getenv("TAPIR_B200_BLOCK_N");
   if (force != nullptr) {
     int v = atoi(force);
-    if (v == 64 || v == 128 || (v == 256 && P <= 2)) return v;
+    if (v == 64 || v == 128) return v;
   }
   if (N <= 64) return 64;
   if (small_problem(m_tiles, N) && m_tiles * ceil_div(N, 128) * 2 <= num_sms()) return 64;
-  return 128;  // 256-wide 1-SM tiles gave no measurable gain (scripts/gemm_bench.py)
+  return 128;
 }
 
 }  // namespace
@@ -1178,11 +658,6 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
   p.out_plane_stride = g.out_plane_stride;
   p.out_P = g.out_P;
   p.err = device_error_flag();
-  {
-    static int dbg = -1;
-    if (dbg < 0) { const char* e = getenv("TAPIR_B200_GEMM_DEBUG"); dbg = e ? atoi(e) : 0; }
-    p.debug_mode = dbg;
-  }
   p.stats = g.stats;
   p.rows_per_frame = g.rows_per_frame > 0 ? g.rows_per_frame : g.M;
   const int P = g.planes;
@@ -1243,16 +718,15 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
       ProfileScope ps(g.tag ? g.tag : "gemm", stream, 2.0 * g.M * g.N * kl,
                       2.0 * P * ((double)g.M * g.C + (double)g.N * g.K) + out_b * g.M * g.N);
       const int grid = p.num_m_tiles < num_sms() ? p.num_m_tiles : num_sms();
-      if (P == 1) conv3x3_halo_kernel<1><<<grid, HaloCfg<1>::kThreads, HaloCfg<1>::kSmemBytes, stream>>>(p);
-      else conv3x3_halo_kernel<2><<<grid, HaloCfg<2>::kThreads, HaloCfg<2>::kSmemBytes, stream>>>(p);
+      if (P == 1) conv3x3_halo_kernel<1><<<grid, kThreads, HaloCfg<1>::kSmemBytes, stream>>>(p);
+      else conv3x3_halo_kernel<2><<<grid, kThreads, HaloCfg<2>::kSmemBytes, stream>>>(p);
       count_launch();
       TAPIR_LAUNCH_CHECK("conv3x3_halo_kernel");
       return kOk;
     }
   }
   // Split-K (deterministic two-pass, below) for problems that cannot half-fill the GPU: on by
-  // default, TAPIR_B200_SPLITK=0 disables.  (Round 1 measured "no gain at K = 2048" with a launch
-  // that only started one CTA per TILE, so the split gave no extra parallelism; fixed in round 2.)
+  // default, TAPIR_B200_SPLITK=0 disables.
   static int splitk_on = -1;
   if (splitk_on < 0) { const char* e = getenv("TAPIR_B200_SPLITK"); splitk_on = (e != nullptr && atoi(e) == 0) ? 0 : 1; }
   // Only where the caller allows it (single-frame streaming steps).  The summation order of a
@@ -1261,9 +735,9 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
   // tests/multi_gpu_check.py shards 1152 rows over two ranks, both demand bit-level agreement).
   const bool splittable = splitk_on && g.allow_splitk && g.splitk_ws != nullptr && g.stats == nullptr &&
                           p.num_k_blocks >= 32;
-  int bn = pick_block_n(p.num_m_tiles, g.N, P);
+  int bn = pick_block_n(p.num_m_tiles, g.N);
   // a small problem that will be split over K keeps 128-wide tiles: the parallelism comes from K,
-  // and wide tiles re-read the A operand half as often (these sizes are L2 -> SM traffic bound)
+  // and wide tiles re-read the A operand half as often
   if (splittable && bn == 64 && g.N > 64 && small_problem(p.num_m_tiles, g.N) &&
       p.num_m_tiles * ceil_div(g.N, 128) * 2 <= num_sms() && getenv("TAPIR_B200_BLOCK_N") == nullptr)
     bn = 128;
@@ -1274,72 +748,6 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
     cuuint64_t str[2] = {(cuuint64_t)g.ldb * 2, (cuuint64_t)plane * 2};
     cuuint32_t box[3] = {(cuuint32_t)kBlockK, (cuuint32_t)bn, 1};
     TAPIR_RETURN_IF(encode_bf16_map(&p.tmB, g.b, 3, dims, str, box, "B"));
-    cuuint32_t boxh[3] = {(cuuint32_t)kBlockK, (cuuint32_t)(bn / 2), 1};
-    TAPIR_RETURN_IF(encode_bf16_map(&p.tmBh, g.b, 3, dims, str, boxh, "B/half"));
-  }
-
-  // 2-SM path (cta_group::2): pair tiles of 256 x {128, 256}
-  if (use_2sm() != 0 && g.N >= 128 && p.num_m_tiles >= 2 && (num_sms() % 2 == 0) &&
-      !small_problem(p.num_m_tiles, g.N)) {
-    int bn2 = use_2sm();
-    static int tail_on = -1;
-    if (tail_on < 0) { const char* e = getenv("TAPIR_B200_GEMM_TAIL"); tail_on = (e != nullptr && atoi(e) == 0) ? 0 : 1; }
-    // Schedule cost per cluster in quarter-chunk units (a full 32-column chunk = 4): full rounds +
-    // the (possibly N-split) tail.  A piece narrower than 128 columns is bound by the shared-memory
-    // reads of its A operand, not by the tensor pipe (per k-step: 4 KB of A + 16 B per column at
-    // 128 B/clk against N/2 cycles of MMA), so a piece of c chunks costs max(4c, 8 + c) - a 32-column
-    // piece costs more than half a 128-column one, which is why pieces are at least 64 columns wide
-    // (measured: with 32-column pieces the ExtraConvs got 15 % slower, not faster).
-    auto tail_plan = [&](int bn, int* first, int* k_out, int* base, int* extra) {
-      const int W = ((p.num_m_tiles + 1) / 2) * ceil_div(g.N, bn);
-      const int C = W < num_sms() / 2 ? W : num_sms() / 2;
-      const int rem = W % C;
-      *first = W; *k_out = 1; *base = bn / 32; *extra = 0;
-      long long cost = (long long)(W / C) * (bn / 32) * 4;
-      if (rem > 0) {
-        int k = tail_on ? C / rem : 1;
-        if (k > bn / 64) k = bn / 64;
-        if (k >= 2 && W > C) {
-          *first = W - rem; *k_out = k; *base = (bn / 32) / k; *extra = (bn / 32) % k;
-          const int c = *base + (*extra > 0 ? 1 : 0);
-          cost += (4 * c > 8 + c) ? 4 * c : 8 + c;
-        } else {
-          cost += (bn / 32) * 4;
-        }
-      }
-      return cost;
-    };
-    int tf, tk, tb, te;
-    if (bn2 != 128 && bn2 != 256) {
-      // auto: the wider tile halves the operand requests but doubles the wave quantum
-      const long long c128 = tail_plan(128, &tf, &tk, &tb, &te);
-      const long long c256 = tail_plan(256, &tf, &tk, &tb, &te);
-      // three planes (the cost volume: 6 MMAs per k-block, only two 96 KB stages fit at 256 columns,
-      // few tiles per CTA so fill / drain matter): no bias towards the wide tile
-      const long long bias = (P == 3) ? 10 : 9;
-      bn2 = (g.N >= 256 && c256 * bias <= c128 * 10) ? 256 : 128;
-    }
-    if (bn2 == 256 && g.N < 256) bn2 = 128;
-    const long long plane = g.b_plane_stride > 0 ? g.b_plane_stride : (long long)g.N * g.ldb;
-    cuuint64_t dims[3] = {(cuuint64_t)g.K, (cuuint64_t)g.N, (cuuint64_t)P};
-    cuuint64_t str[2] = {(cuuint64_t)g.ldb * 2, (cuuint64_t)plane * 2};
-    cuuint32_t boxh[3] = {(cuuint32_t)kBlockK, (cuuint32_t)(bn2 / 2), 1};
-    TAPIR_RETURN_IF(encode_bf16_map(&p.tmBh, g.b, 3, dims, str, boxh, "B/2sm"));
-    cuuint32_t box16[3] = {(cuuint32_t)kBlockK, 16, 1};
-    TAPIR_RETURN_IF(encode_bf16_map(&p.tmB16, g.b, 3, dims, str, box16, "B/16"));
-    p.split_k = 1;
-    p.split_stride = 0;
-    // Tail of the persistent schedule (DESIGN.md 4.1): W tiles on C clusters leave W % C tiles for
-    // a last round that keeps only a few clusters busy for a whole tile time (mixer `up` at 12288
-    // rows: 384 tiles on 74 clusters = 5 rounds + 14 tiles).  Those tiles are cut along N into k
-    // pieces of 32-column chunks with k * (W % C) <= C, so the last round costs about 1/k-th.
-    tail_plan(bn2, &p.tail_first, &p.tail_k, &p.tail_base, &p.tail_extra);
-    if (bn2 == 128 && P == 1) return launch2<128, 1>(p, g, stream);
-    if (bn2 == 128 && P == 2) return launch2<128, 2>(p, g, stream);
-    if (bn2 == 256 && P == 1) return launch2<256, 1>(p, g, stream);
-    if (bn2 == 256 && P == 2) return launch2<256, 2>(p, g, stream);
-    if (bn2 == 128 && P == 3) return launch2<128, 3>(p, g, stream);
-    if (bn2 == 256 && P == 3) return launch2<256, 3>(p, g, stream);
   }
 
   // split-K for problems that cannot fill the GPU (streaming: T = 1): deterministic two-pass
@@ -1347,10 +755,9 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
   p.split_stride = 0;
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int sms = num_sms();
-  // K >= 2048 only (mixer `down` at ~1000 rows, the ExtraConvs of one frame: 8 row tiles x K = 9216
-  // took 56 us on 16 SMs unsplit).  The summation order then depends on the row count; only problems
-  // that cannot half-fill the GPU split, so offline clips keep their exact chunk / permutation
-  // invariance.
+  // K >= 2048 only (mixer `down` at ~1000 rows, the ExtraConvs of one frame).  The summation order
+  // then depends on the row count; only problems that cannot half-fill the GPU split, so offline
+  // clips keep their exact chunk / permutation invariance.
   if (splittable && tiles * 2 <= sms) {
     int S = sms / tiles;
     if (S > 8) S = 8;
@@ -1384,7 +791,6 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
   if (bn == BN && P == PP) return launch<BN, PP>(p, g, stream);
   TAPIR_TC_CASE(64, 1) TAPIR_TC_CASE(64, 2) TAPIR_TC_CASE(64, 3)
   TAPIR_TC_CASE(128, 1) TAPIR_TC_CASE(128, 2) TAPIR_TC_CASE(128, 3)
-  TAPIR_TC_CASE(256, 1) TAPIR_TC_CASE(256, 2)
 #undef TAPIR_TC_CASE
   set_error("gemm_tc: no kernel for BLOCK_N=%d planes=%d", bn, P);
   return kUnsupported;

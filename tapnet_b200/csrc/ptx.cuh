@@ -1,5 +1,5 @@
-// Inline-PTX wrappers for the Blackwell (sm_100a) async machinery used by the GEMM kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM alloc / ld / commit / fences).
+// Inline-PTX wrappers for the Hopper (sm_90a) async machinery used by the GEMM kernels:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA with shared-memory operands).
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -81,205 +81,69 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       : "memory");
 }
 
-// ----------------------------------------------------------------------------- clusters
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+// ----------------------------------------------------------------------------- wgmma
+__device__ __forceinline__ void wgmma_fence() {
+  asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n"
-               "barrier.cluster.wait.acquire.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_commit() {
+  asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
 }
-// TMA load delivered to the same shared-memory offset of every CTA in `mask`; each destination
-// CTA's mbarrier (same offset) receives the complete_tx for the bytes it got.
-__device__ __forceinline__ void tma_load_3d_multicast(void* dst, const CUtensorMap* m, uint64_t* bar,
-                                                      int c0, int c1, int c2, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
-      : "memory");
+// Waits until at most N committed wgmma groups of this warpgroup are still pending.
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Keeps the accumulator registers live across the asynchronous MMAs (no reordering around them).
+template <int R>
+__device__ __forceinline__ void reg_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ----------------------------------------------------------------------------- 2-SM (cta_group::2)
-// In a 2-CTA cluster the shared::cluster address of a CTA's own shared memory carries its rank in
-// bit 24; clearing it addresses the same offset in the leader CTA (rank 0).
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
+// D (64 x N, fp32, wgmma fragment layout) (+)= A (64 x 16) * B (N x 16)^T, both bf16 K-major;
+// N / 2 accumulator registers per thread.
+#define TAPIR_F8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), \
+                    "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define TAPIR_R10(a) "%" #a "0, %" #a "1, %" #a "2, %" #a "3, %" #a "4, %" #a "5, %" #a "6, %" #a "7, " \
+                     "%" #a "8, %" #a "9, "
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, " TAPIR_R10(1) TAPIR_R10(2) "%30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n}\n"
+      : TAPIR_F8(0), TAPIR_F8(8), TAPIR_F8(16), TAPIR_F8(24)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, " TAPIR_R10(1) TAPIR_R10(2) TAPIR_R10(3) TAPIR_R10(4)
+      TAPIR_R10(5) "%60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n}\n"
+      : TAPIR_F8(0), TAPIR_F8(8), TAPIR_F8(16), TAPIR_F8(24), TAPIR_F8(32), TAPIR_F8(40), TAPIR_F8(48),
+        TAPIR_F8(56)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+#undef TAPIR_F8
+#undef TAPIR_R10
 
-// TMA load into THIS CTA's shared memory whose completion is signalled on the LEADER's mbarrier.
-__device__ __forceinline__ void tma_load_3d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar,
-                                                int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_5d_2sm(void* dst, const CUtensorMap* m, uint64_t* bar,
-                                                int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6, %7}], [%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1), "r"(c2),
-      "r"(c3), "r"(c4)
-      : "memory");
-}
-// Arrive on the barrier at this offset in the leader CTA (used by the peer's epilogue warps).
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// D[tmem of both CTAs] (+)= [A_cta0; A_cta1] (256 x 16) * [B_cta0; B_cta1]^T (N x 16); issued by
-// one thread of the leader CTA, operands at the same shared-memory offsets in both CTAs.
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                             uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Completion of the pair's MMAs, signalled on the barrier at this offset in both CTAs.
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)0x3)
-      : "memory");
-}
-
-// ----------------------------------------------------------------------------- tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, bf16/f16 operands, fp32 accumulate.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrives on `bar` once every tcgen05 op previously issued BY THIS THREAD has completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-// Same, arriving on the barrier at this offset in every CTA of `mask` (cluster multicast).
-__device__ __forceinline__ void umma_commit_multicast(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(mask)
-      : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i <- TMEM lane (base+i), r[j] <- column j.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one full 32-byte sector per request.
-// The GEMM epilogue stores one ROW per thread; with 128-bit stores every request was half a
-// sector and the L2 request rate, not bytes, bounded the K=512 GEMMs.
-__device__ __forceinline__ void st_global_v8(void* ptr, const uint32_t (&r)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(ptr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void ld_global_v8(const void* ptr, uint32_t (&r)[8]) {
-  asm volatile("ld.global.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-                 "=r"(r[7])
-               : "l"(ptr));
-}
-
-// Shared-memory matrix descriptor for a K-major operand tile whose rows are 128 bytes
-// (64 bf16) laid out by TMA with CU_TENSOR_MAP_SWIZZLE_128B: 8-row x 128 B swizzle atoms,
-// consecutive atoms 1024 B apart (SBO); LBO is unused for swizzled K-major (canonical 1).
-// Field layout: cute/arch/mma_sm100_desc.hpp (SmemDescriptor), version 1 = sm_100.
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>(1) << 16;
-  d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;  // LayoutType::SWIZZLE_128B
-  return d;
-}
-
-// Same, for a VIEW into a staged tile that does not start on a swizzle-atom boundary: the groups
-// of eight rows are `sbo_bytes` apart (they need not be contiguous) and the first row may sit any
-// number of 128-byte rows into its 1024-byte swizzle pattern.  Measured on B200 (round 2, the
-// halo-patch convolution): the tensor core applies the 128B swizzle from the ABSOLUTE shared-memory
-// address bits, exactly as TMA does when it writes the tile, so such a view needs NO base offset
-// (descriptor bits 49-51 stay 0; declaring the row phase there gives wrong data).
-__device__ __forceinline__ uint64_t make_smem_desc_sw128_view(uint32_t saddr, uint32_t sbo_bytes) {
+// Shared-memory matrix descriptor (sm_90 wgmma) for a K-major operand tile whose rows are 128
+// bytes (64 bf16) laid out by TMA with CU_TENSOR_MAP_SWIZZLE_128B: 8-row x 128 B swizzle atoms,
+// consecutive atoms `sbo_bytes` apart (1024 for a dense tile); LBO is unused for swizzled
+// K-major (canonical 1); layout type 1 = 128B swizzle (bits 62-63).  Advancing K by 16 bf16
+// inside the swizzle row is +32 B of start address (+2 in the 16-byte units of bits 0-13).
+// The hardware applies the 128B swizzle from the absolute shared-memory address bits, as TMA
+// does when it writes the tile, so a view whose first row sits any number of 128-byte rows into
+// its 1024-byte pattern (the halo-patch convolution) needs no base offset (bits 49-51 stay 0).
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t saddr, uint32_t sbo_bytes = 1024) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;  // LayoutType::SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-
-// Instruction descriptor, kind::f16: D=f32 (bits 4-5 = 1), A=B=bf16 (bits 7-9, 10-12 = 1),
-// both K-major (bits 15,16 = 0), N>>3 at bit 17, M>>4 at bit 24.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int m, int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(n >> 3) << 17) |
-         (static_cast<uint32_t>(m >> 4) << 24);
 }
 
 }  // namespace ptx

@@ -1,6 +1,6 @@
 // Refinement loop kernels (SURVEY.md 8(a7)-(a9)): pyramid pooling, fused bilinear-sample +
 // dot local correlation (which also assembles the mixer input row), the depthwise-conv half
-// of each PIPs mixer block, the mixer orchestration around the tcgen05 GEMMs, and the
+// of each PIPs mixer block, the mixer orchestration around the wgmma GEMMs, and the
 // residual update.
 #include "kernels.cuh"
 #include "ptx.cuh"
@@ -350,9 +350,8 @@ __global__ void __launch_bounds__(512, SMALL ? 1 : 2) mixer_dw_kernel(const DwPa
   __syncthreads();
 
   // ---- phase 2: thread = channel c; both depthwise convs + GELU + group sum + skip.
-  // The four channel multipliers are handled as two packed fp32 pairs (fma.rn.f32x2 = FFMA2 on
-  // sm_100: two IEEE FMAs per issue slot, same results as scalar fmaf): 26 packed + 4 scalar
-  // FP32-pipe instructions per channel and frame instead of ~45, plus the 8 MUFU (ex2, rcp).
+  // The four channel multipliers are handled as two fp32 pairs (fma2_rn: IEEE FMAs, same results
+  // as scalar fmaf), plus the 8 MUFU (ex2, rcp) per channel and frame.
   float2 w1p[2][3], w2p[2][3], b1p[2], b2p[2];  // [pair (m0,m1) / (m2,m3)][tap]
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -388,7 +387,7 @@ __global__ void __launch_bounds__(512, SMALL ? 1 : 2) mixer_dw_kernel(const DwPa
       const float2 Y0 = make_float2(y0, y0), Y1 = make_float2(y1, y1), Y2 = make_float2(y2, y2);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const float2 a = __ffma2_rn(w1p[h][2], Y2, __ffma2_rn(w1p[h][1], Y1, __ffma2_rn(w1p[h][0], Y0, b1p[h])));
+        const float2 a = fma2_rn(w1p[h][2], Y2, fma2_rn(w1p[h][1], Y1, fma2_rn(w1p[h][0], Y0, b1p[h])));
         o[h] = gelu_tanh2(a);
       }
     };
@@ -419,7 +418,7 @@ __global__ void __launch_bounds__(512, SMALL ? 1 : 2) mixer_dw_kernel(const DwPa
       float2 t[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h)
-        t[h] = __ffma2_rn(w2p[h][2], cc[h], __ffma2_rn(w2p[h][1], b[h], __ffma2_rn(w2p[h][0], a[h], b2p[h])));
+        t[h] = fma2_rn(w2p[h][2], cc[h], fma2_rn(w2p[h][1], b[h], fma2_rn(w2p[h][0], a[h], b2p[h])));
       const float acc = (((t[0].x + t[0].y) + t[1].x) + t[1].y) + *xrow;
       *yrow = acc;
       *zrow = acc;
@@ -653,7 +652,6 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
     TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     configured.mark();
   }
   {  // nets.py:235 linear
@@ -694,13 +692,15 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
     const int dw_smem = d.QB * (2 * d.TT + kDwHalo) * 512 * (int)sizeof(float);
     {
       ProfileScope ps("mixer.dw", s, (double)rows * 2048 * 12, (double)rows * 512 * (8 + 2 * P));
-      const bool small = d.QB > 1;
+      // SMALL exists for the causal context prefetch.  Its non-causal instantiation is miscompiled
+      // for sm_90 by CUDA 12.9 ptxas (-O1 and up, query loop unrolled): wrong outputs for tiles of
+      // 5+ frames, right at -O0 or not unrolled.  Non-causal tiles run the generic kernel; the
+      // causal one is checked over the same code paths (test_mixer_causal_with_context).
       if (io->causal) {
-        if (small) mixer_dw_kernel<true, true><<<grid, 512, dw_smem, s>>>(d);
+        if (d.QB > 1) mixer_dw_kernel<true, true><<<grid, 512, dw_smem, s>>>(d);
         else mixer_dw_kernel<true, false><<<grid, 512, dw_smem, s>>>(d);
       } else {
-        if (small) mixer_dw_kernel<false, true><<<grid, 512, dw_smem, s>>>(d);
-        else mixer_dw_kernel<false, false><<<grid, 512, dw_smem, s>>>(d);
+        mixer_dw_kernel<false, false><<<grid, 512, dw_smem, s>>>(d);
       }
     }
     count_launch();

@@ -1,7 +1,7 @@
 // Stage A (SURVEY.md 8(a4),(a6)): query-feature sampling, global cost volume and the
 // track / occlusion head.
 //
-// The cost volume itself is the split-bf16 tcgen05 GEMM (planes=3, i.e. fp32-equivalent,
+// The cost volume itself is the split-bf16 wgmma GEMM (planes=3, i.e. fp32-equivalent,
 // because its arg-max must match the reference bit-exactly): cv[n][t*h*w + cell] with
 // M = queries, N = T*h*w cells, K = 256.  `cost_volume_head_kernel` then consumes one
 // 32x32 map per CTA entirely from shared memory: conv3x3 1->16 + ReLU, conv3x3 16->1,
@@ -967,7 +967,7 @@ size_t plan_cv(Arena& a, int N, int T, int gh, int gw, int C, CvPlan* p) {
   p->generic_ctas = 0;
   if (gh != kG || gw != kG) {
     const long long maps = (long long)N * T;
-    const long long cap = 148ll * kGenericCtasPerSm;  // independent of the device: sizes must agree
+    const long long cap = 132ll * kGenericCtasPerSm;  // independent of the device: sizes must agree
     p->generic_ctas = (int)(maps < cap ? maps : cap);
     p->generic_scratch =
         a.take<float>((size_t)p->generic_ctas * (16 * (size_t)(gh + 3) * (gw + 3) + (size_t)gh * gw));

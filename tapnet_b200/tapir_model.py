@@ -1,4 +1,4 @@
-"""B200-native TAPIR / BootsTAPIR inference behind the reference's Python surface.
+"""H100-native TAPIR / BootsTAPIR inference behind the reference's Python surface.
 
 Mirrors `tapnet/torch/tapir_model.py` (reference, 806 LoC): same constructor keywords
 (incl. the `use_casual_conv` spelling, :73-89), same methods and argument meaning
@@ -6,7 +6,7 @@ Mirrors `tapnet/torch/tapir_model.py` (reference, 806 LoC): same constructor key
 `estimate_trajectories` :394, `construct_initial_causal_state` :763,
 `update_query_features` :774), same `FeatureGrids` / `QueryFeatures` tuples (:30-67), same
 state-dict keys (218 tensors, `tapnet_b200/schema.py`), same errors.  Underneath, every stage is
-a hand-written sm_100a kernel reached through the C ABI of `libtapir_b200.so`
+a hand-written sm_90a kernel reached through the C ABI of `libtapir_b200.so`
 (`include/tapir_b200.h`); PyTorch is used for device memory, streams and (multi-GPU)
 `torch.distributed` only.  There is no CPU or eager-PyTorch fallback: tensors must live on a
 CUDA device and the shared library must be built, otherwise the calls raise.
@@ -101,7 +101,7 @@ def _on_model_device(fn):
 
 
 class TAPIR(nn.Module):
-  """TAPIR model (B200 engine).  See the module docstring.
+  """TAPIR model (H100 engine).  See the module docstring.
 
   Extra keyword (not in the reference): `precision` selects the tensor-core arithmetic of the
   dense contractions: 'bf16x3' (default; operands split in two bf16 terms, 3 MMAs, ~16
@@ -567,7 +567,7 @@ class TAPIR(nn.Module):
     updated in place, which saves a 1 GB copy per frame at 1024 points.
 
     `query_chunk_size` only bounds memory in the reference (queries are independent,
-    SURVEY.md 2.2); here chunks are sized by rows (queries x frames) to keep all 148 SMs busy
+    SURVEY.md 2.2); here chunks are sized by rows (queries x frames) to keep all 132 SMs busy
     and the argument is accepted for compatibility.  No query shuffling is done (the
     reference's randperm only changes chunk membership).
     """

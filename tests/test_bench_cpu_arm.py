@@ -1,5 +1,5 @@
 """bench.py's CPU legs: the reference arm must be the UNMODIFIED reference whenever it is importable
-(baseline/_ref on the GPU box, /root/reference in the build container), the oracle port otherwise."""
+(a copy placed under oracle/_ref), the oracle port otherwise."""
 import os
 import sys
 
@@ -14,7 +14,7 @@ from tapnet_b200 import synth  # noqa: E402
 
 def test_cpu_arm_runs_the_unmodified_reference_when_importable():
   have_ref = any(os.path.isfile(os.path.join(r, 'tapnet', 'torch', 'tapir_model.py'))
-                 for r in (os.path.join(ROOT, 'baseline', '_ref'), '/root/reference'))
+                 for r in (os.path.join(ROOT, 'oracle', '_ref'),))
   wl = dict(bench.WORKLOADS['c2'], frames=6)
   video = synth.make_video(6)
   queries = synth.make_queries(32, 6)

@@ -1,4 +1,4 @@
-"""tcgen05 split-bf16 GEMM / implicit 3x3 conv vs an exact fp64 model of the same planes."""
+"""wgmma split-bf16 GEMM / implicit 3x3 conv vs an exact fp64 model of the same planes."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -24,9 +24,8 @@ CASES = [
     (520, 64, 576, 2, False, False, False, 0),
     (16, 8192, 256, 3, False, False, False, 0),
     (20000, 512, 576, 2, True, False, False, 0),
-    # shapes whose persistent schedule ends in a partial round: the tail tiles are cut along N
-    # into pieces of at least 64 columns (mixer `up` and `down`; linear_out: an odd number of row
-    # tiles and pieces that reach beyond N = 388)
+    # shapes whose persistent schedule ends in a partial round (mixer `up` and `down`; linear_out:
+    # an odd number of row tiles and a last column tile that reaches beyond N = 388)
     (12288, 2048, 512, 2, True, True, False, 2),
     (12288, 512, 2048, 2, True, False, True, 0),
     (9600, 388, 512, 2, True, False, False, 0),

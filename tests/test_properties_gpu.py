@@ -123,7 +123,7 @@ def test_c3_graph_replay_tracker_equals_eager_streaming():
   U.record('c3_graph_tracker', frames=T, equal=1)
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason='needs 2 GPUs (gpurun --gpus 2)')
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason='needs 2 GPUs')
 def test_c4_sharded_equals_single_gpu():
   port = 29500 + os.getpid() % 1000
   cmd = [sys.executable, '-m', 'torch.distributed.run', '--nnodes=1', '--nproc-per-node=2',

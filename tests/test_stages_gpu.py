@@ -282,7 +282,7 @@ def _run_mixer(model, x, causal, ctx=None, get_ctx=False):
   return out.cpu().reshape(n, T, 388), new_ctx
 
 
-@pytest.mark.parametrize('T', [1, 5, 24, 50])
+@pytest.mark.parametrize('T', [1, 5, 8, 24, 50])
 def test_mixer_noncausal(T):
   model, sd, cfg = get_model()
   g = torch.Generator().manual_seed(T)
@@ -296,7 +296,9 @@ def test_mixer_noncausal(T):
   assert e < 2e-4 * max(1.0, ref.abs().max().item())
 
 
-@pytest.mark.parametrize('T', [1, 2, 7, 30])
+# T = 5, 7 and 8 run the several-queries-per-CTA variant with one or more unrolled interior trips
+# followed by two or more checked frames, the shape that its non-causal instantiation got wrong
+@pytest.mark.parametrize('T', [1, 2, 5, 7, 8, 12, 30])
 def test_mixer_causal_with_context(T):
   model, sd, cfg = get_model(causal=True)
   g = torch.Generator().manual_seed(100 + T)
