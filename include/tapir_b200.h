@@ -203,6 +203,19 @@ int tapir_gemm(const void* a_planes, int32_t lda, int64_t a_plane_stride, const 
                void* out_planes, int32_t ldp, int64_t out_plane_stride, int32_t out_P,
                double* stats, int32_t rows_per_frame, int32_t impl, void* stream);
 
+/* tapir_gemm plus a split-K scratch buffer.  A non-NULL `splitk_workspace` lets the wgmma path
+ * split K over several CTAs when the problem cannot fill the GPU (K >= 2048, no stats): raw fp32
+ * partial sums go to the workspace and a second kernel sums them in a fixed order and applies the
+ * epilogue.  The split count shrinks until S * M * round_up(N, 8) floats fit in
+ * `splitk_workspace_bytes`; if no split fits, the GEMM runs in one pass.  This is what the
+ * single-frame (streaming) mixer and backbone calls do; the summation order then depends on M. */
+int tapir_gemm_ex(const void* a_planes, int32_t lda, int64_t a_plane_stride, const tapir_linear* b,
+                  int64_t M, int32_t conv3x3, int32_t frames, int32_t H, int32_t W, int32_t C,
+                  const float* residual, int32_t ldr, int32_t act_gelu, float* out_f32,
+                  int32_t ldo, void* out_planes, int32_t ldp, int64_t out_plane_stride,
+                  int32_t out_P, double* stats, int32_t rows_per_frame, int32_t impl,
+                  void* splitk_workspace, size_t splitk_workspace_bytes, void* stream);
+
 /* ---- a3: tapir_model.py:293-392 get_feature_grids (one resolution, one frame chunk) ---- */
 /* utils.py:26-42 bilinear resize, align_corners=False, [frames][H][W][C] -> [frames][oH][oW][C] */
 int tapir_bilinear_resize(const float* src, int32_t frames, int32_t H, int32_t W, int32_t C,

@@ -114,6 +114,10 @@ SIGNATURES = {
                                   c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32,
                                   c_void_p, c_int32, c_void_p, c_int32, c_int64, c_int32, c_void_p,
                                   c_int32, c_int32, c_void_p]),
+    'tapir_gemm_ex': (ctypes.c_int, [c_void_p, c_int32, c_int64, POINTER(Linear), c_int64, c_int32,
+                                     c_int32, c_int32, c_int32, c_int32, c_void_p, c_int32, c_int32,
+                                     c_void_p, c_int32, c_void_p, c_int32, c_int64, c_int32,
+                                     c_void_p, c_int32, c_int32, c_void_p, c_size_t, c_void_p]),
     'tapir_bilinear_resize': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p,
                                              c_int32, c_int32, c_void_p]),
     'tapir_backbone_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32, c_int32, c_int32]),

@@ -45,9 +45,22 @@ int tapir_gemm(const void* a_planes, int32_t lda, int64_t a_plane_stride, const 
                const float* residual, int32_t ldr, int32_t act_gelu, float* out_f32, int32_t ldo,
                void* out_planes, int32_t ldp, int64_t out_plane_stride, int32_t out_P,
                double* stats, int32_t rows_per_frame, int32_t impl, void* stream) {
+  return tapir_gemm_ex(a_planes, lda, a_plane_stride, b, M, conv3x3, frames, H, W, C, residual, ldr,
+                       act_gelu, out_f32, ldo, out_planes, ldp, out_plane_stride, out_P, stats,
+                       rows_per_frame, impl, nullptr, 0, stream);
+}
+
+int tapir_gemm_ex(const void* a_planes, int32_t lda, int64_t a_plane_stride, const tapir_linear* b,
+                  int64_t M, int32_t conv3x3, int32_t frames, int32_t H, int32_t W, int32_t C,
+                  const float* residual, int32_t ldr, int32_t act_gelu, float* out_f32,
+                  int32_t ldo, void* out_planes, int32_t ldp, int64_t out_plane_stride,
+                  int32_t out_P, double* stats, int32_t rows_per_frame, int32_t impl,
+                  void* splitk_workspace, size_t splitk_workspace_bytes, void* stream) {
   Range nvtx_range("tapir_gemm");
   TAPIR_CHECK_ARG(a_planes != nullptr && b != nullptr && b->w != nullptr, "tapir_gemm: null pointer");
   TAPIR_CHECK_ARG(M > 0 && M < (1ll << 31), "tapir_gemm: M out of range");
+  TAPIR_CHECK_ARG((reinterpret_cast<uintptr_t>(splitk_workspace) & 15) == 0,
+                  "tapir_gemm: split-K workspace must be 16-byte aligned");
   GemmArgs g;
   g.mode = conv3x3 ? kGemmConv3x3 : kGemmPlain;
   g.planes = b->planes;
@@ -69,6 +82,9 @@ int tapir_gemm(const void* a_planes, int32_t lda, int64_t a_plane_stride, const 
   g.out_planes = static_cast<__nv_bfloat16*>(out_planes);
   g.ldp = ldp; g.out_plane_stride = out_plane_stride; g.out_P = out_P;
   g.stats = stats; g.rows_per_frame = rows_per_frame;
+  g.splitk_ws = static_cast<float*>(splitk_workspace);
+  g.splitk_ws_bytes = splitk_workspace != nullptr ? splitk_workspace_bytes : 0;
+  g.allow_splitk = splitk_workspace != nullptr;
   if (impl == 1) return gemm_simt(g, S(stream));
   if (impl == 0) return gemm_tc(g, S(stream));
   set_error("tapir_gemm: impl must be 0 (wgmma) or 1 (simt)");

@@ -1,5 +1,6 @@
 """Per-stage parity of the CUDA path (through the C ABI) against the CPU oracle."""
 import ctypes
+import os
 
 import numpy as np
 import pytest
@@ -241,7 +242,8 @@ def test_cost_volume_tracks_any_map_size(shape):
   assert e_p < 1e-3 and e_o < 1e-4 and e_e < 1e-4
 
 
-def _run_mixer(model, x, causal, ctx=None, get_ctx=False):
+def _run_mixer(model, x, causal, ctx=None, get_ctx=False, in_place=False):
+  """in_place: the context output pointers are the context input buffers (the streaming call)."""
   lib = _lib.load()
   pk = model._pack()
   n, T, cin = x.shape
@@ -263,8 +265,11 @@ def _run_mixer(model, x, causal, ctx=None, get_ctx=False):
     io.ctx2_in = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in c2])
   o1 = o2 = None
   if get_ctx:
-    o1 = [torch.empty(n, 2, 512, device=dev) for _ in range(nb)]
-    o2 = [torch.empty(n, 2, 2048, device=dev) for _ in range(nb)]
+    if in_place:
+      o1, o2 = c1, c2
+    else:
+      o1 = [torch.empty(n, 2, 512, device=dev) for _ in range(nb)]
+      o2 = [torch.empty(n, 2, 2048, device=dev) for _ in range(nb)]
     io.ctx1_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o1])
     io.ctx2_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o2])
   io.out, io.ldo = out.data_ptr(), 388
@@ -319,6 +324,118 @@ def test_mixer_causal_with_context(T):
   U.record(f'mixer_causal_T{T}', err=e, err_noctx=e0, ctx_err=ec, scale=ref.abs().max().item())
   s = max(1.0, ref.abs().max().item())
   assert e < 2e-4 * s and e0 < 2e-4 * s and ec < 2e-4 * s
+
+
+def _mixer_queries_per_cta(n, T):
+  """Queries per CTA of the depthwise mixer kernel: a copy of the choice in mixer_forward
+  (tapnet_b200/csrc/refine.cu), with its constants kDwTileMax 24, kDwRowBudget 52, kDwHalo 4,
+  kDwSmallQueries 8 and the H100's 132 SMs."""
+  tt = min(T, 24)
+  qb = min(max(52 // (2 * tt + 4), 1), 8)
+  if qb > 1:
+    per_sm = -(-n * -(-T // tt) // 132)
+    if per_sm < qb:
+      qb = max(per_sm, 2)
+  return min(qb, n)
+
+
+# (T, n) pairs giving every QB from 1 to 8, each with a partial last query group where QB > 1
+MIXER_QB_CASES = [(1, 1001), (1, 801), (1, 700), (3, 531), (4, 401), (5, 301), (2, 263), (12, 5)]
+
+
+def test_mixer_qb_cases_cover_every_queries_per_cta():
+  qbs = [_mixer_queries_per_cta(n, T) for T, n in MIXER_QB_CASES]
+  assert sorted(qbs) == list(range(1, 9)), qbs
+  assert all(qb == 1 or n % qb != 0 for (T, n), qb in zip(MIXER_QB_CASES, qbs))
+
+
+def _oracle_mixer(*args):
+  # n ~ 1000 query rows through twelve blocks: use every core for the fp32 oracle
+  threads = torch.get_num_threads()
+  torch.set_num_threads(max(threads, os.cpu_count() or 1))
+  try:
+    with torch.no_grad():
+      return O.mixer(*args)
+  finally:
+    torch.set_num_threads(threads)
+
+
+def _random_ctx(g, n):
+  ctx = {}
+  for i in range(12):
+    ctx[f'block_{i}_causal_1'] = torch.randn(n, 2, 512, generator=g)
+    ctx[f'block_{i}_causal_2'] = torch.randn(n, 2, 2048, generator=g)
+  return ctx
+
+
+# The causal kernel with several queries per CTA (SMALL) at every QB: the register context window
+# refill for query slots 4-7 and a partial last query group, with and without context
+@pytest.mark.parametrize('T,n', MIXER_QB_CASES,
+                         ids=[f'T{T}_n{n}_qb{_mixer_queries_per_cta(n, T)}' for T, n in MIXER_QB_CASES])
+def test_mixer_causal_every_queries_per_cta(T, n):
+  model, sd, cfg = get_model(causal=True)
+  g = torch.Generator().manual_seed(7 * T + n)
+  x = torch.randn(n, T, 535, generator=g)
+  ctx = _random_ctx(g, n)
+  ref, ref_ctx = _oracle_mixer(sd, x, O.Ctx(), True, {k: v.clone() for k, v in ctx.items()}, True)
+  ref0, ref0_ctx = _oracle_mixer(sd, x, O.Ctx(), True, None, False)
+  got, got_ctx = _run_mixer(model, x, True, ctx, True)
+  got0, _ = _run_mixer(model, x, True, None, False)
+  e = (got - ref).abs().max().item()
+  e0 = (got0 - ref0).abs().max().item()
+  ec = max((got_ctx[k] - ref_ctx[k]).abs().max().item() for k in ref_ctx)
+  qb = _mixer_queries_per_cta(n, T)
+  U.record(f'mixer_causal_qb{qb}_T{T}_n{n}', err=e, err_noctx=e0, ctx_err=ec,
+           scale=ref.abs().max().item())
+  s = max(1.0, ref.abs().max().item())
+  assert e < 2e-4 * s and e0 < 2e-4 * s and ec < 2e-4 * s  # as test_mixer_causal_with_context
+
+
+# The non-causal (generic) kernel with several queries per CTA
+@pytest.mark.parametrize('T,n', [(1, 1001), (3, 531), (5, 301)])
+def test_mixer_noncausal_many_queries_per_cta(T, n):
+  model, sd, cfg = get_model()
+  assert _mixer_queries_per_cta(n, T) >= 3
+  g = torch.Generator().manual_seed(3 * T + n)
+  x = torch.randn(n, T, 535, generator=g)
+  ref, _ = _oracle_mixer(sd, x, O.Ctx(), False)
+  got, _ = _run_mixer(model, x, False)
+  e = (got - ref).abs().max().item()
+  U.record(f'mixer_noncausal_qb{_mixer_queries_per_cta(n, T)}_T{T}_n{n}', err=e,
+           scale=ref.abs().max().item())
+  assert e < 2e-4 * max(1.0, ref.abs().max().item())  # as test_mixer_noncausal
+
+
+@pytest.mark.parametrize('n', [6, 1001])
+def test_mixer_causal_streaming_step_updates_context_in_place(n):
+  """T = 1 with the context output buffers being the input buffers (what OnlineTracker passes)."""
+  model, sd, cfg = get_model(causal=True)
+  g = torch.Generator().manual_seed(n)
+  x = torch.randn(n, 1, 535, generator=g)
+  ctx = _random_ctx(g, n)
+  ref, ref_ctx = _oracle_mixer(sd, x, O.Ctx(), True, {k: v.clone() for k, v in ctx.items()}, True)
+  got, got_ctx = _run_mixer(model, x, True, ctx, True, in_place=True)
+  e = (got - ref).abs().max().item()
+  ec = max((got_ctx[k] - ref_ctx[k]).abs().max().item() for k in ref_ctx)
+  U.record(f'mixer_causal_in_place_n{n}', err=e, ctx_err=ec, scale=ref.abs().max().item())
+  s = max(1.0, ref.abs().max().item())
+  assert e < 2e-4 * s and ec < 2e-4 * s
+
+
+@pytest.mark.parametrize('T,n', [(1, 1001), (3, 531)])
+def test_mixer_query_permutation_is_bit_exact(T, n):
+  """Same n, so the same QB and GEMM schedules: permuting the queries permutes output and new
+  context bit for bit (a query mixed up with its CTA slot would break this)."""
+  model, sd, cfg = get_model(causal=True)
+  g = torch.Generator().manual_seed(11 * T + n)
+  x = torch.randn(n, T, 535, generator=g)
+  ctx = _random_ctx(g, n)
+  perm = torch.randperm(n, generator=g)
+  got, got_ctx = _run_mixer(model, x, True, ctx, True)
+  got_p, got_ctx_p = _run_mixer(model, x[perm], True, {k: v[perm] for k, v in ctx.items()}, True)
+  assert torch.equal(got_p.view(torch.int32), got[perm].view(torch.int32))
+  for k in got_ctx:
+    assert torch.equal(got_ctx_p[k].view(torch.int32), got_ctx[k][perm].view(torch.int32)), k
 
 
 def test_refine_update():
