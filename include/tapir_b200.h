@@ -305,12 +305,30 @@ int tapir_cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, co
                              int32_t* argmax, void* workspace, size_t workspace_bytes,
                              void* stream);
 
+/* The same for B clips in one launch sequence: qfeat [B][N][C], grid [B][T][gh][gw][C],
+ * query_tyx [B][N][3] or NULL; outputs as above over the flattened query b*N + n.  One batched
+ * GEMM and one head launch; clip b's results equal those of a tapir_cost_volume_tracks call on
+ * clip b alone, bit for bit.  B*N <= 65535 for the 32 x 32 map.  B = 1 is
+ * tapir_cost_volume_tracks. */
+size_t tapir_cost_volume_batched_workspace_bytes(int32_t B, int32_t N, int32_t T, int32_t gh,
+                                                 int32_t gw, int32_t C);
+int tapir_cost_volume_tracks_batched(const tapir_head_weights* w, const float* qfeat,
+                                     const float* grid, int32_t B, int32_t N, int32_t T, int32_t gh,
+                                     int32_t gw, int32_t C, const float* query_tyx,
+                                     float softmax_temperature, int32_t init_h, int32_t init_w,
+                                     float* points, float* occ, float* expd, int32_t* argmax,
+                                     void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- a9: tapir_model.py:519-527 avg_pool3d (2,2,1) ---------------------------------- */
 int tapir_pool_pyramid(const float* grid, int32_t T, int32_t h, int32_t w, int32_t C, float* out,
                        void* stream);
 
 /* ---- a7 / a8 ------------------------------------------------------------------------ */
 int tapir_local_corr(const tapir_corr_args* args, void* stream);
+/* `batch` clips in one launch: args->num_points = queries per clip; every level grid is
+ * [batch][T][h][w][C]; pos / occ / expd / features / output rows run over the flattened query
+ * b*num_points + n.  Equal to one tapir_local_corr call per clip, bit for bit. */
+int tapir_local_corr_batched(const tapir_corr_args* args, int32_t batch, void* stream);
 size_t tapir_mixer_workspace_bytes(int64_t rows, int32_t planes);
 int tapir_mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* workspace,
                         size_t workspace_bytes, void* stream);

@@ -21,15 +21,15 @@ for t in $TIERS; do
   case $t in
     gemm_simt)   run gemm_simt "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py -k simt ;;
     gemm_tc)     run gemm_tc "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py -k tc ;;
-    stages_simt) run stages_simt "TAPIR_B200_GEMM=simt" tests/test_stages_gpu.py ;;
-    stages_tc)   run stages_tc "X=1" tests/test_stages_gpu.py ;;
+    stages_simt) run stages_simt "TAPIR_B200_GEMM=simt" tests/test_stages_gpu.py tests/test_batched_gpu.py ;;
+    stages_tc)   run stages_tc "X=1" tests/test_stages_gpu.py tests/test_batched_gpu.py ;;
     e2e_simt)    run e2e_simt "TAPIR_B200_GEMM=simt" tests/test_end_to_end_gpu.py ;;
     e2e_tc)      run e2e_tc "X=1" tests/test_end_to_end_gpu.py ;;
-    props)       run props "X=1" tests/test_properties_gpu.py ;;
+    props)       run props "X=1" tests/test_properties_gpu.py tests/test_batched_gpu.py ;;
     io)          run io "X=1" tests/test_io_gpu.py ;;
     bulk)        run bulk "X=1" tests/test_bulk_gpu.py ;;
     no_halo)     run no_halo "TAPIR_B200_CONV_HALO=0" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_stages_gpu.py tests/test_end_to_end_gpu.py ;;
-    no_splitk)   run no_splitk "TAPIR_B200_SPLITK=0" tests/test_gemm_variants_gpu.py tests/test_stages_gpu.py tests/test_properties_gpu.py ;;
+    no_splitk)   run no_splitk "TAPIR_B200_SPLITK=0" tests/test_gemm_variants_gpu.py tests/test_stages_gpu.py tests/test_properties_gpu.py tests/test_batched_gpu.py ;;
     all)         run all "X=1" tests ;;
   esac
 done

@@ -2,10 +2,17 @@
 
 Per frame: get_feature_grids(1 frame) + estimate_trajectories(T=1, causal state in/out), exactly
 the call pattern of tapnet/pytorch_live_demo.py:62-85.  Reports frames/s and point-frames/s.
+
+--streams 1,2,4,8 instead compares, for each stream count S and each --stream-points value, one
+S-stream OnlineTracker against S single-stream trackers stepped in turn (rounds alternate between
+the two in this process): ms per frame-set (one frame of every stream), aggregate point-frames/s
+and kernel launches per step.
 """
 import argparse
 import json
 import os
+import statistics
+import subprocess
 import sys
 import time
 
@@ -20,11 +27,99 @@ ap = argparse.ArgumentParser()
 ap.add_argument('--frames', type=int, default=250)
 ap.add_argument('--warm', type=int, default=10)
 ap.add_argument('--queries', type=int, default=1024)
+ap.add_argument('--streams', type=str, default='',
+                help='comma-separated stream counts: multi-stream vs single-stream trackers')
+ap.add_argument('--stream-points', type=str, default='8,256', help='points per stream')
+ap.add_argument('--rounds', type=int, default=5, help='alternating timing rounds (--streams)')
 a = ap.parse_args()
 sd = synth.make_state_dict(0)
 model = tapir_model.TAPIR(pyramid_level=1, use_casual_conv=True)
 model.load_state_dict(sd)
 model = model.cuda().eval()
+
+
+def gpu_info():
+  """Name and power limit of the GPU, read in the same run as the numbers."""
+  try:
+    out = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
+                          '-i', str(torch.cuda.current_device())],
+                         capture_output=True, text=True, timeout=30).stdout.strip()
+    name, limit = [x.strip() for x in out.split(',')]
+  except Exception:  # pylint: disable=broad-except
+    name, limit = torch.cuda.get_device_name(), 'unknown'
+  return dict(gpu=name, power_limit=limit)
+
+
+def multi_stream_bench():
+  from tapnet_b200 import _lib, streaming  # pylint: disable=g-import-not-at-top
+  lib = _lib.load()
+  info = gpu_info()
+  print(json.dumps(dict(mode='gpu', **info)))
+  streams = [int(x) for x in a.streams.split(',')]
+  smax = max(streams)
+  clips = torch.cat([synth.make_video(16, seed=1 + s) for s in range(smax)]).cuda()  # [S, 16, H, W, 3]
+  for n in [int(x) for x in a.stream_points.split(',')]:
+    q = torch.cat([synth.make_queries(n, 1, seed=2 + s, frame0_only=True) for s in range(smax)]).cuda()
+    for S in streams:
+      multi = streaming.OnlineTracker(model, 256, 256, n, num_streams=S)
+      multi.init(clips[:S, 0], q[:S])
+      singles = [streaming.OnlineTracker(model, 256, 256, n) for _ in range(S)]
+      for s, trk in enumerate(singles):
+        trk.init(clips[s, 0], q[s])
+
+      def step_multi(t):
+        multi.step(clips[:S, t % 16])
+
+      def step_singles(t):
+        for s, trk in enumerate(singles):
+          trk.step(clips[s, t % 16])
+
+      for _ in range(2):  # captures; a second pass re-captures any graph a later capture outdated
+        for t in range(a.warm):
+          step_multi(t)
+          step_singles(t)
+
+      def timed(fn):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        torch.cuda.synchronize()
+        e0.record()
+        for t in range(a.frames):
+          fn(t)
+        e1.record()
+        torch.cuda.synchronize()
+        return e0.elapsed_time(e1) / a.frames
+
+      ms_multi, ms_single = [], []
+      for _ in range(a.rounds):
+        ms_multi.append(timed(step_multi))
+        ms_single.append(timed(step_singles))
+
+      def launches(trk):  # one eager step (a graph replay does not pass through the counter)
+        trk._frame.copy_(clips[:trk.num_streams, :1])
+        torch.cuda.synchronize()
+        l0 = lib.tapir_launch_count()
+        trk._step_eager()
+        torch.cuda.synchronize()
+        return int(lib.tapir_launch_count() - l0)
+
+      l_multi, l_single = launches(multi), launches(singles[0]) * S
+      for trk in [multi] + singles:
+        trk.close()
+      mm, ms = statistics.median(ms_multi), statistics.median(ms_single)
+      print(json.dumps(dict(
+          mode='multi-stream', streams=S, points_per_stream=n, frames=a.frames, rounds=a.rounds,
+          ms_per_frame_set_multi=round(mm, 3), ms_per_frame_set_singles=round(ms, 3),
+          ms_multi_rounds=[round(x, 3) for x in ms_multi],
+          ms_singles_rounds=[round(x, 3) for x in ms_single],
+          point_frames_per_s_multi=round(S * n * 1e3 / mm, 1),
+          point_frames_per_s_singles=round(S * n * 1e3 / ms, 1),
+          speedup=round(ms / mm, 3), launches_per_step_multi=l_multi,
+          launches_per_step_singles=l_single, **info)), flush=True)
+
+
+if a.streams:
+  multi_stream_bench()
+  sys.exit(0)
 clip = synth.make_video(16).cuda()  # frames are cycled; content does not affect timing
 q = synth.make_queries(a.queries, 1, frame0_only=True).cuda()
 g0 = model.get_feature_grids(clip[:, :1], False)

@@ -146,9 +146,17 @@ SIGNATURES = {
                                                 c_int32, c_int32, c_int32, c_int32, c_void_p,
                                                 c_float, c_int32, c_int32, c_void_p, c_void_p,
                                                 c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    'tapir_cost_volume_batched_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32, c_int32,
+                                                             c_int32, c_int32]),
+    'tapir_cost_volume_tracks_batched': (ctypes.c_int, [POINTER(HeadWeights), c_void_p, c_void_p,
+                                                        c_int32, c_int32, c_int32, c_int32, c_int32,
+                                                        c_int32, c_void_p, c_float, c_int32, c_int32,
+                                                        c_void_p, c_void_p, c_void_p, c_void_p,
+                                                        c_void_p, c_size_t, c_void_p]),
     'tapir_pool_pyramid': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p,
                                           c_void_p]),
     'tapir_local_corr': (ctypes.c_int, [POINTER(CorrArgs), c_void_p]),
+    'tapir_local_corr_batched': (ctypes.c_int, [POINTER(CorrArgs), c_int32, c_void_p]),
     'tapir_mixer_workspace_bytes': (c_size_t, [c_int64, c_int32]),
     'tapir_mixer_forward': (ctypes.c_int, [POINTER(MixerWeights), POINTER(MixerIO), c_void_p,
                                            c_size_t, c_void_p]),

@@ -161,7 +161,12 @@ int tapir_sample_query_features(const float* grid, int32_t T, int32_t gh, int32_
 }
 
 size_t tapir_cost_volume_workspace_bytes(int32_t N, int32_t T, int32_t gh, int32_t gw, int32_t C) {
-  return cost_volume_workspace_bytes(N, T, gh, gw, C);
+  return cost_volume_workspace_bytes(1, N, T, gh, gw, C);
+}
+
+size_t tapir_cost_volume_batched_workspace_bytes(int32_t B, int32_t N, int32_t T, int32_t gh,
+                                                 int32_t gw, int32_t C) {
+  return cost_volume_workspace_bytes(B, N, T, gh, gw, C);
 }
 
 int tapir_cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid,
@@ -171,8 +176,21 @@ int tapir_cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, co
                              int32_t* argmax, void* workspace, size_t workspace_bytes,
                              void* stream) {
   Range nvtx_range("tapir_cost_volume_tracks");
-  return cost_volume_tracks(w, qfeat, grid, N, T, gh, gw, C, query_tyx, softmax_temperature, init_h,
-                            init_w, points, occ, expd, argmax, workspace, workspace_bytes, S(stream));
+  return cost_volume_tracks(w, qfeat, grid, 1, N, T, gh, gw, C, query_tyx, softmax_temperature,
+                            init_h, init_w, points, occ, expd, argmax, workspace, workspace_bytes,
+                            S(stream));
+}
+
+int tapir_cost_volume_tracks_batched(const tapir_head_weights* w, const float* qfeat,
+                                     const float* grid, int32_t B, int32_t N, int32_t T, int32_t gh,
+                                     int32_t gw, int32_t C, const float* query_tyx,
+                                     float softmax_temperature, int32_t init_h, int32_t init_w,
+                                     float* points, float* occ, float* expd, int32_t* argmax,
+                                     void* workspace, size_t workspace_bytes, void* stream) {
+  Range nvtx_range("tapir_cost_volume_tracks_batched");
+  return cost_volume_tracks(w, qfeat, grid, B, N, T, gh, gw, C, query_tyx, softmax_temperature,
+                            init_h, init_w, points, occ, expd, argmax, workspace, workspace_bytes,
+                            S(stream));
 }
 
 int tapir_pool_pyramid(const float* grid, int32_t T, int32_t h, int32_t w, int32_t C, float* out,
@@ -183,7 +201,12 @@ int tapir_pool_pyramid(const float* grid, int32_t T, int32_t h, int32_t w, int32
 
 int tapir_local_corr(const tapir_corr_args* args, void* stream) {
   Range nvtx_range("tapir_local_corr");
-  return local_corr(args, S(stream));
+  return local_corr(args, 1, S(stream));
+}
+
+int tapir_local_corr_batched(const tapir_corr_args* args, int32_t batch, void* stream) {
+  Range nvtx_range("tapir_local_corr_batched");
+  return local_corr(args, batch, S(stream));
 }
 
 size_t tapir_mixer_workspace_bytes(int64_t rows, int32_t planes) {

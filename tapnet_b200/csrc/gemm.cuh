@@ -50,6 +50,14 @@ struct GemmArgs {
   // order, so allowing it by problem size alone would make an offline result depend on how its
   // rows were chunked or sharded (measured: 1.5e-5 on occlusion logits).
   bool allow_splitk = false;
+  // Batched plain GEMM: `batch` independent problems of M x N, batch b reading A rows
+  // [b * a_batch_rows, + M) and B rows [b * b_batch_rows, + N) of the flattened operand planes and
+  // writing out_f32 + b * out_batch_stride.  An m-tile never crosses a batch.  batch > 1 supports
+  // the fp32 output, bias and GELU only, and never splits K.
+  int batch = 1;
+  long long a_batch_rows = 0;      // 0 = M
+  long long b_batch_rows = 0;      // 0 = N
+  long long out_batch_stride = 0;  // elements; 0 = M * ldo
   int k_logical = 0;        // un-padded K for FLOP accounting (0 = K)
   const char* tag = nullptr;  // profiling class name
 };

@@ -17,6 +17,7 @@ constexpr int TM = 64, TN = 64, TK = 16;
 struct SimtParams {
   GemmArgs g;
   long long a_plane, b_plane;
+  long long a_batch_rows, b_batch_rows, out_batch_stride;  // batch = blockIdx.z
 };
 
 __device__ __forceinline__ float load_a(const SimtParams& p, int m, int k) {
@@ -32,7 +33,7 @@ __device__ __forceinline__ float load_a(const SimtParams& p, int m, int k) {
     if (y < 0 || y >= g.H || x < 0 || x >= g.W) return 0.f;
     off = (((long long)f * g.H + y) * g.W + x) * g.C + c;
   } else {
-    off = (long long)m * g.lda + k;
+    off = ((long long)blockIdx.z * p.a_batch_rows + m) * g.lda + k;
   }
   float v = 0.f;
   for (int i = 0; i < g.planes; ++i) v += __bfloat162float(g.a[i * p.a_plane + off]);
@@ -42,7 +43,7 @@ __device__ __forceinline__ float load_a(const SimtParams& p, int m, int k) {
 __device__ __forceinline__ float load_b(const SimtParams& p, int n, int k) {
   const GemmArgs& g = p.g;
   if (n >= g.N) return 0.f;
-  const long long off = (long long)n * g.ldb + k;
+  const long long off = ((long long)blockIdx.z * p.b_batch_rows + n) * g.ldb + k;
   float v = 0.f;
   for (int i = 0; i < g.planes; ++i) v += __bfloat162float(g.b[i * p.b_plane + off]);
   return v;
@@ -54,6 +55,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const SimtParams p) {
   const GemmArgs& g = p.g;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int m0 = blockIdx.x * TM, n0 = blockIdx.y * TN;
+  float* out_f32 = g.out_f32 != nullptr ? g.out_f32 + blockIdx.z * p.out_batch_stride : nullptr;
   float acc[4][4] = {};
   for (int k0 = 0; k0 < g.K; k0 += TK) {
     for (int e = threadIdx.x; e < TM * TK; e += 256) {
@@ -86,7 +88,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const SimtParams p) {
       if (g.bias != nullptr) v += g.bias[n];
       if (g.act == 1) v = gelu_tanh(v);
       if (g.residual != nullptr) v += g.residual[m * g.ldr + n];
-      if (g.out_f32 != nullptr) g.out_f32[m * g.ldo + n] = v;
+      if (out_f32 != nullptr) out_f32[m * g.ldo + n] = v;
       if (g.stats != nullptr) {
         const long long rpf = (g.mode == kGemmConv3x3) ? (long long)g.H * g.W : (g.rows_per_frame > 0 ? g.rows_per_frame : g.M);
         double* dst = g.stats + ((m / rpf) * g.N + n) * 2;
@@ -111,14 +113,19 @@ int gemm_simt(const GemmArgs& g, cudaStream_t stream) {
   TAPIR_RETURN_IF(validate_gemm_args(g));
   SimtParams p;
   p.g = g;
+  p.a_batch_rows = g.a_batch_rows > 0 ? g.a_batch_rows : g.M;
+  p.b_batch_rows = g.b_batch_rows > 0 ? g.b_batch_rows : g.N;
+  p.out_batch_stride = g.out_batch_stride > 0 ? g.out_batch_stride : (long long)g.M * g.ldo;
+  // default plane strides span every batch's rows
   if (g.mode == kGemmConv3x3) {
     p.a_plane = g.a_plane_stride > 0 ? g.a_plane_stride : (long long)g.M * g.C;
   } else {
-    p.a_plane = g.a_plane_stride > 0 ? g.a_plane_stride : (long long)g.M * g.lda;
+    p.a_plane = g.a_plane_stride > 0 ? g.a_plane_stride : ((g.batch - 1) * p.a_batch_rows + g.M) * g.lda;
   }
-  p.b_plane = g.b_plane_stride > 0 ? g.b_plane_stride : (long long)g.N * g.ldb;
-  ProfileScope ps(g.tag ? g.tag : "gemm", stream, 2.0 * g.M * g.N * (g.k_logical > 0 ? g.k_logical : g.K), 0.0);
-  dim3 grid(ceil_div(g.M, TM), ceil_div(g.N, TN));
+  p.b_plane = g.b_plane_stride > 0 ? g.b_plane_stride : ((g.batch - 1) * p.b_batch_rows + g.N) * g.ldb;
+  ProfileScope ps(g.tag ? g.tag : "gemm", stream,
+                  2.0 * g.batch * g.M * g.N * (g.k_logical > 0 ? g.k_logical : g.K), 0.0);
+  dim3 grid(ceil_div(g.M, TM), ceil_div(g.N, TN), g.batch);
   gemm_simt_kernel<<<grid, 256, 0, stream>>>(p);
   count_launch();
   TAPIR_LAUNCH_CHECK("gemm_simt_kernel");

@@ -62,6 +62,8 @@ struct TcParams {
   int rows_per_frame;   // rows of one frame (plain mode; conv tiles never straddle frames)
   int split_k;          // >1: K is split over `split_k` work items; raw fp32 partials go to out_f32
   long long split_stride;  // elements between partial buffers (M * ldo)
+  int m_tiles_per_batch;   // batched plain GEMM: m-tiles of one batch (= num_m_tiles when batch 1)
+  long long a_batch_rows, b_batch_rows, out_batch_stride;
   int* err;
 };
 
@@ -220,11 +222,14 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
   // split-K (small problems that cannot fill the GPU): work item = (tile, k-slice)
   const int S = p.split_k;
   const int num_work = p.num_m_tiles * p.num_n_tiles * S;
-  auto decode = [&](int w, int& m_tile, int& n0, int& kb0, int& kb1) {
+  // work item order (batch, m-tile, n-tile, k-slice); m_tile is the tile within its batch
+  auto decode = [&](int w, int& bat, int& m_tile, int& n0, int& kb0, int& kb1) {
     const int split = w % S;
     const int tile = w / S;
     m_tile = tile / p.num_n_tiles;
     n0 = (tile - m_tile * p.num_n_tiles) * BLOCK_N;
+    bat = m_tile / p.m_tiles_per_batch;
+    m_tile -= bat * p.m_tiles_per_batch;
     kb0 = (int)((long long)nkb * split / S);
     kb1 = (int)((long long)nkb * (split + 1) / S);
     return split;
@@ -236,8 +241,12 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
     int stage = 0;
     uint32_t phase = 0;
     for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-      int m_tile, n0, kb0, kb1;
-      decode(w, m_tile, n0, kb0, kb1);
+      int bat, m_tile, n0, kb0, kb1;
+      decode(w, bat, m_tile, n0, kb0, kb1);
+      // batch = row offset into the flattened operands; rows loaded past the end of a batch
+      // belong to the next one (or are TMA zero fill) and are masked by the epilogue
+      const int a_row0 = (int)(bat * p.a_batch_rows) + m_tile * kBlockM;
+      const int b_row0 = (int)(bat * p.b_batch_rows) + n0;
       int frame = 0, y0 = 0, x0 = 0;
       if (p.mode == kGemmConv3x3) {
         const int per_frame = p.tiles_x * p.tiles_y;
@@ -263,11 +272,11 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
 #pragma unroll
           for (int pl = 0; pl < P; ++pl)
             ptx::tma_load_3d(sa + pl * Cfg::kABytes, &p.tmA, &full_bar[stage], kb * kBlockK,
-                             m_tile * kBlockM, pl);
+                             a_row0, pl);
         }
 #pragma unroll
         for (int pl = 0; pl < P; ++pl)
-          ptx::tma_load_3d(sb + pl * Cfg::kBBytes, &p.tmB, &full_bar[stage], kb * kBlockK, n0, pl);
+          ptx::tma_load_3d(sb + pl * Cfg::kBBytes, &p.tmB, &full_bar[stage], kb * kBlockK, b_row0, pl);
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
       }
     }
@@ -281,8 +290,8 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
   uint32_t phase = 0;
   float acc[BLOCK_N / 2];
   for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-    int m_tile, n0, kb0, kb1;
-    const int split = decode(w, m_tile, n0, kb0, kb1);
+    int bat, m_tile, n0, kb0, kb1;
+    const int split = decode(w, bat, m_tile, n0, kb0, kb1);
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
     int prev = -1;
@@ -326,7 +335,7 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
     if (p.stats != nullptr)
       frame = (p.mode == kGemmConv3x3) ? m_tile / (p.tiles_x * p.tiles_y)
                                        : (int)(((long long)m_tile * kBlockM) / p.rows_per_frame);
-    epilogue<BLOCK_N>(p, acc, row, row_ok, n0, frame, lane, split * p.split_stride);
+    epilogue<BLOCK_N>(p, acc, row, row_ok, n0, frame, lane, split * p.split_stride + bat * p.out_batch_stride);
   }
 }
 
@@ -574,8 +583,8 @@ int launch(const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
   const double kl = g.k_logical > 0 ? g.k_logical : g.K;
   const double out_b = (g.out_f32 ? 4.0 : 0.0) + (g.out_planes ? 2.0 * g.out_P : 0.0) + (g.residual ? 4.0 : 0.0);
   const double a_elems = (g.mode == kGemmConv3x3) ? (double)g.M * g.C : (double)g.M * g.K;
-  ProfileScope ps(g.tag ? g.tag : "gemm", stream, 2.0 * g.M * g.N * kl,
-                  2.0 * P * (a_elems + (double)g.N * g.K) + out_b * g.M * g.N);
+  ProfileScope ps(g.tag ? g.tag : "gemm", stream, 2.0 * g.batch * g.M * g.N * kl,
+                  g.batch * (2.0 * P * (a_elems + (double)g.N * g.K) + out_b * g.M * g.N));
   const int sms = num_sms();
   const int tiles = p.num_m_tiles * p.num_n_tiles * (p.split_k > 1 ? p.split_k : 1);  // work items
   const int grid = tiles < sms ? tiles : sms;
@@ -629,6 +638,18 @@ int validate_gemm_args(const GemmArgs& g) {
     TAPIR_CHECK_ARG(g.out_P >= 1 && g.out_P <= 3 && g.ldp >= g.N, "gemm: bad plane output (out_P=%d ldp=%d)", g.out_P, g.ldp);
   if (g.out_f32 != nullptr) TAPIR_CHECK_ARG(g.ldo >= g.N, "gemm: ldo=%d < N=%d", g.ldo, g.N);
   if (g.residual != nullptr) TAPIR_CHECK_ARG(g.ldr >= g.N, "gemm: ldr=%d < N=%d", g.ldr, g.N);
+  TAPIR_CHECK_ARG(g.batch >= 1 && g.batch <= 65535, "gemm: batch=%d must be 1..65535", g.batch);
+  if (g.batch > 1) {
+    TAPIR_CHECK_ARG(g.mode == kGemmPlain && g.out_f32 != nullptr && g.out_planes == nullptr &&
+                        g.residual == nullptr && g.stats == nullptr,
+                    "gemm: a batched GEMM is plain mode with an fp32 output and no residual or statistics");
+    TAPIR_CHECK_ARG(g.a_batch_rows >= 0 && g.b_batch_rows >= 0 && g.out_batch_stride >= 0,
+                    "gemm: negative batch stride");
+    const long long arows = g.a_batch_rows > 0 ? g.a_batch_rows : g.M;
+    const long long brows = g.b_batch_rows > 0 ? g.b_batch_rows : g.N;
+    TAPIR_CHECK_ARG(arows >= g.M && brows >= g.N && arows * g.batch < (1ll << 31) && brows * g.batch < (1ll << 31),
+                    "gemm: batch strides out of range");
+  }
   if (g.stats != nullptr) {
     TAPIR_CHECK_ARG(g.out_planes == nullptr, "gemm: fused statistics need an fp32-only output");
     if (g.mode == kGemmPlain)
@@ -661,6 +682,11 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
   p.stats = g.stats;
   p.rows_per_frame = g.rows_per_frame > 0 ? g.rows_per_frame : g.M;
   const int P = g.planes;
+  const long long a_batch_rows = g.a_batch_rows > 0 ? g.a_batch_rows : g.M;
+  const long long b_batch_rows = g.b_batch_rows > 0 ? g.b_batch_rows : g.N;
+  p.a_batch_rows = a_batch_rows;
+  p.b_batch_rows = b_batch_rows;
+  p.out_batch_stride = g.out_batch_stride > 0 ? g.out_batch_stride : (long long)g.M * g.ldo;
 
   if (g.mode == kGemmConv3x3) {
     choose_conv_tile(g.H, g.W, &p.tileW, &p.tileH);
@@ -677,9 +703,10 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
     cuuint32_t box[5] = {(cuuint32_t)kBlockK, (cuuint32_t)p.tileW, (cuuint32_t)p.tileH, 1, 1};
     TAPIR_RETURN_IF(encode_bf16_map(&p.tmA, g.a, 5, dims, str, box, "A/conv"));
   } else {
-    p.num_m_tiles = ceil_div(g.M, kBlockM);
-    const long long plane = g.a_plane_stride > 0 ? g.a_plane_stride : (long long)g.M * g.lda;
-    cuuint64_t dims[3] = {(cuuint64_t)g.K, (cuuint64_t)g.M, (cuuint64_t)P};
+    p.num_m_tiles = ceil_div(g.M, kBlockM) * g.batch;
+    const long long a_rows = (g.batch - 1) * a_batch_rows + g.M;
+    const long long plane = g.a_plane_stride > 0 ? g.a_plane_stride : a_rows * g.lda;
+    cuuint64_t dims[3] = {(cuuint64_t)g.K, (cuuint64_t)a_rows, (cuuint64_t)P};
     cuuint64_t str[2] = {(cuuint64_t)g.lda * 2, (cuuint64_t)plane * 2};
     cuuint32_t box[3] = {(cuuint32_t)kBlockK, (cuuint32_t)kBlockM, 1};
     TAPIR_RETURN_IF(encode_bf16_map(&p.tmA, g.a, 3, dims, str, box, "A"));
@@ -734,7 +761,8 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
   // invariance (tests/test_properties_gpu.py re-chunks config 2 into 1776-row chunks,
   // tests/multi_gpu_check.py shards 1152 rows over two ranks, both demand bit-level agreement).
   const bool splittable = splitk_on && g.allow_splitk && g.splitk_ws != nullptr && g.stats == nullptr &&
-                          p.num_k_blocks >= 32;
+                          g.batch == 1 && p.num_k_blocks >= 32;
+  p.m_tiles_per_batch = p.num_m_tiles / g.batch;
   int bn = pick_block_n(p.num_m_tiles, g.N);
   // a small problem that will be split over K keeps 128-wide tiles: the parallelism comes from K,
   // and wide tiles re-read the A operand half as often
@@ -743,8 +771,9 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
     bn = 128;
   p.num_n_tiles = ceil_div(g.N, bn);
   {
-    const long long plane = g.b_plane_stride > 0 ? g.b_plane_stride : (long long)g.N * g.ldb;
-    cuuint64_t dims[3] = {(cuuint64_t)g.K, (cuuint64_t)g.N, (cuuint64_t)P};
+    const long long b_rows = (g.batch - 1) * b_batch_rows + g.N;
+    const long long plane = g.b_plane_stride > 0 ? g.b_plane_stride : b_rows * g.ldb;
+    cuuint64_t dims[3] = {(cuuint64_t)g.K, (cuuint64_t)b_rows, (cuuint64_t)P};
     cuuint64_t str[2] = {(cuuint64_t)g.ldb * 2, (cuuint64_t)plane * 2};
     cuuint32_t box[3] = {(cuuint32_t)kBlockK, (cuuint32_t)bn, 1};
     TAPIR_RETURN_IF(encode_bf16_map(&p.tmB, g.b, 3, dims, str, box, "B"));

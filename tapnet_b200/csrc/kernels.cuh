@@ -63,15 +63,17 @@ int sample_query_features(const float* grid, int T, int gh, int gw, int C, const
 int cost_volume_head(const tapir_head_weights* w, const float* cost_volume, int N, int T,
                      const float* query_tyx, float temperature, int init_h, int init_w,
                      float* points, float* occ, float* expd, int* argmax, cudaStream_t s);
-size_t cost_volume_workspace_bytes(int N, int T, int gh, int gw, int C);
-int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid, int N,
-                       int T, int gh, int gw, int C, const float* query_tyx, float temperature,
+// B clips: qfeat [B][N][C], grid [B][T][gh][gw][C], outputs indexed by flattened query b*N + n
+size_t cost_volume_workspace_bytes(int B, int N, int T, int gh, int gw, int C);
+int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid, int B,
+                       int N, int T, int gh, int gw, int C, const float* query_tyx, float temperature,
                        int init_h, int init_w, float* points, float* occ, float* expd, int* argmax,
                        void* ws, size_t ws_bytes, cudaStream_t s);
 
 // ---- refinement (refine.cu) -------------------------------------------------------------
 int pool_pyramid(const float* grid, int T, int h, int w, int C, float* out, cudaStream_t s);
-int local_corr(const tapir_corr_args* a, cudaStream_t s);
+// a->num_points queries per clip, `batch` clips; level grids are [batch][T][h][w][C]
+int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s);
 size_t mixer_workspace_bytes(long long rows, int planes);
 int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* ws, size_t ws_bytes,
                   cudaStream_t s);

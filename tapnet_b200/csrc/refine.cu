@@ -49,6 +49,7 @@ constexpr int kBoxCells = kBoxRows * kBoxColsMax;
 
 struct CorrParams {
   tapir_corr_args a;
+  int batch;  // clips; query q = b * a.num_points + n reads frame b * T + t of every level
 };
 
 template <int V>  // V = C / 128 float4 per lane
@@ -102,8 +103,11 @@ __global__ void __launch_bounds__(32 * TAPIR_MAX_CORR_LEVELS) local_corr_kernel(
   // CTAs are issued frame-major: the CTAs resident at any time read the grids of one or two
   // frames (3.3 MB per frame at 256^2), which therefore stay in L2; the row order (n, t) of the
   // inputs / outputs would cycle through every frame's grids (all of them exceed L2) per query.
-  const int t = (int)(blockIdx.x / (unsigned)a.num_points);
-  const int n = (int)(blockIdx.x - (unsigned)t * (unsigned)a.num_points);
+  // n is the query flattened over the clips, b its clip.
+  const unsigned nq = (unsigned)a.num_points * (unsigned)p.batch;
+  const int t = (int)(blockIdx.x / nq);
+  const int n = (int)(blockIdx.x - (unsigned)t * nq);
+  const int b = n / a.num_points;
   const long long row = (long long)n * T + t;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float px = a.pos[row * 2 + 0], py = a.pos[row * 2 + 1];
@@ -126,7 +130,7 @@ __global__ void __launch_bounds__(32 * TAPIR_MAX_CORR_LEVELS) local_corr_kernel(
     const int x_last = (int)floorf(pix(cx, 3, gw)) + 1;
     int box_w = x_last - x0 + 1;
     if (box_w < 2) box_w = 2;
-    const float* frame = L.grid + (long long)t * gh * gw * L.C;
+    const float* frame = L.grid + ((long long)b * T + t) * gh * gw * L.C;
     if (box_w > kBoxColsMax) {
       // Wide grids (w/h > 2: the reference spaces the 49 samples gw/gh cells apart in x because it
       // normalises x by h, utils.py:104): the samples' cells no longer fit the 8 x 16 box, so
@@ -552,9 +556,12 @@ int pool_pyramid(const float* grid, int T, int h, int w, int C, float* out, cuda
   return kOk;
 }
 
-int local_corr(const tapir_corr_args* a, cudaStream_t s) {
+int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s) {
   TAPIR_CHECK_ARG(a != nullptr && a->num_levels >= 1 && a->num_levels <= TAPIR_MAX_CORR_LEVELS,
                   "local_corr: bad level count");
+  TAPIR_CHECK_ARG(batch >= 1, "local_corr: bad clip count %d", batch);
+  TAPIR_CHECK_ARG(a->pos && a->occ && a->expd && a->feat_hi && a->feat_lo && a->out_planes,
+                  "local_corr: null pointer");
   TAPIR_CHECK_ARG(a->planes >= 1 && a->planes <= 3 && a->num_points > 0 && a->num_frames > 0,
                   "local_corr: bad shape");
   TAPIR_CHECK_ARG(a->ld >= 388 + 49 * a->num_levels && a->ld % 8 == 0, "local_corr: ld=%d too small", a->ld);
@@ -565,9 +572,11 @@ int local_corr(const tapir_corr_args* a, cudaStream_t s) {
     // (x spacing of the 49 samples is gw/gh cells - a reference quirk; boxes wider than the
     // 16-column table take the per-sample path inside the kernel)
   }
+  const long long rows = (long long)a->num_points * batch * a->num_frames;
+  TAPIR_CHECK_ARG(rows < (1ll << 31), "local_corr: %lld rows exceed one launch", rows);
   CorrParams p;
   p.a = *a;
-  const long long rows = (long long)a->num_points * a->num_frames;
+  p.batch = batch;
   double cell_bytes = 0;
   for (int l = 0; l < a->num_levels; ++l) cell_bytes += 64.0 * a->levels[l].C * 4;
   // SURVEY.md 8(d): N*T*(64 cells * sum C * e + 384*4 + 8 + 147*4)

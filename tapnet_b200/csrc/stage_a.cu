@@ -958,15 +958,16 @@ struct CvPlan {
   int generic_ctas;
 };
 constexpr int kGenericCtasPerSm = 4;
-size_t plan_cv(Arena& a, int N, int T, int gh, int gw, int C, CvPlan* p) {
+// B clips of N queries and T frames each
+size_t plan_cv(Arena& a, int B, int N, int T, int gh, int gw, int C, CvPlan* p) {
   const long long cells = (long long)T * gh * gw;
-  p->q = a.take<__nv_bfloat16>((size_t)N * C * kCvPlanes);
-  p->g = a.take<__nv_bfloat16>((size_t)cells * C * kCvPlanes);
-  p->cv = a.take<float>((size_t)N * cells);
+  p->q = a.take<__nv_bfloat16>((size_t)B * N * C * kCvPlanes);
+  p->g = a.take<__nv_bfloat16>((size_t)B * cells * C * kCvPlanes);
+  p->cv = a.take<float>((size_t)B * N * cells);
   p->generic_scratch = nullptr;
   p->generic_ctas = 0;
   if (gh != kG || gw != kG) {
-    const long long maps = (long long)N * T;
+    const long long maps = (long long)B * N * T;
     const long long cap = 132ll * kGenericCtasPerSm;  // independent of the device: sizes must agree
     p->generic_ctas = (int)(maps < cap ? maps : cap);
     p->generic_scratch =
@@ -976,51 +977,64 @@ size_t plan_cv(Arena& a, int N, int T, int gh, int gw, int C, CvPlan* p) {
 }
 }  // namespace
 
-size_t cost_volume_workspace_bytes(int N, int T, int gh, int gw, int C) {
+size_t cost_volume_workspace_bytes(int B, int N, int T, int gh, int gw, int C) {
+  if (B < 1) return 0;
   Arena a(nullptr, 0);
   CvPlan p;
-  return plan_cv(a, N, T, gh, gw, C, &p) + 256;
+  return plan_cv(a, B, N, T, gh, gw, C, &p) + 256;
 }
 
-int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid, int N,
-                       int T, int gh, int gw, int C, const float* query_tyx, float temperature,
+int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid, int B,
+                       int N, int T, int gh, int gw, int C, const float* query_tyx, float temperature,
                        int init_h, int init_w, float* points, float* occ, float* expd, int* argmax,
                        void* ws, size_t ws_bytes, cudaStream_t s) {
   TAPIR_CHECK_ARG(w && qfeat && grid && points && occ && expd, "cost_volume_tracks: null pointer");
+  TAPIR_CHECK_ARG(B > 0, "cost_volume_tracks: bad clip count B=%d", B);
   TAPIR_CHECK_ARG(N > 0 && T > 0 && C % 64 == 0, "cost_volume_tracks: bad shape N=%d T=%d C=%d", N, T, C);
   TAPIR_CHECK_ARG(gh >= 2 && gw >= 2, "cost_volume_tracks: map %dx%d too small", gh, gw);
+  // the 32 x 32 head launches a (T, queries) grid
+  TAPIR_CHECK_ARG((gh != kG || gw != kG) || (long long)B * N <= 65535,
+                  "cost_volume_tracks: at most 65535 queries per call (B*N=%lld)", (long long)B * N);
   Arena arena(ws, ws_bytes);
   CvPlan p;
-  plan_cv(arena, N, T, gh, gw, C, &p);
+  plan_cv(arena, B, N, T, gh, gw, C, &p);
   if (!arena.ok) {
     set_error("cost_volume_tracks: workspace too small (%zu < %zu)", ws_bytes, arena.off);
     return kWorkspaceTooSmall;
   }
+  // qfeat [B][N][C] -> planes [3][B*N][C]; grid [B][T][gh][gw][C] -> planes [3][B*cells][C]
   const long long cells = (long long)T * gh * gw;
-  TAPIR_RETURN_IF(split_planes(qfeat, C, p.q, C, (long long)N * C, N, C, C, kCvPlanes, s));
-  TAPIR_RETURN_IF(split_planes(grid, C, p.g, C, cells * C, cells, C, C, kCvPlanes, s));
+  const int BN = B * N;
+  TAPIR_RETURN_IF(split_planes(qfeat, C, p.q, C, (long long)BN * C, BN, C, C, kCvPlanes, s));
+  TAPIR_RETURN_IF(split_planes(grid, C, p.g, C, B * cells * C, B * cells, C, C, kCvPlanes, s));
+  // one batched GEMM: cv [B*N][cells], clip b = queries b*N.. against cells b*cells..
   GemmArgs g;
   g.planes = kCvPlanes;
   g.M = N;
   g.N = (int)cells;
   g.K = C;
-  g.a = p.q; g.lda = C; g.a_plane_stride = (long long)N * C;
-  g.b = p.g; g.ldb = C; g.b_plane_stride = cells * C;
+  g.a = p.q; g.lda = C; g.a_plane_stride = (long long)BN * C;
+  g.b = p.g; g.ldb = C; g.b_plane_stride = B * cells * C;
   g.out_f32 = p.cv; g.ldo = (int)cells;
+  g.batch = B;
+  g.a_batch_rows = N;
+  g.b_batch_rows = cells;
+  g.out_batch_stride = (long long)N * cells;
   g.tag = "cost_volume.gemm";
   TAPIR_RETURN_IF(gemm(g, s));
+  // the heads index maps and query_tyx by flattened query b*N + n
   if (gh != kG || gw != kG) {
     // any other initial_resolution (tapir_model.py:86): generic-size head
-    ProfileScope ps("cost_volume.head", s, 2950208.0 / 1024.0 * gh * gw * N * T,
-                    (double)N * T * (4.0 * gh * gw + 16));
+    ProfileScope ps("cost_volume.head", s, 2950208.0 / 1024.0 * gh * gw * BN * T,
+                    (double)BN * T * (4.0 * gh * gw + 16));
     cost_volume_head_generic_kernel<<<p.generic_ctas, 256, 0, s>>>(
-        *w, p.cv, T, N * T, gh, gw, query_tyx, temperature, init_h, init_w, p.generic_scratch, points,
+        *w, p.cv, T, BN * T, gh, gw, query_tyx, temperature, init_h, init_w, p.generic_scratch, points,
         occ, expd, argmax);
     count_launch();
     TAPIR_LAUNCH_CHECK("cost_volume_head_generic_kernel");
     return kOk;
   }
-  return cost_volume_head(w, p.cv, N, T, query_tyx, temperature, init_h, init_w, points, occ, expd,
+  return cost_volume_head(w, p.cv, BN, T, query_tyx, temperature, init_h, init_w, points, occ, expd,
                           argmax, s);
 }
 

@@ -8,6 +8,10 @@ which is ~260 small kernel launches: at a few query points the GPU idles between
 a CUDA graph (fixed frame size and point count) and replays it: same kernels, same results bit for
 bit, no per-launch host cost.  The causal state lives in static device buffers that the graph
 updates in place; `update_query` mirrors `TAPIR.update_query_features` for re-targeting a point.
+
+With `num_streams=S` one tracker follows S camera streams (same frame size, same point count): a
+step runs the backbone over the S frames in one pass and one batched estimate_trajectories over
+the S clips of one frame each (the reference's batch axis), all in one captured graph.
 """
 from typing import Optional, Tuple
 
@@ -18,22 +22,28 @@ from tapnet_b200 import tapir_model
 
 
 class OnlineTracker:
-  """Graph-replayed per-frame step of a causal TAPIR model (`use_casual_conv=True`)."""
+  """Graph-replayed per-frame step of a causal TAPIR model (`use_casual_conv=True`) over
+  `num_streams` camera streams that share one frame size and one point count (pad a stream with
+  dummy points if it tracks fewer)."""
 
   def __init__(self, model: 'tapir_model.TAPIR', height: int, width: int, num_points: int,
-               uint8_frames: bool = False):
+               uint8_frames: bool = False, num_streams: int = 1):
     if not model.use_casual_conv:
       raise ValueError('OnlineTracker needs a causal model: TAPIR(use_casual_conv=True)')
+    if int(num_streams) < 1:
+      raise ValueError(f'num_streams must be >= 1, got {num_streams}')
     self.model = model
     self.hw = (int(height), int(width))
     self.num_points = int(num_points)
+    self.num_streams = int(num_streams)
     self.dev = next(model.parameters()).device
     if self.dev.type != 'cuda':
       raise RuntimeError('OnlineTracker runs on CUDA only')
     # uint8_frames: frames are raw [0, 255] camera frames (what pytorch_live_demo.py:139-141 holds
     # before preprocess_frames); the normalisation runs inside the stem conv's loads
     self._frame_dtype = torch.uint8 if uint8_frames else torch.float32
-    self._frame = torch.zeros(1, 1, height, width, 3, dtype=self._frame_dtype, device=self.dev)
+    self._frame = torch.zeros(self.num_streams, 1, height, width, 3, dtype=self._frame_dtype,
+                              device=self.dev)
     self._graph: Optional[torch.cuda.CUDAGraph] = None
     self._graph_sig = None
     self._pinned = False
@@ -42,12 +52,15 @@ class OnlineTracker:
     self._out = None
 
   # -- pytorch_live_demo.py:44-54 online_model_init
-  def init(self, frame: torch.Tensor, query_points: torch.Tensor):
-    """frame: [H, W, 3] or [1, 1, H, W, 3] float in [-1, 1]; query_points [N, 3] or [1, N, 3] (t,y,x)."""
-    frame = self._as_frame(frame)
+  def init(self, frames: torch.Tensor, query_points: torch.Tensor):
+    """frames: [S, H, W, 3] (or [S, 1, H, W, 3]; [H, W, 3] when S = 1) float in [-1, 1];
+    query_points [S, N, 3] ([N, 3] when S = 1) as (t, y, x), stream s's on its frame s."""
+    frame = self._as_frames(frames)
     qp = query_points.to(self.dev, torch.float32)
     if qp.dim() == 2:
       qp = qp[None]
+    if qp.dim() != 3 or qp.shape[0] != self.num_streams or qp.shape[2] != 3:
+      raise ValueError(f'query_points must be [{self.num_streams}, N, 3], got {tuple(qp.shape)}')
     if qp.shape[1] != self.num_points:
       raise ValueError(f'expected {self.num_points} query points, got {qp.shape[1]}')
     grids = self.model.get_feature_grids(frame, False)
@@ -57,19 +70,31 @@ class OnlineTracker:
         tuple(t.clone() for t in qf.lowres), tuple(t.clone() for t in qf.hires), qf.resolutions)
     n_res = len(qf.resolutions) - 1
     init = self.model.construct_initial_causal_state(self.num_points, n_res)
-    self.state = [{k: v.to(self.dev).clone() for k, v in d.items()} for d in init]
+    # [S, N, 2, 512 | 2048] per block, one tensor per refinement iteration
+    self.state = [{k: v.to(self.dev).expand(self.num_streams, *v.shape[1:]).clone()
+                   for k, v in d.items()} for d in init]
     self._graph = None
     return self.query_features
 
-  def _as_frame(self, frame):
-    frame = frame.to(self.dev, self._frame_dtype, non_blocking=True)
-    if frame.dim() == 3:
-      frame = frame[None, None]
-    if tuple(frame.shape[2:4]) != self.hw:
-      raise ValueError(f'frame size {tuple(frame.shape[2:4])} != {self.hw}')
-    return frame
+  def _as_frames(self, frames, num=None):
+    """[num, 1, H, W, 3] on the device from [num, H, W, 3], [num, 1, H, W, 3] or, for one
+    frame, [H, W, 3]."""
+    num = self.num_streams if num is None else num
+    frames = frames.to(self.dev, self._frame_dtype, non_blocking=True)
+    if frames.dim() == 3:
+      frames = frames[None, None]
+    elif frames.dim() == 4:
+      frames = frames[:, None]
+    if frames.dim() != 5 or frames.shape[1] != 1 or frames.shape[4] != 3:
+      raise ValueError(f'frames must be [S, H, W, 3], got {tuple(frames.shape)}')
+    if frames.shape[0] != num:
+      raise ValueError(f'expected {num} frames (one per stream), got {frames.shape[0]}')
+    if tuple(frames.shape[2:4]) != self.hw:
+      raise ValueError(f'frame size {tuple(frames.shape[2:4])} != {self.hw}')
+    return frames
 
   def _step_eager(self):
+    # all streams in one backbone pass and one batched estimate_trajectories (B = S, T = 1)
     grids = self.model.get_feature_grids(self._frame, False)
     # single-frame step: the causal state is updated in place (causal_context_out = state)
     r = self.model.estimate_trajectories(self.hw, False, grids, self.query_features, None, 64,
@@ -128,12 +153,13 @@ class OnlineTracker:
       pass
 
   # -- pytorch_live_demo.py:62-85 online_model_predict
-  def step(self, frame: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
-    """Returns (tracks [1, N, 1, 2] in frame pixels (x, y), visibles [1, N, 1] bool).  The
-    returned tensors are the graph's static outputs: copy them if they must outlive the next step."""
+  def step(self, frames: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """frames: [S, H, W, 3] ([H, W, 3] when S = 1), one per stream.  Returns (tracks [S, N, 1, 2]
+    in frame pixels (x, y), visibles [S, N, 1] bool).  The returned tensors are the graph's static
+    outputs: copy them if they must outlive the next step."""
     if self.query_features is None:
       raise RuntimeError('call init(frame, query_points) first')
-    self._frame.copy_(self._as_frame(frame))
+    self._frame.copy_(self._as_frames(frames))
     if self._graph is not None and self._graph_sig != self._model_sig():
       self._graph = None  # stale pointers: the model's buffers or weights changed since capture
     if self._graph is None:
@@ -143,15 +169,28 @@ class OnlineTracker:
 
   @property
   def last_logits(self):
-    """(occlusion, expected_dist) logits of the last step, [1, N, 1] each."""
+    """(occlusion, expected_dist) logits of the last step, [S, N, 1] each."""
     return self._out[2], self._out[3]
 
-  def update_query(self, frame: torch.Tensor, query_point: torch.Tensor, idx: int):
-    """Re-targets point `idx` at (t, y, x) = query_point on `frame` (pytorch_live_demo.py:188-200):
-    its features are re-sampled and its causal state zeroed, in place (graph buffers stay valid)."""
-    frame = self._as_frame(frame)
+  def update_query(self, frame: torch.Tensor, query_point: torch.Tensor, idx: int,
+                   stream: int = 0):
+    """Re-targets point `idx` of stream `stream` at (t, y, x) = query_point on `frame` ([H, W, 3],
+    that stream's frame; pytorch_live_demo.py:188-200): its features are re-sampled and its causal
+    state zeroed, in place (graph buffers stay valid).  Other streams are not touched."""
+    if self.query_features is None:
+      raise RuntimeError('call init(frame, query_points) first')
+    if not 0 <= stream < self.num_streams:
+      raise ValueError(f'stream {stream} out of range [0, {self.num_streams})')
+    if not 0 <= idx < self.num_points:
+      raise ValueError(f'point {idx} out of range [0, {self.num_points})')
+    frame = self._as_frames(frame, num=1)
     qp = query_point.to(self.dev, torch.float32).reshape(1, 1, 3)
     grids = self.model.get_feature_grids(frame, False)
     new = self.model.get_query_features(frame, False, qp, grids)
-    self.query_features, self.state = self.model.update_query_features(
-        self.query_features, new, idx, self.state)
+    # TAPIR.update_query_features writes [:, idx] of every stream; only [stream, idx] changes here
+    for dst, src in zip(self.query_features.lowres + self.query_features.hires,
+                        new.lowres + new.hires):
+      dst[stream, idx] = src[0, 0]
+    for d in self.state:
+      for v in d.values():
+        v[stream, idx] = 0

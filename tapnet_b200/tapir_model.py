@@ -82,6 +82,19 @@ def _ptr(t):
   return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
 
+def _groups(B, N, T):
+  """Work groups of estimate_trajectories as (b0, b1, query slice): whole clips b0..b1-1 with all
+  their queries while the group's rows (clips x queries x frames) fit _MAX_ROWS_PER_CHUNK and its
+  queries fit one head / mixer launch (65535); a clip whose rows alone exceed the bound runs on its
+  own in query chunks.  Each group is one launch sequence over its clips."""
+  if N * T <= _MAX_ROWS_PER_CHUNK and N <= 65535:
+    g = max(1, min(B, _MAX_ROWS_PER_CHUNK // (N * T), 65535 // N))
+    return [(b0, min(b0 + g, B), slice(0, N)) for b0 in range(0, B, g)]
+  chunk_q = max(1, min(N, _MAX_ROWS_PER_CHUNK // T, 65535))
+  return [(bi, bi + 1, slice(q0, min(q0 + chunk_q, N)))
+          for bi in range(B) for q0 in range(0, N, chunk_q)]
+
+
 def _on_model_device(fn):
   """Runs a TAPIR method with the model's CUDA device current.  Kernels launch on the current
   device and the C library keeps per-device state (shared-memory attributes, error flag), so
@@ -638,148 +651,145 @@ class TAPIR(nn.Module):
         out['causal_context'] = new_ctx
       return out
 
-    # pooled pyramid level: once per resolution level (the reference recomputes it every
-    # iteration of every chunk, tapir_model.py:519-527)
+    # pooled pyramid levels: once per resolution level over all B*T frames (the reference
+    # recomputes them every iteration of every chunk, tapir_model.py:519-527); each is the 2x2
+    # average of the one before it
     pooled = {}
+    for level in range(1, num_levels_total):
+      g = feature_grids.lowres[level].contiguous()
+      outs = []
+      for _ in range(self.pyramid_level):
+        _, t, gh, gw, c = g.shape
+        out = new(B, t, gh // 2, gw // 2, c)
+        _lib.check(lib.tapir_pool_pyramid(_ptr(g), B * t, gh, gw, c, _ptr(out), stream),
+                   'tapir_pool_pyramid')
+        outs.append(out)
+        g = out
+      pooled[level] = outs
 
-    def pooled_for(level, bi):
-      """The `pyramid_level` pooled grids of a resolution level (each the 2x2 average of the one
-      before it, tapir_model.py:519-527)."""
-      key = (level, bi)
-      if key not in pooled:
-        g = feature_grids.lowres[level][bi].contiguous()
-        outs = []
-        for _ in range(self.pyramid_level):
-          t, gh, gw, c = g.shape
-          out = new(t, gh // 2, gw // 2, c)
-          _lib.check(lib.tapir_pool_pyramid(_ptr(g), t, gh, gw, c, _ptr(out), stream),
-                     'tapir_pool_pyramid')
-          outs.append(out)
-          g = out
-        pooled[key] = outs
-      return pooled[key]
+    for b0, b1, sl in _groups(B, N, T):
+      G = b1 - b0
+      n = sl.stop - sl.start
+      nq = G * n  # queries of the group, flattened over its clips
+      rows = nq * T
+      bs = slice(b0, b1)
+      # every [bs, sl] slice below is contiguous: either whole clips or a query chunk of one clip
+      # ---- stage A: global cost volume + track / occlusion head
+      grid0 = feature_grids.lowres[0][bs].contiguous()
+      _, _, gh0, gw0, c0 = grid0.shape
+      qf0 = query_features.lowres[0][bs, sl].contiguous()
+      qp = None
+      if query_points_in_video is not None:
+        qp = query_points_in_video[bs, sl].to(torch.float32)
+        # utils.convert_grid_coordinates (coords * out / in), tapir_model.py:488-493
+        qp = (qp * self._const([T, ih, iw], dev) / self._const([T, vh, vw], dev)).contiguous()
+      pos = new(nq, T, 2)
+      # outputs are written in place
+      occ0, expd0 = occ_out[0][bs, sl], expd_out[0][bs, sl]
+      nbytes = lib.tapir_cost_volume_batched_workspace_bytes(G, n, T, gh0, gw0, c0)
+      ws = self._workspace('cost_volume', nbytes, dev)
+      _lib.check(lib.tapir_cost_volume_tracks_batched(
+          ctypes.byref(pk['head']), _ptr(qf0), _ptr(grid0), G, n, T, gh0, gw0, c0, _ptr(qp),
+          float(self.softmax_temperature), ih, iw, _ptr(pos), _ptr(occ0), _ptr(expd0),
+          _ptr(am_out[bs, sl]) if am_out is not None else None,
+          _ptr(ws), ws.numel(), stream), 'tapir_cost_volume_tracks_batched')
+      # train2orig (tapir_model.py:435-441)
+      torch.div(pos.view(G, n, T, 2) * self._const([vw, vh], dev), self._const([iw, ih], dev),
+                out=trk_out[0][bs, sl])
 
-    chunk_q = max(1, min(N, _MAX_ROWS_PER_CHUNK // max(T, 1), 65535))
-    for bi in range(B):
-      grid0 = feature_grids.lowres[0][bi].contiguous()
-      _, gh0, gw0, c0 = grid0.shape
-      for q0 in range(0, N, chunk_q):
-        n = min(chunk_q, N - q0)
-        rows = n * T
-        sl = slice(q0, q0 + n)
-        # ---- stage A: global cost volume + track / occlusion head
-        qf0 = query_features.lowres[0][bi, sl].contiguous()
-        qp = None
-        if query_points_in_video is not None:
-          qp = query_points_in_video[bi, sl].to(torch.float32)
-          # utils.convert_grid_coordinates (coords * out / in), tapir_model.py:488-493
-          qp = (qp * self._const([T, ih, iw], dev) / self._const([T, vh, vw], dev)).contiguous()
-        pos = new(n, T, 2)
-        # outputs are written in place: [bi, q0:q0+n] slices of the result tensors are contiguous
-        occ0, expd0 = occ_out[0][bi, sl], expd_out[0][bi, sl]
-        nbytes = lib.tapir_cost_volume_workspace_bytes(n, T, gh0, gw0, c0)
-        ws = self._workspace('cost_volume', nbytes, dev)
-        _lib.check(lib.tapir_cost_volume_tracks(
-            ctypes.byref(pk['head']), _ptr(qf0), _ptr(grid0), n, T, gh0, gw0, c0, _ptr(qp),
-            float(self.softmax_temperature), ih, iw, _ptr(pos), _ptr(occ0), _ptr(expd0),
-            _ptr(am_out[bi, sl]) if am_out is not None else None,
-            _ptr(ws), ws.numel(), stream), 'tapir_cost_volume_tracks')
-        # train2orig (tapir_model.py:435-441)
-        torch.div(pos * self._const([vw, vh], dev), self._const([iw, ih], dev),
-                  out=trk_out[0][bi, sl])
+      # ---- refinement iterations
+      x_planes = new(P, rows, kin, dtype=torch.bfloat16)
+      res = new(rows, 388)
+      feats = [new(nq, T, 384), new(nq, T, 384)]
+      occ, expd = occ0, expd0
+      nbytes = lib.tapir_mixer_workspace_bytes(rows, P)
+      mws = self._workspace('mixer', nbytes, dev)
+      have_feats = False
+      cur = 0
+      for it in range(num_iters):
+        level = it // self.num_pips_iter + 1
+        hires_g = feature_grids.hires[level][bs].contiguous()
+        lowres_g = feature_grids.lowres[level][bs].contiguous()
+        ca = _lib.CorrArgs()
+        grids = [hires_g, lowres_g] + [g[bs] for g in pooled[level]]
+        for li, g in enumerate(grids):
+          ca.levels[li].grid = g.data_ptr()
+          ca.levels[li].h, ca.levels[li].w, ca.levels[li].C = g.shape[2], g.shape[3], g.shape[4]
+        ca.num_levels = L
+        ca.num_points, ca.num_frames = n, T
+        ca.init_h, ca.init_w = ih, iw
+        ca.planes = P
+        ca.pos, ca.occ, ca.expd = pos.data_ptr(), occ.data_ptr(), expd.data_ptr()
+        if have_feats:
+          fsrc = feats[cur]
+          fh = (fsrc.data_ptr(), T * 384, 384)
+          fl = (fsrc.data_ptr() + 128 * 4, T * 384, 384)
+        else:
+          qh = query_features.hires[level][bs, sl].contiguous()
+          ql = query_features.lowres[level][bs, sl].contiguous()
+          fh = (qh.data_ptr(), 128, 0)
+          fl = (ql.data_ptr(), 256, 0)
+        ca.feat_hi, ca.feat_hi_stride_n, ca.feat_hi_stride_t = fh
+        ca.feat_lo, ca.feat_lo_stride_n, ca.feat_lo_stride_t = fl
+        ca.out_planes = x_planes.data_ptr()
+        ca.out_plane_stride = rows * kin
+        ca.ld = kin
+        _lib.check(lib.tapir_local_corr_batched(ctypes.byref(ca), G, stream),
+                   'tapir_local_corr_batched')
 
-        # ---- refinement iterations
-        x_planes = new(P, rows, kin, dtype=torch.bfloat16)
-        res = new(rows, 388)
-        feats = [new(n, T, 384), new(n, T, 384)]
-        occ, expd = occ0, expd0
-        nbytes = lib.tapir_mixer_workspace_bytes(rows, P)
-        mws = self._workspace('mixer', nbytes, dev)
-        have_feats = False
-        cur = 0
-        for it in range(num_iters):
-          level = it // self.num_pips_iter + 1
-          hires_g = feature_grids.hires[level][bi].contiguous()
-          lowres_g = feature_grids.lowres[level][bi].contiguous()
-          ca = _lib.CorrArgs()
-          grids = [hires_g, lowres_g] + (pooled_for(level, bi) if self.pyramid_level else [])
-          for li, g in enumerate(grids):
-            ca.levels[li].grid = g.data_ptr()
-            ca.levels[li].h, ca.levels[li].w, ca.levels[li].C = g.shape[1], g.shape[2], g.shape[3]
-          ca.num_levels = L
-          ca.num_points, ca.num_frames = n, T
-          ca.init_h, ca.init_w = ih, iw
-          ca.planes = P
-          ca.pos, ca.occ, ca.expd = pos.data_ptr(), occ.data_ptr(), expd.data_ptr()
-          if have_feats:
-            fsrc = feats[cur]
-            fh = (fsrc.data_ptr(), T * 384, 384)
-            fl = (fsrc.data_ptr() + 128 * 4, T * 384, 384)
-          else:
-            qh = query_features.hires[level][bi, sl].contiguous()
-            ql = query_features.lowres[level][bi, sl].contiguous()
-            fh = (qh.data_ptr(), 128, 0)
-            fl = (ql.data_ptr(), 256, 0)
-          ca.feat_hi, ca.feat_hi_stride_n, ca.feat_hi_stride_t = fh
-          ca.feat_lo, ca.feat_lo_stride_n, ca.feat_lo_stride_t = fl
-          ca.out_planes = x_planes.data_ptr()
-          ca.out_plane_stride = rows * kin
-          ca.ld = kin
-          _lib.check(lib.tapir_local_corr(ctypes.byref(ca), stream), 'tapir_local_corr')
+        io = _lib.MixerIO()
+        io.x_planes = x_planes.data_ptr()
+        io.x_plane_stride = rows * kin
+        io.ldx = kin
+        io.num_points, io.num_frames = nq, T
+        io.causal = int(self.use_casual_conv)
+        holders = []
+        if causal_context is not None:
+          c1 = [causal_context[it][f'block_{i}_causal_1'][bs, sl].to(device=dev, dtype=torch.float32).contiguous()
+                for i in range(nb)]
+          c2 = [causal_context[it][f'block_{i}_causal_2'][bs, sl].to(device=dev, dtype=torch.float32).contiguous()
+                for i in range(nb)]
+          holders += c1 + c2
+          io.ctx1_in = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in c1])
+          io.ctx2_in = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in c2])
+        o1 = o2 = None
+        if write_ctx:
+          o1 = [new_ctx[it][f'block_{i}_causal_1'][bs, sl] for i in range(nb)]
+          o2 = [new_ctx[it][f'block_{i}_causal_2'][bs, sl] for i in range(nb)]
+          io.ctx1_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o1])
+          io.ctx2_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o2])
+        io.out = res.data_ptr()
+        io.ldo = 388
+        _lib.check(lib.tapir_mixer_forward(ctypes.byref(pk['mixer']), ctypes.byref(io), _ptr(mws),
+                                           mws.numel(), stream), 'tapir_mixer_forward')
 
-          io = _lib.MixerIO()
-          io.x_planes = x_planes.data_ptr()
-          io.x_plane_stride = rows * kin
-          io.ldx = kin
-          io.num_points, io.num_frames = n, T
-          io.causal = int(self.use_casual_conv)
-          holders = []
-          if causal_context is not None:
-            c1 = [causal_context[it][f'block_{i}_causal_1'][bi, sl].to(device=dev, dtype=torch.float32).contiguous()
-                  for i in range(nb)]
-            c2 = [causal_context[it][f'block_{i}_causal_2'][bi, sl].to(device=dev, dtype=torch.float32).contiguous()
-                  for i in range(nb)]
-            holders += c1 + c2
-            io.ctx1_in = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in c1])
-            io.ctx2_in = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in c2])
-          o1 = o2 = None
-          if write_ctx:
-            o1 = [new_ctx[it][f'block_{i}_causal_1'][bi, sl] for i in range(nb)]
-            o2 = [new_ctx[it][f'block_{i}_causal_2'][bi, sl] for i in range(nb)]
-            io.ctx1_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o1])
-            io.ctx2_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o2])
-          io.out = res.data_ptr()
-          io.ldo = 388
-          _lib.check(lib.tapir_mixer_forward(ctypes.byref(pk['mixer']), ctypes.byref(io), _ptr(mws),
-                                             mws.numel(), stream), 'tapir_mixer_forward')
-
-          ua = _lib.UpdateArgs()
-          ua.res, ua.ld_res = res.data_ptr(), 388
-          ua.num_points, ua.num_frames = n, T
-          ua.init_h, ua.init_w = ih, iw
-          rh, rw = feature_grids.resolutions[level]
-          ua.resize_h, ua.resize_w = int(rh), int(rw)
-          ua.video_h, ua.video_w = vh, vw
-          ua.feat_hi, ua.feat_hi_stride_n, ua.feat_hi_stride_t = fh
-          ua.feat_lo, ua.feat_lo_stride_n, ua.feat_lo_stride_t = fl
-          nxt = 1 - cur if have_feats else cur
-          trk_i = trk_out[it + 1][bi, sl]
-          occ_n, expd_n = occ_out[it + 1][bi, sl], expd_out[it + 1][bi, sl]
-          ua.pos = pos.data_ptr()
-          ua.occ_in, ua.expd_in = occ.data_ptr(), expd.data_ptr()
-          ua.occ_out, ua.expd_out = occ_n.data_ptr(), expd_n.data_ptr()
-          ua.feat_out = feats[nxt].data_ptr()
-          ua.tracks_out = trk_i.data_ptr()
-          _lib.check(lib.tapir_refine_update(ctypes.byref(ua), stream), 'tapir_refine_update')
-          cur = nxt
-          have_feats = True
-          occ, expd = occ_n, expd_n
-          if (it + 1) % self.num_pips_iter == 0:
-            # level boundary (tapir_model.py:549-552): features restart from the query,
-            # occlusion / expected_dist revert to the stage-A estimate, positions carry over
-            have_feats = False
-            occ, expd = occ0, expd0
-          del holders
+        ua = _lib.UpdateArgs()
+        ua.res, ua.ld_res = res.data_ptr(), 388
+        ua.num_points, ua.num_frames = nq, T
+        ua.init_h, ua.init_w = ih, iw
+        rh, rw = feature_grids.resolutions[level]
+        ua.resize_h, ua.resize_w = int(rh), int(rw)
+        ua.video_h, ua.video_w = vh, vw
+        ua.feat_hi, ua.feat_hi_stride_n, ua.feat_hi_stride_t = fh
+        ua.feat_lo, ua.feat_lo_stride_n, ua.feat_lo_stride_t = fl
+        nxt = 1 - cur if have_feats else cur
+        trk_i = trk_out[it + 1][bs, sl]
+        occ_n, expd_n = occ_out[it + 1][bs, sl], expd_out[it + 1][bs, sl]
+        ua.pos = pos.data_ptr()
+        ua.occ_in, ua.expd_in = occ.data_ptr(), expd.data_ptr()
+        ua.occ_out, ua.expd_out = occ_n.data_ptr(), expd_n.data_ptr()
+        ua.feat_out = feats[nxt].data_ptr()
+        ua.tracks_out = trk_i.data_ptr()
+        _lib.check(lib.tapir_refine_update(ctypes.byref(ua), stream), 'tapir_refine_update')
+        cur = nxt
+        have_feats = True
+        occ, expd = occ_n, expd_n
+        if (it + 1) % self.num_pips_iter == 0:
+          # level boundary (tapir_model.py:549-552): features restart from the query,
+          # occlusion / expected_dist revert to the stage-A estimate, positions carry over
+          have_feats = False
+          occ, expd = occ0, expd0
+        del holders
 
     out = dict(occlusion=occ_out, tracks=trk_out, expected_dist=expd_out)
     if get_causal_context:
