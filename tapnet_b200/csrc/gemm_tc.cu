@@ -3,10 +3,12 @@
 // One persistent CTA per SM, three warpgroups:
 //   warpgroup 0 (one lane)  TMA producer: cp.async.bulk.tensor tiles of A and B planes into a
 //                           multi-stage shared-memory ring (128B-swizzled, K-major)
-//   warpgroups 1, 2         consumers: each owns 64 rows of the 128-row tile, issues
-//                           wgmma.m64nBLOCK_Nk16 (bf16 operands from shared memory, fp32
-//                           accumulators in registers) and then runs the epilogue from its
-//                           registers: bias / tanh-GELU / residual, fp32 and/or bf16-plane stores
+//   warpgroups 1, 2         consumers: issue wgmma.m64nBLOCK_Nk16 (bf16 operands from shared
+//                           memory, fp32 accumulators in registers) and then run the epilogue
+//                           from their registers: bias / tanh-GELU / residual, fp32 and/or
+//                           bf16-plane stores.  Cooperative schedule (gemm_tc_kernel): each owns
+//                           64 rows of every 128-row tile.  Ping-pong schedule
+//                           (gemm_tc_pingpong_kernel): each owns whole tiles, alternately.
 // full/empty mbarriers between producer and consumers; the producer runs ahead into the next
 // tile while the consumers are in the epilogue of the current one.
 //
@@ -194,55 +196,71 @@ __device__ __forceinline__ void tile_row(const TcParams& p, int m_tile, int r, l
   }
 }
 
-template <int BLOCK_N, int P>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_tc_kernel(const __grid_constant__ TcParams p) {
-  using Cfg = TcCfg<BLOCK_N, P>;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = ptx::smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
-  uint64_t* empty_bar = full_bar + Cfg::kStages;
+// Epilogue of rows [r_base, r_base + 64) of output tile `m_tile`, held by one consumer warpgroup.
+template <int BLOCK_N>
+__device__ __forceinline__ void tile_epilogue(const TcParams& p, const float (&acc)[BLOCK_N / 2], int m_tile,
+                                              int r_base, int n0, int warp, int lane, long long out_off) {
+  const int r0 = r_base + warp * 16 + (lane >> 2);
+  long long row[2];
+  bool row_ok[2];
+  tile_row(p, m_tile, r0, row[0], row_ok[0]);
+  tile_row(p, m_tile, r0 + 8, row[1], row_ok[1]);
+  int frame = 0;
+  if (p.stats != nullptr)
+    frame = (p.mode == kGemmConv3x3) ? m_tile / (p.tiles_x * p.tiles_y)
+                                     : (int)(((long long)m_tile * kBlockM) / p.rows_per_frame);
+  epilogue<BLOCK_N>(p, acc, row, row_ok, n0, frame, lane, out_off);
+}
 
-  const int wg = threadIdx.x >> 7;
-  const int warp = (threadIdx.x >> 5) & 3;  // within the warpgroup
-  const int lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::kStages; ++s) {
-      ptx::mbar_init(&full_bar[s], 1);
-      ptx::mbar_init(&empty_bar[s], kConsumerArrivals);
-    }
-    ptx::fence_barrier_init();
-    ptx::prefetch_tensormap(&p.tmA);
-    ptx::prefetch_tensormap(&p.tmB);
-  }
-  __syncthreads();
-
-  const int nkb = p.num_k_blocks;
-  // split-K (small problems that cannot fill the GPU): work item = (tile, k-slice)
+// Work item w in the order (batch, m-tile, n-tile, k-slice); m_tile is the tile within its batch,
+// [kb0, kb1) its k-blocks.  Returns the k-slice.
+template <int BLOCK_N>
+__device__ __forceinline__ int decode_work(const TcParams& p, int w, int& bat, int& m_tile, int& n0, int& kb0,
+                                           int& kb1) {
   const int S = p.split_k;
-  const int num_work = p.num_m_tiles * p.num_n_tiles * S;
-  // work item order (batch, m-tile, n-tile, k-slice); m_tile is the tile within its batch
-  auto decode = [&](int w, int& bat, int& m_tile, int& n0, int& kb0, int& kb1) {
-    const int split = w % S;
-    const int tile = w / S;
-    m_tile = tile / p.num_n_tiles;
-    n0 = (tile - m_tile * p.num_n_tiles) * BLOCK_N;
-    bat = m_tile / p.m_tiles_per_batch;
-    m_tile -= bat * p.m_tiles_per_batch;
-    kb0 = (int)((long long)nkb * split / S);
-    kb1 = (int)((long long)nkb * (split + 1) / S);
-    return split;
-  };
+  const int split = w % S;
+  const int tile = w / S;
+  m_tile = tile / p.num_n_tiles;
+  n0 = (tile - m_tile * p.num_n_tiles) * BLOCK_N;
+  bat = m_tile / p.m_tiles_per_batch;
+  m_tile -= bat * p.m_tiles_per_batch;
+  kb0 = (int)((long long)p.num_k_blocks * split / S);
+  kb1 = (int)((long long)p.num_k_blocks * (split + 1) / S);
+  return split;
+}
 
-  if (wg == 0) {
-    if (threadIdx.x != 0) return;
-    // ------------------------------------------------------------------ TMA producer
+// Shared-memory ring of both GEMM schedules: kStages stages of P A planes then P B planes, then the
+// full and empty mbarriers.  Initialised by thread 0 before the __syncthreads() that follows.
+template <int BLOCK_N, int P>
+struct Ring {
+  using Cfg = TcCfg<BLOCK_N, P>;
+  uint8_t* smem;
+  uint64_t* full_bar;
+  uint64_t* empty_bar;
+  __device__ __forceinline__ Ring(uint8_t* smem_raw, const TcParams& p, uint32_t empty_arrivals) {
+    const uint32_t raw_addr = ptx::smem_u32(smem_raw);
+    smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
+    full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
+    empty_bar = full_bar + Cfg::kStages;
+    if (threadIdx.x == 0) {
+      for (int s = 0; s < Cfg::kStages; ++s) {
+        ptx::mbar_init(&full_bar[s], 1);
+        ptx::mbar_init(&empty_bar[s], empty_arrivals);
+      }
+      ptx::fence_barrier_init();
+      ptx::prefetch_tensormap(&p.tmA);
+      ptx::prefetch_tensormap(&p.tmB);
+    }
+  }
+
+  // TMA producer (one thread): the k-blocks of this CTA's work items, in order, into the ring.
+  __device__ __forceinline__ void produce(const TcParams& p) const {
+    const int num_work = p.num_m_tiles * p.num_n_tiles * p.split_k;
     int stage = 0;
     uint32_t phase = 0;
     for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
       int bat, m_tile, n0, kb0, kb1;
-      decode(w, bat, m_tile, n0, kb0, kb1);
+      decode_work<BLOCK_N>(p, w, bat, m_tile, n0, kb0, kb1);
       // batch = row offset into the flattened operands; rows loaded past the end of a batch
       // belong to the next one (or are TMA zero fill) and are masked by the epilogue
       const int a_row0 = (int)(bat * p.a_batch_rows) + m_tile * kBlockM;
@@ -280,6 +298,31 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
         if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
       }
     }
+  }
+};
+
+// Cooperative schedule: both consumer warpgroups work on every tile, 64 rows each, and run their
+// epilogues at the same time.  Used for split-K, P = 3 and CTAs with fewer than two tiles.
+template <int BLOCK_N, int P>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_tc_kernel(const __grid_constant__ TcParams p) {
+  using Cfg = TcCfg<BLOCK_N, P>;
+  extern __shared__ uint8_t smem_raw[];
+  const Ring<BLOCK_N, P> ring(smem_raw, p, kConsumerArrivals);
+  uint8_t* smem = ring.smem;
+  uint64_t* full_bar = ring.full_bar;
+  uint64_t* empty_bar = ring.empty_bar;
+
+  const int wg = threadIdx.x >> 7;
+  const int warp = (threadIdx.x >> 5) & 3;  // within the warpgroup
+  const int lane = threadIdx.x & 31;
+  __syncthreads();
+
+  // split-K (small problems that cannot fill the GPU): work item = (tile, k-slice)
+  const int num_work = p.num_m_tiles * p.num_n_tiles * p.split_k;
+
+  if (wg == 0) {
+    if (threadIdx.x == 0) ring.produce(p);
     return;
   }
 
@@ -291,7 +334,7 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
   float acc[BLOCK_N / 2];
   for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
     int bat, m_tile, n0, kb0, kb1;
-    const int split = decode(w, bat, m_tile, n0, kb0, kb1);
+    const int split = decode_work<BLOCK_N>(p, w, bat, m_tile, n0, kb0, kb1);
 #pragma unroll
     for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
     int prev = -1;
@@ -325,17 +368,114 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
     ptx::wgmma_wait<0>();
     ptx::reg_fence(acc);
     if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
+    tile_epilogue<BLOCK_N>(p, acc, m_tile, cw * 64, n0, warp, lane,
+                           split * p.split_stride + bat * p.out_batch_stride);
+  }
+}
 
-    const int r0 = cw * 64 + warp * 16 + (lane >> 2);
-    long long row[2];
-    bool row_ok[2];
-    tile_row(p, m_tile, r0, row[0], row_ok[0]);
-    tile_row(p, m_tile, r0 + 8, row[1], row_ok[1]);
-    int frame = 0;
-    if (p.stats != nullptr)
-      frame = (p.mode == kGemmConv3x3) ? m_tile / (p.tiles_x * p.tiles_y)
-                                       : (int)(((long long)m_tile * kBlockM) / p.rows_per_frame);
-    epilogue<BLOCK_N>(p, acc, row, row_ok, n0, frame, lane, split * p.split_stride + bat * p.out_batch_stride);
+// Ping-pong schedule (no split-K, P <= 2): each consumer warpgroup owns whole 128-row tiles, two
+// m64 wgmma per k step (rows 0-63 and 64-127), and the CTA's tiles alternate between the two.  The
+// warpgroups take turns on the tensor pipe: one issues its tile's whole mainloop, passes the turn
+// and runs its epilogue while the other's MMAs execute, so the epilogue costs no MMA time as long
+// as it is shorter than a mainloop.  The producer is the cooperative one: the ring holds tile t's
+// k-blocks, then tile t + 1's, and each stage is read (and released) by one warpgroup.
+//
+// The turn also keeps the full-barrier parity waits exact: a warpgroup waits on its tile's first
+// stage only after the other has waited on every stage of the tile before, so the stage it waits
+// on has completed all earlier fills and is never a whole phase behind.
+//
+// Every output element sums its K terms in the cooperative kernel's order, so the two schedules
+// give bit-identical outputs (the fused statistics keep its per-warp partials as well; only the
+// order of their fp64 atomics may differ, as it may between two runs of either kernel).
+constexpr int kProducerRegs = 40;
+constexpr int kPingPongRegs = 232;  // 128 accumulators per thread at BLOCK_N = 128
+constexpr uint32_t kTurnBarrier = 1;  // named barriers 1, 2: consumer 0's, consumer 1's turn
+
+template <int BLOCK_N, int P>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
+  using Cfg = TcCfg<BLOCK_N, P>;
+  static_assert(P <= 2, "ping-pong: P = 3 stays cooperative");
+  extern __shared__ uint8_t smem_raw[];
+  const Ring<BLOCK_N, P> ring(smem_raw, p, 4);  // one arrive per warp of the reading warpgroup
+  uint8_t* smem = ring.smem;
+  uint64_t* full_bar = ring.full_bar;
+  uint64_t* empty_bar = ring.empty_bar;
+
+  const int wg = threadIdx.x >> 7;
+  const int warp = (threadIdx.x >> 5) & 3;
+  const int lane = threadIdx.x & 31;
+  __syncthreads();
+
+  if (wg == 0) {
+    ptx::setmaxnreg_dec<kProducerRegs>();
+    if (threadIdx.x == 0) ring.produce(p);
+    return;
+  }
+  ptx::setmaxnreg_inc<kPingPongRegs>();
+
+  const int cw = wg - 1;
+  const int nkb = p.num_k_blocks;
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
+  const int my_tiles = (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  float acc[2][BLOCK_N / 2];  // rows 0-63, rows 64-127
+  for (int t = cw; t < my_tiles; t += 2) {
+    int bat, m_tile, n0, kb0, kb1;
+    decode_work<BLOCK_N>(p, (int)blockIdx.x + t * (int)gridDim.x, bat, m_tile, n0, kb0, kb1);
+    if (t > 0) ptx::named_bar_sync(kTurnBarrier + cw, 256);
+    const long long pos = (long long)t * nkb;  // ring position of the tile's first k-block
+    int stage = (int)(pos % Cfg::kStages);
+    uint32_t phase = (uint32_t)(pos / Cfg::kStages) & 1u;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[h][i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < nkb; ++kb) {
+      ptx::mbar_wait(&full_bar[stage], phase, p.err, 104);
+      const uint32_t sa = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
+      const uint32_t sb = sa + P * Cfg::kABytes;
+      uint32_t accumulate = (kb > 0) ? 1u : 0u;
+      ptx::wgmma_fence();
+#pragma unroll
+      for (int i = 0; i < P; ++i) {
+#pragma unroll
+        for (int j = 0; j < P - i; ++j) {
+          const uint64_t adesc0 = ptx::make_smem_desc_sw128(sa + i * Cfg::kABytes);
+          const uint64_t adesc1 = ptx::make_smem_desc_sw128(sa + i * Cfg::kABytes + 64 * 128);
+          const uint64_t bdesc = ptx::make_smem_desc_sw128(sb + j * Cfg::kBBytes);
+#pragma unroll
+          for (int k = 0; k < kBlockK / kMmaK; ++k) {
+            wgmma_bf16<BLOCK_N>(acc[0], adesc0 + 2 * k, bdesc + 2 * k, accumulate);
+            wgmma_bf16<BLOCK_N>(acc[1], adesc1 + 2 * k, bdesc + 2 * k, accumulate);
+            accumulate = 1u;
+          }
+        }
+      }
+      ptx::wgmma_commit();
+      ptx::wgmma_wait<1>();
+      ptx::reg_fence(acc[0]);
+      ptx::reg_fence(acc[1]);
+      if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
+    }
+    // every MMA of this tile is issued: the other warpgroup's tile, if it has one, may start
+    if (t + 1 < my_tiles) ptx::named_bar_arrive(kTurnBarrier + (1 - cw), 256);
+    ptx::wgmma_wait<0>();
+    ptx::reg_fence(acc[0]);
+    ptx::reg_fence(acc[1]);
+    if (lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
+    // one copy of the epilogue code for both halves: it runs while the other warpgroup's mainloop
+    // executes from the same instruction cache
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      tile_epilogue<BLOCK_N>(p, acc[0], m_tile, 64 * h, n0, warp, lane, bat * p.out_batch_stride);
+      if (h == 0) {
+#pragma unroll
+        for (int i = 0; i < BLOCK_N / 2; ++i) acc[0][i] = acc[1][i];
+      }
+    }
   }
 }
 
@@ -571,13 +711,15 @@ void choose_conv_tile(int H, int W, int* tw, int* th) {
   }
 }
 
-template <int BLOCK_N, int P>
+template <int BLOCK_N, int P, bool PINGPONG = false>
 int launch(const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
   using Cfg = TcCfg<BLOCK_N, P>;
+  void (*kernel)(TcParams);
+  if constexpr (PINGPONG) kernel = gemm_tc_pingpong_kernel<BLOCK_N, P>;
+  else kernel = gemm_tc_kernel<BLOCK_N, P>;
   static PerDeviceOnce configured;
   if (configured.pending()) {
-    TAPIR_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BLOCK_N, P>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    TAPIR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     configured.mark();
   }
   const double kl = g.k_logical > 0 ? g.k_logical : g.K;
@@ -588,9 +730,32 @@ int launch(const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
   const int sms = num_sms();
   const int tiles = p.num_m_tiles * p.num_n_tiles * (p.split_k > 1 ? p.split_k : 1);  // work items
   const int grid = tiles < sms ? tiles : sms;
-  gemm_tc_kernel<BLOCK_N, P><<<grid, kThreads, Cfg::kSmemBytes, stream>>>(p);
+  kernel<<<grid, kThreads, Cfg::kSmemBytes, stream>>>(p);
   count_launch();
-  TAPIR_LAUNCH_CHECK("gemm_tc_kernel");
+  TAPIR_LAUNCH_CHECK(PINGPONG ? "gemm_tc_pingpong_kernel" : "gemm_tc_kernel");
+  return kOk;
+}
+
+// Ping-pong hides a tile's epilogue behind the other warpgroup's mainloop.  It needs at least two
+// tiles per CTA, and measured on H100 it loses to the cooperative kernel when CTAs get fewer than
+// four tiles of short (< 16 k-block) mainloops: mixer linear_in / linear_out, 2.9 tiles of 8-9
+// k-blocks, ran 10-22 % slower.  Split-K work items, P = 3 and batched GEMMs (only the P = 3 cost
+// volume is batched) stay cooperative.  TAPIR_B200_GEMM_SCHEDULE=coop|pingpong forces one schedule
+// wherever both are legal; it is read on every call and any other value is an error.
+int pick_pingpong(int tiles, int num_k_blocks, int P, int batch, bool* pingpong) {
+  *pingpong = false;
+  const char* force = getenv("TAPIR_B200_GEMM_SCHEDULE");
+  if (force != nullptr && strcmp(force, "coop") != 0 && strcmp(force, "pingpong") != 0) {
+    set_error("TAPIR_B200_GEMM_SCHEDULE=%s: expected coop or pingpong", force);
+    return kBadArgument;
+  }
+  if (P > 2 || batch > 1) return kOk;
+  if (force != nullptr) {
+    *pingpong = strcmp(force, "pingpong") == 0;
+    return kOk;
+  }
+  const int sms = num_sms();
+  *pingpong = tiles >= 2 * sms && (tiles >= 4 * sms || num_k_blocks >= 16);
   return kOk;
 }
 
@@ -816,6 +981,14 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
     }
   }
 
+  bool pingpong = false;
+  TAPIR_RETURN_IF(pick_pingpong(tiles, p.num_k_blocks, P, g.batch, &pingpong));
+  if (pingpong) {
+#define TAPIR_TC_PINGPONG(BN, PP) \
+    if (bn == BN && P == PP) return launch<BN, PP, true>(p, g, stream);
+    TAPIR_TC_PINGPONG(64, 1) TAPIR_TC_PINGPONG(64, 2) TAPIR_TC_PINGPONG(128, 1) TAPIR_TC_PINGPONG(128, 2)
+#undef TAPIR_TC_PINGPONG
+  }
 #define TAPIR_TC_CASE(BN, PP) \
   if (bn == BN && P == PP) return launch<BN, PP>(p, g, stream);
   TAPIR_TC_CASE(64, 1) TAPIR_TC_CASE(64, 2) TAPIR_TC_CASE(64, 3)

@@ -59,6 +59,28 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int* e
   }
 }
 
+// ----------------------------------------------------------------------------- named barriers
+// bar.sync waits until `count` threads (whole warps) have reached barrier `id`; bar.arrive counts
+// the calling warp towards it without waiting.  Id 0 is __syncthreads().
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// ----------------------------------------------------------------------------- registers
+// Moves registers between warpgroups of a running CTA: every warp of the warpgroup executes the
+// same instruction; .dec returns registers to the CTA's pool, .inc waits until the pool has them.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
 // ----------------------------------------------------------------------------- TMA
 __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
