@@ -100,6 +100,25 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[B
   const bool vec_o = p.out_f32 != nullptr && (p.ldo & 1) == 0 && (reinterpret_cast<uintptr_t>(p.out_f32) & 7) == 0;
   const bool vec_p = p.out_planes != nullptr && (p.ldp & 1) == 0 && (p.out_plane_stride & 1) == 0 &&
                      (reinterpret_cast<uintptr_t>(p.out_planes) & 3) == 0;
+  // the two rows' operands, addressed once (null where the GEMM has no such tensor)
+  const float* res_row[2];
+  float* out_row[2];
+  __nv_bfloat16* pl_row[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    res_row[h] = p.residual != nullptr ? p.residual + row[h] * (long long)p.ldr : nullptr;
+    out_row[h] = p.out_f32 != nullptr ? p.out_f32 + out_off + row[h] * (long long)p.ldo : nullptr;
+    pl_row[h] = p.out_planes != nullptr ? p.out_planes + row[h] * (long long)p.ldp : nullptr;
+  }
+  if (p.residual != nullptr) {
+    // both rows' residual segments into L1 up front: the loads below then do not each wait on L2
+    const int c = n0 + 32 * (lane & 3);
+    if ((lane & 3) < BLOCK_N / 32 && c < p.N) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (row_ok[h]) asm volatile("prefetch.global.L1 [%0];" ::"l"(res_row[h] + c));
+    }
+  }
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int c = n0 + 8 * j + 2 * (lane & 3);
@@ -116,9 +135,8 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[B
       if (!row_ok[h] || !ok0) continue;
       if (p.bias != nullptr) { v0 += b0; v1 += b1; }
       if (p.act == 1) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
-      const long long r = row[h];
       if (p.residual != nullptr) {
-        const float* rp = p.residual + r * (long long)p.ldr + c;
+        const float* rp = res_row[h] + c;
         if (ok1 && vec_r) {
           const float2 t = *reinterpret_cast<const float2*>(rp);
           v0 += t.x; v1 += t.y;
@@ -128,7 +146,7 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[B
         }
       }
       if (p.out_f32 != nullptr) {
-        float* o = p.out_f32 + out_off + r * (long long)p.ldo + c;
+        float* o = out_row[h] + c;
         if (ok1 && vec_o) {
           *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
         } else {
@@ -144,8 +162,10 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[B
       }
       if (p.out_planes != nullptr) {
         // successive bf16 terms of v: plane q holds bf16(v - sum_{s<q} plane s)
-        for (int q = 0; q < p.out_P; ++q) {
-          __nv_bfloat16* o = p.out_planes + q * p.out_plane_stride + r * (long long)p.ldp + c;
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+          if (q == p.out_P) break;
+          __nv_bfloat16* o = pl_row[h] + q * p.out_plane_stride + c;
           if (ok1 && vec_p) {
             *reinterpret_cast<uint32_t*>(o) = bf16x2_split(v0, v1);
           } else {
