@@ -3,7 +3,7 @@
 # and leaves logs + a JSON report in gpurun_out/.  Usage: gpurun -- bash scripts/gpu_ci.sh [tiers]
 cd "$(dirname "$0")/.." || exit 1
 mkdir -p gpurun_out
-TIERS=${*:-"gemm_simt gemm_tc stages_simt stages_tc head_simt e2e_simt e2e_tc"}
+TIERS=${*:-"gemm_simt gemm_tc stages_simt stages_tc e2e_simt e2e_tc"}
 nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm,memory.total --format=csv > gpurun_out/gpu_info.txt 2>&1
 rc=0
 run() {  # name, env, pytest args...
@@ -23,7 +23,6 @@ for t in $TIERS; do
     gemm_tc)     run gemm_tc "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_schedule_gpu.py -k tc ;;
     stages_simt) run stages_simt "TAPIR_B200_GEMM=simt" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py ;;
     stages_tc)   run stages_tc "X=1" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py ;;
-    head_simt)   run head_simt "TAPIR_B200_HEAD=simt" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py ;;
     e2e_simt)    run e2e_simt "TAPIR_B200_GEMM=simt" tests/test_end_to_end_gpu.py ;;
     e2e_tc)      run e2e_tc "X=1" tests/test_end_to_end_gpu.py ;;
     props)       run props "X=1" tests/test_properties_gpu.py tests/test_batched_gpu.py ;;

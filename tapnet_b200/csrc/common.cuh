@@ -91,11 +91,6 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
 
 // tanh-approximated GELU, F.gelu(x, approximate='tanh') (nets.py:59,102,160):
 //   0.5 x (1 + tanh(k (x + 0.044715 x^3))) == x * sigmoid(2 k (x + 0.044715 x^3))
@@ -161,21 +156,6 @@ __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16 (&out)[P]) {
     out[i] = __float2bfloat16_rn(r);
     r = r - __bfloat162float(out[i]);
   }
-}
-
-// Same split step with integer-ALU rounding only (round-to-nearest-even on the raw bits), which
-// keeps the conversion unit out of the dependency chain.  Bit-identical to cvt.rn for finite x.
-__device__ __forceinline__ uint32_t bf16x2_split_alu(float& a, float& b) {
-  uint32_t ua = __float_as_uint(a), ub = __float_as_uint(b);
-  ua = (ua + 0x7fffu + ((ua >> 16) & 1u)) & 0xffff0000u;
-  ub = (ub + 0x7fffu + ((ub >> 16) & 1u)) & 0xffff0000u;
-  a -= __uint_as_float(ua);
-  b -= __uint_as_float(ub);
-  return __byte_perm(ua, ub, 0x7632);  // low half = bf16(a), high half = bf16(b)
-}
-
-__device__ __forceinline__ uint32_t pack_bf16x2(__nv_bfloat16 a, __nv_bfloat16 b) {
-  return (uint32_t)__bfloat16_as_ushort(a) | ((uint32_t)__bfloat16_as_ushort(b) << 16);
 }
 
 #endif  // __CUDACC__

@@ -60,9 +60,6 @@ int tapvid_counts(const tapir_tapvid_args* a, cudaStream_t s);
 // ---- stage A (stage_a.cu) ---------------------------------------------------------------
 int sample_query_features(const float* grid, int T, int gh, int gw, int C, const float* query_tyx,
                           int N, int vT, int vH, int vW, float* out, cudaStream_t s);
-int cost_volume_head(const tapir_head_weights* w, const float* cost_volume, int N, int T,
-                     const float* query_tyx, float temperature, int init_h, int init_w,
-                     float* points, float* occ, float* expd, int* argmax, cudaStream_t s);
 // B clips: qfeat [B][N][C], grid [B][T][gh][gw][C], outputs indexed by flattened query b*N + n
 size_t cost_volume_workspace_bytes(int B, int N, int T, int gh, int gw, int C);
 int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid, int B,

@@ -3,13 +3,13 @@
 //
 // The cost volume itself is the split-bf16 wgmma GEMM (planes=3, i.e. fp32-equivalent,
 // because its arg-max must match the reference bit-exactly): cv[n][t*h*w + cell] with
-// M = queries, N = T*h*w cells, K = 256.  `cost_volume_head_kernel` then consumes one
-// 32x32 map per CTA entirely from shared memory: conv3x3 1->16 + ReLU, conv3x3 16->1,
-// temperature soft-max, arg-max, radius-5 soft arg-max, and the occlusion branch
-// (pad(0,2,0,2), conv3x3 stride 2 16->32 + ReLU, spatial mean, 32->16->2 MLP).
+// M = queries, N = T*h*w cells, K = 256.  A head kernel then turns every map into a track point:
+// conv3x3 1->16 + ReLU, conv3x3 16->1, temperature soft-max, arg-max, radius-5 soft arg-max, and
+// the occlusion branch (pad(0,2,0,2), conv3x3 stride 2 16->32 + ReLU, spatial mean, 32->16->2
+// MLP).  32x32 maps (initial_resolution 256 x 256) run `cost_volume_head_tc_kernel`, one map at a
+// time per persistent CTA from shared memory with the strided conv on the tensor cores; every
+// other map size runs `cost_volume_head_generic_kernel`.
 #include <cfloat>
-#include <cstdlib>
-#include <cstring>
 
 #include "kernels.cuh"
 
@@ -59,30 +59,22 @@ __global__ void __launch_bounds__(128) sample_query_kernel(const float* __restri
   }
 }
 
-// ------------------------------------------------------------------------ a6 head
-constexpr int kG = 32;            // cost-volume map side (initial_resolution 256 / stride 8)
-constexpr int kOccW = kG + 3;     // 35: index -1 .. 33 (1 left halo for hid2, 2 right for hid3)
-constexpr int kOccPlane = kOccW * kOccW;
-
-struct HeadSmem {
-  float cv[(kG + 2) * (kG + 2)];     // zero-padded cost map
-  float occ[16 * kOccPlane];         // ReLU(hid1) with halo, channel-major
-  float w3[16 * 9 * 32];             // hid3 weights as [ci][tap][co]
-  // hid1 / hid2 weights, 9 taps padded to 12 per channel: three broadcast LDS.128 per channel
-  __align__(16) float w1[16 * 12];
-  __align__(16) float w2[16 * 12];
-  float b1[16], b3[32];
-  float w4[16 * 32], b4[16], w5[2 * 16], b5[2];
-  float red_f[8 * 4];
-  int red_i[8];
-  float mean32[8][32];
-  float bcast[4];
-  int bcast_i;
+// ------------------------------------------------------------------------ a6 head, shared parts
+// Single-barrier block reductions over NW warps: each warp's result goes to the reduction's own
+// slot, then EVERY thread folds the NW partials itself in ascending warp order (broadcast loads
+// instead of two more barriers; the tensor-core head spent 21 % of its stall samples on
+// barriers).  A head gives each reduction of a map its own slot and writes a slot again only in
+// the next map, after at least one more __syncthreads, so that write comes after every read.
+template <int NW>
+struct RedSlot {
+  float f[NW * 3];
+  int i[NW];
 };
 
-__device__ __forceinline__ void block_reduce_max_first(float v, int idx, HeadSmem& sm, float* out_v,
-                                                       int* out_i) {
-  // maximum value; among equal values the LOWEST index (torch.argmax on CPU)
+// maximum value; among equal values the LOWEST index (torch.argmax on CPU)
+template <int NW>
+__device__ __forceinline__ void block_max_first(float v, int idx, RedSlot<NW>& s, float* out_v,
+                                                int* out_i) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     const float ov = __shfl_xor_sync(0xffffffffu, v, o);
@@ -90,215 +82,64 @@ __device__ __forceinline__ void block_reduce_max_first(float v, int idx, HeadSme
     if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
   }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) { s.f[warp] = v; s.i[warp] = idx; }
   __syncthreads();
-  if (lane == 0) { sm.red_f[warp] = v; sm.red_i[warp] = idx; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float bv = sm.red_f[0];
-    int bi = sm.red_i[0];
-    for (int k = 1; k < 8; ++k)
-      if (sm.red_f[k] > bv || (sm.red_f[k] == bv && sm.red_i[k] < bi)) { bv = sm.red_f[k]; bi = sm.red_i[k]; }
-    sm.bcast[0] = bv;
-    sm.bcast_i = bi;
+  float bv = s.f[0];
+  int bi = s.i[0];
+#pragma unroll
+  for (int k = 1; k < NW; ++k) {
+    const float kv = s.f[k];
+    const int ki = s.i[k];
+    if (kv > bv || (kv == bv && ki < bi)) { bv = kv; bi = ki; }
   }
-  __syncthreads();
-  *out_v = sm.bcast[0];
-  *out_i = sm.bcast_i;
+  *out_v = bv;
+  *out_i = bi;
 }
 
-__device__ __forceinline__ void block_reduce_sum3(float a, float b, float c, HeadSmem& sm, float* oa,
-                                                  float* ob, float* oc) {
+template <int NW>
+__device__ __forceinline__ void block_sum3(float a, float b, float c, RedSlot<NW>& s, float* oa,
+                                           float* ob, float* oc) {
   a = warp_sum(a); b = warp_sum(b); c = warp_sum(c);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) { s.f[warp * 3] = a; s.f[warp * 3 + 1] = b; s.f[warp * 3 + 2] = c; }
   __syncthreads();
-  if (lane == 0) { sm.red_f[warp * 4] = a; sm.red_f[warp * 4 + 1] = b; sm.red_f[warp * 4 + 2] = c; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float x = 0, y = 0, z = 0;
-    for (int k = 0; k < 8; ++k) { x += sm.red_f[k * 4]; y += sm.red_f[k * 4 + 1]; z += sm.red_f[k * 4 + 2]; }
-    sm.bcast[0] = x; sm.bcast[1] = y; sm.bcast[2] = z;
-  }
-  __syncthreads();
-  *oa = sm.bcast[0]; *ob = sm.bcast[1]; *oc = sm.bcast[2];
+  float x = 0, y = 0, z = 0;
+#pragma unroll
+  for (int k = 0; k < NW; ++k) { x += s.f[k * 3]; y += s.f[k * 3 + 1]; z += s.f[k * 3 + 2]; }
+  *oa = x; *ob = y; *oc = z;
 }
 
-__global__ void __launch_bounds__(256) cost_volume_head_kernel(
-    const tapir_head_weights w, const float* __restrict__ cost_volume, int T,
-    const float* __restrict__ query_tyx, float temperature, int init_h, int init_w,
-    float* __restrict__ points, float* __restrict__ occ_out, float* __restrict__ expd_out,
-    int* __restrict__ argmax_out) {
-  extern __shared__ __align__(16) uint8_t head_smem_raw[];
-  HeadSmem& sm = *reinterpret_cast<HeadSmem*>(head_smem_raw);
-  const int t = blockIdx.x, n = blockIdx.y;
-  const int tid = threadIdx.x;
-  const float* cv = cost_volume + ((long long)n * T + t) * (kG * kG);
-
-  // ---- stage weights and the zero-padded map
-  for (int i = tid; i < (kG + 2) * (kG + 2); i += 256) sm.cv[i] = 0.f;
-  for (int i = tid; i < 16 * kOccPlane; i += 256) sm.occ[i] = 0.f;
-  for (int i = tid; i < 16 * 9 * 32; i += 256) {
-    const int co = i & 31, tap = (i >> 5) % 9, ci = i / (32 * 9);
-    sm.w3[i] = w.hid3_w[(co * 16 + ci) * 9 + tap];
+// The rest of map (n, t) after the spatial mean of hid3, run by warp 0 alone with shuffles
+// (lane = channel of `mean`): hid4 32 -> 16 + ReLU, occ_out 16 -> 2, the soft arg-max (tx, ty) / tw
+// of a gh x gw map scaled to initial_resolution pixels, the query-frame passthrough and the
+// stores.  w4, b4, w5, b5 are the hid4 and occ_out weights.
+__device__ __forceinline__ void head_tail(float mean, const float* w4, const float* b4, const float* w5,
+                                          const float* b5, float tx, float ty, float tw, int am, int gh,
+                                          int gw, int n, int t, int T, const float* query_tyx, int init_h,
+                                          int init_w, float* points, float* occ_out, float* expd_out,
+                                          int* argmax_out) {
+  const int lane = threadIdx.x & 31;
+  float a = (lane < 16) ? b4[lane] : 0.f;  // hid4: 32 -> 16, ReLU
+#pragma unroll
+  for (int k = 0; k < 32; ++k) {
+    const float mk = __shfl_sync(0xffffffffu, mean, k);
+    if (lane < 16) a = fmaf(mk, w4[lane * 32 + k], a);
   }
-  if (tid < 192) {
-    const int co = tid / 12, k = tid - co * 12;
-    sm.w1[tid] = (k < 9) ? w.hid1_w[co * 9 + k] : 0.f;
-    sm.w2[tid] = (k < 9) ? w.hid2_w[co * 9 + k] : 0.f;
+  a = fmaxf(a, 0.f);
+  float o2 = (lane < 2) ? b5[lane] : 0.f;  // occ_out: 16 -> 2
+#pragma unroll
+  for (int k = 0; k < 16; ++k) {
+    const float hk = __shfl_sync(0xffffffffu, a, k);
+    if (lane < 2) o2 = fmaf(hk, w5[lane * 16 + k], o2);
   }
-  if (tid < 16) { sm.b1[tid] = w.hid1_b[tid]; sm.b4[tid] = w.hid4_b[tid]; }
-  if (tid < 32) { sm.b3[tid] = w.hid3_b[tid]; sm.w5[tid] = w.occ_w[tid]; }
-  if (tid < 2) sm.b5[tid] = w.occ_b[tid];
-  for (int i = tid; i < 512; i += 256) sm.w4[i] = w.hid4_w[i];
-  __syncthreads();
-  for (int i = tid; i < kG * kG; i += 256) sm.cv[((i >> 5) + 1) * (kG + 2) + (i & 31) + 1] = cv[i];
-  __syncthreads();
-
-  // ---- hid1: conv3x3 1->16 (padding 1) + ReLU.  Thread = row y, 4 consecutive x.
-  const int y = tid >> 3, x0 = (tid & 7) * 4;
-  {
-    float win[3][6];
-#pragma unroll
-    for (int r = 0; r < 3; ++r)
-#pragma unroll
-      for (int c = 0; c < 6; ++c) win[r][c] = sm.cv[(y + r) * (kG + 2) + x0 + c];
-    for (int co = 0; co < 16; ++co) {
-      float a[4] = {sm.b1[co], sm.b1[co], sm.b1[co], sm.b1[co]};
-#pragma unroll
-      for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-          const float wv = sm.w1[co * 12 + ky * 3 + kx];
-#pragma unroll
-          for (int p = 0; p < 4; ++p) a[p] = fmaf(win[ky][kx + p], wv, a[p]);
-        }
-#pragma unroll
-      for (int p = 0; p < 4; ++p) sm.occ[co * kOccPlane + (y + 1) * kOccW + (x0 + p + 1)] = fmaxf(a[p], 0.f);
-    }
-  }
-  __syncthreads();
-
-  // ---- hid2: conv3x3 16->1 (padding 1), x temperature
-  float heat[4];
-  {
-    const float b2 = w.hid2_b[0];
-    float a[4] = {b2, b2, b2, b2};
-    for (int ci = 0; ci < 16; ++ci) {
-      const float* op = sm.occ + ci * kOccPlane;
-#pragma unroll
-      for (int ky = 0; ky < 3; ++ky) {
-        float row[6];
-#pragma unroll
-        for (int c = 0; c < 6; ++c) row[c] = op[(y + ky) * kOccW + x0 + c];
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-          const float wv = sm.w2[ci * 12 + ky * 3 + kx];
-#pragma unroll
-          for (int p = 0; p < 4; ++p) a[p] = fmaf(row[kx + p], wv, a[p]);
-        }
-      }
-    }
-#pragma unroll
-    for (int p = 0; p < 4; ++p) heat[p] = a[p] * temperature;
-  }
-
-  // ---- softmax over the 1024 cells, argmax of the PROBABILITIES (first index on ties),
-  //      soft arg-max within radius 5 (utils.py:116-150)
-  float lmax = fmaxf(fmaxf(heat[0], heat[1]), fmaxf(heat[2], heat[3]));
-  int dummy;
-  float gmax;
-  block_reduce_max_first(lmax, 0, sm, &gmax, &dummy);
-  float e[4], lsum = 0.f;
-#pragma unroll
-  for (int p = 0; p < 4; ++p) { e[p] = expf(heat[p] - gmax); lsum += e[p]; }
-  float gsum, u1, u2;
-  block_reduce_sum3(lsum, 0.f, 0.f, sm, &gsum, &u1, &u2);
-  float prob[4];
-  float pbest = -1.f;
-  int ibest = 0;
-#pragma unroll
-  for (int p = 0; p < 4; ++p) {
-    prob[p] = e[p] / gsum;
-    if (prob[p] > pbest) { pbest = prob[p]; ibest = y * kG + x0 + p; }
-  }
-  float pm;
-  int am;
-  block_reduce_max_first(pbest, ibest, sm, &pm, &am);
-  const float cx = (float)(am & 31) + 0.5f, cy = (float)(am >> 5) + 0.5f;
-  float sx = 0.f, sy = 0.f, sw = 0.f;
-#pragma unroll
-  for (int p = 0; p < 4; ++p) {
-    const float px = (float)(x0 + p) + 0.5f, py = (float)y + 0.5f;
-    const float dx = px - cx, dy = py - cy;
-    if (dx * dx + dy * dy < 25.f) { sx += px * prob[p]; sy += py * prob[p]; sw += prob[p]; }
-  }
-  float tx, ty, tw;
-  block_reduce_sum3(sx, sy, sw, sm, &tx, &ty, &tw);
-
-  // ---- hid3: pad(0,2,0,2), conv3x3 stride 2 16->32 + ReLU; thread = one of 16x16 outputs
-  {
-    const int oy = tid >> 4, ox = tid & 15;
-    float acc[32];
-#pragma unroll
-    for (int c = 0; c < 32; ++c) acc[c] = sm.b3[c];
-    for (int ci = 0; ci < 16; ++ci) {
-      const float* op = sm.occ + ci * kOccPlane + (2 * oy + 1) * kOccW + (2 * ox + 1);
-#pragma unroll
-      for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-        for (int kx = 0; kx < 3; ++kx) {
-          const float v = op[ky * kOccW + kx];
-          const float4* wr = reinterpret_cast<const float4*>(sm.w3 + (ci * 9 + ky * 3 + kx) * 32);
-#pragma unroll
-          for (int g = 0; g < 8; ++g) {
-            const float4 w4 = wr[g];
-            acc[4 * g + 0] = fmaf(v, w4.x, acc[4 * g + 0]);
-            acc[4 * g + 1] = fmaf(v, w4.y, acc[4 * g + 1]);
-            acc[4 * g + 2] = fmaf(v, w4.z, acc[4 * g + 2]);
-            acc[4 * g + 3] = fmaf(v, w4.w, acc[4 * g + 3]);
-          }
-        }
-    }
-    // spatial mean over the 256 outputs: warp-level transpose-reduce, then across 8 warps
-    const int lane = tid & 31, warp = tid >> 5;
-#pragma unroll
-    for (int c = 0; c < 32; ++c) acc[c] = fmaxf(acc[c], 0.f);
-#pragma unroll
-    for (int s = 16; s >= 1; s >>= 1) {
-#pragma unroll
-      for (int j = 0; j < s; ++j) {
-        const bool up = (lane & s) != 0;
-        const float send = up ? acc[j] : acc[j + s];
-        const float keep = up ? acc[j + s] : acc[j];
-        acc[j] = keep + __shfl_xor_sync(0xffffffffu, send, s);
-      }
-    }
-    sm.mean32[warp][lane] = acc[0];  // lane l holds channel l summed over the warp
-  }
-  __syncthreads();
-  if (tid < 32) {
-    float m = 0.f;
-    for (int k = 0; k < 8; ++k) m += sm.mean32[k][tid];
-    sm.mean32[0][tid] = m * (1.0f / 256.0f);
-  }
-  __syncthreads();
-  if (tid < 16) {
-    float a = sm.b4[tid];
-    for (int k = 0; k < 32; ++k) a = fmaf(sm.mean32[0][k], sm.w4[tid * 32 + k], a);
-    sm.mean32[1][tid] = fmaxf(a, 0.f);
-  }
-  __syncthreads();
-  if (tid < 2) {
-    float a = sm.b5[tid];
-    for (int k = 0; k < 16; ++k) a = fmaf(sm.mean32[1][k], sm.w5[tid * 16 + k], a);
-    const long long o = (long long)n * T + t;
-    if (tid == 0) occ_out[o] = a; else expd_out[o] = a;
-  }
-  if (tid == 0) {
-    const long long o = (long long)n * T + t;
+  const long long o = (long long)n * T + t;
+  if (lane == 0) occ_out[o] = o2;
+  if (lane == 1) expd_out[o] = o2;
+  if (lane == 0) {
     const float den = fmaxf(tw, 1e-12f);
     // utils.py:165-169: cell units -> initial_resolution pixels (coords * out / in)
-    float px = __fdiv_rn(__fmul_rn(tx / den, (float)init_w), (float)kG);
-    float py = __fdiv_rn(__fmul_rn(ty / den, (float)init_h), (float)kG);
+    float px = __fdiv_rn(__fmul_rn(tx / den, (float)init_w), (float)gw);
+    float py = __fdiv_rn(__fmul_rn(ty / den, (float)init_h), (float)gh);
     if (query_tyx != nullptr) {
       // utils.py:171-191: on the query frame the track passes through the query point
       const float qf = rintf(query_tyx[n * 3 + 0]);
@@ -310,129 +151,41 @@ __global__ void __launch_bounds__(256) cost_volume_head_kernel(
   }
 }
 
-
-// ------------------------------------------------------------------------ a6 head, tensor-core hid3
-// Same arithmetic as cost_volume_head_kernel, re-organised so that the 16->32 stride-2 conv
-// (80 % of the head FLOPs) runs on the tensor cores as a split-bf16 implicit GEMM per map:
+// ------------------------------------------------------------------------ a6 head, 32 x 32 maps
+// One persistent CTA per SM walks the maps.  The 16->32 stride-2 conv (80 % of the head FLOPs)
+// runs on the tensor cores as a split-bf16 implicit GEMM per map:
 // M = 256 output pixels, N = 32 channels, K = 9 taps x 16 input channels (one m16n8k16 k-step per
 // tap), three MMAs per product (hi*hi + hi*lo + lo*hi), fp32 accumulation.  ReLU(hid1) is kept as
 // bf16 hi/lo planes in channel-last order (A fragments are plain 32-bit shared loads), and the
 // 16->1 conv is evaluated in exact fp32 from registers as nine per-tap channel dot products
 // (`stap`) that are then gathered - so the soft-argmax path never sees bf16.
+constexpr int kG = 32;            // cost-volume map side (initial_resolution 256 / stride 8)
+constexpr int kOccW = kG + 3;     // 35: index -1 .. 33 (1 left halo for hid2, 2 right for hid3)
+constexpr int kOccPlane = kOccW * kOccW;
 constexpr int kHT = 512;                       // threads per map
 constexpr int kPixW = 9;                       // 32-bit words per pixel: 16 bf16 + 1 pad (bank spread)
 constexpr int kPlaneWords = kOccPlane * kPixW; // 35 x 35 pixels
 constexpr int kTapW = (kG + 2) * (kG + 2);
 
-// W3S = 32-bit words per hid3 weight row.  With the pixel stride (9) every weight-fragment load
-// of phase D was 2-way bank conflicted (lane group g = 7 lands on the banks of g = 0: 49 M of the
-// 145 M shared wavefronts per launch, profiles/r01_ncu_summary.md); 12 makes {12 g + tq} distinct
-// mod 32.  Validated against the whole parity suite in round 2 (gpurun_out/head_w3s.log).
+// kW3Stride = 32-bit words per hid3 weight row.  With the pixel stride (9) every weight-fragment
+// load of phase D was 2-way bank conflicted (lane group g = 7 lands on the banks of g = 0: 49 M of
+// the 145 M shared wavefronts per launch); 12 makes {12 g + tq} distinct mod 32.
 constexpr int kW3Stride = 12;
-template <int W3S>
 struct HeadTcSmem {
   float cv[kTapW];
   float stap[9 * kTapW];
   uint32_t occ_hi[kPlaneWords], occ_lo[kPlaneWords];
-  uint32_t w3_hi[9 * 32 * W3S], w3_lo[9 * 32 * W3S];  // [tap][co][ci pairs]
+  uint32_t w3_hi[9 * 32 * kW3Stride], w3_lo[9 * 32 * kW3Stride];  // [tap][co][ci pairs]
   // hid1 / hid2 weights, 9 taps padded to 12 per channel: three broadcast LDS.128 per channel
   __align__(16) float w1[16 * 12];
   __align__(16) float w2[16 * 12];
   float b1[16], b3[32];
   float w4[16 * 32], b4[16], w5[2 * 16], b5[2];
-  float red_f[16 * 4];
-  int red_i[16];
   float mean32[16][32];
-  float bcast[4];
-  int bcast_i;
   // one slot per block reduction of a map (4 per map): a slot is rewritten only in the next map,
-  // at least one __syncthreads later, so every reduction needs a single barrier
-  float slot_f[4][16 * 3];
-  int slot_i[4][16];
+  // after the barrier before the tail and the barrier that publishes the next map
+  RedSlot<16> slot[4];
 };
-
-// Single-barrier block reductions (16 warps): warp results go to a private slot, then EVERY thread
-// folds the 16 partials itself in the same fixed order (16 broadcast LDS instead of two more
-// barriers; the head kernel spent 21 % of its stall samples on barriers).
-template <class SM>
-__device__ __forceinline__ void block_max_first_1s(float v, int idx, SM& sm, int slot, float* out_v,
-                                                   int* out_i) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, v, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-    if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
-  }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { sm.slot_f[slot][warp] = v; sm.slot_i[slot][warp] = idx; }
-  __syncthreads();
-  float bv = sm.slot_f[slot][0];
-  int bi = sm.slot_i[slot][0];
-#pragma unroll
-  for (int k = 1; k < 16; ++k) {
-    const float kv = sm.slot_f[slot][k];
-    const int ki = sm.slot_i[slot][k];
-    if (kv > bv || (kv == bv && ki < bi)) { bv = kv; bi = ki; }
-  }
-  *out_v = bv;
-  *out_i = bi;
-}
-
-template <class SM>
-__device__ __forceinline__ void block_sum3_1s(float a, float b, float c, SM& sm, int slot, float* oa,
-                                              float* ob, float* oc) {
-  a = warp_sum(a); b = warp_sum(b); c = warp_sum(c);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { sm.slot_f[slot][warp * 3] = a; sm.slot_f[slot][warp * 3 + 1] = b; sm.slot_f[slot][warp * 3 + 2] = c; }
-  __syncthreads();
-  float x = 0, y = 0, z = 0;
-#pragma unroll
-  for (int k = 0; k < 16; ++k) { x += sm.slot_f[slot][k * 3]; y += sm.slot_f[slot][k * 3 + 1]; z += sm.slot_f[slot][k * 3 + 2]; }
-  *oa = x; *ob = y; *oc = z;
-}
-
-template <class SM>
-__device__ __forceinline__ void block_max_first(float v, int idx, SM& sm, int nwarps, float* out_v,
-                                                int* out_i) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float ov = __shfl_xor_sync(0xffffffffu, v, o);
-    const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
-    if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
-  }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) { sm.red_f[warp] = v; sm.red_i[warp] = idx; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float bv = sm.red_f[0];
-    int bi = sm.red_i[0];
-    for (int k = 1; k < nwarps; ++k)
-      if (sm.red_f[k] > bv || (sm.red_f[k] == bv && sm.red_i[k] < bi)) { bv = sm.red_f[k]; bi = sm.red_i[k]; }
-    sm.bcast[0] = bv;
-    sm.bcast_i = bi;
-  }
-  __syncthreads();
-  *out_v = sm.bcast[0];
-  *out_i = sm.bcast_i;
-}
-
-template <class SM>
-__device__ __forceinline__ void block_sum3(float a, float b, float c, SM& sm, int nwarps, float* oa,
-                                           float* ob, float* oc) {
-  a = warp_sum(a); b = warp_sum(b); c = warp_sum(c);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) { sm.red_f[warp * 4] = a; sm.red_f[warp * 4 + 1] = b; sm.red_f[warp * 4 + 2] = c; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float x = 0, y = 0, z = 0;
-    for (int k = 0; k < nwarps; ++k) { x += sm.red_f[k * 4]; y += sm.red_f[k * 4 + 1]; z += sm.red_f[k * 4 + 2]; }
-    sm.bcast[0] = x; sm.bcast[1] = y; sm.bcast[2] = z;
-  }
-  __syncthreads();
-  *oa = sm.bcast[0]; *ob = sm.bcast[1]; *oc = sm.bcast[2];
-}
 
 __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
   asm volatile(
@@ -442,17 +195,15 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
 }
 
-static_assert(sizeof(HeadTcSmem<kW3Stride>) <= 227 * 1024,
-              "head kernel shared memory exceeds the 227 KB opt-in limit");
+static_assert(sizeof(HeadTcSmem) <= 227 * 1024, "head kernel shared memory exceeds the 227 KB opt-in limit");
 
-template <int W3S>
 __global__ void __launch_bounds__(kHT, 1) cost_volume_head_tc_kernel(
     const tapir_head_weights w, const float* __restrict__ cost_volume, int T, int num_maps,
     const float* __restrict__ query_tyx, float temperature, int init_h, int init_w,
     float* __restrict__ points, float* __restrict__ occ_out, float* __restrict__ expd_out,
     int* __restrict__ argmax_out) {
   extern __shared__ __align__(16) uint8_t head_tc_smem_raw[];
-  HeadTcSmem<W3S>& sm = *reinterpret_cast<HeadTcSmem<W3S>*>(head_tc_smem_raw);
+  HeadTcSmem& sm = *reinterpret_cast<HeadTcSmem*>(head_tc_smem_raw);
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
 
@@ -466,8 +217,8 @@ __global__ void __launch_bounds__(kHT, 1) cost_volume_head_tc_kernel(
     float v0 = w.hid3_w[(co * 16 + 2 * cp) * 9 + tap], v1 = w.hid3_w[(co * 16 + 2 * cp + 1) * 9 + tap];
     const uint32_t hi = bf16x2_split(v0, v1);
     const uint32_t lo = bf16x2_split(v0, v1);
-    sm.w3_hi[(tap * 32 + co) * W3S + cp] = hi;
-    sm.w3_lo[(tap * 32 + co) * W3S + cp] = lo;
+    sm.w3_hi[(tap * 32 + co) * kW3Stride + cp] = hi;
+    sm.w3_lo[(tap * 32 + co) * kW3Stride + cp] = lo;
   }
   if (tid < 192) {
     const int co = tid / 12, k = tid - co * 12;
@@ -579,12 +330,12 @@ __global__ void __launch_bounds__(kHT, 1) cost_volume_head_tc_kernel(
   }
   int dummy;
   float gmax;
-  block_max_first_1s(fmaxf(heat[0], heat[1]), 0, sm, 0, &gmax, &dummy);
+  block_max_first(fmaxf(heat[0], heat[1]), 0, sm.slot[0], &gmax, &dummy);
   float e[2];
   e[0] = expf(heat[0] - gmax);
   e[1] = expf(heat[1] - gmax);
   float gsum, u1, u2;
-  block_sum3_1s(e[0] + e[1], 0.f, 0.f, sm, 1, &gsum, &u1, &u2);
+  block_sum3(e[0] + e[1], 0.f, 0.f, sm.slot[1], &gsum, &u1, &u2);
   float prob[2];
   float pbest = -1.f;
   int ibest = 0;
@@ -595,7 +346,7 @@ __global__ void __launch_bounds__(kHT, 1) cost_volume_head_tc_kernel(
   }
   float pm;
   int am;
-  block_max_first_1s(pbest, ibest, sm, 2, &pm, &am);
+  block_max_first(pbest, ibest, sm.slot[2], &pm, &am);
   const float cx = (float)(am & 31) + 0.5f, cy = (float)(am >> 5) + 0.5f;
   float sx = 0.f, sy = 0.f, sw = 0.f;
 #pragma unroll
@@ -605,7 +356,7 @@ __global__ void __launch_bounds__(kHT, 1) cost_volume_head_tc_kernel(
     if (dx * dx + dy * dy < 25.f) { sx += px * prob[p]; sy += py * prob[p]; sw += prob[p]; }
   }
   float tx, ty, tw;
-  block_sum3_1s(sx, sy, sw, sm, 3, &tx, &ty, &tw);
+  block_sum3(sx, sy, sw, sm.slot[3], &tx, &ty, &tw);
 
   // ---- phase D: hid3 (pad(0,2,0,2), conv3x3 stride 2, 16->32) on the tensor cores.
   // warp = output row oy (16 output pixels = one m16 tile), 4 n8 tiles, one k16 step per tap.
@@ -628,7 +379,7 @@ __global__ void __launch_bounds__(kHT, 1) cost_volume_head_tc_kernel(
       al[2] = sm.occ_lo[pa + tq + 4]; al[3] = sm.occ_lo[pb + tq + 4];
 #pragma unroll
       for (int nt = 0; nt < 4; ++nt) {
-        const int wb = (tap * 32 + nt * 8 + g) * W3S + tq;
+        const int wb = (tap * 32 + nt * 8 + g) * kW3Stride + tq;
         uint32_t bh[2] = {sm.w3_hi[wb], sm.w3_hi[wb + 4]};
         uint32_t bl[2] = {sm.w3_lo[wb], sm.w3_lo[wb + 4]};
         mma_bf16_16816(acc[nt], al, bh);
@@ -659,35 +410,8 @@ __global__ void __launch_bounds__(kHT, 1) cost_volume_head_tc_kernel(
     float m = 0.f;
 #pragma unroll
     for (int k = 0; k < 16; ++k) m += sm.mean32[k][lane];
-    m *= (1.0f / 256.0f);                       // lane = channel
-    float a = (lane < 16) ? sm.b4[lane] : 0.f;  // hid4: 32 -> 16, ReLU
-#pragma unroll
-    for (int k = 0; k < 32; ++k) {
-      const float mk = __shfl_sync(0xffffffffu, m, k);
-      if (lane < 16) a = fmaf(mk, sm.w4[lane * 32 + k], a);
-    }
-    a = fmaxf(a, 0.f);
-    float o2 = (lane < 2) ? sm.b5[lane] : 0.f;  // occ_out: 16 -> 2
-#pragma unroll
-    for (int k = 0; k < 16; ++k) {
-      const float hk = __shfl_sync(0xffffffffu, a, k);
-      if (lane < 2) o2 = fmaf(hk, sm.w5[lane * 16 + k], o2);
-    }
-    const long long o = (long long)n * T + t;
-    if (lane == 0) occ_out[o] = o2;
-    if (lane == 1) expd_out[o] = o2;
-    if (lane == 0) {
-      const float den = fmaxf(tw, 1e-12f);
-      float px = __fdiv_rn(__fmul_rn(tx / den, (float)init_w), (float)kG);
-      float py = __fdiv_rn(__fmul_rn(ty / den, (float)init_h), (float)kG);
-      if (query_tyx != nullptr) {
-        const float qf = rintf(query_tyx[n * 3 + 0]);
-        if (qf == (float)t) { px = query_tyx[n * 3 + 2]; py = query_tyx[n * 3 + 1]; }
-      }
-      points[o * 2 + 0] = px;
-      points[o * 2 + 1] = py;
-      if (argmax_out != nullptr) argmax_out[o] = am;
-    }
+    head_tail(m * (1.0f / 256.0f), sm.w4, sm.b4, sm.w5, sm.b5, tx, ty, tw, am, kG, kG, n, t, T, query_tyx,
+              init_h, init_w, points, occ_out, expd_out, argmax_out);
   }
   }  // map loop
 }
@@ -695,66 +419,21 @@ __global__ void __launch_bounds__(kHT, 1) cost_volume_head_tc_kernel(
 
 // ------------------------------------------------------------------------ a6 head, any map size
 // initial_resolution != (256, 256) (constructor argument, tapir_model.py:86) gives a cost map that
-// is not 32 x 32.  Same arithmetic as the kernels above for a gh x gw map: one CTA per map,
+// is not 32 x 32.  The same head as the tensor-core kernel's for a gh x gw map: one CTA per map,
 // ReLU(hid1) and the heat map staged in a per-CTA slice of the caller's workspace (L2 resident).
 // A correctness path (every published checkpoint / demo uses 256 x 256), not a tuned one.
-struct GenericRed {
-  float f[8 * 4];
-  int i[8];
-  float mean32[8][32];
-  float out[4];
-  int out_i;
-};
-
-__device__ __forceinline__ void generic_max_first(float v, int idx, GenericRed& r, float* ov, int* oi) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float xv = __shfl_xor_sync(0xffffffffu, v, o);
-    const int xi = __shfl_xor_sync(0xffffffffu, idx, o);
-    if (xv > v || (xv == v && xi < idx)) { v = xv; idx = xi; }
-  }
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) { r.f[warp] = v; r.i[warp] = idx; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float bv = r.f[0];
-    int bi = r.i[0];
-    for (int k = 1; k < 8; ++k)
-      if (r.f[k] > bv || (r.f[k] == bv && r.i[k] < bi)) { bv = r.f[k]; bi = r.i[k]; }
-    r.out[0] = bv;
-    r.out_i = bi;
-  }
-  __syncthreads();
-  *ov = r.out[0];
-  *oi = r.out_i;
-}
-
-__device__ __forceinline__ void generic_sum3(float a, float b, float c, GenericRed& r, float* oa,
-                                             float* ob, float* oc) {
-  a = warp_sum(a); b = warp_sum(b); c = warp_sum(c);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  __syncthreads();
-  if (lane == 0) { r.f[warp * 4] = a; r.f[warp * 4 + 1] = b; r.f[warp * 4 + 2] = c; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    float x = 0, y = 0, z = 0;
-    for (int k = 0; k < 8; ++k) { x += r.f[k * 4]; y += r.f[k * 4 + 1]; z += r.f[k * 4 + 2]; }
-    r.out[0] = x; r.out[1] = y; r.out[2] = z;
-  }
-  __syncthreads();
-  *oa = r.out[0]; *ob = r.out[1]; *oc = r.out[2];
-}
-
 __global__ void __launch_bounds__(256) cost_volume_head_generic_kernel(
     const tapir_head_weights w, const float* __restrict__ cost_volume, int T, int num_maps, int gh,
     int gw, const float* __restrict__ query_tyx, float temperature, int init_h, int init_w,
     float* __restrict__ scratch, float* __restrict__ points, float* __restrict__ occ_out,
     float* __restrict__ expd_out, int* __restrict__ argmax_out) {
-  __shared__ GenericRed red;
-  __shared__ float w1s[16 * 9], b1s[16], w2s[16 * 9], w3s[32 * 16 * 9], b3s[32], w4s[16 * 32], b4s[16],
-      w5s[2 * 16], b5s[2];
+  __shared__ float w1s[16 * 9], b1s[16], w2s[16 * 9], w3s[32 * 16 * 9], b3s[32];
+  __shared__ float mean32[8][32];  // [warp][channel] sums of ReLU(hid3)
+  // one slot per block reduction of a map (4 per map): a slot is written again only in the next
+  // map, and the map loop starts with __syncthreads(), so that write comes after every read
+  __shared__ RedSlot<8> slot[4];
   const int tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
   const int pw = gw + 3, ph = gh + 3;  // index -1 .. size+1 (1 halo before, 2 after)
   const int plane = pw * ph;
   const int cells = gh * gw;
@@ -762,10 +441,8 @@ __global__ void __launch_bounds__(256) cost_volume_head_generic_kernel(
   float* heat = occ + 16 * plane;                                    // [gh][gw]
   for (int i = tid; i < 16 * 9; i += 256) { w1s[i] = w.hid1_w[i]; w2s[i] = w.hid2_w[i]; }
   for (int i = tid; i < 32 * 16 * 9; i += 256) w3s[i] = w.hid3_w[i];
-  for (int i = tid; i < 512; i += 256) w4s[i] = w.hid4_w[i];
-  if (tid < 16) { b1s[tid] = w.hid1_b[tid]; b4s[tid] = w.hid4_b[tid]; }
-  if (tid < 32) { b3s[tid] = w.hid3_b[tid]; w5s[tid] = w.occ_w[tid]; }
-  if (tid < 2) b5s[tid] = w.occ_b[tid];
+  if (tid < 16) b1s[tid] = w.hid1_b[tid];
+  if (tid < 32) b3s[tid] = w.hid3_b[tid];
   for (int i = tid; i < 16 * plane; i += 256) occ[i] = 0.f;  // halos stay zero for every map
   const float b2 = w.hid2_b[0];
   const int oh = (gh - 1) / 2 + 1, ow = (gw - 1) / 2 + 1;  // pad (0,2,0,2), 3x3, stride 2, no padding
@@ -809,11 +486,11 @@ __global__ void __launch_bounds__(256) cost_volume_head_generic_kernel(
     }
     int dummy;
     float gmax;
-    generic_max_first(lmax, 0, red, &gmax, &dummy);
+    block_max_first(lmax, 0, slot[0], &gmax, &dummy);
     float lsum = 0.f;
     for (int i = tid; i < cells; i += 256) lsum += expf(heat[i] - gmax);
     float gsum, u1, u2;
-    generic_sum3(lsum, 0.f, 0.f, red, &gsum, &u1, &u2);
+    block_sum3(lsum, 0.f, 0.f, slot[1], &gsum, &u1, &u2);
     float pbest = -1.f;
     int ibest = 0;
     for (int i = tid; i < cells; i += 256) {  // ascending i: the first maximum is kept
@@ -822,7 +499,7 @@ __global__ void __launch_bounds__(256) cost_volume_head_generic_kernel(
     }
     float pm;
     int am;
-    generic_max_first(pbest, ibest, red, &pm, &am);
+    block_max_first(pbest, ibest, slot[2], &pm, &am);
     const float cx = (float)(am % gw) + 0.5f, cy = (float)(am / gw) + 0.5f;
     float sx = 0.f, sy = 0.f, sw = 0.f;
     for (int i = tid; i < cells; i += 256) {
@@ -835,7 +512,7 @@ __global__ void __launch_bounds__(256) cost_volume_head_generic_kernel(
       }
     }
     float tx, ty, tw;
-    generic_sum3(sx, sy, sw, red, &tx, &ty, &tw);
+    block_sum3(sx, sy, sw, slot[3], &tx, &ty, &tw);
     // hid3: conv3x3 stride 2 16 -> 32 on the (0,2,0,2)-padded activation, ReLU, spatial mean
     float msum[32];
 #pragma unroll
@@ -857,45 +534,18 @@ __global__ void __launch_bounds__(256) cost_volume_head_generic_kernel(
 #pragma unroll
       for (int c = 0; c < 32; ++c) msum[c] += fmaxf(acc[c], 0.f);
     }
-    {
-      const int lane = tid & 31, warp = tid >> 5;
 #pragma unroll
-      for (int c = 0; c < 32; ++c) {
-        const float v = warp_sum(msum[c]);
-        if (lane == 0) red.mean32[warp][c] = v;
-      }
+    for (int c = 0; c < 32; ++c) {
+      const float v = warp_sum(msum[c]);
+      if (lane == 0) mean32[warp][c] = v;
     }
     __syncthreads();
-    if (tid < 32) {
+    // the MLP reads its 2.2 KB of weights through L1 rather than staging them in shared memory
+    if (warp == 0) {
       float m = 0.f;
-      for (int k = 0; k < 8; ++k) m += red.mean32[k][tid];
-      red.mean32[0][tid] = m / (float)(oh * ow);
-    }
-    __syncthreads();
-    if (tid < 16) {
-      float a = b4s[tid];
-      for (int k = 0; k < 32; ++k) a = fmaf(red.mean32[0][k], w4s[tid * 32 + k], a);
-      red.mean32[1][tid] = fmaxf(a, 0.f);
-    }
-    __syncthreads();
-    if (tid < 2) {
-      float a = b5s[tid];
-      for (int k = 0; k < 16; ++k) a = fmaf(red.mean32[1][k], w5s[tid * 16 + k], a);
-      const long long o = (long long)n * T + t;
-      if (tid == 0) occ_out[o] = a; else expd_out[o] = a;
-    }
-    if (tid == 0) {
-      const long long o = (long long)n * T + t;
-      const float den = fmaxf(tw, 1e-12f);
-      float px = __fdiv_rn(__fmul_rn(tx / den, (float)init_w), (float)gw);
-      float py = __fdiv_rn(__fmul_rn(ty / den, (float)init_h), (float)gh);
-      if (query_tyx != nullptr) {
-        const float qf = rintf(query_tyx[n * 3 + 0]);
-        if (qf == (float)t) { px = query_tyx[n * 3 + 2]; py = query_tyx[n * 3 + 1]; }
-      }
-      points[o * 2 + 0] = px;
-      points[o * 2 + 1] = py;
-      if (argmax_out != nullptr) argmax_out[o] = am;
+      for (int k = 0; k < 8; ++k) m += mean32[k][lane];
+      head_tail(m / (float)(oh * ow), w.hid4_w, w.hid4_b, w.occ_w, w.occ_b, tx, ty, tw, am, gh, gw, n, t, T,
+                query_tyx, init_h, init_w, points, occ_out, expd_out, argmax_out);
     }
   }
 }
@@ -910,41 +560,6 @@ int sample_query_features(const float* grid, int T, int gh, int gw, int C, const
   sample_query_kernel<<<N, 128, 0, s>>>(grid, T, gh, gw, C, query_tyx, vT, vH, vW, out);
   count_launch();
   TAPIR_LAUNCH_CHECK("sample_query_kernel");
-  return kOk;
-}
-
-int cost_volume_head(const tapir_head_weights* w, const float* cost_volume, int N, int T,
-                     const float* query_tyx, float temperature, int init_h, int init_w,
-                     float* points, float* occ, float* expd, int* argmax, cudaStream_t s) {
-  static int use_simt = -1;
-  static PerDeviceOnce configured;
-  if (use_simt < 0) {
-    const char* e = getenv("TAPIR_B200_HEAD");
-    use_simt = (e != nullptr && strcmp(e, "simt") == 0) ? 1 : 0;
-  }
-  if (configured.pending()) {
-    TAPIR_CUDA(cudaFuncSetAttribute(cost_volume_head_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)sizeof(HeadSmem)));
-    TAPIR_CUDA(cudaFuncSetAttribute(cost_volume_head_tc_kernel<kW3Stride>,
-                                    cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)sizeof(HeadTcSmem<kW3Stride>)));
-    configured.mark();
-  }
-  TAPIR_CHECK_ARG(N <= 65535, "cost_volume_head: at most 65535 queries per call (got %d)", N);
-  // SURVEY.md 8(d): head = 2,950,208 FLOP per (n,t); 4 KB map in, 16 B out
-  ProfileScope ps("cost_volume.head", s, 2950208.0 * N * T, (double)N * T * (4096 + 16));
-  dim3 grid(T, N);
-  if (use_simt) {
-    cost_volume_head_kernel<<<grid, 256, sizeof(HeadSmem), s>>>(*w, cost_volume, T, query_tyx, temperature,
-                                                               init_h, init_w, points, occ, expd, argmax);
-  } else {
-    const int maps = N * T;
-    const int ctas = maps < num_sms() ? maps : num_sms();
-    cost_volume_head_tc_kernel<kW3Stride><<<ctas, kHT, sizeof(HeadTcSmem<kW3Stride>), s>>>(
-        *w, cost_volume, T, maps, query_tyx, temperature, init_h, init_w, points, occ, expd, argmax);
-  }
-  count_launch();
-  TAPIR_LAUNCH_CHECK("cost_volume_head_kernel");
   return kOk;
 }
 
@@ -992,7 +607,8 @@ int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const fl
   TAPIR_CHECK_ARG(B > 0, "cost_volume_tracks: bad clip count B=%d", B);
   TAPIR_CHECK_ARG(N > 0 && T > 0 && C % 64 == 0, "cost_volume_tracks: bad shape N=%d T=%d C=%d", N, T, C);
   TAPIR_CHECK_ARG(gh >= 2 && gw >= 2, "cost_volume_tracks: map %dx%d too small", gh, gw);
-  // the 32 x 32 head launches a (T, queries) grid
+  // the documented per-call query limit for 32 x 32 maps (tapir_cost_volume_tracks_batched), the
+  // same as the mixer's that refines these tracks
   TAPIR_CHECK_ARG((gh != kG || gw != kG) || (long long)B * N <= 65535,
                   "cost_volume_tracks: at most 65535 queries per call (B*N=%lld)", (long long)B * N);
   Arena arena(ws, ws_bytes);
@@ -1023,19 +639,32 @@ int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const fl
   g.tag = "cost_volume.gemm";
   TAPIR_RETURN_IF(gemm(g, s));
   // the heads index maps and query_tyx by flattened query b*N + n
-  if (gh != kG || gw != kG) {
-    // any other initial_resolution (tapir_model.py:86): generic-size head
-    ProfileScope ps("cost_volume.head", s, 2950208.0 / 1024.0 * gh * gw * BN * T,
-                    (double)BN * T * (4.0 * gh * gw + 16));
-    cost_volume_head_generic_kernel<<<p.generic_ctas, 256, 0, s>>>(
-        *w, p.cv, T, BN * T, gh, gw, query_tyx, temperature, init_h, init_w, p.generic_scratch, points,
-        occ, expd, argmax);
+  const int maps = BN * T;
+  if (gh == kG && gw == kG) {
+    static PerDeviceOnce configured;
+    if (configured.pending()) {
+      TAPIR_CUDA(cudaFuncSetAttribute(cost_volume_head_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)sizeof(HeadTcSmem)));
+      configured.mark();
+    }
+    // SURVEY.md 8(d): head = 2,950,208 FLOP per (n,t); 4 KB map in, 16 B out
+    ProfileScope ps("cost_volume.head", s, 2950208.0 * BN * T, (double)BN * T * (4096 + 16));
+    const int ctas = maps < num_sms() ? maps : num_sms();
+    cost_volume_head_tc_kernel<<<ctas, kHT, sizeof(HeadTcSmem), s>>>(
+        *w, p.cv, T, maps, query_tyx, temperature, init_h, init_w, points, occ, expd, argmax);
     count_launch();
-    TAPIR_LAUNCH_CHECK("cost_volume_head_generic_kernel");
+    TAPIR_LAUNCH_CHECK("cost_volume_head_tc_kernel");
     return kOk;
   }
-  return cost_volume_head(w, p.cv, BN, T, query_tyx, temperature, init_h, init_w, points, occ, expd,
-                          argmax, s);
+  // any other initial_resolution (tapir_model.py:86): generic-size head
+  ProfileScope ps("cost_volume.head", s, 2950208.0 / 1024.0 * gh * gw * BN * T,
+                  (double)BN * T * (4.0 * gh * gw + 16));
+  cost_volume_head_generic_kernel<<<p.generic_ctas, 256, 0, s>>>(
+      *w, p.cv, T, maps, gh, gw, query_tyx, temperature, init_h, init_w, p.generic_scratch, points, occ,
+      expd, argmax);
+  count_launch();
+  TAPIR_LAUNCH_CHECK("cost_volume_head_generic_kernel");
+  return kOk;
 }
 
 }  // namespace tapir

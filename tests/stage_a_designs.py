@@ -11,7 +11,7 @@ whose heat map is exactly temperature * map, so that the designed geometry (ties
 radius-5 window) is the geometry the soft-argmax sees.
 
 tests/test_stage_a_cases.py checks on the CPU that each family can catch the bug it targets;
-tests/test_stage_a_gpu.py runs the families through the three heads.
+tests/test_stage_a_gpu.py runs the families through the two heads.
 """
 from typing import NamedTuple, Tuple
 
@@ -38,7 +38,7 @@ HEAD_PREFIX = 'torch_cost_volume_track_mods.'
 HEAD_KEYS = ('hid1', 'hid2', 'hid3', 'hid4', 'occ_out')
 
 # 32 x 32 heads and their pixel-to-thread mappings; every other map size runs the generic head
-HEADS_32 = ('tc', 'simt')
+HEADS_32 = ('tc',)
 GENERIC_SIZES = ((2, 2), (3, 5), (5, 3), (7, 64), (64, 7), (31, 32), (32, 31), (33, 33), (96, 128))
 
 
@@ -102,8 +102,6 @@ def owner(head, gh, gw, i):
   y, x = divmod(i, gw)
   if head == 'tc':        # 512 threads: 2 consecutive x per thread, 16 threads per row
     tid = y * 16 + x // 2
-  elif head == 'simt':    # 256 threads: 4 consecutive x per thread, 8 threads per row
-    tid = y * 8 + x // 4
   else:                   # generic: cell i belongs to thread i mod 256
     tid = i % 256
   return tid >> 5, tid & 31
@@ -152,7 +150,7 @@ def _pairs(gh, gw, head, bumps):
   start = (gh // 3) * gw + gw // 4
   order = list(range(start, cells)) + list(range(start))
   out = {}
-  # two bumps never share a thread of the 32 x 32 heads (2 or 4 consecutive x)
+  # two bumps never share a thread of the 32 x 32 head (2 consecutive x)
   levels = ('lane', 'warp') if bumps and head in HEADS_32 else ('thread', 'lane', 'warp')
   for level in levels:
     for a in order:

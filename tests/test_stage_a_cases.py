@@ -1,6 +1,6 @@
 """The designed stage-A cost maps can catch the bugs they target (CPU only, float64 reference).
 
-tests/test_stage_a_gpu.py runs these designs through the three track heads.  Here each family is
+tests/test_stage_a_gpu.py runs these designs through the two track heads.  Here each family is
 checked on its own: tie maps really tie, the radius plateau really moves the point when the
 d^2 == 25 cells are counted, the query times really separate rint from round-half-away, and the
 saturated maps really underflow exp in fp32."""
@@ -34,7 +34,7 @@ def test_tie_designs_tie_exactly_at_every_level(kind):
   """Every designed tie has two exactly equal maximal probabilities in float64, the lower index
   first.  Together the tie maps reach every tie level of every head's pixel-to-thread mapping:
   inside a thread, across lanes and across warps (the synthetic head needs two separated bumps,
-  which never share a thread of the 32 x 32 heads)."""
+  which never share a thread of the 32 x 32 head)."""
   sd64 = _sd64(kind)
   covered = set()
   for gh, gw in SIZES:
@@ -53,7 +53,7 @@ def test_tie_designs_tie_exactly_at_every_level(kind):
             covered.add((head, D.tie_level(head, gh, gw, a, b)))
   want = {(h, l) for h in D.HEADS_32 + ('generic',) for l in ('thread', 'lane', 'warp')}
   if kind == 'synth':
-    want -= {('tc', 'thread'), ('simt', 'thread')}
+    want -= {('tc', 'thread')}
   assert want <= covered, sorted(want - covered)
 
 

@@ -1,4 +1,4 @@
-"""Stage A against a float64 reference: the three track heads on designed cost maps, and
+"""Stage A against a float64 reference: the two track heads on designed cost maps, and
 query-feature sampling, through the C ABI.
 
 Designed maps (tests/stage_a_designs.py) reach the heads through tapir_cost_volume_tracks_batched:
@@ -15,13 +15,9 @@ does).  Per map:
     elsewhere wherever the arg-max agrees;
   * logits within 1e-4 (synthetic head) or 1e-4 * max(1, |ref|) (identity head, large logits).
 
-Output buffers carry NaN guards.  The SIMT head is chosen once per process (TAPIR_B200_HEAD=simt),
-so its cases run in one child interpreter and are compared here."""
+Output buffers carry NaN guards."""
 import ctypes
 import functools
-import os
-import subprocess
-import sys
 from typing import NamedTuple
 
 import numpy as np
@@ -36,7 +32,6 @@ from tapnet_b200 import _lib  # noqa: E402
 from tests import gpu_util as U  # noqa: E402
 from tests import stage_a_designs as D  # noqa: E402
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GUARD = 16   # elements of NaN fill before and after every output
 STRIDE = 8   # initial-resolution pixels per cost-map cell
 SAMPLE_TOL = 1e-5
@@ -69,7 +64,7 @@ def _cases_32():
         out.append(Case(B, N, 5, 32, 32, kind, temp, True))
   out.append(Case(1, 24, 5, 32, 32, 'synth', 20.0, False))
   out.append(Case(3, 8, 5, 32, 32, 'identity', 20.0, False))
-  # B * N = 65535: the largest query count the heads accept (the SIMT head's grid.y)
+  # B * N = 65535: the largest query count a call with 32 x 32 maps accepts
   out += [Case(1, 65535, 1, 32, 32, kind, 20.0, True) for kind in D.HEAD_KINDS]
   out += [Case(1, 40, 6, 32, 32, 'synth', temp, True, 'unit') for temp in (20.0, 1.0)]
   return out
@@ -201,30 +196,6 @@ def _run(case):
   return {name: body.view(shape[name]).cpu() for name, (_, body) in outs.items()}
 
 
-def run_simt_child(path):
-  """Entry point of the child interpreter that runs every 32 x 32 case with the SIMT head."""
-  assert os.environ.get('TAPIR_B200_HEAD') == 'simt'
-  torch.save({c.id: _run(c) for c in CASES_32}, path)
-
-
-_SIMT_CHILD = """
-import sys
-sys.path.insert(0, {root!r})
-from tests import test_stage_a_gpu as M
-M.run_simt_child(sys.argv[1])
-"""
-
-
-@pytest.fixture(scope='module')
-def simt_outputs(tmp_path_factory):
-  path = str(tmp_path_factory.mktemp('simt_head') / 'outputs.pt')
-  env = dict(os.environ, TAPIR_B200_HEAD='simt')
-  p = subprocess.run([sys.executable, '-c', _SIMT_CHILD.format(root=ROOT), path], capture_output=True,
-                     text=True, timeout=900, env=env)
-  assert p.returncode == 0, p.stderr[-3000:]
-  return torch.load(path)
-
-
 # ------------------------------------------------------------------------- comparison
 def _check(case, head, got):
   B, N, T, gh, gw = case.B, case.N, case.T, case.gh, case.gw
@@ -296,20 +267,10 @@ def _check(case, head, got):
       f'logits: occ {rel_occ.max().item():.3e}, expd {rel_exp.max().item():.3e}'
 
 
-def _head_in_process():
-  return 'simt' if os.environ.get('TAPIR_B200_HEAD') == 'simt' else 'tc'
-
-
 @pytest.mark.parametrize('case', CASES_32, ids=[c.id for c in CASES_32])
 def test_head_32x32_tc(case):
-  """The default head of 32 x 32 maps (the tensor-core head unless TAPIR_B200_HEAD=simt)."""
-  _check(case, _head_in_process(), _run(case))
-
-
-@pytest.mark.parametrize('case', CASES_32, ids=[c.id for c in CASES_32])
-def test_head_32x32_simt(case, simt_outputs):
-  """The all-SIMT head (TAPIR_B200_HEAD=simt), run in a child interpreter."""
-  _check(case, 'simt', simt_outputs[case.id])
+  """The tensor-core head: every 32 x 32 map."""
+  _check(case, 'tc', _run(case))
 
 
 @pytest.mark.parametrize('case', CASES_GENERIC, ids=[c.id for c in CASES_GENERIC])
