@@ -261,6 +261,50 @@ int tapir_ingest_frames(const uint8_t* src, int32_t frames, int32_t H, int32_t W
                         int32_t crop_x, int32_t crop_h, int32_t crop_w, float* dst, int32_t oH,
                         int32_t oW, void* stream);
 
+/* 8-bit YUV 4:2:0 frames as video decoders (NV12) and cameras (NV12 / I420) deliver them.
+ * Luma sample (r, c) of frame f is y[f * y_frame_stride + r * y_pitch + c]; chroma sample
+ * (r, c) is u[f * u_frame_stride + r * u_pitch + c * chroma_step] (v likewise), with chroma
+ * planes of ceil(H/2) x ceil(W/2) samples.  I420: chroma_step 1; NV12: chroma_step 2 and
+ * v = u + 1 (the interleaved UV plane).  Strides and pitches are in bytes.
+ *
+ * Conversion contract: pixel (r, c) of the full frame uses chroma sample (r >> 1, c >> 1)
+ * (nearest, no interpolation; a crop window keeps absolute coordinates).  With D = U - 128,
+ * E = V - 128 and C = Y - 16, k = 298 (limited range) or C = Y, k = 256 (full range):
+ *   R = (k*C + cr*E + 128) >> 8, G = (k*C - gu*D - gv*E + 128) >> 8, B = (k*C + bu*D + 128) >> 8
+ * (arithmetic shift, then clamped to [0, 255]), where (cr, gu, gv, bu) is
+ *   BT.601 limited (409, 100, 208, 516)   BT.709 limited (459, 55, 136, 541)
+ *   BT.601 full    (359,  88, 183, 454)   BT.709 full    (403, 48, 120, 475).
+ * Everything after that is the uint8 RGB path (x / 255 * 2 - 1, each operation rounded), so a
+ * YUV frame gives bit for bit the results of the uint8 RGB frame the conversion produces. */
+typedef struct tapir_yuv420_frames {
+  const uint8_t* y;
+  const uint8_t* u;
+  const uint8_t* v;
+  int64_t y_frame_stride, u_frame_stride, v_frame_stride;
+  int64_t y_pitch, u_pitch, v_pitch;
+  int32_t chroma_step;     /* 1 (I420) or 2 (NV12) */
+  int32_t H, W;            /* full frame (luma samples) */
+  int32_t y0, x0, h, w;    /* crop window inside the frame */
+  int32_t matrix;          /* 601 or 709 */
+  int32_t full_range;      /* 0: limited (16-235 luma), 1: full (0-255) */
+  int32_t reserved;
+} tapir_yuv420_frames;
+
+/* Crop window of `frames` frames -> uint8 RGB [frames][h][w][3] (dense). */
+int tapir_yuv420_to_rgb(const tapir_yuv420_frames* src, int32_t frames, uint8_t* dst, void* stream);
+
+/* tapir_ingest_frames for YUV 4:2:0: crop window -> RGB -> [-1,1] -> bilinear resize to
+ * [frames][oH][oW][3] float, one pass; each of the four taps is converted, then the uint8
+ * arithmetic runs unchanged. */
+int tapir_ingest_frames_yuv420(const tapir_yuv420_frames* src, int32_t frames, float* dst,
+                               int32_t oH, int32_t oW, void* stream);
+
+/* tapir_backbone_forward_ex on the crop window (h x w) of YUV 4:2:0 frames: the conversion and
+ * the normalisation run inside the stem conv's loads; same launches as the uint8 reader. */
+int tapir_backbone_forward_yuv420(const tapir_backbone_weights* w, const tapir_yuv420_frames* video,
+                                  int32_t frames, float* lowres, float* hires, void* workspace,
+                                  size_t workspace_bytes, void* hires_ready_event, void* stream);
+
 /* ---- SURVEY 8f row 2: output post-processing (the step after the path) ---------------- */
 /* pytorch_live_demo.py:57-59 / utils/model_utils.py:376-389:
  * visible[i] = (1 - sigmoid(occ[i])) * (1 - sigmoid(expd[i])) > 0.5 */

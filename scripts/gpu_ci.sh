@@ -27,6 +27,7 @@ for t in $TIERS; do
     e2e_tc)      run e2e_tc "X=1" tests/test_end_to_end_gpu.py ;;
     props)       run props "X=1" tests/test_properties_gpu.py tests/test_batched_gpu.py ;;
     io)          run io "X=1" tests/test_io_gpu.py ;;
+    yuv)         run yuv "X=1" tests/test_yuv_gpu.py ;;
     bulk)        run bulk "X=1" tests/test_bulk_gpu.py ;;
     no_halo)     run no_halo "TAPIR_B200_CONV_HALO=0" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_stages_gpu.py tests/test_end_to_end_gpu.py ;;
     no_splitk)   run no_splitk "TAPIR_B200_SPLITK=0" tests/test_gemm_variants_gpu.py tests/test_stages_gpu.py tests/test_properties_gpu.py tests/test_batched_gpu.py ;;

@@ -9,3 +9,11 @@ for tool in memcheck racecheck synccheck; do
       > gpurun_out/sanitizer_$tool.log 2>&1
   echo "sanitizer $tool rc=$? $(grep -E 'ERROR SUMMARY|RACECHECK SUMMARY' gpurun_out/sanitizer_$tool.log | tail -1)"
 done
+# then the YUV 4:2:0 readers (stem loader, ingest taps, conversion kernel) on pitched, cropped
+# frames; the sanitizer's findings and summary go to stdout
+for tool in memcheck racecheck; do
+  timeout 1800 compute-sanitizer --tool $tool --print-limit 20 \
+      python -m pytest -q -m gpu -p no:cacheprovider tests/test_yuv_gpu.py -k "not every_triple" \
+      2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+  echo "sanitizer yuv $tool rc=${PIPESTATUS[0]}"
+done

@@ -98,6 +98,15 @@ class TapvidArgs(Structure):
               ('counts', c_void_p)]
 
 
+class Yuv420Frames(Structure):
+  _fields_ = [('y', c_void_p), ('u', c_void_p), ('v', c_void_p),
+              ('y_frame_stride', c_int64), ('u_frame_stride', c_int64), ('v_frame_stride', c_int64),
+              ('y_pitch', c_int64), ('u_pitch', c_int64), ('v_pitch', c_int64),
+              ('chroma_step', c_int32), ('H', c_int32), ('W', c_int32),
+              ('y0', c_int32), ('x0', c_int32), ('h', c_int32), ('w', c_int32),
+              ('matrix', c_int32), ('full_range', c_int32), ('reserved', c_int32)]
+
+
 TAPVID_COUNTERS = 18
 
 # name -> (restype, argtypes); this table is also what tests/test_abi.py checks against
@@ -135,6 +144,12 @@ SIGNATURES = {
                                            c_void_p]),
     'tapir_ingest_frames': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32,
                                            c_int32, c_int32, c_void_p, c_int32, c_int32, c_void_p]),
+    'tapir_yuv420_to_rgb': (ctypes.c_int, [POINTER(Yuv420Frames), c_int32, c_void_p, c_void_p]),
+    'tapir_ingest_frames_yuv420': (ctypes.c_int, [POINTER(Yuv420Frames), c_int32, c_void_p,
+                                                  c_int32, c_int32, c_void_p]),
+    'tapir_backbone_forward_yuv420': (ctypes.c_int, [POINTER(BackboneWeights), POINTER(Yuv420Frames),
+                                                     c_int32, c_void_p, c_void_p, c_void_p,
+                                                     c_size_t, c_void_p, c_void_p]),
     'tapir_postprocess_occlusions': (ctypes.c_int, [c_void_p, c_void_p, c_int64, c_void_p,
                                                     c_void_p]),
     'tapir_tapvid_counts': (ctypes.c_int, [POINTER(TapvidArgs), c_void_p]),

@@ -142,6 +142,31 @@ int tapir_ingest_frames(const uint8_t* src, int32_t frames, int32_t H, int32_t W
   return ingest_frames(src, frames, H, W, crop_y, crop_x, crop_h, crop_w, dst, oH, oW, S(stream));
 }
 
+int tapir_yuv420_to_rgb(const tapir_yuv420_frames* src, int32_t frames, uint8_t* dst, void* stream) {
+  Range nvtx_range("tapir_yuv420_to_rgb");
+  Yuv420Reader r;
+  TAPIR_RETURN_IF(make_yuv420_reader(src, frames, "tapir_yuv420_to_rgb", &r));
+  return yuv420_to_rgb(r, frames, src->h, src->w, dst, S(stream));
+}
+
+int tapir_ingest_frames_yuv420(const tapir_yuv420_frames* src, int32_t frames, float* dst,
+                               int32_t oH, int32_t oW, void* stream) {
+  Range nvtx_range("tapir_ingest_frames_yuv420");
+  Yuv420Reader r;
+  TAPIR_RETURN_IF(make_yuv420_reader(src, frames, "tapir_ingest_frames_yuv420", &r));
+  return ingest_frames_yuv420(r, frames, src->h, src->w, dst, oH, oW, S(stream));
+}
+
+int tapir_backbone_forward_yuv420(const tapir_backbone_weights* w, const tapir_yuv420_frames* video,
+                                  int32_t frames, float* lowres, float* hires, void* workspace,
+                                  size_t workspace_bytes, void* hires_ready_event, void* stream) {
+  Range nvtx_range("tapir_backbone_forward_yuv420");
+  Yuv420Reader r;
+  TAPIR_RETURN_IF(make_yuv420_reader(video, frames, "tapir_backbone_forward_yuv420", &r));
+  return backbone_forward(w, nullptr, 0, frames, video->h, video->w, lowres, hires, workspace,
+                          workspace_bytes, S(stream), static_cast<cudaEvent_t>(hires_ready_event), &r);
+}
+
 int tapir_postprocess_occlusions(const float* occ, const float* expd, int64_t n, uint8_t* visible,
                                  void* stream) {
   Range nvtx_range("tapir_postprocess_occlusions");

@@ -45,23 +45,58 @@ __device__ __forceinline__ float stem_load(const uint8_t* p) {
   return __fsub_rn(__fmul_rn(__fdiv_rn((float)*p, 255.f), 2.f), 1.f);
 }
 
+// Patch loaders: value of channel c at pixel (y, x) of frame f of the H x W input.
 template <typename In>
-__global__ void __launch_bounds__(256, 1) stem_conv_kernel(const In* __restrict__ video,
+struct StemRgb {
+  static constexpr int kTableFloats = 0;
+  const In* __restrict__ video;
+  __device__ __forceinline__ void prepare(float*) const {}
+  __device__ __forceinline__ float operator()(const float*, int f, int H, int W, int y, int x,
+                                              int c) const {
+    const In v = __ldg(video + (((long long)f * H + y) * W + x) * 3 + c);
+    return stem_load(&v);
+  }
+};
+
+// YUV 4:2:0: the integer conversion gives the uint8 RGB byte, and a per-CTA table of the 256
+// stem_load values gives exactly the float the uint8 loader computes from that byte.
+struct StemYuv420 {
+  static constexpr int kTableFloats = 256;
+  Yuv420Reader src;
+  __device__ __forceinline__ void prepare(float* table) const {
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) {
+      const uint8_t b = (uint8_t)i;
+      table[i] = stem_load(&b);
+    }
+    __syncthreads();
+  }
+  __device__ __forceinline__ float operator()(const float* table, int f, int, int, int y, int x,
+                                              int c) const {
+    uint8_t rgb[3];
+    src.pixel(f, y, x, rgb);
+    return table[c == 0 ? rgb[0] : (c == 1 ? rgb[1] : rgb[2])];
+  }
+};
+
+template <typename Load>
+__global__ void __launch_bounds__(256, 1) stem_conv_kernel(const Load load,
                                                            const float* __restrict__ w, int H, int W,
                                                            float* __restrict__ out) {
   extern __shared__ float stem_smem[];
   float* ws = stem_smem;                    // [147][64]
   float* patch = stem_smem + 147 * 64;      // [37][69][3]
+  float* table = patch + kStemPatchY * kStemPatchX * 3;  // [Load::kTableFloats]
   const int OH = H / 2, OW = W / 2;
   const int f = blockIdx.z;
   const int oy0 = blockIdx.y * kStemTileY, ox0 = blockIdx.x * kStemTileX;
   for (int i = threadIdx.x; i < 147 * 64; i += 256) ws[i] = w[i];
+  load.prepare(table);
   const int iy0 = 2 * oy0 - 2, ix0 = 2 * ox0 - 2;
   for (int i = threadIdx.x; i < kStemPatchY * kStemPatchX * 3; i += 256) {
     const int c = i % 3, px = (i / 3) % kStemPatchX, py = i / (3 * kStemPatchX);
     const int y = iy0 + py, x = ix0 + px;
     float v = 0.f;
-    if (y >= 0 && y < H && x >= 0 && x < W) v = stem_load(video + (((long long)f * H + y) * W + x) * 3 + c);
+    if (y >= 0 && y < H && x >= 0 && x < W) v = load(table, f, H, W, y, x, c);
     patch[i] = v;
   }
   __syncthreads();
@@ -375,27 +410,39 @@ int split_planes(const float* src, long long ld_src, __nv_bfloat16* dst, long lo
   return kOk;
 }
 
-int stem_conv(const void* video, int video_u8, const float* w_packed, int frames, int H, int W,
-              float* out, cudaStream_t s) {
+template <typename Load>
+int launch_stem_conv(const Load& load, const float* w_packed, int frames, int H, int W, float* out,
+                     double input_bytes, cudaStream_t s) {
   TAPIR_CHECK_ARG(H % 2 == 0 && W % 2 == 0, "stem_conv: H, W must be even");
-  const int smem = (147 * 64 + kStemPatchY * kStemPatchX * 3) * (int)sizeof(float);
+  const int smem = (147 * 64 + kStemPatchY * kStemPatchX * 3 + Load::kTableFloats) * (int)sizeof(float);
   static PerDeviceOnce configured;
   if (configured.pending()) {
-    TAPIR_CUDA(cudaFuncSetAttribute(stem_conv_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    TAPIR_CUDA(cudaFuncSetAttribute(stem_conv_kernel<uint8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    TAPIR_CUDA(cudaFuncSetAttribute(stem_conv_kernel<Load>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     configured.mark();
   }
   ProfileScope ps("backbone.stem_conv", s, 2.0 * frames * (H / 2) * (W / 2) * 64 * 147,
-                  (double)frames * H * W * 3 * (video_u8 ? 1 : 4) +
-                      (double)frames * (H / 2) * (W / 2) * 64 * 4);
+                  input_bytes + (double)frames * (H / 2) * (W / 2) * 64 * 4);
   dim3 grid(ceil_div(W / 2, kStemTileX), ceil_div(H / 2, kStemTileY), frames);
-  if (video_u8)
-    stem_conv_kernel<uint8_t><<<grid, 256, smem, s>>>(static_cast<const uint8_t*>(video), w_packed, H, W, out);
-  else
-    stem_conv_kernel<float><<<grid, 256, smem, s>>>(static_cast<const float*>(video), w_packed, H, W, out);
+  stem_conv_kernel<Load><<<grid, 256, smem, s>>>(load, w_packed, H, W, out);
   count_launch();
   TAPIR_LAUNCH_CHECK("stem_conv_kernel");
   return kOk;
+}
+
+int stem_conv(const void* video, int video_u8, const float* w_packed, int frames, int H, int W,
+              float* out, cudaStream_t s) {
+  const double in_bytes = (double)frames * H * W * 3 * (video_u8 ? 1 : 4);
+  if (video_u8)
+    return launch_stem_conv(StemRgb<uint8_t>{static_cast<const uint8_t*>(video)}, w_packed, frames,
+                            H, W, out, in_bytes, s);
+  return launch_stem_conv(StemRgb<float>{static_cast<const float*>(video)}, w_packed, frames, H, W,
+                          out, in_bytes, s);
+}
+
+int stem_conv_yuv420(const Yuv420Reader& video, const float* w_packed, int frames, int H, int W,
+                     float* out, cudaStream_t s) {
+  return launch_stem_conv(StemYuv420{video}, w_packed, frames, H, W, out,
+                          (double)frames * H * W * 1.5, s);
 }
 
 int instnorm_stats(const float* x, int frames, long long hw, int C, double* sums, cudaStream_t s) {
@@ -562,9 +609,10 @@ int backbone_stem(const tapir_backbone_weights* w, const void* video_chunk, int 
 
 int backbone_forward(const tapir_backbone_weights* w, const void* video, int video_u8, int frames,
                      int H, int W, float* lowres, float* hires, void* ws, size_t ws_bytes,
-                     cudaStream_t s, cudaEvent_t hires_ready) {
-  // video == nullptr: the stem output of all `frames` frames is already in the workspace
-  // (tapir_backbone_stem, called per frame chunk while later chunks are still in flight on PCIe)
+                     cudaStream_t s, cudaEvent_t hires_ready, const Yuv420Reader* yuv) {
+  // video == nullptr and yuv == nullptr: the stem output of all `frames` frames is already in
+  // the workspace (tapir_backbone_stem, called per frame chunk while later chunks are still in
+  // flight on PCIe).  yuv != nullptr: the stem reads the H x W window of YUV 4:2:0 frames.
   TAPIR_CHECK_ARG(w != nullptr && lowres != nullptr && hires != nullptr, "backbone_forward: null pointer");
   TAPIR_CHECK_ARG(frames > 0 && H % 8 == 0 && W % 8 == 0 && H >= 16 && W >= 16,
                   "backbone_forward: image resolution must be a multiple of 8 (H=%d W=%d)", H, W);
@@ -580,7 +628,10 @@ int backbone_forward(const tapir_backbone_weights* w, const void* video, int vid
 
   int h = H / 2, wd = W / 2;
   float* x = bp.buf[0];
-  if (video != nullptr) TAPIR_RETURN_IF(stem_conv(video, video_u8, w->stem_w, frames, H, W, x, s));
+  if (yuv != nullptr)
+    TAPIR_RETURN_IF(stem_conv_yuv420(*yuv, w->stem_w, frames, H, W, x, s));
+  else if (video != nullptr)
+    TAPIR_RETURN_IF(stem_conv(video, video_u8, w->stem_w, frames, H, W, x, s));
   int xi = 0;  // index of the buffer holding x
   // InstanceNorm statistics are accumulated by the epilogue of the GEMM that produces the
   // tensor (fp64 atomics into bp.sums[.]); only the stem output needs the stand-alone pass.  The

@@ -46,13 +46,26 @@ __global__ void __launch_bounds__(256) preprocess_u8_kernel(const uint8_t* __res
   if (blockIdx.x == 0 && threadIdx.x < (n & 3)) dst[(n4 << 2) + threadIdx.x] = lut[src[(n4 << 2) + threadIdx.x]];
 }
 
+// uint8 RGB pixel (y, x) of the crop window at (cy, cx) of frame f of an H x W frame.
+struct RgbWindow {
+  const uint8_t* __restrict__ src;
+  int H, W, cy, cx;
+  __device__ __forceinline__ void pixel(long long f, int y, int x, uint8_t (&rgb)[3]) const {
+    const uint8_t* p = src + (f * H + cy) * (long long)W * 3 + (long long)cx * 3 + ((long long)y * W + x) * 3;
+    rgb[0] = p[0];
+    rgb[1] = p[1];
+    rgb[2] = p[2];
+  }
+};
+
 // crop + normalise + resize.  A CTA walks over runs of 256 consecutive output pixels: one thread
 // computes one pixel (3 channels) into shared memory, then the run's 768 floats leave as float4
 // rows (the direct 12-byte-strided stores would touch every sector three times).  The resize is
 // F.interpolate(mode='bilinear', align_corners=False) of the normalised crop, i.e. the same
-// arithmetic as bilinear_resize_kernel (backbone.cu) applied after normalise_u8.
-__global__ void __launch_bounds__(256) ingest_frames_kernel(const uint8_t* __restrict__ src, int H,
-                                                            int W, int cy, int cx, int ch, int cw,
+// arithmetic as bilinear_resize_kernel (backbone.cu) applied after normalise_u8.  Src gives the
+// uint8 RGB pixels of the ch x cw window (RgbWindow, or Yuv420Reader converting each tap).
+template <typename Src>
+__global__ void __launch_bounds__(256) ingest_frames_kernel(const Src src, int ch, int cw,
                                                             float* __restrict__ dst, int oH, int oW,
                                                             long long total, bool dst_aligned16) {
   __shared__ float lut[256];
@@ -77,10 +90,10 @@ __global__ void __launch_bounds__(256) ingest_frames_kernel(const uint8_t* __res
         oy = (int)(r % oH);
         f = r / oH;
       }
-      const uint8_t* b = src + (f * H + cy) * (long long)W * 3 + (long long)cx * 3;
       float* o = stage + threadIdx.x * 3;
       if (same) {
-        const uint8_t* p = b + ((long long)oy * W + ox) * 3;
+        uint8_t p[3];
+        src.pixel(f, oy, ox, p);
         o[0] = lut[p[0]];
         o[1] = lut[p[1]];
         o[2] = lut[p[2]];
@@ -93,10 +106,11 @@ __global__ void __launch_bounds__(256) ingest_frames_kernel(const uint8_t* __res
         const int y1 = y0 + ((y0 < ch - 1) ? 1 : 0), x1 = x0 + ((x0 < cw - 1) ? 1 : 0);
         const float ly = fy - y0, lx = fx - x0;
         const float hy = 1.f - ly, hx = 1.f - lx;
-        const uint8_t* p00 = b + ((long long)y0 * W + x0) * 3;
-        const uint8_t* p01 = b + ((long long)y0 * W + x1) * 3;
-        const uint8_t* p10 = b + ((long long)y1 * W + x0) * 3;
-        const uint8_t* p11 = b + ((long long)y1 * W + x1) * 3;
+        uint8_t p00[3], p01[3], p10[3], p11[3];
+        src.pixel(f, y0, x0, p00);
+        src.pixel(f, y0, x1, p01);
+        src.pixel(f, y1, x0, p10);
+        src.pixel(f, y1, x1, p11);
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
           const float v00 = lut[p00[c]], v01 = lut[p01[c]];
@@ -114,6 +128,23 @@ __global__ void __launch_bounds__(256) ingest_frames_kernel(const uint8_t* __res
       for (int e = threadIdx.x; e < (int)left * 3; e += 256) dst[i0 * 3 + e] = stage[e];
     }
     __syncthreads();
+  }
+}
+
+// YUV 4:2:0 crop window -> dense uint8 RGB [frames][h][w][3]; one thread per pixel.
+__global__ void __launch_bounds__(256) yuv420_to_rgb_kernel(const Yuv420Reader src, int h, int w,
+                                                            uint8_t* __restrict__ dst,
+                                                            long long total) {
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int x = (int)(i % w);
+    const long long r = i / w;
+    const int y = (int)(r % h);
+    uint8_t p[3];
+    src.pixel(r / h, y, x, p);
+    dst[i * 3 + 0] = p[0];
+    dst[i * 3 + 1] = p[1];
+    dst[i * 3 + 2] = p[2];
   }
 }
 
@@ -204,11 +235,34 @@ int ingest_frames(const uint8_t* src, int frames, int H, int W, int crop_y, int 
     preprocess_u8_kernel<<<grid_for(n / 4 / 4 + 1), 256, 0, s>>>(src, dst, n);
   } else {
     ingest_frames_kernel<<<grid_for(total), 256, 0, s>>>(
-        src, H, W, crop_y, crop_x, crop_h, crop_w, dst, oH, oW, total,
+        RgbWindow{src, H, W, crop_y, crop_x}, crop_h, crop_w, dst, oH, oW, total,
         (reinterpret_cast<uintptr_t>(dst) & 15) == 0);
   }
   count_launch();
   TAPIR_LAUNCH_CHECK("ingest_frames_kernel");
+  return kOk;
+}
+
+int ingest_frames_yuv420(const Yuv420Reader& src, int frames, int h, int w, float* dst, int oH,
+                         int oW, cudaStream_t s) {
+  TAPIR_CHECK_ARG(dst && frames > 0 && h > 0 && w > 0 && oH > 0 && oW > 0,
+                  "ingest_frames_yuv420: bad arguments");
+  const long long total = (long long)frames * oH * oW;
+  ProfileScope ps("ingest_frames_yuv420", s, 0.0, (double)frames * h * w * 1.5 + (double)total * 12);
+  ingest_frames_kernel<<<grid_for(total), 256, 0, s>>>(src, h, w, dst, oH, oW, total,
+                                                       (reinterpret_cast<uintptr_t>(dst) & 15) == 0);
+  count_launch();
+  TAPIR_LAUNCH_CHECK("ingest_frames_kernel");
+  return kOk;
+}
+
+int yuv420_to_rgb(const Yuv420Reader& src, int frames, int h, int w, uint8_t* dst, cudaStream_t s) {
+  TAPIR_CHECK_ARG(dst && frames > 0 && h > 0 && w > 0, "yuv420_to_rgb: bad arguments");
+  const long long total = (long long)frames * h * w;
+  ProfileScope ps("yuv420_to_rgb", s, 0.0, (double)total * 4.5);
+  yuv420_to_rgb_kernel<<<grid_for(total), 256, 0, s>>>(src, h, w, dst, total);
+  count_launch();
+  TAPIR_LAUNCH_CHECK("yuv420_to_rgb_kernel");
   return kOk;
 }
 

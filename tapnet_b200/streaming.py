@@ -12,6 +12,10 @@ updates in place; `update_query` mirrors `TAPIR.update_query_features` for re-ta
 With `num_streams=S` one tracker follows S camera streams (same frame size, same point count): a
 step runs the backbone over the S frames in one pass and one batched estimate_trajectories over
 the S clips of one frame each (the reference's batch axis), all in one captured graph.
+
+With `yuv420=True` the tracker takes `live.YUV420Frames` (NV12 / I420 camera or decoder frames):
+it keeps static Y / U / V buffers of the camera frame, a step copies the 1.5 B/px planes into them
+and replays the graph, and the crop window and colour matrix are fixed at construction.
 """
 from typing import Optional, Tuple
 
@@ -27,11 +31,20 @@ class OnlineTracker:
   dummy points if it tracks fewer)."""
 
   def __init__(self, model: 'tapir_model.TAPIR', height: int, width: int, num_points: int,
-               uint8_frames: bool = False, num_streams: int = 1):
+               uint8_frames: bool = False, num_streams: int = 1, yuv420: bool = False,
+               window: Optional[Tuple[int, int, int, int]] = None, matrix: str = 'bt601',
+               full_range: bool = False):
+    """height x width: the frame size.  With yuv420=True that is the camera frame and `window`
+    (y0, x0, h, w; e.g. `live.center_square_window(height, width)`) the crop that is tracked, in
+    whose pixels the tracks are; `matrix` / `full_range` describe the YUV frames."""
     if not model.use_casual_conv:
       raise ValueError('OnlineTracker needs a causal model: TAPIR(use_casual_conv=True)')
     if int(num_streams) < 1:
       raise ValueError(f'num_streams must be >= 1, got {num_streams}')
+    if yuv420 and uint8_frames:
+      raise ValueError('uint8_frames and yuv420 are exclusive')
+    if not yuv420 and window is not None:
+      raise ValueError('window is only supported with yuv420=True')
     self.model = model
     self.hw = (int(height), int(width))
     self.num_points = int(num_points)
@@ -42,8 +55,19 @@ class OnlineTracker:
     # uint8_frames: frames are raw [0, 255] camera frames (what pytorch_live_demo.py:139-141 holds
     # before preprocess_frames); the normalisation runs inside the stem conv's loads
     self._frame_dtype = torch.uint8 if uint8_frames else torch.float32
-    self._frame = torch.zeros(self.num_streams, 1, height, width, 3, dtype=self._frame_dtype,
-                              device=self.dev)
+    self._yuv = None
+    if yuv420:
+      H, W = self.hw
+      ch, cw = (H + 1) // 2, (W + 1) // 2
+      planes = [torch.zeros(self.num_streams, 1, *hw, dtype=torch.uint8, device=self.dev)
+                for hw in ((H, W), (ch, cw), (ch, cw))]
+      # the graph's input: static planes of the camera frame, fixed window and matrix
+      self._yuv = live.YUV420Frames(*planes, matrix=matrix, full_range=full_range, window=window)
+      self._frame = self._yuv
+      self.hw = tuple(self._yuv.window[2:])
+    else:
+      self._frame = torch.zeros(self.num_streams, 1, height, width, 3, dtype=self._frame_dtype,
+                                device=self.dev)
     self._graph: Optional[torch.cuda.CUDAGraph] = None
     self._graph_sig = None
     self._pinned = False
@@ -78,8 +102,11 @@ class OnlineTracker:
 
   def _as_frames(self, frames, num=None):
     """[num, 1, H, W, 3] on the device from [num, H, W, 3], [num, 1, H, W, 3] or, for one
-    frame, [H, W, 3]."""
+    frame, [H, W, 3].  YUV trackers: YUV420Frames [num, 1, ...] of the camera frame size, in the
+    tracker's window and matrix, returned as they are."""
     num = self.num_streams if num is None else num
+    if self._yuv is not None:
+      return self._check_yuv(frames, num)
     frames = frames.to(self.dev, self._frame_dtype, non_blocking=True)
     if frames.dim() == 3:
       frames = frames[None, None]
@@ -91,6 +118,24 @@ class OnlineTracker:
       raise ValueError(f'expected {num} frames (one per stream), got {frames.shape[0]}')
     if tuple(frames.shape[2:4]) != self.hw:
       raise ValueError(f'frame size {tuple(frames.shape[2:4])} != {self.hw}')
+    return frames
+
+  def _check_yuv(self, frames, num):
+    if not isinstance(frames, live.YUV420Frames):
+      raise ValueError('this tracker was built with yuv420=True: pass live.YUV420Frames')
+    ref = self._yuv
+    if frames.frame_size != ref.frame_size:
+      raise ValueError(f'frame size {frames.frame_size} != {ref.frame_size}')
+    if (frames.window, frames.matrix, frames.full_range) != (ref.window, ref.matrix,
+                                                             ref.full_range):
+      raise ValueError(f'frames have window {frames.window}, {frames.matrix}, full_range='
+                       f'{frames.full_range}; the tracker was built for {ref.window}, '
+                       f'{ref.matrix}, full_range={ref.full_range}')
+    if frames.device != self.dev:
+      raise ValueError(f'frames on {frames.device}, tracker on {self.dev}')
+    if tuple(frames.y.shape[:2]) != (num, 1):
+      raise ValueError(f'expected YUV420Frames of [{num}, 1] frames, got '
+                       f'{list(frames.y.shape[:2])}')
     return frames
 
   def _step_eager(self):
@@ -159,7 +204,12 @@ class OnlineTracker:
     outputs: copy them if they must outlive the next step."""
     if self.query_features is None:
       raise RuntimeError('call init(frame, query_points) first')
-    self._frame.copy_(self._as_frames(frames))
+    if self._yuv is not None:
+      src = self._as_frames(frames)
+      for dst, plane in zip((self._yuv.y, self._yuv.u, self._yuv.v), (src.y, src.u, src.v)):
+        dst.copy_(plane)
+    else:
+      self._frame.copy_(self._as_frames(frames))
     if self._graph is not None and self._graph_sig != self._model_sig():
       self._graph = None  # stale pointers: the model's buffers or weights changed since capture
     if self._graph is None:

@@ -20,6 +20,7 @@ import torch
 from torch import nn
 
 from tapnet_b200 import _lib
+from tapnet_b200 import live
 from tapnet_b200 import schema
 
 
@@ -398,7 +399,8 @@ class TAPIR(nn.Module):
       refinement_resolutions: Optional[List[Tuple[int, int]]] = None,
       hires_ready_events: Optional[list] = None,
   ) -> FeatureGrids:
-    """Reference tapir_model.py:293-392.  video: [B, T, H, W, 3] float in [-1, 1].
+    """Reference tapir_model.py:293-392.  video: [B, T, H, W, 3] float in [-1, 1] (or uint8
+    [0, 255], or a device-resident `live.YUV420Frames` clip whose crop window is the video).
 
     `hires_ready_events` (extension, used by tapnet_b200.distributed): a list that receives one
     (hires tensor, torch.cuda.Event) pair per distinct resolution; the event fires as soon as
@@ -422,8 +424,13 @@ class TAPIR(nn.Module):
     # preprocess_frames, pytorch_live_demo.py:30-41): normalised inside the stem conv's loads
     # (or inside the resize), so the 4x larger float video never exists.  Extension of the
     # reference surface; float video behaves exactly as before.
-    video_u8 = video.dtype == torch.uint8
-    video = video.contiguous() if video_u8 else video.to(torch.float32).contiguous()
+    # YUV 4:2:0 frames (extension): at the frame's own size the stem conv converts inside its
+    # loads; a resized pass converts each bilinear tap in the ingest kernel.  Bit for bit the
+    # results of the uint8 RGB frames the conversion produces.
+    yuv = isinstance(video, live.YUV420Frames)
+    video_u8 = not yuv and video.dtype == torch.uint8
+    if not yuv:
+      video = video.contiguous() if video_u8 else video.to(torch.float32).contiguous()
     n, f, vh, vw, _ = video.shape
     host_src = None
     if host_video:
@@ -452,7 +459,12 @@ class TAPIR(nn.Module):
             frames_src = video  # align_corners=False resize to the same size is the identity
           else:
             frames_src = torch.empty(n, f, h, w, 3, dtype=torch.float32, device=dev)
-            if video_u8:
+            if yuv:
+              desc = video.c_struct()
+              _lib.check(lib.tapir_ingest_frames_yuv420(ctypes.byref(desc), n * f,
+                                                        _ptr(frames_src), h, w, stream),
+                         'tapir_ingest_frames_yuv420')
+            elif video_u8:
               _lib.check(lib.tapir_ingest_frames(_ptr(video), n * f, vh, vw, 0, 0, vh, vw,
                                                  _ptr(frames_src), h, w, stream),
                          'tapir_ingest_frames')
@@ -467,7 +479,8 @@ class TAPIR(nn.Module):
         nf = n * f
         latent = torch.empty(n, f, h // 8, w // 8, self.lowres_dim, dtype=torch.float32, device=dev)
         hires = torch.empty(n, f, h // 4, w // 4, self.highres_dim, dtype=torch.float32, device=dev)
-        flat_src = frames_src.view(nf, h, w, 3)
+        src_yuv = frames_src is video and yuv
+        flat_src = None if src_yuv else frames_src.view(nf, h, w, 3)
         flat_lo = latent.view(nf, h // 8, w // 8, self.lowres_dim)
         flat_hi = hires.view(nf, h // 4, w // 4, self.highres_dim)
         # frames are independent in the backbone (InstanceNorm per frame, LayerNorm per
@@ -506,11 +519,19 @@ class TAPIR(nn.Module):
               _lib.check(lib.tapir_backbone_stem(
                   ctypes.byref(pk['backbone']), _ptr(flat_src[a:]), int(video_u8), c, h, w, a - s0,
                   b - a, _ptr(ws), ws.numel(), stream), 'tapir_backbone_stem')
+          ready = ctypes.c_void_p(ev.cuda_event) if (ev is not None and last) else None
+          if src_yuv:
+            desc = video.c_struct(s0)
+            _lib.check(lib.tapir_backbone_forward_yuv420(
+                ctypes.byref(pk['backbone']), ctypes.byref(desc), c, _ptr(flat_lo[s0:]),
+                _ptr(flat_hi[s0:]), _ptr(ws), ws.numel(), ready, stream),
+                       'tapir_backbone_forward_yuv420')
+            continue
           _lib.check(lib.tapir_backbone_forward_ex(
               ctypes.byref(pk['backbone']), None if streamed else _ptr(flat_src[s0:]),
               int(flat_src.dtype == torch.uint8),
               c, h, w, _ptr(flat_lo[s0:]), _ptr(flat_hi[s0:]), _ptr(ws), ws.numel(),
-              ctypes.c_void_p(ev.cuda_event) if (ev is not None and last) else None, stream),
+              ready, stream),
                      'tapir_backbone_forward')
         if streamed:
           host_src = None  # the whole clip is on the device now (later passes resize from it)
