@@ -220,6 +220,44 @@ int tapir_gemm_ex(const void* a_planes, int32_t lda, int64_t a_plane_stride, con
 /* utils.py:26-42 bilinear resize, align_corners=False, [frames][H][W][C] -> [frames][oH][oW][C] */
 int tapir_bilinear_resize(const float* src, int32_t frames, int32_t H, int32_t W, int32_t C,
                           float* dst, int32_t oH, int32_t oW, void* stream);
+
+/* The backbone's memory-bound building blocks, one kernel each (what tapir_backbone_forward runs
+ * around its GEMMs).  Every argument is checked before any CUDA call: a NULL pointer, an
+ * unsupported C, planes outside 1..3, frames above 65535 (where frames run on a grid dimension)
+ * or a pointer / plane stride misaligned for the kernel's vector accesses returns 1.  Planes are
+ * bf16 [planes][...] at `plane_stride` elements, each the fp32 residual of the ones before. */
+/* nets.py:395-402,420: F.pad(x, (2, 4, 2, 4)) then the 7x7 stride-2 conv 3 -> 64, no bias.
+ * video [frames][H][W][3] fp32 in [-1,1], or uint8 [0,255] when video_u8 != 0 (normalised as
+ * x / 255 * 2 - 1 in fp32, each operation rounded); H, W even; w_packed [7][7][3][64] is
+ * initial_conv.weight.permute(2, 3, 1, 0); out [frames][H/2][W/2][64]. */
+int tapir_stem_conv(const void* video, int32_t video_u8, const float* w_packed, int32_t frames,
+                    int32_t H, int32_t W, float* out, void* stream);
+/* InstanceNorm statistics of x [frames][hw][C], C in {64, 128, 256}: sums [frames][C][2] fp64
+ * (sum, sum of squares), zeroed by the call, then accumulated in fp64. */
+int tapir_instnorm_stats(const float* x, int32_t frames, int64_t hw, int32_t C, double* sums,
+                         void* stream);
+/* nets.py:280-286,315-316: relu(InstanceNorm(x) * w + b) (biased variance, eps 1e-5) from the
+ * sums of tapir_instnorm_stats, split into `planes` bf16 planes [frames][hw][C].  zero_next
+ * (nullable) receives 0.0 in its first frames * 2 * zero_channels doubles. */
+int tapir_instnorm_relu_split(const float* x, const double* sums, const float* w, const float* b,
+                              int32_t frames, int64_t hw, int32_t C, void* out_planes,
+                              int64_t plane_stride, int32_t planes, double* zero_next,
+                              int32_t zero_channels, void* stream);
+/* nets.py:258-267,320: the rows of a stride-2 conv over F.pad(x, (0, 2, 0, 2)).  in_planes
+ * [planes][frames][H][W][C] bf16 (H, W even, C % 8 == 0) -> out_planes
+ * [planes][frames][H/2][W/2][taps][C]; taps 9: tap (ky, kx) = ky * 3 + kx reads
+ * in[2y + ky][2x + kx] (zero outside), taps 1: in[2y][2x]. */
+int tapir_im2col_s2(const void* in_planes, int64_t in_plane_stride, int32_t frames, int32_t H,
+                    int32_t W, int32_t C, int32_t taps, void* out_planes, int64_t out_plane_stride,
+                    int32_t planes, void* stream);
+/* LayerNorm over the last dimension (eps 1e-5), C in {256, 512}: x [rows][C] -> y [rows][C]
+ * fp32 (nullable) and / or `planes` bf16 planes [rows][C] (planes_out nullable); b nullable
+ * (nets.py:37-39,56 with bias, :118-120,138-140 without). */
+int tapir_layernorm_split(const float* x, int64_t rows, int32_t C, const float* w, const float* b,
+                          float* y, void* planes_out, int64_t plane_stride, int32_t planes,
+                          void* stream);
+/* tapir_model.py:370-381: x / sqrt(max(sum x^2, 1e-12)) per row, C in {128, 256}. */
+int tapir_l2_normalize(const float* x, int64_t rows, int32_t C, float* out, void* stream);
 size_t tapir_backbone_workspace_bytes(int32_t frames, int32_t H, int32_t W, int32_t extra_convs,
                                       int32_t planes);
 /* video [frames][H][W][3] in [-1,1] -> lowres [frames][H/8][W/8][256], hires

@@ -17,3 +17,9 @@ for tool in memcheck racecheck; do
       2>&1 | grep -E '^=========|passed|failed' | tail -n 25
   echo "sanitizer yuv $tool rc=${PIPESTATUS[0]}"
 done
+# then the backbone's memory-bound kernels one at a time, with NaN guards around every output
+# (stem conv, instance norm, im2col, layer norm, L2 norm, resize)
+timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
+    python -m pytest -q -m gpu -p no:cacheprovider tests/test_backbone_ops_gpu.py -k "not backbone_vs and not frame_chunks" \
+    2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+echo "sanitizer backbone_ops memcheck rc=${PIPESTATUS[0]}"

@@ -129,6 +129,18 @@ SIGNATURES = {
                                      c_void_p, c_int32, c_int32, c_void_p, c_size_t, c_void_p]),
     'tapir_bilinear_resize': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p,
                                              c_int32, c_int32, c_void_p]),
+    'tapir_stem_conv': (ctypes.c_int, [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int32,
+                                       c_void_p, c_void_p]),
+    'tapir_instnorm_stats': (ctypes.c_int, [c_void_p, c_int32, c_int64, c_int32, c_void_p,
+                                            c_void_p]),
+    'tapir_instnorm_relu_split': (ctypes.c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int32,
+                                                 c_int64, c_int32, c_void_p, c_int64, c_int32,
+                                                 c_void_p, c_int32, c_void_p]),
+    'tapir_im2col_s2': (ctypes.c_int, [c_void_p, c_int64, c_int32, c_int32, c_int32, c_int32,
+                                       c_int32, c_void_p, c_int64, c_int32, c_void_p]),
+    'tapir_layernorm_split': (ctypes.c_int, [c_void_p, c_int64, c_int32, c_void_p, c_void_p,
+                                             c_void_p, c_void_p, c_int64, c_int32, c_void_p]),
+    'tapir_l2_normalize': (ctypes.c_int, [c_void_p, c_int64, c_int32, c_void_p, c_void_p]),
     'tapir_backbone_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32, c_int32, c_int32]),
     'tapir_backbone_forward': (ctypes.c_int, [POINTER(BackboneWeights), c_void_p, c_int32, c_int32,
                                               c_int32, c_void_p, c_void_p, c_void_p, c_size_t,

@@ -99,6 +99,106 @@ int tapir_bilinear_resize(const float* src, int32_t frames, int32_t H, int32_t W
   return bilinear_resize(src, frames, H, W, C, dst, oH, oW, S(stream));
 }
 
+// The backbone's HBM-bound building blocks.  The internal functions trust their callers
+// (backbone_forward, mixer_forward); these entry points check every argument first, so a bad one
+// returns kBadArgument before any CUDA call.
+namespace {
+constexpr int kMaxGridFrames = 65535;  // frames run on gridDim.y / gridDim.z
+
+bool aligned(const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) % bytes) == 0; }
+}  // namespace
+
+int tapir_stem_conv(const void* video, int32_t video_u8, const float* w_packed, int32_t frames,
+                    int32_t H, int32_t W, float* out, void* stream) {
+  Range nvtx_range("tapir_stem_conv");
+  TAPIR_CHECK_ARG(video && w_packed && out, "tapir_stem_conv: null pointer");
+  TAPIR_CHECK_ARG(frames > 0 && frames <= kMaxGridFrames, "tapir_stem_conv: frames=%d", frames);
+  TAPIR_CHECK_ARG(H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0,
+                  "tapir_stem_conv: H=%d W=%d must be positive and even", H, W);
+  TAPIR_CHECK_ARG(aligned(out, 16) && (video_u8 || aligned(video, 4)),
+                  "tapir_stem_conv: out must be 16-byte aligned, a float video 4-byte aligned");
+  return stem_conv(video, video_u8 ? 1 : 0, w_packed, frames, H, W, out, S(stream));
+}
+
+int tapir_instnorm_stats(const float* x, int32_t frames, int64_t hw, int32_t C, double* sums,
+                         void* stream) {
+  Range nvtx_range("tapir_instnorm_stats");
+  TAPIR_CHECK_ARG(x && sums, "tapir_instnorm_stats: null pointer");
+  TAPIR_CHECK_ARG(frames > 0 && frames <= kMaxGridFrames && hw > 0,
+                  "tapir_instnorm_stats: frames=%d hw=%lld", frames, (long long)hw);
+  TAPIR_CHECK_ARG(C == 64 || C == 128 || C == 256, "tapir_instnorm_stats: C=%d unsupported", C);
+  TAPIR_CHECK_ARG(aligned(x, 16) && aligned(sums, 8),
+                  "tapir_instnorm_stats: x must be 16-byte and sums 8-byte aligned");
+  return instnorm_stats(x, frames, hw, C, sums, S(stream));
+}
+
+int tapir_instnorm_relu_split(const float* x, const double* sums, const float* w, const float* b,
+                              int32_t frames, int64_t hw, int32_t C, void* out_planes,
+                              int64_t plane_stride, int32_t planes, double* zero_next,
+                              int32_t zero_channels, void* stream) {
+  Range nvtx_range("tapir_instnorm_relu_split");
+  TAPIR_CHECK_ARG(x && sums && w && b && out_planes, "tapir_instnorm_relu_split: null pointer");
+  TAPIR_CHECK_ARG(frames > 0 && frames <= kMaxGridFrames && hw > 0,
+                  "tapir_instnorm_relu_split: frames=%d hw=%lld", frames, (long long)hw);
+  TAPIR_CHECK_ARG(C == 64 || C == 128 || C == 256, "tapir_instnorm_relu_split: C=%d unsupported", C);
+  TAPIR_CHECK_ARG(planes >= 1 && planes <= 3, "tapir_instnorm_relu_split: planes=%d", planes);
+  TAPIR_CHECK_ARG(planes == 1 || plane_stride >= (long long)frames * hw * C,
+                  "tapir_instnorm_relu_split: planes overlap (plane_stride=%lld)", (long long)plane_stride);
+  TAPIR_CHECK_ARG(aligned(x, 16) && aligned(sums, 8) && aligned(out_planes, 8) && plane_stride % 4 == 0,
+                  "tapir_instnorm_relu_split: x must be 16-byte aligned, sums and out_planes 8-byte "
+                  "aligned, plane_stride a multiple of 4");
+  TAPIR_CHECK_ARG(zero_next == nullptr || (zero_channels > 0 && aligned(zero_next, 8)),
+                  "tapir_instnorm_relu_split: zero_next needs zero_channels > 0 and 8-byte alignment");
+  return instnorm_relu_split(x, sums, w, b, frames, hw, C, static_cast<__nv_bfloat16*>(out_planes),
+                             plane_stride, planes, zero_next, zero_channels, S(stream));
+}
+
+int tapir_im2col_s2(const void* in_planes, int64_t in_plane_stride, int32_t frames, int32_t H,
+                    int32_t W, int32_t C, int32_t taps, void* out_planes, int64_t out_plane_stride,
+                    int32_t planes, void* stream) {
+  Range nvtx_range("tapir_im2col_s2");
+  TAPIR_CHECK_ARG(in_planes && out_planes, "tapir_im2col_s2: null pointer");
+  TAPIR_CHECK_ARG(frames > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0,
+                  "tapir_im2col_s2: frames=%d H=%d W=%d (H, W positive and even)", frames, H, W);
+  TAPIR_CHECK_ARG(C > 0 && C % 8 == 0, "tapir_im2col_s2: C=%d must be a positive multiple of 8", C);
+  TAPIR_CHECK_ARG(taps == 1 || taps == 9, "tapir_im2col_s2: taps=%d must be 1 or 9", taps);
+  TAPIR_CHECK_ARG(planes >= 1 && planes <= 3, "tapir_im2col_s2: planes=%d", planes);
+  TAPIR_CHECK_ARG(aligned(in_planes, 16) && aligned(out_planes, 16) && in_plane_stride % 8 == 0 &&
+                      out_plane_stride % 8 == 0,
+                  "tapir_im2col_s2: planes must be 16-byte aligned, plane strides multiples of 8");
+  return im2col_s2(static_cast<const __nv_bfloat16*>(in_planes), in_plane_stride, frames, H, W, C, taps,
+                   static_cast<__nv_bfloat16*>(out_planes), out_plane_stride, planes, S(stream));
+}
+
+int tapir_layernorm_split(const float* x, int64_t rows, int32_t C, const float* w, const float* b,
+                          float* y, void* planes_out, int64_t plane_stride, int32_t planes,
+                          void* stream) {
+  Range nvtx_range("tapir_layernorm_split");
+  TAPIR_CHECK_ARG(x && w, "tapir_layernorm_split: null pointer");
+  TAPIR_CHECK_ARG(y || planes_out, "tapir_layernorm_split: y and planes_out are both NULL");
+  TAPIR_CHECK_ARG(rows > 0 && rows < (1ll << 34), "tapir_layernorm_split: rows=%lld", (long long)rows);
+  TAPIR_CHECK_ARG(C == 256 || C == 512, "tapir_layernorm_split: C=%d unsupported", C);
+  TAPIR_CHECK_ARG(planes_out == nullptr || (planes >= 1 && planes <= 3),
+                  "tapir_layernorm_split: planes=%d", planes);
+  TAPIR_CHECK_ARG(planes_out == nullptr || planes == 1 || plane_stride >= rows * C,
+                  "tapir_layernorm_split: planes overlap (plane_stride=%lld)", (long long)plane_stride);
+  TAPIR_CHECK_ARG(aligned(x, 16) && aligned(w, 16) && aligned(b, 16) && aligned(y, 16) &&
+                      aligned(planes_out, 8) && plane_stride % 4 == 0,
+                  "tapir_layernorm_split: x, w, b, y must be 16-byte aligned, planes_out 8-byte "
+                  "aligned, plane_stride a multiple of 4");
+  return layernorm_split(x, rows, C, w, b, y, static_cast<__nv_bfloat16*>(planes_out), plane_stride,
+                         planes_out ? planes : 0, S(stream));
+}
+
+int tapir_l2_normalize(const float* x, int64_t rows, int32_t C, float* out, void* stream) {
+  Range nvtx_range("tapir_l2_normalize");
+  TAPIR_CHECK_ARG(x && out, "tapir_l2_normalize: null pointer");
+  TAPIR_CHECK_ARG(rows > 0 && rows < (1ll << 34), "tapir_l2_normalize: rows=%lld", (long long)rows);
+  TAPIR_CHECK_ARG(C == 128 || C == 256, "tapir_l2_normalize: C=%d unsupported", C);
+  TAPIR_CHECK_ARG(aligned(x, 16) && aligned(out, 16), "tapir_l2_normalize: x and out must be 16-byte aligned");
+  return l2_normalize(x, rows, C, out, S(stream));
+}
+
 size_t tapir_backbone_workspace_bytes(int32_t frames, int32_t H, int32_t W, int32_t extra_convs,
                                       int32_t planes) {
   return backbone_workspace_bytes(frames, H, W, extra_convs, planes);
