@@ -414,6 +414,18 @@ int tapir_local_corr_batched(const tapir_corr_args* args, int32_t batch, void* s
 size_t tapir_mixer_workspace_bytes(int64_t rows, int32_t planes);
 int tapir_mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* workspace,
                         size_t workspace_bytes, void* stream);
+/* The depthwise half of one mixer block, the kernel tapir_mixer_forward runs between its GEMMs
+ * (nets.py:143-181 up to the channel MLP): x [n][T][512] fp32 -> z = x + group sum of the two
+ * depthwise convs [n][T][512] fp32, and LayerNorm_1(z) * ln1_w as `planes` bf16 planes
+ * [planes][n*T][512] at `plane_stride` elements.  causal != 0: causal convs, with the optional
+ * context of tapir_mixer_io (ctx1 [n][2][512], ctx2 [n][2][2048]; NULL = zero context / not
+ * requested); a non-causal call takes no context pointers.  A context output may be its input
+ * buffer only at T = 1.  Every argument is checked before any CUDA call (NULLs, n in 1..65535,
+ * T >= 1, planes 1..3, overlapping planes, 16-byte alignment of x, z, the contexts and the
+ * LayerNorm weights): a bad one returns 1. */
+int tapir_mixer_dw(const tapir_mixer_block* blk, const float* x, int32_t n, int32_t T, int32_t causal,
+                   const float* ctx1_in, const float* ctx2_in, float* ctx1_out, float* ctx2_out, float* z,
+                   void* planes_out, int64_t plane_stride, int32_t planes, void* stream);
 int tapir_refine_update(const tapir_update_args* args, void* stream);
 
 #ifdef __cplusplus

@@ -21,8 +21,8 @@ for t in $TIERS; do
   case $t in
     gemm_simt)   run gemm_simt "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py -k simt ;;
     gemm_tc)     run gemm_tc "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_schedule_gpu.py -k tc ;;
-    stages_simt) run stages_simt "TAPIR_B200_GEMM=simt" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py tests/test_backbone_ops_gpu.py ;;
-    stages_tc)   run stages_tc "X=1" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py tests/test_backbone_ops_gpu.py ;;
+    stages_simt) run stages_simt "TAPIR_B200_GEMM=simt" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py tests/test_backbone_ops_gpu.py tests/test_refine_ops_gpu.py ;;
+    stages_tc)   run stages_tc "X=1" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py tests/test_backbone_ops_gpu.py tests/test_refine_ops_gpu.py ;;
     e2e_simt)    run e2e_simt "TAPIR_B200_GEMM=simt" tests/test_end_to_end_gpu.py ;;
     e2e_tc)      run e2e_tc "X=1" tests/test_end_to_end_gpu.py ;;
     props)       run props "X=1" tests/test_properties_gpu.py tests/test_batched_gpu.py ;;

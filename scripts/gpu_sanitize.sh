@@ -23,3 +23,10 @@ timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
     python -m pytest -q -m gpu -p no:cacheprovider tests/test_backbone_ops_gpu.py -k "not backbone_vs and not frame_chunks" \
     2>&1 | grep -E '^=========|passed|failed' | tail -n 25
 echo "sanitizer backbone_ops memcheck rc=${PIPESTATUS[0]}"
+# then the refinement kernels one at a time (local correlation, pooling, track update, the mixer's
+# depthwise block), leaving out the production-shape cases
+timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
+    python -m pytest -q -m gpu -p no:cacheprovider tests/test_refine_ops_gpu.py \
+    -k "not production_shape and not streaming_shape and not clip_shape and not pl1_1024 and not n1001 and not n801 and not n700" \
+    2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+echo "sanitizer refine_ops memcheck rc=${PIPESTATUS[0]}"

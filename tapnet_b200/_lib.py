@@ -187,6 +187,9 @@ SIGNATURES = {
     'tapir_mixer_workspace_bytes': (c_size_t, [c_int64, c_int32]),
     'tapir_mixer_forward': (ctypes.c_int, [POINTER(MixerWeights), POINTER(MixerIO), c_void_p,
                                            c_size_t, c_void_p]),
+    'tapir_mixer_dw': (ctypes.c_int, [POINTER(MixerBlock), c_void_p, c_int32, c_int32, c_int32, c_void_p,
+                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32,
+                                      c_void_p]),
     'tapir_refine_update': (ctypes.c_int, [POINTER(UpdateArgs), c_void_p]),
 }
 

@@ -321,16 +321,50 @@ int tapir_cost_volume_tracks_batched(const tapir_head_weights* w, const float* q
 int tapir_pool_pyramid(const float* grid, int32_t T, int32_t h, int32_t w, int32_t C, float* out,
                        void* stream) {
   Range nvtx_range("tapir_pool_pyramid");
+  TAPIR_CHECK_ARG(grid && out, "tapir_pool_pyramid: null pointer");
+  TAPIR_CHECK_ARG(T > 0 && h >= 2 && w >= 2 && C > 0 && C % 4 == 0,
+                  "tapir_pool_pyramid: T=%d h=%d w=%d C=%d (h, w >= 2, C a positive multiple of 4)", T, h, w, C);
+  TAPIR_CHECK_ARG(aligned(grid, 16) && aligned(out, 16), "tapir_pool_pyramid: grid and out must be 16-byte aligned");
   return pool_pyramid(grid, T, h, w, C, out, S(stream));
 }
 
+// The correlation kernel reads the level grids and the query features as float4 and writes the
+// output planes as bf16 pairs.
+namespace {
+int check_corr_args(const tapir_corr_args* a, int batch, const char* fn) {
+  TAPIR_CHECK_ARG(a != nullptr && a->num_levels >= 1 && a->num_levels <= TAPIR_MAX_CORR_LEVELS,
+                  "%s: bad level count", fn);
+  TAPIR_CHECK_ARG(batch >= 1, "%s: bad clip count %d", fn, batch);
+  TAPIR_CHECK_ARG(a->pos && a->occ && a->expd && a->feat_hi && a->feat_lo && a->out_planes, "%s: null pointer", fn);
+  TAPIR_CHECK_ARG(a->init_h >= 1 && a->init_w >= 1, "%s: init_h=%d init_w=%d", fn, a->init_h, a->init_w);
+  for (int l = 0; l < a->num_levels; ++l) {
+    const tapir_corr_level& L = a->levels[l];
+    TAPIR_CHECK_ARG(L.h >= 1 && L.w >= 1, "%s: level %d is %d x %d", fn, l, L.h, L.w);
+    TAPIR_CHECK_ARG(aligned(L.grid, 16), "%s: level %d grid must be 16-byte aligned", fn, l);
+  }
+  TAPIR_CHECK_ARG(aligned(a->feat_hi, 16) && aligned(a->feat_lo, 16) && a->feat_hi_stride_n >= 0 &&
+                      a->feat_hi_stride_t >= 0 && a->feat_lo_stride_n >= 0 && a->feat_lo_stride_t >= 0 &&
+                      a->feat_hi_stride_n % 4 == 0 && a->feat_hi_stride_t % 4 == 0 &&
+                      a->feat_lo_stride_n % 4 == 0 && a->feat_lo_stride_t % 4 == 0,
+                  "%s: feat_hi, feat_lo must be 16-byte aligned, their strides non-negative multiples of 4", fn);
+  TAPIR_CHECK_ARG(aligned(a->out_planes, 4) && a->out_plane_stride % 2 == 0,
+                  "%s: out_planes must be 4-byte aligned, out_plane_stride even", fn);
+  const long long rows = (long long)a->num_points * batch * a->num_frames;
+  TAPIR_CHECK_ARG(a->planes <= 1 || a->out_plane_stride >= rows * a->ld,
+                  "%s: planes overlap (out_plane_stride=%lld)", fn, (long long)a->out_plane_stride);
+  return kOk;
+}
+}  // namespace
+
 int tapir_local_corr(const tapir_corr_args* args, void* stream) {
   Range nvtx_range("tapir_local_corr");
+  TAPIR_RETURN_IF(check_corr_args(args, 1, "tapir_local_corr"));
   return local_corr(args, 1, S(stream));
 }
 
 int tapir_local_corr_batched(const tapir_corr_args* args, int32_t batch, void* stream) {
   Range nvtx_range("tapir_local_corr_batched");
+  TAPIR_RETURN_IF(check_corr_args(args, batch, "tapir_local_corr_batched"));
   return local_corr(args, batch, S(stream));
 }
 
@@ -344,8 +378,60 @@ int tapir_mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, 
   return mixer_forward(w, io, workspace, workspace_bytes, S(stream));
 }
 
+namespace {
+bool overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
+  const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
+  return pa < pb + b_bytes && pb < pa + a_bytes;
+}
+}  // namespace
+
+int tapir_mixer_dw(const tapir_mixer_block* blk, const float* x, int32_t n, int32_t T, int32_t causal,
+                   const float* ctx1_in, const float* ctx2_in, float* ctx1_out, float* ctx2_out, float* z,
+                   void* planes_out, int64_t plane_stride, int32_t planes, void* stream) {
+  Range nvtx_range("tapir_mixer_dw");
+  TAPIR_CHECK_ARG(blk && x && z && planes_out, "tapir_mixer_dw: null pointer");
+  TAPIR_CHECK_ARG(blk->ln_w && blk->dw1_w && blk->dw1_b && blk->dw2_w && blk->dw2_b && blk->ln1_w,
+                  "tapir_mixer_dw: null weight pointer");
+  TAPIR_CHECK_ARG(n >= 1 && n <= 65535 && T >= 1, "tapir_mixer_dw: n=%d T=%d (n in 1..65535, T >= 1)", n, T);
+  TAPIR_CHECK_ARG(planes >= 1 && planes <= 3, "tapir_mixer_dw: planes=%d", planes);
+  const long long rows = (long long)n * T;
+  TAPIR_CHECK_ARG(planes == 1 || plane_stride >= rows * 512,
+                  "tapir_mixer_dw: planes overlap (plane_stride=%lld)", (long long)plane_stride);
+  TAPIR_CHECK_ARG(aligned(x, 16) && aligned(z, 16) && aligned(ctx1_in, 16) && aligned(ctx2_in, 16) &&
+                      aligned(ctx1_out, 16) && aligned(ctx2_out, 16) && aligned(blk->ln_w, 16) &&
+                      aligned(blk->ln1_w, 16) && aligned(planes_out, 8) && plane_stride % 4 == 0,
+                  "tapir_mixer_dw: x, z, contexts and LayerNorm weights must be 16-byte aligned, "
+                  "planes_out 8-byte aligned, plane_stride a multiple of 4");
+  TAPIR_CHECK_ARG(!overlap(x, rows * 512 * 4, z, rows * 512 * 4), "tapir_mixer_dw: x and z overlap");
+  TAPIR_CHECK_ARG(causal || !(ctx1_in || ctx2_in || ctx1_out || ctx2_out),
+                  "tapir_mixer_dw: context pointers on a non-causal call");
+  // T > 24 runs several CTAs per query: one would read a context slot another has overwritten.
+  // T = 1 reads both slots before writing (the streaming step updates its context in place).
+  const size_t c1 = (size_t)n * 2 * 512 * 4, c2 = (size_t)n * 2 * 2048 * 4;
+  TAPIR_CHECK_ARG(!overlap(ctx1_in, ctx1_in ? c1 : 0, ctx1_out, ctx1_out ? c1 : 0) ||
+                      (T == 1 && ctx1_in == ctx1_out),
+                  "tapir_mixer_dw: ctx1_in and ctx1_out overlap (allowed only as the same buffer at T = 1)");
+  TAPIR_CHECK_ARG(!overlap(ctx2_in, ctx2_in ? c2 : 0, ctx2_out, ctx2_out ? c2 : 0) ||
+                      (T == 1 && ctx2_in == ctx2_out),
+                  "tapir_mixer_dw: ctx2_in and ctx2_out overlap (allowed only as the same buffer at T = 1)");
+  return mixer_dw(*blk, x, n, T, causal != 0, ctx1_in, ctx2_in, ctx1_out, ctx2_out, z,
+                  static_cast<__nv_bfloat16*>(planes_out), plane_stride, planes, S(stream));
+}
+
 int tapir_refine_update(const tapir_update_args* args, void* stream) {
   Range nvtx_range("tapir_refine_update");
+  const tapir_update_args* a = args;
+  TAPIR_CHECK_ARG(a != nullptr && a->res && a->pos && a->feat_out && a->occ_out && a->expd_out && a->feat_hi &&
+                      a->feat_lo && a->occ_in && a->expd_in,
+                  "tapir_refine_update: null pointer");
+  const long long rows = (long long)a->num_points * a->num_frames;
+  TAPIR_CHECK_ARG(a->num_points >= 1 && a->num_frames >= 1 && rows < (1ll << 31),
+                  "tapir_refine_update: num_points=%d num_frames=%d (rows must be in 1..2^31-1)", a->num_points,
+                  a->num_frames);
+  TAPIR_CHECK_ARG(a->ld_res >= 388, "tapir_refine_update: ld_res=%d < 388", a->ld_res);
+  TAPIR_CHECK_ARG(a->init_h >= 1 && a->init_w >= 1 && a->resize_h >= 1 && a->resize_w >= 1 &&
+                      (a->tracks_out == nullptr || (a->video_h >= 1 && a->video_w >= 1)),
+                  "tapir_refine_update: sizes must be positive");
   return refine_update(args, S(stream));
 }
 

@@ -82,6 +82,11 @@ int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s);
 size_t mixer_workspace_bytes(long long rows, int planes);
 int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* ws, size_t ws_bytes,
                   cudaStream_t s);
+// The depthwise half of one mixer block (everything before its channel MLP) on x [n][T][512]:
+// z [n][T][512] and LN_1(z) * w as bf16 planes [planes][n*T][512].  Context pointers: causal only.
+int mixer_dw(const tapir_mixer_block& blk, const float* x, int n, int T, bool causal, const float* ctx1_in,
+             const float* ctx2_in, float* ctx1_out, float* ctx2_out, float* z, __nv_bfloat16* planes_out,
+             long long plane_stride, int planes, cudaStream_t s);
 int refine_update(const tapir_update_args* a, cudaStream_t s);
 
 }  // namespace tapir

@@ -632,6 +632,59 @@ GemmArgs lin(const tapir_linear& l) {
 }
 }  // namespace
 
+int mixer_dw(const tapir_mixer_block& blk, const float* x, int n, int T, bool causal, const float* ctx1_in,
+             const float* ctx2_in, float* ctx1_out, float* ctx2_out, float* z, __nv_bfloat16* planes_out,
+             long long plane_stride, int planes, cudaStream_t s) {
+  static PerDeviceOnce configured;
+  if (configured.pending()) {
+    const int max_smem = kDwRowBudget * 512 * (int)sizeof(float);
+    TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
+    configured.mark();
+  }
+  const long long rows = (long long)n * T;
+  DwParams d;
+  d.x = x; d.z = z;
+  d.planes_out = planes_out; d.plane_stride = plane_stride; d.planes = planes;
+  d.T = T; d.N = n;
+  d.TT = T < kDwTileMax ? T : kDwTileMax;
+  d.QB = kDwRowBudget / (2 * d.TT + kDwHalo);
+  if (d.QB < 1) d.QB = 1;
+  if (d.QB > kDwSmallQueries) d.QB = kDwSmallQueries;
+  // few rows in total (streaming): fewer queries per CTA so that every SM gets one
+  // (the several-queries-per-CTA variant runs one CTA per SM: aim at exactly one round)
+  if (d.QB > 1) {
+    const long long per_sm = ceil_div_ll((long long)n * ceil_div(T, d.TT), num_sms());
+    if (per_sm < d.QB) d.QB = per_sm < 2 ? 2 : (int)per_sm;
+  }
+  if (d.QB > n) d.QB = n;
+  d.ln_w = blk.ln_w; d.w1 = blk.dw1_w; d.b1 = blk.dw1_b; d.w2 = blk.dw2_w; d.b2 = blk.dw2_b;
+  d.ln1_w = blk.ln1_w;
+  d.ctx1_in = ctx1_in;
+  d.ctx2_in = ctx2_in;
+  d.ctx1_out = ctx1_out;
+  d.ctx2_out = ctx2_out;
+  dim3 grid(ceil_div(T, d.TT), ceil_div(n, d.QB));
+  const int dw_smem = d.QB * (2 * d.TT + kDwHalo) * 512 * (int)sizeof(float);
+  {
+    ProfileScope ps("mixer.dw", s, (double)rows * 2048 * 12, (double)rows * 512 * (8 + 2 * planes));
+    // SMALL exists for the causal context prefetch.  Its non-causal instantiation is miscompiled
+    // for sm_90 by CUDA 12.9 ptxas (-O1 and up, query loop unrolled): wrong outputs for tiles of
+    // 5+ frames, right at -O0 or not unrolled.  Non-causal tiles run the generic kernel; the
+    // causal one is checked over the same code paths (test_mixer_causal_with_context).
+    if (causal) {
+      if (d.QB > 1) mixer_dw_kernel<true, true><<<grid, 512, dw_smem, s>>>(d);
+      else mixer_dw_kernel<true, false><<<grid, 512, dw_smem, s>>>(d);
+    } else {
+      mixer_dw_kernel<false, false><<<grid, 512, dw_smem, s>>>(d);
+    }
+  }
+  count_launch();
+  TAPIR_LAUNCH_CHECK("mixer_dw_kernel");
+  return kOk;
+}
+
 size_t mixer_workspace_bytes(long long rows, int planes) {
   Arena a(nullptr, 0);
   MixerPlan m;
@@ -655,14 +708,6 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
     set_error("mixer_forward: workspace too small (%zu < %zu)", ws_bytes, arena.off);
     return kWorkspaceTooSmall;
   }
-  static PerDeviceOnce configured;
-  if (configured.pending()) {
-    const int max_smem = kDwRowBudget * 512 * (int)sizeof(float);
-    TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    TAPIR_CUDA(cudaFuncSetAttribute(mixer_dw_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
-    configured.mark();
-  }
   {  // nets.py:235 linear
     GemmArgs g = lin(w->linear);
     g.tag = "mixer.linear_in";
@@ -676,44 +721,9 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
   }
   for (int b = 0; b < w->num_blocks; ++b) {
     const tapir_mixer_block& blk = w->blocks[b];
-    DwParams d;
-    d.x = m.xa; d.z = m.xb;
-    d.planes_out = m.y; d.plane_stride = rows * 512; d.planes = P;
-    d.T = T; d.N = n;
-    d.TT = T < kDwTileMax ? T : kDwTileMax;
-    d.QB = kDwRowBudget / (2 * d.TT + kDwHalo);
-    if (d.QB < 1) d.QB = 1;
-    if (d.QB > kDwSmallQueries) d.QB = kDwSmallQueries;
-    // few rows in total (streaming): fewer queries per CTA so that every SM gets one
-    // (the several-queries-per-CTA variant runs one CTA per SM: aim at exactly one round)
-    if (d.QB > 1) {
-      const long long per_sm = ceil_div_ll((long long)n * ceil_div(T, d.TT), num_sms());
-      if (per_sm < d.QB) d.QB = per_sm < 2 ? 2 : (int)per_sm;
-    }
-    if (d.QB > n) d.QB = n;
-    d.ln_w = blk.ln_w; d.w1 = blk.dw1_w; d.b1 = blk.dw1_b; d.w2 = blk.dw2_w; d.b2 = blk.dw2_b;
-    d.ln1_w = blk.ln1_w;
-    d.ctx1_in = io->ctx1_in ? io->ctx1_in[b] : nullptr;
-    d.ctx2_in = io->ctx2_in ? io->ctx2_in[b] : nullptr;
-    d.ctx1_out = io->ctx1_out ? io->ctx1_out[b] : nullptr;
-    d.ctx2_out = io->ctx2_out ? io->ctx2_out[b] : nullptr;
-    dim3 grid(ceil_div(T, d.TT), ceil_div(n, d.QB));
-    const int dw_smem = d.QB * (2 * d.TT + kDwHalo) * 512 * (int)sizeof(float);
-    {
-      ProfileScope ps("mixer.dw", s, (double)rows * 2048 * 12, (double)rows * 512 * (8 + 2 * P));
-      // SMALL exists for the causal context prefetch.  Its non-causal instantiation is miscompiled
-      // for sm_90 by CUDA 12.9 ptxas (-O1 and up, query loop unrolled): wrong outputs for tiles of
-      // 5+ frames, right at -O0 or not unrolled.  Non-causal tiles run the generic kernel; the
-      // causal one is checked over the same code paths (test_mixer_causal_with_context).
-      if (io->causal) {
-        if (d.QB > 1) mixer_dw_kernel<true, true><<<grid, 512, dw_smem, s>>>(d);
-        else mixer_dw_kernel<true, false><<<grid, 512, dw_smem, s>>>(d);
-      } else {
-        mixer_dw_kernel<false, false><<<grid, 512, dw_smem, s>>>(d);
-      }
-    }
-    count_launch();
-    TAPIR_LAUNCH_CHECK("mixer_dw_kernel");
+    TAPIR_RETURN_IF(mixer_dw(blk, m.xa, n, T, io->causal != 0, io->ctx1_in ? io->ctx1_in[b] : nullptr,
+                             io->ctx2_in ? io->ctx2_in[b] : nullptr, io->ctx1_out ? io->ctx1_out[b] : nullptr,
+                             io->ctx2_out ? io->ctx2_out[b] : nullptr, m.xb, m.y, rows * 512, P, s));
     {
       GemmArgs g = lin(blk.up);
       g.tag = "mixer.up";

@@ -129,81 +129,6 @@ def test_cost_volume_tracks():
   assert e_p < 1e-3 and e_o < 1e-4 and e_e < 1e-4
 
 
-# (pyramid_level, gh, gw, use_last).  24 x 72 is a 3:1 panoramic grid: the reference spaces the x
-# samples gw/gh = 3 cells apart (x is normalised by h, utils.py:104), wider than the 16-column
-# cell box, so the kernel's per-sample path is exercised (levels 0/1) next to the box path.
-@pytest.mark.parametrize('cfg_case', [(1, 32, 32, True), (1, 40, 48, True), (0, 32, 32, False),
-                                      (1, 24, 72, True)])
-def test_local_corr(cfg_case):
-  pyr, gh, gw, use_last = cfg_case
-  model, sd, cfg = get_model(pyramid_level=pyr, extra_convs=(pyr == 1))
-  lib = _lib.load()
-  T, N = 3, 37
-  hires = _unit_grid(T, 2 * gh, 2 * gw, 128, 7)
-  lowres = _unit_grid(T, gh, gw, 256, 8)
-  g = torch.Generator().manual_seed(9)
-  pos = torch.rand(1, N, T, 2, generator=g) * 256
-  pos[0, 0, 0] = torch.tensor([0.0, 0.0])          # corner: zero padding
-  pos[0, 1, 0] = torch.tensor([255.99, 255.99])
-  pos[0, 2, 0] = torch.tensor([128.0, 64.0])       # exactly-integer sample positions
-  pos[0, 3, 0] = torch.tensor([-20.0, 300.0])      # fully outside
-  occ = torch.randn(1, N, T, generator=g)
-  expd = torch.randn(1, N, T, generator=g)
-  qh = torch.randn(1, N, 128, generator=g)
-  ql = torch.randn(1, N, 256, generator=g)
-  last = torch.randn(1, N, T, 384, generator=g) if use_last else None
-  pyramid = [hires, lowres]
-  queries = [qh, ql]
-  if pyr:
-    pyramid.append(torch.nn.functional.avg_pool3d(lowres, (2, 2, 1), (2, 2, 1)))
-    queries.append(ql)
-  ref = O.local_correlation(cfg, queries, pyramid, pos, last)  # [1,N,T,49L]
-  L = 2 + pyr
-  kin = 388 + 49 * L
-  kpad = (kin + 63) // 64 * 64
-  P = 3
-  dev = 'cuda'
-  grids_d = [p[0].cuda().contiguous() for p in pyramid]
-  if pyr:
-    pooled = torch.empty_like(grids_d[2])
-    _lib.check(lib.tapir_pool_pyramid(U.ptr(grids_d[1]), T, gh, gw, 256, U.ptr(pooled), U.stream()), 'pool')
-    torch.cuda.synchronize()
-    e_pool = maxerr(pooled, pyramid[2][0])
-    U.record(f'pool_{gh}x{gw}', err=e_pool)
-    assert e_pool < 1e-6
-    grids_d[2] = pooled
-  out = torch.empty(P, N * T, kpad, dtype=torch.bfloat16, device=dev)
-  ca = _lib.CorrArgs()
-  for i, gd in enumerate(grids_d):
-    ca.levels[i].grid = gd.data_ptr()
-    ca.levels[i].h, ca.levels[i].w, ca.levels[i].C = gd.shape[1], gd.shape[2], gd.shape[3]
-  ca.num_levels, ca.num_points, ca.num_frames = L, N, T
-  ca.init_h, ca.init_w, ca.planes = 256, 256, P
-  pos_d, occ_d, expd_d = pos[0].cuda().contiguous(), occ[0].cuda().contiguous(), expd[0].cuda().contiguous()
-  ca.pos, ca.occ, ca.expd = pos_d.data_ptr(), occ_d.data_ptr(), expd_d.data_ptr()
-  if use_last:
-    last_d = last[0].cuda().contiguous()
-    ca.feat_hi, ca.feat_hi_stride_n, ca.feat_hi_stride_t = last_d.data_ptr(), T * 384, 384
-    ca.feat_lo, ca.feat_lo_stride_n, ca.feat_lo_stride_t = last_d.data_ptr() + 512, T * 384, 384
-    feats_ref = last[0]
-  else:
-    qh_d, ql_d = qh[0].cuda().contiguous(), ql[0].cuda().contiguous()
-    ca.feat_hi, ca.feat_hi_stride_n, ca.feat_hi_stride_t = qh_d.data_ptr(), 128, 0
-    ca.feat_lo, ca.feat_lo_stride_n, ca.feat_lo_stride_t = ql_d.data_ptr(), 256, 0
-    feats_ref = torch.cat([qh[0], ql[0]], -1)[:, None].expand(-1, T, -1)
-  ca.out_planes, ca.out_plane_stride, ca.ld = out.data_ptr(), N * T * kpad, kpad
-  _lib.check(lib.tapir_local_corr(ctypes.byref(ca), U.stream()), 'local_corr')
-  torch.cuda.synchronize()
-  row = out.float().sum(0).cpu().reshape(N, T, kpad)
-  e_corr = (row[..., 388:kin] - ref[0]).abs().max().item()
-  e_feat = (row[..., 4:388] - feats_ref).abs().max().item()
-  e_head = max(row[..., :2].abs().max().item(), (row[..., 2] - occ[0]).abs().max().item(),
-               (row[..., 3] - expd[0]).abs().max().item(), row[..., kin:].abs().max().item())
-  U.record(f'local_corr_pyr{pyr}_{gh}x{gw}_last{int(use_last)}', corr_err=e_corr, feat_err=e_feat,
-           head_err=e_head, corr_scale=ref.abs().max().item())
-  assert e_corr < 2e-5 * max(1.0, ref.abs().max().item()) and e_feat < 1e-6 and e_head < 1e-6
-
-
 @pytest.mark.parametrize('shape', [(24, 40), (48, 16)])
 def test_cost_volume_tracks_any_map_size(shape):
   """initial_resolution != (256, 256) (ctor argument, tapir_model.py:86): the cost map is not
