@@ -3,6 +3,8 @@
   python scripts/gemm_bench.py               every shape under the dispatcher's own choice
   python scripts/gemm_bench.py --schedules   the offline clip's GEMM shapes under both wgmma
                                              schedules (TAPIR_B200_GEMM_SCHEDULE), alternated
+  python scripts/gemm_bench.py --tile-cost   time per launch against tile count at constant MMA
+                                             work, both schedules and BLOCK_N = 64 / 128
 """
 import argparse
 import ctypes
@@ -126,15 +128,87 @@ def compare_schedules(rounds, reps):
     print(f'{name:34s} {cells[0]:>24s} {cells[1]:>24s} {1 - med["pingpong"] / med["coop"]:6.1%}', flush=True)
 
 
+# GEMMs of mixer `up`'s MMA work (12288 x 2048 x 512) with fewer, longer tiles: same k-blocks per
+# CTA, 4x fewer tiles from the first shape to the last two
+TILE_COST_SHAPES = [(12288, 2048, 512), (12288, 1024, 1024), (12288, 512, 2048), (3072, 2048, 2048)]
+TILE_COST_EPILOGUES = [('f32', dict(bias=False), 4),
+                       ('gelu+plane', dict(gelu=True, planes_out=1, f32_out=False), 2),
+                       ('gelu+planes', dict(gelu=True, planes_out=2, f32_out=False), 4)]
+
+
+def _card():
+  """Card name, power limit and max SM clock, read now (nvidia-smi queries only)."""
+  import subprocess  # pylint: disable=g-import-not-at-top
+  q = 'name,power.limit,clocks.max.sm,clocks.sm'
+  try:
+    out = subprocess.run(['nvidia-smi', '-i', str(torch.cuda.current_device()), f'--query-gpu={q}',
+                          '--format=csv,noheader'], capture_output=True, text=True, timeout=30).stdout
+    return out.strip()
+  except (OSError, subprocess.SubprocessError):
+    return f'{torch.cuda.get_device_name()} (nvidia-smi unavailable)'
+
+
+def _with_env(env, fn):
+  old = {k: os.environ.get(k) for k in env}
+  os.environ.update(env)
+  try:
+    return fn()
+  finally:
+    for k, v in old.items():
+      if v is None:
+        os.environ.pop(k, None)
+      else:
+        os.environ[k] = v
+
+
+def tile_cost(rounds, reps):
+  """Time per launch against tile count at constant MMA work: every shape x epilogue x schedule x
+  BLOCK_N, alternated `rounds` times in this process (L2 flushed before every launch), median of
+  all launches.  Per tile and per k-block figures divide by the busiest CTA's share."""
+  sms = torch.cuda.get_device_properties(0).multi_processor_count
+  print(f'card: {_card()}')
+  calls = {}
+  for M, N, K in TILE_COST_SHAPES:
+    for epi, kw, _ in TILE_COST_EPILOGUES:
+      calls[(M, N, K, epi)] = make(M, N, K, **kw)[0]
+  out_bytes = {epi: b for epi, _, b in TILE_COST_EPILOGUES}
+  configs = [(shape_epi, sched, bn) for shape_epi in calls for sched in ('coop', 'pingpong') for bn in (128, 64)]
+  ts = {c: [] for c in configs}
+  for _ in range(rounds):
+    for c in configs:
+      shape_epi, sched, bn = c
+      env = {'TAPIR_B200_GEMM_SCHEDULE': sched, 'TAPIR_B200_BLOCK_N': str(bn)}
+      ts[c] += _with_env(env, lambda: time_ms(calls[shape_epi], reps, True))
+  print(f'{"M x N x K":>18s} {"epilogue":>12s} {"sched":>8s} {"BN":>3s} {"tiles":>5s} {"t/CTA":>5s} '
+        f'{"kb/t":>4s} {"us/launch (min-max)":>22s} {"us/tile":>8s} {"us/kblk":>8s} {"TF/s":>6s} {"out MB":>7s}')
+  for c in configs:
+    (M, N, K, epi), sched, bn = c
+    tiles = -(-M // 128) * -(-N // bn)
+    per_cta = -(-tiles // sms)
+    kb = K // 64
+    med = statistics.median(ts[c]) * 1e3
+    tf = 2.0 * M * N * K * 3 / (med * 1e-6) / 1e12  # P = 2: three bf16 MMAs per product
+    out_mb = M * N * out_bytes[epi] / 1e6
+    rng = f'{med:8.1f} ({min(ts[c]) * 1e3:.1f}-{max(ts[c]) * 1e3:.1f})'
+    print(f'{f"{M} x {N} x {K}":>18s} {epi:>12s} {sched:>8s} {bn:3d} {tiles:5d} {per_cta:5d} {kb:4d} '
+          f'{rng:>22s} {med / per_cta:8.2f} {med / (per_cta * kb) * (128 / bn):8.3f} {tf:6.1f} {out_mb:7.1f}',
+          flush=True)
+
+
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--schedules', action='store_true', help='compare the two wgmma schedules')
+  ap.add_argument('--tile-cost', action='store_true',
+                  help='time per launch against tile count at constant MMA work')
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--reps', type=int, default=10)
   a = ap.parse_args()
   print(f'peak {PEAK:g} TFLOP/s bf16 ({PEAK_SOURCE}); {torch.cuda.get_device_name()}')
   if a.schedules:
     compare_schedules(a.rounds, a.reps)
+    return
+  if a.tile_cost:
+    tile_cost(a.rounds, a.reps)
     return
   print('BLOCK_N override:', os.environ.get('TAPIR_B200_BLOCK_N', 'auto'))
   print('schedule override:', os.environ.get('TAPIR_B200_GEMM_SCHEDULE', 'auto'))

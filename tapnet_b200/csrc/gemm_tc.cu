@@ -89,9 +89,61 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[BLOCK_N / 2], uint64_t ade
   else ptx::wgmma_m64n128k16(d, adesc, bdesc, accumulate);
 }
 
+// Epilogue of a whole 64 x BLOCK_N accumulator whose rows and columns all exist, with the
+// options fixed at compile time and vector accesses only: straight-line code without branches,
+// so the compiler interleaves the independent column groups.  Each element goes through the
+// same operations in the same order as in `epilogue` below, so the results are bit-identical.
+template <int BLOCK_N, bool BIAS, bool GELU, bool RESID, bool F32, int PLANES, bool STATS>
+__device__ __forceinline__ void epilogue_full(const TcParams& p, const float (&acc)[BLOCK_N / 2],
+                                              const float* const (&res_row)[2], float* const (&out_row)[2],
+                                              __nv_bfloat16* const (&pl_row)[2], int n0, int frame, int lane) {
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int c = n0 + 8 * j + 2 * (lane & 3);
+    float b0 = 0.f, b1 = 0.f;
+    if constexpr (BIAS) { b0 = __ldg(p.bias + c); b1 = __ldg(p.bias + c + 1); }
+    float st[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      if constexpr (BIAS) { v0 += b0; v1 += b1; }
+      if constexpr (GELU) { v0 = gelu_tanh(v0); v1 = gelu_tanh(v1); }
+      if constexpr (RESID) {
+        const float2 t = *reinterpret_cast<const float2*>(res_row[h] + c);
+        v0 += t.x; v1 += t.y;
+      }
+      if constexpr (F32) *reinterpret_cast<float2*>(out_row[h] + c) = make_float2(v0, v1);
+      if constexpr (STATS) { st[0] += v0; st[2] += v0 * v0; st[1] += v1; st[3] += v1 * v1; }
+#pragma unroll
+      for (int q = 0; q < PLANES; ++q)
+        *reinterpret_cast<uint32_t*>(pl_row[h] + q * p.out_plane_stride + c) = bf16x2_split(v0, v1);
+    }
+    if constexpr (STATS) {
+#pragma unroll
+      for (int s = 4; s < 32; s <<= 1)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) st[e] += __shfl_xor_sync(0xffffffffu, st[e], s);
+      if (lane < 4) {
+        double* dst = p.stats + ((long long)frame * p.N + c) * 2;
+        atomicAdd(dst, (double)st[0]);
+        atomicAdd(dst + 1, (double)st[2]);
+        atomicAdd(dst + 2, (double)st[1]);
+        atomicAdd(dst + 3, (double)st[3]);
+      }
+    }
+  }
+}
+
 // Epilogue of one consumer warpgroup from its 64 x BLOCK_N accumulator in the wgmma fragment
 // layout: lane l of warp w holds tile rows 16 w + l / 4 (h = 0) and + 8 (h = 1), columns
 // 8 j + 2 (l % 4) + {0, 1} in acc[4 j + 2 h + {0, 1}].  row[h] / row_ok[h]: the global rows.
+//
+// Tiles inside the output with the common option sets (GELU and two bf16 planes; fp32 with or
+// without residual and fused statistics; each with or without bias) take `epilogue_full`.
+// Everything else (edge tiles, other plane counts, unaligned tensors) takes the general
+// loop below, whose runtime option tests split every column group into short dependent
+// branches: measured on H100 at 700 W, it kept one warpgroup 17 us (fp32 store) to 28 us (GELU +
+// planes) on a 128 x 128 tile, two to three times the other warpgroup's 8-k-block mainloop.
 template <int BLOCK_N>
 __device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[BLOCK_N / 2],
                                          const long long (&row)[2], const bool (&row_ok)[2], int n0,
@@ -118,6 +170,23 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[B
       for (int h = 0; h < 2; ++h)
         if (row_ok[h]) asm volatile("prefetch.global.L1 [%0];" ::"l"(res_row[h] + c));
     }
+  }
+  if (n0 + BLOCK_N <= p.N && row_ok[0] && row_ok[1]) {
+    const bool bias = p.bias != nullptr, resid = p.residual != nullptr, stats = p.stats != nullptr;
+#define TAPIR_EPI_FULL(B, G, R, F, PL, S)                                                  \
+    if (bias == B && resid == R && stats == S)                                              \
+      return epilogue_full<BLOCK_N, B, G, R, F, PL, S>(p, acc, res_row, out_row, pl_row, n0, frame, lane);
+    if (p.act == 1 && !resid && !stats && p.out_f32 == nullptr && p.out_P == 2 && vec_p) {
+      TAPIR_EPI_FULL(true, true, false, false, 2, false)
+      TAPIR_EPI_FULL(false, true, false, false, 2, false)
+    }
+    if (p.act == 0 && p.out_planes == nullptr && vec_o && (!resid || vec_r)) {
+      TAPIR_EPI_FULL(true, false, true, true, 0, true) TAPIR_EPI_FULL(true, false, true, true, 0, false)
+      TAPIR_EPI_FULL(true, false, false, true, 0, true) TAPIR_EPI_FULL(true, false, false, true, 0, false)
+      TAPIR_EPI_FULL(false, false, true, true, 0, true) TAPIR_EPI_FULL(false, false, true, true, 0, false)
+      TAPIR_EPI_FULL(false, false, false, true, 0, true) TAPIR_EPI_FULL(false, false, false, true, 0, false)
+    }
+#undef TAPIR_EPI_FULL
   }
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
