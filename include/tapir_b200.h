@@ -368,6 +368,22 @@ typedef struct {
 } tapir_tapvid_args;
 int tapir_tapvid_counts(const tapir_tapvid_args* args, void* stream);
 
+/* ---- f5: visualisation (the step after the path) ------------------------------------- */
+/* tapnet/utils/viz_utils.py:47-124 paint_point_track, bit for bit: frames [T][H][W][3] uint8 ->
+ * out (same shape, must not overlap frames) with a dot of radius round(min(H, W) * 0.015) at
+ * every visible point, painted in index order.  tracks [N][T][2] (x, y) float (tracks_fp64 = 0)
+ * or double (1); the + 0.5 to the dot centre is taken in that dtype.  visibles [N][T] uint8
+ * (non-zero paints), colors [N][3] uint8.  Points with a NaN coordinate are skipped (undefined in
+ * the reference).  N = 0 copies the frames.  Workspace: tapir_paint_point_track_workspace_bytes
+ * (T, N) bytes, 16-byte aligned (NULL when N = 0).  Two launches; stream-ordered, no host sync.
+ * A bad argument (negative size, NULL pointer, small workspace, out overlapping frames) returns
+ * 1 before any CUDA call. */
+size_t tapir_paint_point_track_workspace_bytes(int32_t frames, int32_t points);
+int tapir_paint_point_track(const uint8_t* frames, int32_t T, int32_t H, int32_t W,
+                            const void* tracks, int32_t tracks_fp64, const uint8_t* visibles,
+                            int32_t N, const uint8_t* colors, uint8_t* out, void* workspace,
+                            size_t workspace_bytes, void* stream);
+
 /* ---- a4: tapir_model.py:217-291 + utils.py:45-73 (trilinear, border clamp) ---------- */
 /* query_tyx [N][3] in video coordinates (vT,vH,vW) -> out [N][C] */
 int tapir_sample_query_features(const float* grid, int32_t T, int32_t gh, int32_t gw, int32_t C,

@@ -191,6 +191,10 @@ SIGNATURES = {
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32,
                                       c_void_p]),
     'tapir_refine_update': (ctypes.c_int, [POINTER(UpdateArgs), c_void_p]),
+    'tapir_paint_point_track_workspace_bytes': (c_size_t, [c_int32, c_int32]),
+    'tapir_paint_point_track': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int32,
+                                               c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_size_t,
+                                               c_void_p]),
 }
 
 _lib = None

@@ -435,4 +435,35 @@ int tapir_refine_update(const tapir_update_args* args, void* stream) {
   return refine_update(args, S(stream));
 }
 
+size_t tapir_paint_point_track_workspace_bytes(int32_t frames, int32_t points) {
+  return paint_point_track_workspace_bytes(frames, points);
+}
+
+int tapir_paint_point_track(const uint8_t* frames, int32_t T, int32_t H, int32_t W, const void* tracks,
+                            int32_t tracks_fp64, const uint8_t* visibles, int32_t N, const uint8_t* colors,
+                            uint8_t* out, void* workspace, size_t workspace_bytes, void* stream) {
+  Range nvtx_range("tapir_paint_point_track");
+  TAPIR_CHECK_ARG(T >= 0 && H >= 0 && W >= 0 && N >= 0,
+                  "tapir_paint_point_track: negative size (T=%d H=%d W=%d N=%d)", T, H, W, N);
+  TAPIR_CHECK_ARG(tracks_fp64 == 0 || tracks_fp64 == 1, "tapir_paint_point_track: tracks_fp64=%d", tracks_fp64);
+  const long long tiles_per_frame = ((H + 31ll) / 32) * ((W + 31ll) / 32);
+  TAPIR_CHECK_ARG(tiles_per_frame == 0 || T <= INT32_MAX / tiles_per_frame,
+                  "tapir_paint_point_track: %d frames of %d x %d exceed one launch grid", T, H, W);
+  const long long pixels = (long long)T * H * W;
+  if (pixels == 0) return kOk;
+  TAPIR_CHECK_ARG(frames && out, "tapir_paint_point_track: null frames / out");
+  TAPIR_CHECK_ARG(!overlap(frames, (size_t)pixels * 3, out, (size_t)pixels * 3),
+                  "tapir_paint_point_track: out overlaps frames (painting is not in place)");
+  if (N > 0) {
+    TAPIR_CHECK_ARG(tracks && visibles && colors && workspace, "tapir_paint_point_track: null pointer");
+    TAPIR_CHECK_ARG(aligned(tracks, tracks_fp64 ? 8 : 4) && aligned(workspace, 16),
+                    "tapir_paint_point_track: tracks must be aligned to their dtype, workspace 16-byte aligned");
+    const size_t need = paint_point_track_workspace_bytes(T, N);
+    TAPIR_CHECK_ARG(workspace_bytes >= need, "tapir_paint_point_track: workspace %zu bytes < %zu",
+                    workspace_bytes, need);
+  }
+  return paint_point_track(frames, T, H, W, tracks, tracks_fp64, visibles, N, colors, out, workspace,
+                           S(stream));
+}
+
 }  // extern "C"

@@ -65,6 +65,14 @@ int postprocess_occlusions(const float* occ, const float* expd, long long n, uin
                            cudaStream_t s);
 int tapvid_counts(const tapir_tapvid_args* a, cudaStream_t s);
 
+// ---- point-track painting (paint.cu; viz_utils.py:47-124) ---------------------------------
+int paint_radius(int H, int W);
+size_t paint_point_track_workspace_bytes(long long frames, long long points);
+// Arguments checked by tapir_paint_point_track; T * ceil(H/32) * ceil(W/32) fits a grid.
+int paint_point_track(const uint8_t* frames, int T, int H, int W, const void* tracks, int tracks_fp64,
+                      const uint8_t* visibles, int N, const uint8_t* colors, uint8_t* out, void* ws,
+                      cudaStream_t s);
+
 // ---- stage A (stage_a.cu) ---------------------------------------------------------------
 int sample_query_features(const float* grid, int T, int gh, int gw, int C, const float* query_tyx,
                           int N, int vT, int vH, int vW, float* out, cudaStream_t s);
