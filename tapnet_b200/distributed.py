@@ -89,7 +89,7 @@ def sharded_forward(model, video: torch.Tensor, query_points: torch.Tensor, gath
   rank only touches its own frame / query slices).  Returns the same dict as TAPIR.forward
   (on every rank if gather_outputs, else only this rank's query shard).
   """
-  from tapnet_b200.tapir_model import FeatureGrids  # pylint: disable=g-import-not-at-top
+  from tapnet_b200.tapir_model import FeatureGrids, refined_average  # pylint: disable=g-import-not-at-top
   world = dist.get_world_size(group)
   rank = dist.get_rank(group)
   T = video.shape[1]
@@ -154,12 +154,7 @@ def sharded_forward(model, video: torch.Tensor, query_points: torch.Tensor, gath
   qp = query_points[:, q0:q1]
   qf = model.get_query_features(video, False, qp, grids)
   tr = model.estimate_trajectories(video.shape[-3:-1], False, grids, qf, qp, None)
-  p = model.num_pips_iter
-  out = dict(
-      occlusion=torch.mean(torch.stack(tr['occlusion'][p::p]), dim=0),
-      tracks=torch.mean(torch.stack(tr['tracks'][p::p]), dim=0),
-      expected_dist=torch.mean(torch.stack(tr['expected_dist'][p::p]), dim=0),
-  )
+  out = refined_average(tr, model.num_pips_iter)
   if gather_outputs and world > 1:
     out = {k: gather_queries(v, N, 1, group) for k, v in out.items()}
   return out

@@ -16,20 +16,11 @@ never materialised as float.  `YUV420Frames` carries NV12 / I420 device frames (
 cameras) the same way, the colour conversion fused into the same reads; `yuv420_to_rgb`
 converts alone.  CUDA only; raises without the shared library.
 """
-import ctypes
 from typing import Optional, Tuple
 
 import torch
 
 from tapnet_b200 import _lib
-
-
-def _ptr(t):
-  return ctypes.c_void_p(t.data_ptr())
-
-
-def _stream():
-  return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _require_cuda(t, what):
@@ -155,8 +146,7 @@ def _descriptor(y, u, v, window, matrix, full_range, frame0=0):
   y0, x0, h, w = window
   f = int(frame0)
   desc = _lib.Yuv420Frames(
-      y.data_ptr() + f * y.stride(0), u.data_ptr() + f * u.stride(0),
-      v.data_ptr() + f * v.stride(0), y.stride(0), u.stride(0), v.stride(0),
+      y[f:].data_ptr(), u[f:].data_ptr(), v[f:].data_ptr(), y.stride(0), u.stride(0), v.stride(0),
       y.stride(1), u.stride(1), v.stride(1), step, H, W, y0, x0, h, w, _MATRICES[matrix],
       int(bool(full_range)), 0)
   return desc, (y, u, v)
@@ -170,9 +160,7 @@ def yuv420_to_rgb(frames: YUV420Frames) -> torch.Tensor:
   n = out.shape[0] * out.shape[1]
   if n > 0:
     with torch.cuda.device(frames.device):
-      desc = frames.c_struct()
-      _lib.check(_lib.load().tapir_yuv420_to_rgb(ctypes.byref(desc), n, _ptr(out), _stream()),
-                 'tapir_yuv420_to_rgb')
+      _lib.yuv420_to_rgb(frames, out)
   return out
 
 
@@ -184,10 +172,7 @@ def _ingest_yuv420(frames: YUV420Frames, window, resolution) -> torch.Tensor:
   out = torch.empty(B, T, oh, ow, 3, dtype=torch.float32, device=frames.device)
   if B * T > 0:
     with torch.cuda.device(frames.device):
-      desc = frames.c_struct()
-      _lib.check(_lib.load().tapir_ingest_frames_yuv420(ctypes.byref(desc), B * T, _ptr(out), oh,
-                                                        ow, _stream()),
-                 'tapir_ingest_frames_yuv420')
+      _lib.ingest_frames(frames, out)
   return out
 
 
@@ -204,16 +189,11 @@ def ingest_frames(frames, window: Optional[Tuple[int, int, int, int]] = None,
     raise ValueError('ingest_frames: expected uint8 frames [..., H, W, 3]')
   frames = frames.contiguous()
   H, W = int(frames.shape[-3]), int(frames.shape[-2])
-  lead = tuple(frames.shape[:-3])
-  n = 1
-  for d in lead:
-    n *= int(d)
   y0, x0, ch, cw = (0, 0, H, W) if window is None else (int(v) for v in window)
   oh, ow = (ch, cw) if resolution is None else (int(resolution[0]), int(resolution[1]))
-  out = torch.empty(*lead, oh, ow, 3, dtype=torch.float32, device=frames.device)
-  if n > 0:
-    _lib.check(_lib.load().tapir_ingest_frames(_ptr(frames), n, H, W, y0, x0, ch, cw, _ptr(out),
-                                               oh, ow, _stream()), 'tapir_ingest_frames')
+  out = torch.empty(*frames.shape[:-3], oh, ow, 3, dtype=torch.float32, device=frames.device)
+  if frames.shape[:-3].numel() > 0:
+    _lib.ingest_frames(frames, out, (y0, x0, ch, cw))
   return out
 
 
@@ -231,9 +211,7 @@ def postprocess_occlusions(occlusions: torch.Tensor, expected_dist: torch.Tensor
   expd = expected_dist.to(torch.float32).contiguous()
   out = torch.empty(occ.shape, dtype=torch.uint8, device=occ.device)
   if occ.numel() > 0:
-    _lib.check(_lib.load().tapir_postprocess_occlusions(_ptr(occ), _ptr(expd), occ.numel(),
-                                                        _ptr(out), _stream()),
-               'tapir_postprocess_occlusions')
+    _lib.postprocess_occlusions(occ, expd, out)
   return out.view(torch.bool)
 
 

@@ -8,7 +8,6 @@ divided (float64, 0/0 -> nan as in numpy).  The visibility threshold of
 `postprocess_occlusions` can be fused in by passing the two logit tensors instead of
 `pred_occluded`.
 """
-import ctypes
 from typing import Mapping, Optional
 
 import torch
@@ -41,33 +40,14 @@ def tapvid_counts(query_points, gt_occluded, gt_tracks, pred_occluded, pred_trac
   qp = _dev_tensor(query_points, torch.float32, dev)
   go = _dev_tensor(gt_occluded, torch.uint8, dev)
   gt = _dev_tensor(gt_tracks, torch.float32, dev)
-  if tuple(qp.shape) != (B, N, 3) or tuple(go.shape) != (B, N, T) or tuple(gt.shape) != (B, N, T, 2):
-    raise ValueError('tapvid_counts: inconsistent shapes')
-  args = _lib.TapvidArgs()
-  keep = [qp, go, gt, pt]
+  po = logits = None
   if pred_logits is not None:
-    occ = _dev_tensor(pred_logits[0], torch.float32, dev)
-    expd = _dev_tensor(pred_logits[1], torch.float32, dev)
-    if tuple(occ.shape) != (B, N, T) or tuple(expd.shape) != (B, N, T):
-      raise ValueError('tapvid_counts: logits must be [B, N, T]')
-    keep += [occ, expd]
-    args.pred_occluded = None
-    args.pred_occ_logits, args.pred_expd_logits = occ.data_ptr(), expd.data_ptr()
+    logits = tuple(_dev_tensor(x, torch.float32, dev) for x in pred_logits[:2])
   else:
     po = _dev_tensor(pred_occluded, torch.uint8, dev)
-    if tuple(po.shape) != (B, N, T):
-      raise ValueError('tapvid_counts: pred_occluded must be [B, N, T]')
-    keep.append(po)
-    args.pred_occluded = po.data_ptr()
   counts = torch.empty(B, N, _lib.TAPVID_COUNTERS, dtype=torch.int32, device=dev)
-  args.query_points, args.gt_occluded, args.gt_tracks = qp.data_ptr(), go.data_ptr(), gt.data_ptr()
-  args.pred_tracks = pt.data_ptr()
-  args.B, args.N, args.T, args.query_mode = B, N, T, _MODES[query_mode]
-  args.counts = counts.data_ptr()
-  stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
   with torch.cuda.device(dev):
-    _lib.check(_lib.load().tapir_tapvid_counts(ctypes.byref(args), stream), 'tapir_tapvid_counts')
-  del keep
+    _lib.tapvid_counts(qp, go, gt, po, pt, _MODES[query_mode], counts, logits)
   return counts
 
 

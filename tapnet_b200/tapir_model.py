@@ -11,7 +11,6 @@ a hand-written sm_90a kernel reached through the C ABI of `libtapir_b200.so`
 `torch.distributed` only.  There is no CPU or eager-PyTorch fallback: tensors must live on a
 CUDA device and the shared library must be built, otherwise the calls raise.
 """
-import ctypes
 import math
 from typing import Any, List, Mapping, NamedTuple, Optional, Sequence, Tuple
 
@@ -79,10 +78,6 @@ _MAX_BACKBONE_PIXELS = 96 * 256 * 256
 _H2D_SUBCHUNKS = 6
 
 
-def _ptr(t):
-  return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
 def _groups(B, N, T):
   """Work groups of estimate_trajectories as (b0, b1, query slice): whole clips b0..b1-1 with all
   their queries while the group's rows (clips x queries x frames) fit _MAX_ROWS_PER_CHUNK and its
@@ -94,6 +89,21 @@ def _groups(B, N, T):
   chunk_q = max(1, min(N, _MAX_ROWS_PER_CHUNK // T, 65535))
   return [(bi, bi + 1, slice(q0, min(q0 + chunk_q, N)))
           for bi in range(B) for q0 in range(0, N, chunk_q)]
+
+
+def _ctx_lists(d, nb, index, fix=lambda t: t):
+  """The [index] slices of one iteration's causal context dict as two per-block lists (causal_1,
+  causal_2), each passed through `fix`."""
+  return ([fix(d[f'block_{i}_causal_1'][index]) for i in range(nb)],
+          [fix(d[f'block_{i}_causal_2'][index]) for i in range(nb)])
+
+
+def refined_average(trajectories, num_pips_iter):
+  """occlusion / tracks / expected_dist averaged over the estimates that end each refinement
+  level, as the reference's forward returns them (tapir_model.py:203-210)."""
+  p = num_pips_iter
+  return {k: torch.mean(torch.stack(trajectories[k][p::p]), dim=0)
+          for k in ('occlusion', 'tracks', 'expected_dist')}
 
 
 def _on_model_device(fn):
@@ -223,11 +233,6 @@ class TAPIR(nn.Module):
         raise RuntimeError(f'tensor on {t.device}, model on {dev}')
     return dev
 
-  def _stream(self, dev=None):
-    # the current stream OF THE MODEL'S DEVICE (every public method runs its launches inside
-    # `torch.cuda.device(dev)`, so the C side's per-device caches and the pointers agree)
-    return ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
   def _copy_stream(self, dev):
     key = str(dev)
     if key not in self._copy_streams:
@@ -263,99 +268,9 @@ class TAPIR(nn.Module):
     sig = self._param_sig()
     if self._packed is not None and self._packed_sig == sig:
       return self._packed
-    lib = _lib.load()
     sd = {k: v.detach() for k, v in self.state_dict().items()}
-    dev = next(self.parameters()).device
-    P = self._planes
-    keep = []  # tensors referenced by raw pointers below
-    stream = self._stream(dev)
-
-    def f32(t):
-      t = t.to(device=dev, dtype=torch.float32).contiguous().clone()
-      keep.append(t)
-      return t
-
-    def linear(w2d, bias, planes=P):
-      w2d = f32(w2d)
-      n, k = w2d.shape
-      kp = (k + 63) // 64 * 64
-      dst = torch.empty(planes, n, kp, dtype=torch.bfloat16, device=dev)
-      keep.append(dst)
-      _lib.check(lib.tapir_split_planes(_ptr(w2d), k, _ptr(dst), kp, n * kp, n, k, kp, planes,
-                                        stream), 'tapir_split_planes')
-      b = f32(bias) if bias is not None else None
-      return _lib.Linear(w=dst.data_ptr(), bias=(b.data_ptr() if b is not None else None), N=n,
-                         K=kp, planes=planes, k_logical=k)
-
-    def conv(wkey, bkey=None):
-      w = sd[wkey]
-      co = w.shape[0]
-      w2d = w.permute(0, 2, 3, 1).reshape(co, -1)  # K order (ky, kx, cin)
-      return linear(w2d, sd[bkey] if bkey else None)
-
-    bw = _lib.BackboneWeights()
-    stem = f32(sd['resnet_torch.initial_conv.weight'].permute(2, 3, 1, 0))  # [7,7,3,64]
-    bw.stem_w = stem.data_ptr()
-    cin = 64
-    bi = 0
-    for g, (cout, stride) in enumerate(zip(schema.GROUP_CHANNELS, schema.GROUP_STRIDES)):
-      for b in range(2):
-        p = f'resnet_torch.block_groups.{g}.blocks.{b}.'
-        blk = bw.blocks[bi]
-        blk.cin = cin if b == 0 else cout
-        blk.cout = cout
-        blk.stride = stride if b == 0 else 1
-        blk.has_proj = 1 if b == 0 else 0
-        if b == 0:
-          blk.proj = conv(p + 'proj_conv.weight')
-        blk.conv0 = conv(p + 'conv_0.weight')
-        blk.conv1 = conv(p + 'conv_1.weight')
-        blk.bn0_w = f32(sd[p + 'bn_0.weight']).data_ptr()
-        blk.bn0_b = f32(sd[p + 'bn_0.bias']).data_ptr()
-        blk.bn1_w = f32(sd[p + 'bn_1.weight']).data_ptr()
-        blk.bn1_b = f32(sd[p + 'bn_1.bias']).data_ptr()
-        bi += 1
-      cin = cout
-    bw.num_extra = schema.NUM_EXTRA_CONV_BLOCKS if self._has_extra else 0
-    for i in range(bw.num_extra):
-      p = f'extra_convs.blocks.{i}.'
-      eb = bw.extra[i]
-      eb.ln_w = f32(sd[p + 'layer_norm.weight']).data_ptr()
-      eb.ln_b = f32(sd[p + 'layer_norm.bias']).data_ptr()
-      eb.conv = conv(p + 'conv.weight', p + 'conv.bias')
-      eb.conv1 = conv(p + 'conv_1.weight', p + 'conv_1.bias')
-    bw.planes = P
-
-    hw = _lib.HeadWeights()
-    m = 'torch_cost_volume_track_mods.'
-    for name, key in (('hid1', 'hid1'), ('hid2', 'hid2'), ('hid3', 'hid3'), ('hid4', 'hid4'),
-                      ('occ', 'occ_out')):
-      setattr(hw, name + '_w', f32(sd[m + key + '.weight']).data_ptr())
-      setattr(hw, name + '_b', f32(sd[m + key + '.bias']).data_ptr())
-
-    mw = _lib.MixerWeights()
-    x = 'torch_pips_mixer.'
-    mw.linear = linear(sd[x + 'linear.weight'], sd[x + 'linear.bias'])
-    mw.linear_1 = linear(sd[x + 'linear_1.weight'], sd[x + 'linear_1.bias'])
-    mw.ln_w = f32(sd[x + 'layer_norm.weight']).data_ptr()
-    nb = len([k for k in sd if k.startswith(x + 'blocks.') and k.endswith('.layer_norm.weight')])
-    mw.num_blocks = nb
-    mw.planes = P
-    for i in range(nb):
-      p = f'{x}blocks.{i}.'
-      blk = mw.blocks[i]
-      blk.ln_w = f32(sd[p + 'layer_norm.weight']).data_ptr()
-      blk.dw1_w = f32(sd[p + 'mlp1_up.weight']).data_ptr()
-      blk.dw1_b = f32(sd[p + 'mlp1_up.bias']).data_ptr()
-      blk.dw2_w = f32(sd[p + 'mlp1_up_1.weight']).data_ptr()
-      blk.dw2_b = f32(sd[p + 'mlp1_up_1.bias']).data_ptr()
-      blk.ln1_w = f32(sd[p + 'layer_norm_1.weight']).data_ptr()
-      blk.up = linear(sd[p + 'conv_channels_mixer.mlp2_up.weight'],
-                      sd[p + 'conv_channels_mixer.mlp2_up.bias'])
-      blk.down = linear(sd[p + 'conv_channels_mixer.mlp2_down.weight'],
-                        sd[p + 'conv_channels_mixer.mlp2_down.bias'])
-    self._packed = dict(backbone=bw, head=hw, mixer=mw, keep=keep,
-                        mixer_in=int(mw.linear.K), num_blocks=nb)
+    self._packed = _lib.pack_weights(sd, self._planes, self._has_extra,
+                                     next(self.parameters()).device)
     self._packed_sig = sig
     return self._packed
 
@@ -381,11 +296,8 @@ class TAPIR(nn.Module):
                                              refinement_resolutions)
     trajectories = self.estimate_trajectories(video.shape[-3:-1], is_training, feature_grids,
                                               query_features, query_points, query_chunk_size)
-    p = self.num_pips_iter
     return dict(
-        occlusion=torch.mean(torch.stack(trajectories['occlusion'][p::p]), dim=0),
-        tracks=torch.mean(torch.stack(trajectories['tracks'][p::p]), dim=0),
-        expected_dist=torch.mean(torch.stack(trajectories['expected_dist'][p::p]), dim=0),
+        **refined_average(trajectories, self.num_pips_iter),
         unrefined_occlusion=trajectories['occlusion'][:-1],
         unrefined_tracks=trajectories['tracks'][:-1],
         unrefined_expected_dist=trajectories['expected_dist'][:-1],
@@ -410,15 +322,13 @@ class TAPIR(nn.Module):
       refinement_resolutions = generate_default_resolutions(video.shape[2:4],
                                                             self.initial_resolution)
     all_required = [tuple(self.initial_resolution)] + [tuple(r) for r in refinement_resolutions]
-    for resolution in all_required:
-      if resolution[0] % 8 != 0 or resolution[1] % 8 != 0:
-        raise ValueError('Image resolution must be a multiple of 8.')
+    if any(r[0] % 8 != 0 or r[1] % 8 != 0 for r in all_required):
+      raise ValueError('Image resolution must be a multiple of 8.')
     # A HOST clip (ideally pinned) is accepted too (extension): its frames are copied to the
     # device in chunks on a copy stream and the stem convolution - the only reader of the video -
     # runs chunk by chunk behind them, so PCIe time hides behind compute.
     host_video = video.device.type == 'cpu'
     dev = self._device_check(None if host_video else video)
-    lib = _lib.load()
     pk = self._pack()
     # uint8 video = raw [0,255] frames (what the reference's callers hold before
     # preprocess_frames, pytorch_live_demo.py:30-41): normalised inside the stem conv's loads
@@ -427,10 +337,8 @@ class TAPIR(nn.Module):
     # YUV 4:2:0 frames (extension): at the frame's own size the stem conv converts inside its
     # loads; a resized pass converts each bilinear tap in the ingest kernel.  Bit for bit the
     # results of the uint8 RGB frames the conversion produces.
-    yuv = isinstance(video, live.YUV420Frames)
-    video_u8 = not yuv and video.dtype == torch.uint8
-    if not yuv:
-      video = video.contiguous() if video_u8 else video.to(torch.float32).contiguous()
+    if not isinstance(video, live.YUV420Frames):
+      video = video.contiguous() if video.dtype == torch.uint8 else video.to(torch.float32).contiguous()
     n, f, vh, vw, _ = video.shape
     host_src = None
     if host_video:
@@ -444,101 +352,72 @@ class TAPIR(nn.Module):
     curr_resolution = (-1, -1)
     latent = hires = None
     shape_hw = None
-    stream = self._stream(dev)
     for resolution in all_required:
-      if resolution[0] % 8 != 0 or resolution[1] % 8 != 0:
-        raise ValueError('Image resolution must be a multiple of 8.')
       if not _is_same_res(curr_resolution, resolution):
         # reference quirk (:337): the PREVIOUS resolution is compared with the video size
         if _is_same_res(curr_resolution, video.shape[-3:-1]):
           h, w = vh, vw
-          frames_src = video
         else:
           h, w = int(resolution[0]), int(resolution[1])
-          if (h, w) == (vh, vw):
-            frames_src = video  # align_corners=False resize to the same size is the identity
-          else:
-            frames_src = torch.empty(n, f, h, w, 3, dtype=torch.float32, device=dev)
-            if yuv:
-              desc = video.c_struct()
-              _lib.check(lib.tapir_ingest_frames_yuv420(ctypes.byref(desc), n * f,
-                                                        _ptr(frames_src), h, w, stream),
-                         'tapir_ingest_frames_yuv420')
-            elif video_u8:
-              _lib.check(lib.tapir_ingest_frames(_ptr(video), n * f, vh, vw, 0, 0, vh, vw,
-                                                 _ptr(frames_src), h, w, stream),
-                         'tapir_ingest_frames')
-            else:
-              _lib.check(lib.tapir_bilinear_resize(_ptr(video), n * f, vh, vw, 3,
-                                                   _ptr(frames_src), h, w, stream),
-                         'tapir_bilinear_resize')
-        if h % 8 != 0 or w % 8 != 0:
-          raise ValueError('Image resolution must be a multiple of 8.')
+        frames = video  # align_corners=False resize to the same size is the identity
+        if (h, w) != (vh, vw):
+          frames = torch.empty(n, f, h, w, 3, dtype=torch.float32, device=dev)
+          _lib.resample_frames(video, frames)
         curr_resolution = resolution
         shape_hw = (h, w)
-        nf = n * f
-        latent = torch.empty(n, f, h // 8, w // 8, self.lowres_dim, dtype=torch.float32, device=dev)
-        hires = torch.empty(n, f, h // 4, w // 4, self.highres_dim, dtype=torch.float32, device=dev)
-        src_yuv = frames_src is video and yuv
-        flat_src = None if src_yuv else frames_src.view(nf, h, w, 3)
-        flat_lo = latent.view(nf, h // 8, w // 8, self.lowres_dim)
-        flat_hi = hires.view(nf, h // 4, w // 4, self.highres_dim)
-        # frames are independent in the backbone (InstanceNorm per frame, LayerNorm per
-        # pixel), so the frame-chunk size only bounds the workspace; the reference's
-        # feature_extractor_chunk_size (:346-360) has the same role.
-        chunk = max(1, _MAX_BACKBONE_PIXELS // (h * w))
-        chunk = min(chunk, nf)
-        nbytes = lib.tapir_backbone_workspace_bytes(chunk, h, w, int(self._has_extra), self._planes)
-        ws = self._workspace('backbone', nbytes, dev)
-        ev = None
-        if hires_ready_events is not None:
-          ev = torch.cuda.Event()
-          ev.record(torch.cuda.current_stream(dev))  # materialises the CUDA event handle
-          hires_ready_events.append((hires, ev))
-        streamed = host_src is not None and frames_src is video
-        if streamed:
-          main = torch.cuda.current_stream(dev)
-          cs = self._copy_stream(dev)
-          cs.wait_stream(main)  # the staging buffer's previous owner is done
-          host_flat = host_src.view(nf, h, w, 3)
-        for s0 in range(0, nf, chunk):
-          c = min(chunk, nf - s0)
-          last = s0 + c >= nf
-          if streamed:
-            # sub-chunks of >= ~4 MB (each costs ~70 us of host time: copy, event, stem launch),
-            # at most _H2D_SUBCHUNKS per pass
-            nsub = max(1, min(_H2D_SUBCHUNKS, (c * h * w * 3 * flat_src.element_size()) >> 22))
-            sub = max(1, -(-c // nsub))
-            for a in range(s0, s0 + c, sub):
-              b = min(a + sub, s0 + c)
-              with torch.cuda.stream(cs):
-                flat_src[a:b].copy_(host_flat[a:b], non_blocking=True)
-                arrived = torch.cuda.Event()
-                arrived.record(cs)
-              main.wait_event(arrived)
-              _lib.check(lib.tapir_backbone_stem(
-                  ctypes.byref(pk['backbone']), _ptr(flat_src[a:]), int(video_u8), c, h, w, a - s0,
-                  b - a, _ptr(ws), ws.numel(), stream), 'tapir_backbone_stem')
-          ready = ctypes.c_void_p(ev.cuda_event) if (ev is not None and last) else None
-          if src_yuv:
-            desc = video.c_struct(s0)
-            _lib.check(lib.tapir_backbone_forward_yuv420(
-                ctypes.byref(pk['backbone']), ctypes.byref(desc), c, _ptr(flat_lo[s0:]),
-                _ptr(flat_hi[s0:]), _ptr(ws), ws.numel(), ready, stream),
-                       'tapir_backbone_forward_yuv420')
-            continue
-          _lib.check(lib.tapir_backbone_forward_ex(
-              ctypes.byref(pk['backbone']), None if streamed else _ptr(flat_src[s0:]),
-              int(flat_src.dtype == torch.uint8),
-              c, h, w, _ptr(flat_lo[s0:]), _ptr(flat_hi[s0:]), _ptr(ws), ws.numel(),
-              ready, stream),
-                     'tapir_backbone_forward')
-        if streamed:
+        latent, hires = self._backbone_pass(pk, frames, host_src if frames is video else None,
+                                            hires_ready_events, dev)
+        if frames is video:
           host_src = None  # the whole clip is on the device now (later passes resize from it)
       feature_grid.append(latent)
       hires_feats.append(hires)
       resize_im_shape.append(torch.Size(shape_hw))
     return FeatureGrids(tuple(feature_grid), tuple(hires_feats), tuple(resize_im_shape))
+
+  def _backbone_pass(self, pk, frames, host_src, hires_ready_events, dev):
+    """Feature grids (lowres, hires) of every frame of `frames` ([B, T, h, w, 3] on the device, or
+    a YUV clip).  host_src: the host clip whose copy `frames` is yet to be, streamed in here."""
+    n, f, h, w, _ = frames.shape
+    nf = n * f
+    latent = torch.empty(n, f, h // 8, w // 8, self.lowres_dim, dtype=torch.float32, device=dev)
+    hires = torch.empty(n, f, h // 4, w // 4, self.highres_dim, dtype=torch.float32, device=dev)
+    src = frames if isinstance(frames, live.YUV420Frames) else frames.view(nf, h, w, 3)
+    flat_lo = latent.view(nf, h // 8, w // 8, self.lowres_dim)
+    flat_hi = hires.view(nf, h // 4, w // 4, self.highres_dim)
+    # frames are independent in the backbone (InstanceNorm per frame, LayerNorm per
+    # pixel), so the frame-chunk size only bounds the workspace; the reference's
+    # feature_extractor_chunk_size (:346-360) has the same role.
+    chunk = min(max(1, _MAX_BACKBONE_PIXELS // (h * w)), nf)
+    ws = self._workspace('backbone', _lib.backbone_workspace_bytes(pk['backbone'], chunk, h, w), dev)
+    ev = None
+    if hires_ready_events is not None:
+      ev = torch.cuda.Event()
+      ev.record(torch.cuda.current_stream(dev))  # materialises the CUDA event handle
+      hires_ready_events.append((hires, ev))
+    streamed = host_src is not None
+    if streamed:
+      main = torch.cuda.current_stream(dev)
+      cs = self._copy_stream(dev)
+      cs.wait_stream(main)  # the staging buffer's previous owner is done
+      host_flat = host_src.view(nf, h, w, 3)
+    for s0 in range(0, nf, chunk):
+      c = min(chunk, nf - s0)
+      if streamed:
+        # sub-chunks of >= ~4 MB (each costs ~70 us of host time: copy, event, stem launch),
+        # at most _H2D_SUBCHUNKS per pass
+        nsub = max(1, min(_H2D_SUBCHUNKS, (c * h * w * 3 * src.element_size()) >> 22))
+        sub = max(1, -(-c // nsub))
+        for a in range(s0, s0 + c, sub):
+          b = min(a + sub, s0 + c)
+          with torch.cuda.stream(cs):
+            src[a:b].copy_(host_flat[a:b], non_blocking=True)
+            arrived = torch.cuda.Event()
+            arrived.record(cs)
+          main.wait_event(arrived)
+          _lib.backbone_stem(pk['backbone'], src[a:b], c, a - s0, ws)
+      _lib.backbone_forward(pk['backbone'], src, flat_lo[s0:s0 + c], flat_hi[s0:s0 + c], ws,
+                            ev if s0 + c >= nf else None, frame0=s0, stem_done=streamed)
+    return latent, hires
 
   @_on_model_device
   def get_query_features(
@@ -553,9 +432,6 @@ class TAPIR(nn.Module):
     if feature_grids is None:
       feature_grids = self.get_feature_grids(video, is_training, refinement_resolutions)
     dev = self._device_check(query_points)
-    lib = _lib.load()
-    stream = self._stream(dev)
-    shape = video.shape
     qp = query_points.to(torch.float32).contiguous()
     b, nq, _ = qp.shape
     query_feats, hires_query_feats = [], []
@@ -567,12 +443,9 @@ class TAPIR(nn.Module):
         outs = []
         for grid in (lo_grid, hi_grid):
           grid = grid.contiguous()
-          _, t, gh, gw, c = grid.shape
-          out = torch.empty(b, nq, c, dtype=torch.float32, device=dev)
+          out = torch.empty(b, nq, grid.shape[-1], dtype=torch.float32, device=dev)
           for bi in range(b if nq > 0 else 0):
-            _lib.check(lib.tapir_sample_query_features(
-                _ptr(grid[bi]), t, gh, gw, c, _ptr(qp[bi]), nq, int(shape[1]), int(shape[2]),
-                int(shape[3]), _ptr(out[bi]), stream), 'tapir_sample_query_features')
+            _lib.sample_query_features(grid[bi], qp[bi], video.shape[1:4], out[bi])
           outs.append(out)
         cache[key] = outs
       query_feats.append(cache[key][0])
@@ -607,18 +480,12 @@ class TAPIR(nn.Module):
     """
     del is_training, query_chunk_size
     dev = self._device_check(query_features.lowres[0])
-    lib = _lib.load()
     pk = self._pack()
-    stream = self._stream(dev)
-    P = self._planes
-    ih, iw = self.initial_resolution
-    vh, vw = int(video_size[0]), int(video_size[1])
+    video_hw = (int(video_size[0]), int(video_size[1]))
     num_levels_total = len(feature_grids.lowres)
     num_iters = self.num_pips_iter * (num_levels_total - 1)
     B, N = query_features.lowres[0].shape[:2]
     T = feature_grids.lowres[0].shape[1]
-    L = self.pyramid_level + 2
-    kin = pk['mixer_in']
     nb = pk['num_blocks']
 
     def new(*shape, dtype=torch.float32):
@@ -627,6 +494,83 @@ class TAPIR(nn.Module):
     occ_out = [new(B, N, T) for _ in range(num_iters + 1)]
     expd_out = [new(B, N, T) for _ in range(num_iters + 1)]
     trk_out = [new(B, N, T, 2) for _ in range(num_iters + 1)]
+    new_ctx = self._new_causal_context(causal_context, get_causal_context, causal_context_out,
+                                       num_iters, nb, B, N, T, dev)
+    write_ctx = get_causal_context and causal_context is not None
+    am_out = None
+    if self.capture_stage_a_argmax:
+      am_out = torch.empty(B, N, T, dtype=torch.int32, device=dev)
+      self.last_stage_a_argmax = am_out
+    out = dict(occlusion=occ_out, tracks=trk_out, expected_dist=expd_out)
+    if get_causal_context:
+      out['causal_context'] = new_ctx
+    if N == 0 or T == 0:
+      # nothing to track (the reference fails in torch.cat on an empty chunk list,
+      # tapir_model.py:556-559; returning correctly shaped empty tensors is the useful behaviour)
+      return out
+
+    # pooled pyramid levels: once per resolution level over all B*T frames (the reference
+    # recomputes them every iteration of every chunk, tapir_model.py:519-527); each is the 2x2
+    # average of the one before it
+    pooled = {}
+    for level in range(1, num_levels_total):
+      g = feature_grids.lowres[level].contiguous()
+      outs = []
+      for _ in range(self.pyramid_level):
+        _, t, gh, gw, c = g.shape
+        pooled_g = new(B, t, gh // 2, gw // 2, c)
+        _lib.pool_pyramid(g, pooled_g)
+        outs.append(pooled_g)
+        g = pooled_g
+      pooled[level] = outs
+
+    for b0, b1, sl in _groups(B, N, T):
+      bs = slice(b0, b1)
+      nq = (b1 - b0) * (sl.stop - sl.start)  # queries of the group, flattened over its clips
+      # every [bs, sl] slice below is contiguous: either whole clips or a query chunk of one clip
+      occ0, expd0 = occ_out[0][bs, sl], expd_out[0][bs, sl]  # outputs are written in place
+      qp = query_points_in_video[bs, sl] if query_points_in_video is not None else None
+      pos = self._stage_a(pk, feature_grids.lowres[0][bs].contiguous(),
+                          query_features.lowres[0][bs, sl].contiguous(), qp, video_hw, occ0, expd0,
+                          trk_out[0][bs, sl], am_out[bs, sl] if am_out is not None else None, dev)
+
+      # ---- refinement iterations
+      x_planes = new(self._planes, nq * T, pk['mixer_in'], dtype=torch.bfloat16)
+      res = new(nq, T, 388)
+      feats = [new(nq, T, 384), new(nq, T, 384)]
+      mws = self._workspace('mixer', _lib.mixer_workspace_bytes(x_planes), dev)
+      occ, expd = occ0, expd0
+      fsrc = None  # the previous iteration's features; None: start from the query features
+      for it in range(num_iters):
+        level = it // self.num_pips_iter + 1
+        levels = ([feature_grids.hires[level][bs].contiguous(),
+                   feature_grids.lowres[level][bs].contiguous()] + [g[bs] for g in pooled[level]])
+        if fsrc is not None:
+          feat = (fsrc[..., :128], fsrc[..., 128:])
+        else:
+          feat = tuple(q[bs, sl].contiguous().view(nq, 1, -1).expand(nq, T, -1)
+                       for q in (query_features.hires[level], query_features.lowres[level]))
+        ctx = [None] * 4
+        if causal_context is not None:
+          ctx[:2] = _ctx_lists(causal_context[it], nb, (bs, sl),
+                               lambda t: t.to(device=dev, dtype=torch.float32).contiguous())
+        if write_ctx:
+          ctx[2:] = _ctx_lists(new_ctx[it], nb, (bs, sl))
+        fdst = feats[1] if fsrc is feats[0] else feats[0]
+        occ_n, expd_n = occ_out[it + 1][bs, sl], expd_out[it + 1][bs, sl]
+        self._refine(pk, levels, pos, occ, expd, feat, x_planes, res, ctx, mws, occ_n, expd_n,
+                     fdst, trk_out[it + 1][bs, sl], feature_grids.resolutions[level], video_hw)
+        fsrc, occ, expd = fdst, occ_n, expd_n
+        if (it + 1) % self.num_pips_iter == 0:
+          # level boundary (tapir_model.py:549-552): features restart from the query,
+          # occlusion / expected_dist revert to the stage-A estimate, positions carry over
+          fsrc, occ, expd = None, occ0, expd0
+    return out
+
+  def _new_causal_context(self, causal_context, get_causal_context, causal_context_out, num_iters,
+                          nb, B, N, T, dev):
+    """Checks the causal context arguments of estimate_trajectories; returns the list of dicts the
+    call fills with the new context (None when get_causal_context is False)."""
     # Causal context bookkeeping follows nets.py:143-176: a block only produces a new context
     # when it was GIVEN one (new_causal_context is filled inside `if causal_context is not None`),
     # so get_causal_context without causal_context yields empty dicts, exactly like the reference.
@@ -642,7 +586,6 @@ class TAPIR(nn.Module):
             if tuple(d[key].shape) != (B, N, 2, width):
               raise ValueError(f'causal_context[{key}] has shape {tuple(d[key].shape)}, expected '
                                f'{(B, N, 2, width)}')
-    new_ctx = None
     if get_causal_context and causal_context is not None and causal_context_out is not None:
       if T != 1 and any(causal_context_out[it][k].data_ptr() == causal_context[it][k].data_ptr()
                         for it in range(num_iters) for k in causal_context[it]):
@@ -652,170 +595,49 @@ class TAPIR(nn.Module):
         for k, v in d.items():
           if not (v.is_contiguous() and v.dtype == torch.float32 and v.device == dev):
             raise ValueError(f'causal_context_out[{k}] must be a contiguous fp32 tensor on {dev}')
-    elif get_causal_context:
-      new_ctx = [{} for _ in range(num_iters)]
-      if causal_context is not None:
-        for d in new_ctx:
-          for i in range(nb):
-            d[f'block_{i}_causal_1'] = new(B, N, 2, 512)
-            d[f'block_{i}_causal_2'] = new(B, N, 2, 2048)
-    write_ctx = get_causal_context and causal_context is not None
-    am_out = None
-    if self.capture_stage_a_argmax:
-      am_out = torch.empty(B, N, T, dtype=torch.int32, device=dev)
-      self.last_stage_a_argmax = am_out
-    if N == 0 or T == 0:
-      # nothing to track (the reference fails in torch.cat on an empty chunk list,
-      # tapir_model.py:556-559; returning correctly shaped empty tensors is the useful behaviour)
-      out = dict(occlusion=occ_out, tracks=trk_out, expected_dist=expd_out)
-      if get_causal_context:
-        out['causal_context'] = new_ctx
-      return out
+      return new_ctx
+    if not get_causal_context:
+      return None
+    new_ctx = [{} for _ in range(num_iters)]
+    if causal_context is not None:
+      for d in new_ctx:
+        for i in range(nb):
+          d[f'block_{i}_causal_1'] = torch.empty(B, N, 2, 512, dtype=torch.float32, device=dev)
+          d[f'block_{i}_causal_2'] = torch.empty(B, N, 2, 2048, dtype=torch.float32, device=dev)
+    return new_ctx
 
-    # pooled pyramid levels: once per resolution level over all B*T frames (the reference
-    # recomputes them every iteration of every chunk, tapir_model.py:519-527); each is the 2x2
-    # average of the one before it
-    pooled = {}
-    for level in range(1, num_levels_total):
-      g = feature_grids.lowres[level].contiguous()
-      outs = []
-      for _ in range(self.pyramid_level):
-        _, t, gh, gw, c = g.shape
-        out = new(B, t, gh // 2, gw // 2, c)
-        _lib.check(lib.tapir_pool_pyramid(_ptr(g), B * t, gh, gw, c, _ptr(out), stream),
-                   'tapir_pool_pyramid')
-        outs.append(out)
-        g = out
-      pooled[level] = outs
+  def _stage_a(self, pk, grid, qfeat, query_points, video_hw, occ, expd, tracks, argmax, dev):
+    """Stage A for one group of clips: the global cost volume and the track / occlusion head of
+    qfeat [G, n, 256] against grid [G, T, h, w, 256].  Writes occ, expd [G, n, T], tracks
+    [G, n, T, 2] (video pixels) and, unless None, argmax; returns the positions [G, n, T, 2] in
+    initial-resolution pixels."""
+    G, n = qfeat.shape[:2]
+    T = grid.shape[1]
+    ih, iw = self.initial_resolution
+    vh, vw = video_hw
+    qp = None
+    if query_points is not None:
+      qp = query_points.to(torch.float32)
+      # utils.convert_grid_coordinates (coords * out / in), tapir_model.py:488-493
+      qp = (qp * self._const([T, ih, iw], dev) / self._const([T, vh, vw], dev)).contiguous()
+    pos = torch.empty(G, n, T, 2, dtype=torch.float32, device=dev)
+    ws = self._workspace('cost_volume', _lib.cost_volume_workspace_bytes(qfeat, grid), dev)
+    _lib.cost_volume_tracks(pk['head'], qfeat, grid, qp, self.softmax_temperature, (ih, iw), pos,
+                            occ, expd, argmax, ws)
+    # train2orig (tapir_model.py:435-441)
+    torch.div(pos * self._const([vw, vh], dev), self._const([iw, ih], dev), out=tracks)
+    return pos
 
-    for b0, b1, sl in _groups(B, N, T):
-      G = b1 - b0
-      n = sl.stop - sl.start
-      nq = G * n  # queries of the group, flattened over its clips
-      rows = nq * T
-      bs = slice(b0, b1)
-      # every [bs, sl] slice below is contiguous: either whole clips or a query chunk of one clip
-      # ---- stage A: global cost volume + track / occlusion head
-      grid0 = feature_grids.lowres[0][bs].contiguous()
-      _, _, gh0, gw0, c0 = grid0.shape
-      qf0 = query_features.lowres[0][bs, sl].contiguous()
-      qp = None
-      if query_points_in_video is not None:
-        qp = query_points_in_video[bs, sl].to(torch.float32)
-        # utils.convert_grid_coordinates (coords * out / in), tapir_model.py:488-493
-        qp = (qp * self._const([T, ih, iw], dev) / self._const([T, vh, vw], dev)).contiguous()
-      pos = new(nq, T, 2)
-      # outputs are written in place
-      occ0, expd0 = occ_out[0][bs, sl], expd_out[0][bs, sl]
-      nbytes = lib.tapir_cost_volume_batched_workspace_bytes(G, n, T, gh0, gw0, c0)
-      ws = self._workspace('cost_volume', nbytes, dev)
-      _lib.check(lib.tapir_cost_volume_tracks_batched(
-          ctypes.byref(pk['head']), _ptr(qf0), _ptr(grid0), G, n, T, gh0, gw0, c0, _ptr(qp),
-          float(self.softmax_temperature), ih, iw, _ptr(pos), _ptr(occ0), _ptr(expd0),
-          _ptr(am_out[bs, sl]) if am_out is not None else None,
-          _ptr(ws), ws.numel(), stream), 'tapir_cost_volume_tracks_batched')
-      # train2orig (tapir_model.py:435-441)
-      torch.div(pos.view(G, n, T, 2) * self._const([vw, vh], dev), self._const([iw, ih], dev),
-                out=trk_out[0][bs, sl])
-
-      # ---- refinement iterations
-      x_planes = new(P, rows, kin, dtype=torch.bfloat16)
-      res = new(rows, 388)
-      feats = [new(nq, T, 384), new(nq, T, 384)]
-      occ, expd = occ0, expd0
-      nbytes = lib.tapir_mixer_workspace_bytes(rows, P)
-      mws = self._workspace('mixer', nbytes, dev)
-      have_feats = False
-      cur = 0
-      for it in range(num_iters):
-        level = it // self.num_pips_iter + 1
-        hires_g = feature_grids.hires[level][bs].contiguous()
-        lowres_g = feature_grids.lowres[level][bs].contiguous()
-        ca = _lib.CorrArgs()
-        grids = [hires_g, lowres_g] + [g[bs] for g in pooled[level]]
-        for li, g in enumerate(grids):
-          ca.levels[li].grid = g.data_ptr()
-          ca.levels[li].h, ca.levels[li].w, ca.levels[li].C = g.shape[2], g.shape[3], g.shape[4]
-        ca.num_levels = L
-        ca.num_points, ca.num_frames = n, T
-        ca.init_h, ca.init_w = ih, iw
-        ca.planes = P
-        ca.pos, ca.occ, ca.expd = pos.data_ptr(), occ.data_ptr(), expd.data_ptr()
-        if have_feats:
-          fsrc = feats[cur]
-          fh = (fsrc.data_ptr(), T * 384, 384)
-          fl = (fsrc.data_ptr() + 128 * 4, T * 384, 384)
-        else:
-          qh = query_features.hires[level][bs, sl].contiguous()
-          ql = query_features.lowres[level][bs, sl].contiguous()
-          fh = (qh.data_ptr(), 128, 0)
-          fl = (ql.data_ptr(), 256, 0)
-        ca.feat_hi, ca.feat_hi_stride_n, ca.feat_hi_stride_t = fh
-        ca.feat_lo, ca.feat_lo_stride_n, ca.feat_lo_stride_t = fl
-        ca.out_planes = x_planes.data_ptr()
-        ca.out_plane_stride = rows * kin
-        ca.ld = kin
-        _lib.check(lib.tapir_local_corr_batched(ctypes.byref(ca), G, stream),
-                   'tapir_local_corr_batched')
-
-        io = _lib.MixerIO()
-        io.x_planes = x_planes.data_ptr()
-        io.x_plane_stride = rows * kin
-        io.ldx = kin
-        io.num_points, io.num_frames = nq, T
-        io.causal = int(self.use_casual_conv)
-        holders = []
-        if causal_context is not None:
-          c1 = [causal_context[it][f'block_{i}_causal_1'][bs, sl].to(device=dev, dtype=torch.float32).contiguous()
-                for i in range(nb)]
-          c2 = [causal_context[it][f'block_{i}_causal_2'][bs, sl].to(device=dev, dtype=torch.float32).contiguous()
-                for i in range(nb)]
-          holders += c1 + c2
-          io.ctx1_in = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in c1])
-          io.ctx2_in = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in c2])
-        o1 = o2 = None
-        if write_ctx:
-          o1 = [new_ctx[it][f'block_{i}_causal_1'][bs, sl] for i in range(nb)]
-          o2 = [new_ctx[it][f'block_{i}_causal_2'][bs, sl] for i in range(nb)]
-          io.ctx1_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o1])
-          io.ctx2_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o2])
-        io.out = res.data_ptr()
-        io.ldo = 388
-        _lib.check(lib.tapir_mixer_forward(ctypes.byref(pk['mixer']), ctypes.byref(io), _ptr(mws),
-                                           mws.numel(), stream), 'tapir_mixer_forward')
-
-        ua = _lib.UpdateArgs()
-        ua.res, ua.ld_res = res.data_ptr(), 388
-        ua.num_points, ua.num_frames = nq, T
-        ua.init_h, ua.init_w = ih, iw
-        rh, rw = feature_grids.resolutions[level]
-        ua.resize_h, ua.resize_w = int(rh), int(rw)
-        ua.video_h, ua.video_w = vh, vw
-        ua.feat_hi, ua.feat_hi_stride_n, ua.feat_hi_stride_t = fh
-        ua.feat_lo, ua.feat_lo_stride_n, ua.feat_lo_stride_t = fl
-        nxt = 1 - cur if have_feats else cur
-        trk_i = trk_out[it + 1][bs, sl]
-        occ_n, expd_n = occ_out[it + 1][bs, sl], expd_out[it + 1][bs, sl]
-        ua.pos = pos.data_ptr()
-        ua.occ_in, ua.expd_in = occ.data_ptr(), expd.data_ptr()
-        ua.occ_out, ua.expd_out = occ_n.data_ptr(), expd_n.data_ptr()
-        ua.feat_out = feats[nxt].data_ptr()
-        ua.tracks_out = trk_i.data_ptr()
-        _lib.check(lib.tapir_refine_update(ctypes.byref(ua), stream), 'tapir_refine_update')
-        cur = nxt
-        have_feats = True
-        occ, expd = occ_n, expd_n
-        if (it + 1) % self.num_pips_iter == 0:
-          # level boundary (tapir_model.py:549-552): features restart from the query,
-          # occlusion / expected_dist revert to the stage-A estimate, positions carry over
-          have_feats = False
-          occ, expd = occ0, expd0
-        del holders
-
-    out = dict(occlusion=occ_out, tracks=trk_out, expected_dist=expd_out)
-    if get_causal_context:
-      out['causal_context'] = new_ctx
-    return out
+  def _refine(self, pk, levels, pos, occ, expd, feat, x_planes, res, ctx, mws, occ_out, expd_out,
+              feat_out, tracks_out, resize_hw, video_hw):
+    """One refinement iteration (the refine_pips call, reference tapir_model.py:529-542): local correlation around pos
+    over the pyramid `levels`, the mixer, and the update of pos (in place), occlusion, expected
+    distance, features (hi, lo views `feat` -> feat_out) and tracks.  ctx: the mixer's causal
+    context lists (ctx1_in, ctx2_in, ctx1_out, ctx2_out), None where absent."""
+    _lib.local_corr(levels, pos, occ, expd, *feat, x_planes, self.initial_resolution)
+    _lib.mixer_forward(pk['mixer'], x_planes, res, self.use_casual_conv, *ctx, mws)
+    _lib.refine_update(res, pos, occ, expd, *feat, occ_out, expd_out, feat_out, tracks_out,
+                       self.initial_resolution, resize_hw, video_hw)
 
   def construct_initial_causal_state(self, num_points, num_resolutions=1):
     """Reference tapir_model.py:763-772 (the same dict object repeated, CPU tensors)."""

@@ -15,7 +15,6 @@ colormap divides by zero there); points with a NaN coordinate are not painted (u
 reference); the frame count of `frames` and `point_tracks` must agree.
 """
 import colorsys
-import ctypes
 import random
 
 import numpy as np
@@ -119,15 +118,10 @@ def paint_point_track(frames, point_tracks, visibles, colormap=None):
   vis_d = (_to_device(vis, dev) != 0).contiguous()   # bool: one byte, 0 / 1
   colors_d = _to_device(colors, dev)
   out = torch.empty_like(frames_d)
-  lib = _lib.load()
   with torch.cuda.device(dev):
-    ws_bytes = int(lib.tapir_paint_point_track_workspace_bytes(T, N))
-    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
-    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(lib.tapir_paint_point_track(
-        frames_d.data_ptr(), T, H, W, tracks_d.data_ptr(), int(tracks_d.dtype == torch.float64),
-        vis_d.data_ptr(), N, colors_d.data_ptr(), out.data_ptr(), ws.data_ptr(), ws_bytes, stream),
-        'tapir_paint_point_track')
+    ws_bytes = int(_lib.load().tapir_paint_point_track_workspace_bytes(T, N))
+    ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)[:ws_bytes]
+    _lib.paint_point_track(frames_d, tracks_d, vis_d, colors_d, out, ws)
   return out if on_device else out.cpu().numpy()
 
 

@@ -38,24 +38,31 @@ def record(name, **vals):
   print(f'[report] {name}: ' + ', '.join(f'{k}={v}' for k, v in REPORT[name].items()))
 
 
-def ptr(t):
-  return ctypes.c_void_p(t.data_ptr()) if t is not None else None
-
-
-def stream():
-  return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+ptr, stream = _lib.ptr, _lib.stream
 
 
 def split(x, planes, kpad=None):
   """fp32 [rows, cols] (cuda) -> bf16 planes [P, rows, kpad] through tapir_split_planes."""
-  lib = _lib.load()
   x = x.contiguous().float()
   rows, cols = x.shape
-  kpad = kpad or cols
-  out = torch.empty(planes, rows, kpad, dtype=torch.bfloat16, device=x.device)
-  _lib.check(lib.tapir_split_planes(ptr(x), cols, ptr(out), kpad, rows * kpad, rows, cols, kpad,
-                                    planes, stream()), 'split')
+  out = torch.empty(planes, rows, kpad or cols, dtype=torch.bfloat16, device=x.device)
+  _lib.split_planes(x, out)
   return out
+
+
+GUARD = 16  # elements of NaN fill before and after every guarded() output
+
+
+def guarded(n, dtype=torch.float32):
+  """A NaN-filled buffer (-7 for integers) with GUARD elements either side of an n-element body."""
+  fill = -7 if not dtype.is_floating_point else float('nan')
+  buf = torch.full((n + 2 * GUARD,), fill, dtype=dtype, device='cuda')
+  return buf, buf[GUARD:GUARD + n]
+
+
+def guards_intact(buf):
+  g = torch.cat([buf[:GUARD], buf[-GUARD:]])
+  return bool(torch.isnan(g.float()).all()) if buf.dtype.is_floating_point else bool((g == -7).all())
 
 
 def planes_matmul_fp64(a_pl, b_pl):

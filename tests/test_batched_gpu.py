@@ -21,25 +21,12 @@ from tests.test_stages_gpu import get_model  # noqa: E402
 
 TRACK_TOL = 1e-3
 LOGIT_TOL = 1e-4
-GUARD = 16  # elements of NaN fill before and after every output
 
 
 def _unit(*shape, seed):
   g = torch.Generator().manual_seed(seed)
   x = torch.randn(*shape, generator=g)
   return x / x.norm(dim=-1, keepdim=True)
-
-
-def _guarded(n, dtype=torch.float32):
-  """A NaN-filled buffer (-7 for integers) with GUARD elements either side of an n-element body."""
-  fill = -7 if not dtype.is_floating_point else float('nan')
-  buf = torch.full((n + 2 * GUARD,), fill, dtype=dtype, device='cuda')
-  return buf, buf[GUARD:GUARD + n]
-
-
-def _guards_intact(buf):
-  g = torch.cat([buf[:GUARD], buf[-GUARD:]])
-  return bool(torch.isnan(g.float()).all()) if buf.dtype.is_floating_point else bool((g == -7).all())
 
 
 # ------------------------------------------------------------------------- entry points
@@ -63,16 +50,13 @@ def test_cost_volume_batched_equals_per_clip(B, N, T, gh, gw):
   outs = {}
   for name, per, dt in (('pts', 2, torch.float32), ('occ', 1, torch.float32), ('expd', 1, torch.float32),
                         ('am', 1, torch.int32)):
-    outs[name] = _guarded(B * N * T * per, dt)
-  nbytes = lib.tapir_cost_volume_batched_workspace_bytes(B, N, T, gh, gw, C)
-  ws = torch.empty(nbytes, dtype=torch.uint8, device='cuda')
-  _lib.check(lib.tapir_cost_volume_tracks_batched(
-      ctypes.byref(pk['head']), U.ptr(qf), U.ptr(grid), B, N, T, gh, gw, C, U.ptr(qp), 20.0, ih, iw,
-      U.ptr(outs['pts'][1]), U.ptr(outs['occ'][1]), U.ptr(outs['expd'][1]), U.ptr(outs['am'][1]),
-      U.ptr(ws), nbytes, U.stream()), 'cost_volume_batched')
+    outs[name] = U.guarded(B * N * T * per, dt)
+  ws = torch.empty(_lib.cost_volume_workspace_bytes(qf, grid), dtype=torch.uint8, device='cuda')
+  _lib.cost_volume_tracks(pk['head'], qf, grid, qp, 20.0, (ih, iw), outs['pts'][1].view(B, N, T, 2),
+                          *(outs[k][1].view(B, N, T) for k in ('occ', 'expd', 'am')), ws)
   torch.cuda.synchronize()
   for name, (buf, _) in outs.items():
-    assert _guards_intact(buf), f'{name}: bytes outside the output were written'
+    assert U.guards_intact(buf), f'{name}: bytes outside the output were written'
   nb1 = lib.tapir_cost_volume_workspace_bytes(N, T, gh, gw, C)
   ws1 = torch.empty(nb1, dtype=torch.uint8, device='cuda')
   for b in range(B):
@@ -110,42 +94,28 @@ def test_local_corr_batched_equals_per_clip(B, N, T, pyr, gh, gw):
   per_row = pyr == 2  # per-(query, frame) features (refinement) or per-query ones (first iteration)
   if per_row:
     feat = torch.randn(B, N, T, 384, generator=g).cuda()
-    fh = lambda f: (f.data_ptr(), T * 384, 384)  # noqa: E731
-    fl = lambda f: (f.data_ptr() + 512, T * 384, 384)  # noqa: E731
-    feats = (feat,)
+    feats = lambda bsl, nq: (feat[bsl].view(nq, T, 384)[..., :128], feat[bsl].view(nq, T, 384)[..., 128:])  # noqa: E731
   else:
     qh = torch.randn(B, N, 128, generator=g).cuda()
     ql = torch.randn(B, N, 256, generator=g).cuda()
-    feats = (qh, ql)
+    feats = lambda bsl, nq: tuple(q[bsl].reshape(nq, 1, -1).expand(nq, T, -1) for q in (qh, ql))  # noqa: E731
 
   def args(bsl, nclips):
-    ca = _lib.CorrArgs()
-    for i, gd in enumerate(grids):
-      ca.levels[i].grid = gd[bsl].data_ptr()
-      ca.levels[i].h, ca.levels[i].w, ca.levels[i].C = gd.shape[2], gd.shape[3], gd.shape[4]
-    ca.num_levels, ca.num_points, ca.num_frames = L, N, T
-    ca.init_h, ca.init_w, ca.planes = 256, 256, P
-    ca.pos, ca.occ, ca.expd = pos[bsl].data_ptr(), occ[bsl].data_ptr(), expd[bsl].data_ptr()
-    if per_row:
-      ca.feat_hi, ca.feat_hi_stride_n, ca.feat_hi_stride_t = fh(feats[0][bsl])
-      ca.feat_lo, ca.feat_lo_stride_n, ca.feat_lo_stride_t = fl(feats[0][bsl])
-    else:
-      ca.feat_hi, ca.feat_hi_stride_n, ca.feat_hi_stride_t = feats[0][bsl].data_ptr(), 128, 0
-      ca.feat_lo, ca.feat_lo_stride_n, ca.feat_lo_stride_t = feats[1][bsl].data_ptr(), 256, 0
     rows = nclips * N * T
-    buf, body = _guarded(P * rows * kpad, torch.bfloat16)
-    ca.out_planes, ca.out_plane_stride, ca.ld = body.data_ptr(), rows * kpad, kpad
+    buf, body = U.guarded(P * rows * kpad, torch.bfloat16)
+    ca = _lib.corr_args([gd[bsl] for gd in grids], pos[bsl], occ[bsl], expd[bsl], *feats(bsl, nclips * N),
+                        body.view(P, rows, kpad), (256, 256))
     return ca, buf, body.view(P, nclips, N * T, kpad)
 
   ca, buf, got = args(slice(0, B), B)
   _lib.check(lib.tapir_local_corr_batched(ctypes.byref(ca), B, U.stream()), 'local_corr_batched')
   torch.cuda.synchronize()
-  assert _guards_intact(buf)
+  assert U.guards_intact(buf)
   for b in range(B):
     ca1, buf1, want = args(slice(b, b + 1), 1)
     _lib.check(lib.tapir_local_corr(ctypes.byref(ca1), U.stream()), 'local_corr')
     torch.cuda.synchronize()
-    assert _guards_intact(buf1)
+    assert U.guards_intact(buf1)
     assert torch.equal(got[:, b].view(torch.int16), want[:, 0].view(torch.int16)), f'clip {b}'
 
 

@@ -35,34 +35,22 @@ def run_local_corr(levels, pos, feats, init_hw, batch, P, ld, per_row):
   read at stride 384 with the low half 128 floats in (what the refinement loop passes after its
   first iteration); else per-query vectors at stride_t 0 (feats must then be constant over t)."""
   Q, T, _ = pos.shape
-  N = Q // batch
-  L = len(levels)
   rows = Q * T
   grids = [g.cuda().contiguous() for g in levels]
-  ca = _lib.CorrArgs()
-  for i, g in enumerate(grids):
-    ca.levels[i].grid = g.data_ptr()
-    ca.levels[i].h, ca.levels[i].w, ca.levels[i].C = g.shape[2], g.shape[3], g.shape[4]
-  ca.num_levels, ca.num_points, ca.num_frames = L, N, T
-  ca.init_h, ca.init_w = init_hw
-  ca.planes = P
   occ = torch.randn(Q, T, generator=torch.Generator().manual_seed(rows))
   expd = torch.randn(Q, T, generator=torch.Generator().manual_seed(rows + 1))
   pos_d, occ_d, expd_d = pos.cuda().contiguous(), occ.cuda(), expd.cuda()
-  ca.pos, ca.occ, ca.expd = pos_d.data_ptr(), occ_d.data_ptr(), expd_d.data_ptr()
   if per_row:
     fr = torch.cat(feats, -1).cuda().contiguous()
-    ca.feat_hi, ca.feat_hi_stride_n, ca.feat_hi_stride_t = fr.data_ptr(), T * 384, 384
-    ca.feat_lo, ca.feat_lo_stride_n, ca.feat_lo_stride_t = fr.data_ptr() + 128 * 4, T * 384, 384
+    fh, fl = fr[..., :128], fr[..., 128:]
   else:
-    fh, fl = feats[0][:, 0].cuda().contiguous(), feats[1][:, 0].cuda().contiguous()
-    ca.feat_hi, ca.feat_hi_stride_n, ca.feat_hi_stride_t = fh.data_ptr(), 128, 0
-    ca.feat_lo, ca.feat_lo_stride_n, ca.feat_lo_stride_t = fl.data_ptr(), 256, 0
+    fh, fl = (f[:, 0].cuda().contiguous()[:, None].expand(Q, T, -1) for f in feats)
   out = Guarded(rows * ld, torch.bfloat16, P)
-  ca.out_planes, ca.out_plane_stride, ca.ld = out.ptr().value, out.stride, ld
-  fn = (lambda: lib().tapir_local_corr(ctypes.byref(ca), U.stream())) if batch == 1 else (
-      lambda: lib().tapir_local_corr_batched(ctypes.byref(ca), batch, U.stream()))
-  _lib.check(fn(), 'tapir_local_corr')
+  args = (grids, pos_d, occ_d, expd_d, fh, fl, out.body().view(P, rows, ld), init_hw)
+  if batch == 1:
+    _lib.check(lib().tapir_local_corr(ctypes.byref(_lib.corr_args(*args)), U.stream()), 'tapir_local_corr')
+  else:
+    _lib.local_corr(*args)
   torch.cuda.synchronize()
   assert out.guards_untouched()
   return out.body().cpu().view(P, Q, T, ld), occ, expd
@@ -155,28 +143,18 @@ def test_refine_update_bit_exact(n, T, per_row, alias, tracks, init, resize, vid
     feat = feat[:, :1].expand(n, T, 384).contiguous()
   d = lambda t: t.cuda().contiguous()  # noqa: E731
   res_d, pos_d, occ_d, expd_d = d(res), d(pos), d(occ), d(expd)
-  ua = _lib.UpdateArgs()
-  ua.res, ua.ld_res, ua.num_points, ua.num_frames = res_d.data_ptr(), ld, n, T
-  ua.init_h, ua.init_w = init
-  ua.resize_h, ua.resize_w = resize
-  ua.video_h, ua.video_w = video
   if per_row:
     fd = d(feat)
-    ua.feat_hi, ua.feat_hi_stride_n, ua.feat_hi_stride_t = fd.data_ptr(), T * 384, 384
-    ua.feat_lo, ua.feat_lo_stride_n, ua.feat_lo_stride_t = fd.data_ptr() + 512, T * 384, 384
+    fh, fl = fd[..., :128], fd[..., 128:]
   else:
-    fh, fl = d(feat[:, 0, :128]), d(feat[:, 0, 128:])
-    ua.feat_hi, ua.feat_hi_stride_n, ua.feat_hi_stride_t = fh.data_ptr(), 128, 0
-    ua.feat_lo, ua.feat_lo_stride_n, ua.feat_lo_stride_t = fl.data_ptr(), 256, 0
+    fh, fl = (d(f)[:, None].expand(n, T, -1) for f in (feat[:, 0, :128], feat[:, 0, 128:]))
   rows = n * T
   occ_o = None if alias else Guarded(rows, torch.float32)
   expd_o, feat_o = Guarded(rows, torch.float32), Guarded(rows * 384, torch.float32)
   trk = Guarded(rows * 2, torch.float32) if tracks else None
-  ua.pos, ua.occ_in, ua.expd_in = pos_d.data_ptr(), occ_d.data_ptr(), expd_d.data_ptr()
-  ua.occ_out = occ_d.data_ptr() if alias else occ_o.ptr().value
-  ua.expd_out, ua.feat_out = expd_o.ptr().value, feat_o.ptr().value
-  ua.tracks_out = trk.ptr().value if tracks else None
-  _lib.check(lib().tapir_refine_update(ctypes.byref(ua), U.stream()), 'tapir_refine_update')
+  _lib.refine_update(res_d, pos_d, occ_d, expd_d, fh, fl, occ_d if alias else occ_o.body().view(n, T),
+                     expd_o.body().view(n, T), feat_o.body().view(n, T, 384),
+                     trk.body().view(n, T, 2) if tracks else None, init, resize, video)
   torch.cuda.synchronize()
   for o in (occ_o, expd_o, feat_o, trk):
     assert o is None or o.guards_untouched()

@@ -16,8 +16,8 @@ does).  Per map:
   * logits within 1e-4 (synthetic head) or 1e-4 * max(1, |ref|) (identity head, large logits).
 
 Output buffers carry NaN guards."""
-import ctypes
 import functools
+import math
 from typing import NamedTuple
 
 import numpy as np
@@ -32,7 +32,6 @@ from tapnet_b200 import _lib  # noqa: E402
 from tests import gpu_util as U  # noqa: E402
 from tests import stage_a_designs as D  # noqa: E402
 
-GUARD = 16   # elements of NaN fill before and after every output
 STRIDE = 8   # initial-resolution pixels per cost-map cell
 SAMPLE_TOL = 1e-5
 
@@ -162,37 +161,21 @@ def _head_weights(kind):
   return _HEADS[kind][0]
 
 
-def _guarded(n, dtype=torch.float32):
-  fill = -7 if not dtype.is_floating_point else float('nan')
-  buf = torch.full((n + 2 * GUARD,), fill, dtype=dtype, device='cuda')
-  return buf, buf[GUARD:GUARD + n]
-
-
-def _guards_intact(buf):
-  g = torch.cat([buf[:GUARD], buf[-GUARD:]])
-  return bool(torch.isnan(g.float()).all()) if buf.dtype.is_floating_point else bool((g == -7).all())
-
-
 def _run(case):
   """Runs one case through tapir_cost_volume_tracks_batched; returns CPU outputs."""
-  lib = _lib.load()
   inp = _inputs(case.B, case.N, case.T, case.gh, case.gw, case.source)
   B, N, T, gh, gw = case.B, case.N, case.T, case.gh, case.gw
   grid, qf = inp['grid'].cuda().contiguous(), inp['qf'].cuda().contiguous()
   qp = inp['qp'].cuda().contiguous() if case.queries else None
-  outs = {name: _guarded(B * N * T * per, dt) for name, per, dt in
-          (('pts', 2, torch.float32), ('occ', 1, torch.float32), ('expd', 1, torch.float32),
-           ('am', 1, torch.int32))}
-  nbytes = lib.tapir_cost_volume_batched_workspace_bytes(B, N, T, gh, gw, D.C)
-  ws = torch.empty(nbytes, dtype=torch.uint8, device='cuda')
-  _lib.check(lib.tapir_cost_volume_tracks_batched(
-      ctypes.byref(_head_weights(case.kind)), U.ptr(qf), U.ptr(grid), B, N, T, gh, gw, D.C, U.ptr(qp),
-      case.temp, gh * STRIDE, gw * STRIDE, U.ptr(outs['pts'][1]), U.ptr(outs['occ'][1]),
-      U.ptr(outs['expd'][1]), U.ptr(outs['am'][1]), U.ptr(ws), nbytes, U.stream()), case.id)
+  shape = {'pts': (B, N, T, 2), 'occ': (B, N, T), 'expd': (B, N, T), 'am': (B, N, T)}
+  outs = {name: U.guarded(math.prod(shape[name]), dt) for name, dt in
+          (('pts', torch.float32), ('occ', torch.float32), ('expd', torch.float32), ('am', torch.int32))}
+  ws = torch.empty(_lib.cost_volume_workspace_bytes(qf, grid), dtype=torch.uint8, device='cuda')
+  _lib.cost_volume_tracks(_head_weights(case.kind), qf, grid, qp, case.temp, (gh * STRIDE, gw * STRIDE),
+                          *(body.view(shape[name]) for name, (_, body) in outs.items()), ws)
   torch.cuda.synchronize()
   for name, (buf, _) in outs.items():
-    assert _guards_intact(buf), f'{case.id}: {name}: bytes outside the output were written'
-  shape = {'pts': (B, N, T, 2), 'occ': (B, N, T), 'expd': (B, N, T), 'am': (B, N, T)}
+    assert U.guards_intact(buf), f'{case.id}: {name}: bytes outside the output were written'
   return {name: body.view(shape[name]).cpu() for name, (_, body) in outs.items()}
 
 
@@ -328,11 +311,11 @@ def test_sample_query_features(case, C):
   grid = grid / grid.norm(dim=-1, keepdim=True)  # unit features, as the backbone's grids
   q, n_special = _sample_queries(N, vT, vH, vW, gh, gw, seed=C + N)
   grid_d, q_d = grid.cuda().contiguous(), q.cuda().contiguous()
-  buf, out = _guarded(N * C)
+  buf, out = U.guarded(N * C)
   _lib.check(lib.tapir_sample_query_features(U.ptr(grid_d), T, gh, gw, C, U.ptr(q_d), N, vT, vH, vW,
                                              U.ptr(out), U.stream()), 'sample_query_features')
   torch.cuda.synchronize()
-  assert _guards_intact(buf), 'bytes outside the output were written'
+  assert U.guards_intact(buf), 'bytes outside the output were written'
   ref = _sample_reference(grid.double(), q, vT, vH, vW)
   err = (out.view(N, C).cpu().double() - ref).abs()
   U.record(f'sample_query_T{T}_{gh}x{gw}_C{C}_N{N}', err=err.max(), err_special=err[:n_special].max())

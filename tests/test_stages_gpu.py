@@ -1,5 +1,4 @@
 """Per-stage parity of the CUDA path (through the C ABI) against the CPU oracle."""
-import ctypes
 import os
 
 import numpy as np
@@ -90,6 +89,14 @@ def test_query_features():
   assert e1 < 1e-5 and e2 < 1e-5
 
 
+def _run_cost_volume(model, qf, grid, qp, init_hw, *outs):
+  """Stage A of one clip (qf [1, N, 256], grid [1, T, h, w, 256], qp [1, N, 3] on the CPU) into the
+  [N, T, ...] CUDA outputs (points, occ, expd, argmax)."""
+  qf, grid, qp = (t.cuda().contiguous() for t in (qf, grid, qp))
+  ws = torch.empty(_lib.cost_volume_workspace_bytes(qf, grid), dtype=torch.uint8, device='cuda')
+  _lib.cost_volume_tracks(model._pack()['head'], qf, grid, qp, 20.0, init_hw, *(o[None] for o in outs), ws)
+
+
 def _unit_grid(T, h, w, c, seed):
   g = torch.Generator().manual_seed(seed)
   x = torch.randn(1, T, h, w, c, generator=g)
@@ -98,8 +105,6 @@ def _unit_grid(T, h, w, c, seed):
 
 def test_cost_volume_tracks():
   model, sd, cfg = get_model()
-  lib = _lib.load()
-  pk = model._pack()
   T, N = 6, 40
   grid = _unit_grid(T, 32, 32, 256, 5)
   # queries = features sampled from the grid itself (+ noise) so heat maps are peaked
@@ -115,12 +120,7 @@ def test_cost_volume_tracks():
   o_occ = torch.empty(N, T, device=dev)
   o_exp = torch.empty(N, T, device=dev)
   o_am = torch.empty(N, T, dtype=torch.int32, device=dev)
-  nbytes = lib.tapir_cost_volume_workspace_bytes(N, T, 32, 32, 256)
-  ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-  qf_d, grid_d, qp_d = qf[0].cuda().contiguous(), grid[0].cuda().contiguous(), qp[0].cuda().contiguous()
-  _lib.check(lib.tapir_cost_volume_tracks(
-      ctypes.byref(pk['head']), U.ptr(qf_d), U.ptr(grid_d), N, T, 32, 32, 256, U.ptr(qp_d), 20.0, 256,
-      256, U.ptr(o_pts), U.ptr(o_occ), U.ptr(o_exp), U.ptr(o_am), U.ptr(ws), nbytes, U.stream()), 'cv')
+  _run_cost_volume(model, qf, grid, qp, (256, 256), o_pts, o_occ, o_exp, o_am)
   torch.cuda.synchronize()
   agree = (o_am.cpu().long() == am[0]).float().mean().item()
   e_p, e_o, e_e = maxerr(o_pts, pts[0]), maxerr(o_occ, occ[0]), maxerr(o_exp, expd[0])
@@ -135,8 +135,6 @@ def test_cost_volume_tracks_any_map_size(shape):
   32 x 32 and the generic-size head runs.  Same checks as the 32 x 32 case."""
   gh, gw = shape
   model, sd, cfg = get_model()
-  lib = _lib.load()
-  pk = model._pack()
   T, N = 3, 20
   grid = _unit_grid(T, gh, gw, 256, 15)
   g = torch.Generator().manual_seed(16)
@@ -153,12 +151,7 @@ def test_cost_volume_tracks_any_map_size(shape):
   o_occ = torch.empty(N, T, device=dev)
   o_exp = torch.empty(N, T, device=dev)
   o_am = torch.empty(N, T, dtype=torch.int32, device=dev)
-  nbytes = lib.tapir_cost_volume_workspace_bytes(N, T, gh, gw, 256)
-  ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-  qf_d, grid_d, qp_d = qf[0].cuda().contiguous(), grid[0].cuda().contiguous(), qp[0].cuda().contiguous()
-  _lib.check(lib.tapir_cost_volume_tracks(
-      ctypes.byref(pk['head']), U.ptr(qf_d), U.ptr(grid_d), N, T, gh, gw, 256, U.ptr(qp_d), 20.0, ih,
-      iw, U.ptr(o_pts), U.ptr(o_occ), U.ptr(o_exp), U.ptr(o_am), U.ptr(ws), nbytes, U.stream()), 'cv')
+  _run_cost_volume(model, qf, grid, qp, (ih, iw), o_pts, o_occ, o_exp, o_am)
   torch.cuda.synchronize()
   agree = (o_am.cpu().long() == am[0]).float().mean().item()
   e_p, e_o, e_e = maxerr(o_pts, pts[0]), maxerr(o_occ, occ[0]), maxerr(o_exp, expd[0])
@@ -169,39 +162,24 @@ def test_cost_volume_tracks_any_map_size(shape):
 
 def _run_mixer(model, x, causal, ctx=None, get_ctx=False, in_place=False):
   """in_place: the context output pointers are the context input buffers (the streaming call)."""
-  lib = _lib.load()
   pk = model._pack()
   n, T, cin = x.shape
-  kpad = pk['mixer_in']
-  P = model._planes
   dev = 'cuda'
-  xp = U.split(x.reshape(n * T, cin).cuda(), P, kpad)
-  out = torch.empty(n * T, 388, device=dev)
-  io = _lib.MixerIO()
-  io.x_planes, io.x_plane_stride, io.ldx = xp.data_ptr(), n * T * kpad, kpad
-  io.num_points, io.num_frames, io.causal = n, T, int(causal)
+  xp = U.split(x.reshape(n * T, cin).cuda(), model._planes, pk['mixer_in'])
+  out = torch.empty(n, T, 388, device=dev)
   nb = pk['num_blocks']
-  keep = []
+  c1 = c2 = o1 = o2 = None
   if ctx is not None:
     c1 = [ctx[f'block_{i}_causal_1'].cuda().contiguous() for i in range(nb)]
     c2 = [ctx[f'block_{i}_causal_2'].cuda().contiguous() for i in range(nb)]
-    keep += c1 + c2
-    io.ctx1_in = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in c1])
-    io.ctx2_in = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in c2])
-  o1 = o2 = None
   if get_ctx:
     if in_place:
       o1, o2 = c1, c2
     else:
       o1 = [torch.empty(n, 2, 512, device=dev) for _ in range(nb)]
       o2 = [torch.empty(n, 2, 2048, device=dev) for _ in range(nb)]
-    io.ctx1_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o1])
-    io.ctx2_out = (ctypes.c_void_p * nb)(*[t.data_ptr() for t in o2])
-  io.out, io.ldo = out.data_ptr(), 388
-  nbytes = lib.tapir_mixer_workspace_bytes(n * T, P)
-  ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-  _lib.check(lib.tapir_mixer_forward(ctypes.byref(pk['mixer']), ctypes.byref(io), U.ptr(ws), nbytes,
-                                     U.stream()), 'mixer')
+  ws = torch.empty(_lib.mixer_workspace_bytes(xp), dtype=torch.uint8, device=dev)
+  _lib.mixer_forward(pk['mixer'], xp, out, causal, c1, c2, o1, o2, ws)
   torch.cuda.synchronize()
   new_ctx = None
   if get_ctx:
@@ -364,26 +342,18 @@ def test_mixer_query_permutation_is_bit_exact(T, n):
 
 
 def test_refine_update():
-  lib = _lib.load()
   g = torch.Generator().manual_seed(11)
   n, T = 5, 4
   res = torch.randn(n * T, 388, generator=g)
   pos = torch.rand(n, T, 2, generator=g) * 256
   occ, expd = torch.randn(n, T, generator=g), torch.randn(n, T, generator=g)
   feat = torch.randn(n, T, 384, generator=g)
-  ua = _lib.UpdateArgs()
   d = lambda t: t.cuda().contiguous()  # noqa: E731
   res_d, pos_d, occ_d, expd_d, feat_d = d(res), d(pos), d(occ), d(expd), d(feat)
   occ_o, expd_o = torch.empty_like(occ_d), torch.empty_like(expd_d)
   feat_o, trk = torch.empty_like(feat_d), torch.empty_like(pos_d)
-  ua.res, ua.ld_res, ua.num_points, ua.num_frames = res_d.data_ptr(), 388, n, T
-  ua.init_h, ua.init_w, ua.resize_h, ua.resize_w, ua.video_h, ua.video_w = 256, 256, 320, 384, 480, 640
-  ua.feat_hi, ua.feat_hi_stride_n, ua.feat_hi_stride_t = feat_d.data_ptr(), T * 384, 384
-  ua.feat_lo, ua.feat_lo_stride_n, ua.feat_lo_stride_t = feat_d.data_ptr() + 512, T * 384, 384
-  ua.pos, ua.occ_in, ua.expd_in = pos_d.data_ptr(), occ_d.data_ptr(), expd_d.data_ptr()
-  ua.occ_out, ua.expd_out, ua.feat_out, ua.tracks_out = (occ_o.data_ptr(), expd_o.data_ptr(),
-                                                          feat_o.data_ptr(), trk.data_ptr())
-  _lib.check(lib.tapir_refine_update(ctypes.byref(ua), U.stream()), 'update')
+  _lib.refine_update(res_d.view(n, T, 388), pos_d, occ_d, expd_d, feat_d[..., :128], feat_d[..., 128:], occ_o,
+                     expd_o, feat_o, trk, (256, 256), (320, 384), (480, 640))
   torch.cuda.synchronize()
   r = res.reshape(n, T, 388)
   new_pos = pos + r[..., :2] * torch.tensor([256.0, 256.0]) / torch.tensor([384.0, 320.0])
