@@ -19,8 +19,8 @@ run() {  # name, env, pytest args...
 }
 for t in $TIERS; do
   case $t in
-    gemm_simt)   run gemm_simt "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py -k simt ;;
-    gemm_tc)     run gemm_tc "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_schedule_gpu.py -k tc ;;
+    gemm_simt)   run gemm_simt "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_exact_gpu.py -k simt ;;
+    gemm_tc)     run gemm_tc "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_schedule_gpu.py tests/test_gemm_exact_gpu.py -k tc ;;
     stages_simt) run stages_simt "TAPIR_B200_GEMM=simt" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py tests/test_backbone_ops_gpu.py tests/test_refine_ops_gpu.py ;;
     stages_tc)   run stages_tc "X=1" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py tests/test_backbone_ops_gpu.py tests/test_refine_ops_gpu.py ;;
     e2e_simt)    run e2e_simt "TAPIR_B200_GEMM=simt" tests/test_end_to_end_gpu.py ;;
@@ -29,8 +29,8 @@ for t in $TIERS; do
     io)          run io "X=1" tests/test_io_gpu.py ;;
     yuv)         run yuv "X=1" tests/test_yuv_gpu.py ;;
     bulk)        run bulk "X=1" tests/test_bulk_gpu.py ;;
-    no_halo)     run no_halo "TAPIR_B200_CONV_HALO=0" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_stages_gpu.py tests/test_end_to_end_gpu.py ;;
-    no_splitk)   run no_splitk "TAPIR_B200_SPLITK=0" tests/test_gemm_variants_gpu.py tests/test_stages_gpu.py tests/test_properties_gpu.py tests/test_batched_gpu.py "tests/test_backbone_ops_gpu.py::test_backbone_vs_fp64_oracle" "tests/test_backbone_ops_gpu.py::test_backbone_frame_chunks_are_independent" ;;
+    no_halo)     run no_halo "TAPIR_B200_CONV_HALO=0" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_exact_gpu.py tests/test_stages_gpu.py tests/test_end_to_end_gpu.py ;;
+    no_splitk)   run no_splitk "TAPIR_B200_SPLITK=0" tests/test_gemm_variants_gpu.py tests/test_gemm_exact_gpu.py tests/test_stages_gpu.py tests/test_properties_gpu.py tests/test_batched_gpu.py "tests/test_backbone_ops_gpu.py::test_backbone_vs_fp64_oracle" "tests/test_backbone_ops_gpu.py::test_backbone_frame_chunks_are_independent" ;;
     all)         run all "X=1" tests ;;
   esac
 done

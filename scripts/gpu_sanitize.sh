@@ -30,3 +30,9 @@ timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
     -k "not production_shape and not streaming_shape and not clip_shape and not pl1_1024 and not n1001 and not n801 and not n700" \
     2>&1 | grep -E '^=========|passed|failed' | tail -n 25
 echo "sanitizer refine_ops memcheck rc=${PIPESTATUS[0]}"
+# then every GEMM epilogue path (whole-tile and general epilogues, split-K reduction, halo
+# convolution, SIMT) and tapir_split_planes, with NaN-filled padding around every output
+timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
+    python -m pytest -q -m gpu -p no:cacheprovider tests/test_gemm_exact_gpu.py \
+    2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+echo "sanitizer gemm_exact memcheck rc=${PIPESTATUS[0]}"
