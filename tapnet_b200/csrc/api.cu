@@ -61,21 +61,13 @@ int tapir_gemm_ex(const void* a_planes, int32_t lda, int64_t a_plane_stride, con
   TAPIR_CHECK_ARG(M > 0 && M < (1ll << 31), "tapir_gemm: M out of range");
   TAPIR_CHECK_ARG((reinterpret_cast<uintptr_t>(splitk_workspace) & 15) == 0,
                   "tapir_gemm: split-K workspace must be 16-byte aligned");
-  GemmArgs g;
+  GemmArgs g = gemm_args(*b);
   g.mode = conv3x3 ? kGemmConv3x3 : kGemmPlain;
-  g.planes = b->planes;
   g.M = (int)M;
-  g.N = b->N;
-  g.K = b->K;
   g.a = static_cast<const __nv_bfloat16*>(a_planes);
   g.lda = lda;
   g.a_plane_stride = a_plane_stride;
   g.frames = frames; g.H = H; g.W = W; g.C = C;
-  g.b = static_cast<const __nv_bfloat16*>(b->w);
-  g.ldb = b->K;
-  g.b_plane_stride = (long long)b->N * b->K;
-  g.bias = b->bias;
-  g.k_logical = b->k_logical;
   g.residual = residual; g.ldr = ldr;
   g.act = act_gelu ? 1 : 0;
   g.out_f32 = out_f32; g.ldo = ldo;

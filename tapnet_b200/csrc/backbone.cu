@@ -568,16 +568,10 @@ size_t plan_backbone(Arena& a, int frames, int H, int W, int extra, int planes, 
   return a.off;
 }
 
-GemmArgs linear_args(const tapir_linear& l) {
-  GemmArgs g;
-  g.planes = l.planes;
-  g.N = l.N;
-  g.K = l.K;
-  g.b = static_cast<const __nv_bfloat16*>(l.w);
-  g.ldb = l.K;
-  g.b_plane_stride = (long long)l.N * l.K;
-  g.bias = l.bias;
-  g.k_logical = l.k_logical;
+// An ExtraConv GEMM: split-K only for single-frame (streaming) passes, see GemmArgs::allow_splitk.
+GemmArgs extra_conv_args(const tapir_linear& l, const BackbonePlan& bp, int frames) {
+  GemmArgs g = gemm_args(l);
+  g.splitk_ws = bp.splitk; g.splitk_ws_bytes = kBackboneSplitKBytes; g.allow_splitk = (frames == 1);
   return g;
 }
 
@@ -654,7 +648,7 @@ int backbone_forward(const tapir_backbone_weights* w, const void* video, int vid
                                         bp.act, bp.act_plane, P, fuse ? bp.sums[cur ^ 1] : nullptr, b.cout, s));
     const float* shortcut = x;
     if (b.has_proj) {
-      GemmArgs g = linear_args(b.proj);
+      GemmArgs g = gemm_args(b.proj);
       g.tag = "backbone.proj";
       g.M = (int)m_out;
       g.out_f32 = shortcut_buf;
@@ -669,7 +663,7 @@ int backbone_forward(const tapir_backbone_weights* w, const void* video, int vid
       shortcut = shortcut_buf;
     }
     {
-      GemmArgs g = linear_args(b.conv0);
+      GemmArgs g = gemm_args(b.conv0);
       g.tag = "backbone.conv";
       g.M = (int)m_out;
       g.out_f32 = hbuf;
@@ -694,7 +688,7 @@ int backbone_forward(const tapir_backbone_weights* w, const void* video, int vid
                                         b.cout, bp.act, bp.act_plane, P, next_stats ? bp.sums[cur] : nullptr,
                                         b.cout, s));
     {
-      GemmArgs g = linear_args(b.conv1);
+      GemmArgs g = gemm_args(b.conv1);
       g.tag = "backbone.conv";
       g.mode = kGemmConv3x3;
       g.M = (int)m_out;
@@ -723,9 +717,8 @@ int backbone_forward(const tapir_backbone_weights* w, const void* video, int vid
     float* xnew = bp.buf[(xi + 2) & 3];
     TAPIR_RETURN_IF(layernorm_split(x, m, 256, b.ln_w, b.ln_b, y, bp.act, bp.act_plane, P, s));
     {
-      GemmArgs g = linear_args(b.conv);
+      GemmArgs g = extra_conv_args(b.conv, bp, frames);
       g.tag = "backbone.extra_conv";
-      g.splitk_ws = bp.splitk; g.splitk_ws_bytes = kBackboneSplitKBytes; g.allow_splitk = (frames == 1);
       g.mode = kGemmConv3x3;
       g.M = (int)m;
       g.a = bp.act; g.a_plane_stride = bp.act_plane;
@@ -735,9 +728,8 @@ int backbone_forward(const tapir_backbone_weights* w, const void* video, int vid
       TAPIR_RETURN_IF(gemm(g, s));
     }
     {
-      GemmArgs g = linear_args(b.conv1);
+      GemmArgs g = extra_conv_args(b.conv1, bp, frames);
       g.tag = "backbone.extra_conv";
-      g.splitk_ws = bp.splitk; g.splitk_ws_bytes = kBackboneSplitKBytes; g.allow_splitk = (frames == 1);
       g.mode = kGemmConv3x3;
       g.M = (int)m;
       g.a = bp.col; g.a_plane_stride = bp.col_plane;

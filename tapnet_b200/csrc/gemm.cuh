@@ -11,6 +11,7 @@
 // in fp32 (tapir_model.py:665,720; nets.py convs/linears), and its parity budget (1e-3 px,
 // 1e-4 logits) cannot be met by single-pass bf16 (tests/test_precision_policy.py).
 #pragma once
+#include "../../include/tapir_b200.h"
 #include "common.cuh"
 
 namespace tapir {
@@ -61,6 +62,20 @@ struct GemmArgs {
   int k_logical = 0;        // un-padded K for FLOP accounting (0 = K)
   const char* tag = nullptr;  // profiling class name
 };
+
+// A GEMM with weight `l` as its B operand and bias; the caller sets A, M and the outputs.
+inline GemmArgs gemm_args(const tapir_linear& l) {
+  GemmArgs g;
+  g.planes = l.planes;
+  g.N = l.N;
+  g.K = l.K;
+  g.b = static_cast<const __nv_bfloat16*>(l.w);
+  g.ldb = l.K;
+  g.b_plane_stride = (long long)l.N * l.K;
+  g.bias = l.bias;
+  g.k_logical = l.k_logical;
+  return g;
+}
 
 int validate_gemm_args(const GemmArgs& g);
 // wgmma + TMA implementation (the product path).

@@ -318,35 +318,103 @@ __device__ __forceinline__ int decode_work(const TcParams& p, int w, int& bat, i
   return split;
 }
 
+// Position in a ring of STAGES stages: the stage, and the parity of its current fill.
+template <int STAGES>
+struct StageCursor {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void advance() {
+    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+  }
+};
+
+// The dynamic shared memory from its first 1024-byte boundary: the 128B swizzle of TMA and wgmma
+// repeats every 1024 B of absolute address.
+__device__ __forceinline__ uint8_t* aligned_smem(uint8_t* smem_raw) {
+  return smem_raw + ((1024u - (ptx::smem_u32(smem_raw) & 1023u)) & 1023u);
+}
+
+// Thread 0's set-up before the __syncthreads() that follows: the barriers of one or two stage
+// rings laid out one after the other at `bars`, each as full[stages] (one arrival: the producer's
+// expect_tx) then empty[stages] (`empty_arrivals` each), and a prefetch of the producer's maps.
+__device__ __forceinline__ void init_rings(uint64_t* bars, uint32_t empty_arrivals, const CUtensorMap* map_a,
+                                           const CUtensorMap* map_b, int stages0, int stages1 = 0) {
+  if (threadIdx.x != 0) return;
+  const int ring_stages[2] = {stages0, stages1};
+  for (const int stages : ring_stages) {
+    for (int s = 0; s < stages; ++s) {
+      ptx::mbar_init(&bars[s], 1);
+      ptx::mbar_init(&bars[stages + s], empty_arrivals);
+    }
+    bars += 2 * stages;
+  }
+  ptx::fence_barrier_init();
+  ptx::prefetch_tensormap(map_a);
+  ptx::prefetch_tensormap(map_b);
+}
+
+// The MMAs of one k-block, in the order of every kernel (plane pair (i, j), then k step), into
+// HALVES m64 accumulators (A rows 64 h on, 8 KB apart).  A plane i starts at a + i * a_plane with
+// its 8-row swizzle atoms `a_sbo` bytes apart; B plane j at b + j * b_plane.
+template <int BLOCK_N, int P, int HALVES>
+__device__ __forceinline__ void mma_k_block(float (&acc)[HALVES][BLOCK_N / 2], uint32_t a, uint32_t a_plane,
+                                            uint32_t a_sbo, uint32_t b, uint32_t b_plane, uint32_t accumulate) {
+#pragma unroll
+  for (int i = 0; i < P; ++i) {
+#pragma unroll
+    for (int j = 0; j < P - i; ++j) {
+      uint64_t adesc[HALVES];
+#pragma unroll
+      for (int h = 0; h < HALVES; ++h) adesc[h] = ptx::make_smem_desc_sw128(a + i * a_plane + h * 64 * 128, a_sbo);
+      const uint64_t bdesc = ptx::make_smem_desc_sw128(b + j * b_plane);
+#pragma unroll
+      for (int k = 0; k < kBlockK / kMmaK; ++k) {
+#pragma unroll
+        for (int h = 0; h < HALVES; ++h) wgmma_bf16<BLOCK_N>(acc[h], adesc[h] + 2 * k, bdesc + 2 * k, accumulate);
+        accumulate = 1u;
+      }
+    }
+  }
+}
+
+// One consumer k-block: waits for its stage to fill, issues its MMAs as one wgmma group, and
+// once the previous k-block's group has retired releases that k-block's stage (empty[prev]; none
+// before a tile's first k-block, prev < 0) with one arrival per warp.
+template <int BLOCK_N, int P, int HALVES>
+__device__ __forceinline__ void consume_k_block(float (&acc)[HALVES][BLOCK_N / 2], uint64_t* full, uint32_t parity,
+                                                const TcParams& p, int err_code, uint32_t a, uint32_t a_plane,
+                                                uint32_t a_sbo, uint32_t b, uint32_t b_plane, uint32_t accumulate,
+                                                uint64_t* empty, int prev, int lane) {
+  ptx::mbar_wait(full, parity, p.err, err_code);
+  ptx::wgmma_fence();
+  mma_k_block<BLOCK_N, P, HALVES>(acc, a, a_plane, a_sbo, b, b_plane, accumulate);
+  ptx::wgmma_commit();
+  // the previous k-block's MMAs have retired once at most this group is pending
+  ptx::wgmma_wait<1>();
+#pragma unroll
+  for (int h = 0; h < HALVES; ++h) ptx::reg_fence(acc[h]);
+  if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
+}
+
 // Shared-memory ring of both GEMM schedules: kStages stages of P A planes then P B planes, then the
-// full and empty mbarriers.  Initialised by thread 0 before the __syncthreads() that follows.
+// full and empty mbarriers.
 template <int BLOCK_N, int P>
 struct Ring {
   using Cfg = TcCfg<BLOCK_N, P>;
   uint8_t* smem;
   uint64_t* full_bar;
   uint64_t* empty_bar;
-  __device__ __forceinline__ Ring(uint8_t* smem_raw, const TcParams& p, uint32_t empty_arrivals) {
-    const uint32_t raw_addr = ptx::smem_u32(smem_raw);
-    smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-    full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes);
-    empty_bar = full_bar + Cfg::kStages;
-    if (threadIdx.x == 0) {
-      for (int s = 0; s < Cfg::kStages; ++s) {
-        ptx::mbar_init(&full_bar[s], 1);
-        ptx::mbar_init(&empty_bar[s], empty_arrivals);
-      }
-      ptx::fence_barrier_init();
-      ptx::prefetch_tensormap(&p.tmA);
-      ptx::prefetch_tensormap(&p.tmB);
-    }
+  __device__ __forceinline__ Ring(uint8_t* smem_raw, const TcParams& p, uint32_t empty_arrivals)
+      : smem(aligned_smem(smem_raw)),
+        full_bar(reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes)),
+        empty_bar(full_bar + Cfg::kStages) {
+    init_rings(full_bar, empty_arrivals, &p.tmA, &p.tmB, Cfg::kStages);
   }
 
   // TMA producer (one thread): the k-blocks of this CTA's work items, in order, into the ring.
   __device__ __forceinline__ void produce(const TcParams& p) const {
     const int num_work = p.num_m_tiles * p.num_n_tiles * p.split_k;
-    int stage = 0;
-    uint32_t phase = 0;
+    StageCursor<Cfg::kStages> cur;
     for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
       int bat, m_tile, n0, kb0, kb1;
       decode_work<BLOCK_N>(p, w, bat, m_tile, n0, kb0, kb1);
@@ -363,9 +431,9 @@ struct Ring {
         x0 = (r % p.tiles_x) * p.tileW;
       }
       for (int kb = kb0; kb < kb1; ++kb) {
-        ptx::mbar_wait(&empty_bar[stage], phase ^ 1u, p.err, 101);
-        ptx::mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-        uint8_t* sa = smem + stage * Cfg::kStageBytes;
+        ptx::mbar_wait(&empty_bar[cur.stage], cur.phase ^ 1u, p.err, 101);
+        ptx::mbar_arrive_expect_tx(&full_bar[cur.stage], Cfg::kStageBytes);
+        uint8_t* sa = smem + cur.stage * Cfg::kStageBytes;
         uint8_t* sb = sa + P * Cfg::kABytes;
         if (p.mode == kGemmConv3x3) {
           const int tap = kb / p.cblocks;
@@ -373,18 +441,18 @@ struct Ring {
           const int ky = tap / 3, kx = tap - ky * 3;
 #pragma unroll
           for (int pl = 0; pl < P; ++pl)
-            ptx::tma_load_5d(sa + pl * Cfg::kABytes, &p.tmA, &full_bar[stage], cb * kBlockK,
+            ptx::tma_load_5d(sa + pl * Cfg::kABytes, &p.tmA, &full_bar[cur.stage], cb * kBlockK,
                              x0 + kx - 1, y0 + ky - 1, frame, pl);
         } else {
 #pragma unroll
           for (int pl = 0; pl < P; ++pl)
-            ptx::tma_load_3d(sa + pl * Cfg::kABytes, &p.tmA, &full_bar[stage], kb * kBlockK,
+            ptx::tma_load_3d(sa + pl * Cfg::kABytes, &p.tmA, &full_bar[cur.stage], kb * kBlockK,
                              a_row0, pl);
         }
 #pragma unroll
         for (int pl = 0; pl < P; ++pl)
-          ptx::tma_load_3d(sb + pl * Cfg::kBBytes, &p.tmB, &full_bar[stage], kb * kBlockK, b_row0, pl);
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
+          ptx::tma_load_3d(sb + pl * Cfg::kBBytes, &p.tmB, &full_bar[cur.stage], kb * kBlockK, b_row0, pl);
+        cur.advance();
       }
     }
   }
@@ -398,9 +466,6 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
   using Cfg = TcCfg<BLOCK_N, P>;
   extern __shared__ uint8_t smem_raw[];
   const Ring<BLOCK_N, P> ring(smem_raw, p, kConsumerArrivals);
-  uint8_t* smem = ring.smem;
-  uint64_t* full_bar = ring.full_bar;
-  uint64_t* empty_bar = ring.empty_bar;
 
   const int wg = threadIdx.x >> 7;
   const int warp = (threadIdx.x >> 5) & 3;  // within the warpgroup
@@ -418,46 +483,25 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
   // -------------------------------------------------------------------- consumers
   const int cw = wg - 1;                        // rows [64 cw, 64 cw + 64) of the tile
   const uint32_t a_off = (uint32_t)cw * 64 * 128;  // their A rows: eight whole swizzle atoms
-  int stage = 0;
-  uint32_t phase = 0;
-  float acc[BLOCK_N / 2];
+  StageCursor<Cfg::kStages> cur;
+  float acc[1][BLOCK_N / 2];
   for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
     int bat, m_tile, n0, kb0, kb1;
     const int split = decode_work<BLOCK_N>(p, w, bat, m_tile, n0, kb0, kb1);
 #pragma unroll
-    for (int i = 0; i < BLOCK_N / 2; ++i) acc[i] = 0.f;
+    for (int i = 0; i < BLOCK_N / 2; ++i) acc[0][i] = 0.f;
     int prev = -1;
     for (int kb = kb0; kb < kb1; ++kb) {
-      ptx::mbar_wait(&full_bar[stage], phase, p.err, 103);
-      const uint32_t sa = ptx::smem_u32(smem + stage * Cfg::kStageBytes) + a_off;
-      const uint32_t sb = ptx::smem_u32(smem + stage * Cfg::kStageBytes) + P * Cfg::kABytes;
-      uint32_t accumulate = (kb > kb0) ? 1u : 0u;
-      ptx::wgmma_fence();
-#pragma unroll
-      for (int i = 0; i < P; ++i) {
-#pragma unroll
-        for (int j = 0; j < P - i; ++j) {
-          const uint64_t adesc = ptx::make_smem_desc_sw128(sa + i * Cfg::kABytes);
-          const uint64_t bdesc = ptx::make_smem_desc_sw128(sb + j * Cfg::kBBytes);
-#pragma unroll
-          for (int k = 0; k < kBlockK / kMmaK; ++k) {
-            wgmma_bf16<BLOCK_N>(acc, adesc + 2 * k, bdesc + 2 * k, accumulate);
-            accumulate = 1u;
-          }
-        }
-      }
-      ptx::wgmma_commit();
-      // the previous k-block's MMAs have retired once at most this group is pending
-      ptx::wgmma_wait<1>();
-      ptx::reg_fence(acc);
-      if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
+      const uint32_t sa = ptx::smem_u32(ring.smem + cur.stage * Cfg::kStageBytes);
+      consume_k_block<BLOCK_N, P, 1>(acc, &ring.full_bar[cur.stage], cur.phase, p, 103, sa + a_off, Cfg::kABytes,
+                                     1024, sa + P * Cfg::kABytes, Cfg::kBBytes, kb > kb0, ring.empty_bar, prev, lane);
+      prev = cur.stage;
+      cur.advance();
     }
     ptx::wgmma_wait<0>();
-    ptx::reg_fence(acc);
-    if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
-    tile_epilogue<BLOCK_N>(p, acc, m_tile, cw * 64, n0, warp, lane,
+    ptx::reg_fence(acc[0]);
+    if (prev >= 0 && lane == 0) ptx::mbar_arrive(&ring.empty_bar[prev]);
+    tile_epilogue<BLOCK_N>(p, acc[0], m_tile, cw * 64, n0, warp, lane,
                            split * p.split_stride + bat * p.out_batch_stride);
   }
 }
@@ -487,9 +531,6 @@ gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
   static_assert(P <= 2, "ping-pong: P = 3 stays cooperative");
   extern __shared__ uint8_t smem_raw[];
   const Ring<BLOCK_N, P> ring(smem_raw, p, 4);  // one arrive per warp of the reading warpgroup
-  uint8_t* smem = ring.smem;
-  uint64_t* full_bar = ring.full_bar;
-  uint64_t* empty_bar = ring.empty_bar;
 
   const int wg = threadIdx.x >> 7;
   const int warp = (threadIdx.x >> 5) & 3;
@@ -513,48 +554,25 @@ gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
     decode_work<BLOCK_N>(p, (int)blockIdx.x + t * (int)gridDim.x, bat, m_tile, n0, kb0, kb1);
     if (t > 0) ptx::named_bar_sync(kTurnBarrier + cw, 256);
     const long long pos = (long long)t * nkb;  // ring position of the tile's first k-block
-    int stage = (int)(pos % Cfg::kStages);
-    uint32_t phase = (uint32_t)(pos / Cfg::kStages) & 1u;
+    StageCursor<Cfg::kStages> cur{(int)(pos % Cfg::kStages), (uint32_t)(pos / Cfg::kStages) & 1u};
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) acc[h][i] = 0.f;
     int prev = -1;
     for (int kb = 0; kb < nkb; ++kb) {
-      ptx::mbar_wait(&full_bar[stage], phase, p.err, 104);
-      const uint32_t sa = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
-      const uint32_t sb = sa + P * Cfg::kABytes;
-      uint32_t accumulate = (kb > 0) ? 1u : 0u;
-      ptx::wgmma_fence();
-#pragma unroll
-      for (int i = 0; i < P; ++i) {
-#pragma unroll
-        for (int j = 0; j < P - i; ++j) {
-          const uint64_t adesc0 = ptx::make_smem_desc_sw128(sa + i * Cfg::kABytes);
-          const uint64_t adesc1 = ptx::make_smem_desc_sw128(sa + i * Cfg::kABytes + 64 * 128);
-          const uint64_t bdesc = ptx::make_smem_desc_sw128(sb + j * Cfg::kBBytes);
-#pragma unroll
-          for (int k = 0; k < kBlockK / kMmaK; ++k) {
-            wgmma_bf16<BLOCK_N>(acc[0], adesc0 + 2 * k, bdesc + 2 * k, accumulate);
-            wgmma_bf16<BLOCK_N>(acc[1], adesc1 + 2 * k, bdesc + 2 * k, accumulate);
-            accumulate = 1u;
-          }
-        }
-      }
-      ptx::wgmma_commit();
-      ptx::wgmma_wait<1>();
-      ptx::reg_fence(acc[0]);
-      ptx::reg_fence(acc[1]);
-      if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == Cfg::kStages) { stage = 0; phase ^= 1u; }
+      const uint32_t sa = ptx::smem_u32(ring.smem + cur.stage * Cfg::kStageBytes);
+      consume_k_block<BLOCK_N, P, 2>(acc, &ring.full_bar[cur.stage], cur.phase, p, 104, sa, Cfg::kABytes, 1024,
+                                     sa + P * Cfg::kABytes, Cfg::kBBytes, kb > 0, ring.empty_bar, prev, lane);
+      prev = cur.stage;
+      cur.advance();
     }
     // every MMA of this tile is issued: the other warpgroup's tile, if it has one, may start
     if (t + 1 < my_tiles) ptx::named_bar_arrive(kTurnBarrier + (1 - cw), 256);
     ptx::wgmma_wait<0>();
     ptx::reg_fence(acc[0]);
     ptx::reg_fence(acc[1]);
-    if (lane == 0) ptx::mbar_arrive(&empty_bar[prev]);
+    if (lane == 0) ptx::mbar_arrive(&ring.empty_bar[prev]);
     // one copy of the epilogue code for both halves: it runs while the other warpgroup's mainloop
     // executes from the same instruction cache
 #pragma unroll 1
@@ -582,13 +600,14 @@ constexpr int kHaloRowBytes = 2048;                        // 16 pixels x 128 B
 constexpr int kHaloPatchRows = kHaloTileH + 2;
 constexpr int kHaloPatchBytes = kHaloPatchRows * kHaloRowBytes;  // per plane
 constexpr int kHaloRowLoadBytes = (kHaloTileW + 2) * 128;  // what one TMA row load delivers
+constexpr int kHaloPatchStages = 2;
 constexpr int kHaloBStages = 4;
 constexpr int kHaloBBytes = 64 * 128;                      // per plane and tap
 template <int P>
 struct HaloCfg {
   static constexpr int kPatchStage = P * kHaloPatchBytes;
   static constexpr int kBStage = P * kHaloBBytes;
-  static constexpr int kSmemBytes = 1024 + 2 * kPatchStage + kHaloBStages * kBStage + kBarrierBytes;
+  static constexpr int kSmemBytes = 1024 + kHaloPatchStages * kPatchStage + kHaloBStages * kBStage + kBarrierBytes;
   static_assert(kSmemBytes <= kSmemLimit, "halo conv: shared memory");
 };
 
@@ -597,10 +616,9 @@ __global__ void __launch_bounds__(kThreads, 1)
 conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
   using Cfg = HaloCfg<P>;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = ptx::smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
-  uint8_t* patch = smem;                                   // [2][P][18][2048]
-  uint8_t* bring = smem + 2 * Cfg::kPatchStage;            // [4][P][64][128]
+  uint8_t* smem = aligned_smem(smem_raw);
+  uint8_t* patch = smem;                                           // [2][P][18][2048]
+  uint8_t* bring = smem + kHaloPatchStages * Cfg::kPatchStage;     // [4][P][64][128]
   uint64_t* bars = reinterpret_cast<uint64_t*>(bring + kHaloBStages * Cfg::kBStage);
   uint64_t* pfull = bars;                    // [2]
   uint64_t* pempty = bars + 2;               // [2]
@@ -610,88 +628,64 @@ conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
   const int wg = threadIdx.x >> 7;
   const int warp = (threadIdx.x >> 5) & 3;
   const int lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < 2; ++s) { ptx::mbar_init(&pfull[s], 1); ptx::mbar_init(&pempty[s], kConsumerArrivals); }
-    for (int s = 0; s < kHaloBStages; ++s) { ptx::mbar_init(&bfull[s], 1); ptx::mbar_init(&bempty[s], kConsumerArrivals); }
-    ptx::fence_barrier_init();
-    ptx::prefetch_tensormap(&p.tmPatch);
-    ptx::prefetch_tensormap(&p.tmB);
-  }
+  init_rings(bars, kConsumerArrivals, &p.tmPatch, &p.tmB, kHaloPatchStages, kHaloBStages);
   __syncthreads();
   const int num_work = p.num_m_tiles;
   const int per_frame = p.tiles_x * p.tiles_y;
 
   if (wg == 0) {
     if (threadIdx.x != 0) return;
-    int ps = 0, bs = 0;
-    uint32_t pphase = 0, bphase = 0;
+    StageCursor<kHaloPatchStages> pc;
+    StageCursor<kHaloBStages> bc;
     for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
       const int frame = w / per_frame;
       const int r = w - frame * per_frame;
       const int y0 = (r / p.tiles_x) * kHaloTileH, x0 = (r % p.tiles_x) * kHaloTileW;
-      ptx::mbar_wait(&pempty[ps], pphase ^ 1u, p.err, 401);
-      ptx::mbar_arrive_expect_tx(&pfull[ps], (uint32_t)(P * kHaloPatchRows * kHaloRowLoadBytes));
+      ptx::mbar_wait(&pempty[pc.stage], pc.phase ^ 1u, p.err, 401);
+      ptx::mbar_arrive_expect_tx(&pfull[pc.stage], (uint32_t)(P * kHaloPatchRows * kHaloRowLoadBytes));
       for (int pl = 0; pl < P; ++pl)
         for (int pr = 0; pr < kHaloPatchRows; ++pr)
-          ptx::tma_load_5d(patch + ps * Cfg::kPatchStage + pl * kHaloPatchBytes + pr * kHaloRowBytes, &p.tmPatch,
-                           &pfull[ps], 0, x0 - 1, y0 - 1 + pr, frame, pl);
-      if (++ps == 2) { ps = 0; pphase ^= 1u; }
+          ptx::tma_load_5d(patch + pc.stage * Cfg::kPatchStage + pl * kHaloPatchBytes + pr * kHaloRowBytes,
+                           &p.tmPatch, &pfull[pc.stage], 0, x0 - 1, y0 - 1 + pr, frame, pl);
+      pc.advance();
       for (int tap = 0; tap < 9; ++tap) {
-        ptx::mbar_wait(&bempty[bs], bphase ^ 1u, p.err, 402);
-        ptx::mbar_arrive_expect_tx(&bfull[bs], (uint32_t)Cfg::kBStage);
+        ptx::mbar_wait(&bempty[bc.stage], bc.phase ^ 1u, p.err, 402);
+        ptx::mbar_arrive_expect_tx(&bfull[bc.stage], (uint32_t)Cfg::kBStage);
 #pragma unroll
         for (int pl = 0; pl < P; ++pl)
-          ptx::tma_load_3d(bring + bs * Cfg::kBStage + pl * kHaloBBytes, &p.tmB, &bfull[bs], tap * kBlockK, 0, pl);
-        if (++bs == kHaloBStages) { bs = 0; bphase ^= 1u; }
+          ptx::tma_load_3d(bring + bc.stage * Cfg::kBStage + pl * kHaloBBytes, &p.tmB, &bfull[bc.stage],
+                           tap * kBlockK, 0, pl);
+        bc.advance();
       }
     }
     return;
   }
 
   const int cw = wg - 1;
-  int ps = 0, bs = 0;
-  uint32_t pphase = 0, bphase = 0;
-  float acc[32];
+  StageCursor<kHaloPatchStages> pc;
+  StageCursor<kHaloBStages> bc;
+  float acc[1][32];
   for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) acc[i] = 0.f;
-    ptx::mbar_wait(&pfull[ps], pphase, p.err, 404);
-    const uint32_t pbase = ptx::smem_u32(patch + ps * Cfg::kPatchStage) + (uint32_t)cw * 8 * kHaloRowBytes;
-    uint32_t accumulate = 0u;
+    for (int i = 0; i < 32; ++i) acc[0][i] = 0.f;
+    ptx::mbar_wait(&pfull[pc.stage], pc.phase, p.err, 404);
+    const uint32_t pbase = ptx::smem_u32(patch + pc.stage * Cfg::kPatchStage) + (uint32_t)cw * 8 * kHaloRowBytes;
     int prev = -1;
     for (int tap = 0; tap < 9; ++tap) {
       const int ky = tap / 3, kx = tap - ky * 3;
-      ptx::mbar_wait(&bfull[bs], bphase, p.err, 405);
-      const uint32_t sb = ptx::smem_u32(bring + bs * Cfg::kBStage);
-      ptx::wgmma_fence();
-#pragma unroll
-      for (int i = 0; i < P; ++i) {
-#pragma unroll
-        for (int j = 0; j < P - i; ++j) {
-          const uint64_t adesc = ptx::make_smem_desc_sw128(
-              pbase + i * kHaloPatchBytes + ky * kHaloRowBytes + kx * 128, kHaloRowBytes);
-          const uint64_t bdesc = ptx::make_smem_desc_sw128(sb + j * kHaloBBytes);
-#pragma unroll
-          for (int k = 0; k < kBlockK / kMmaK; ++k) {
-            ptx::wgmma_m64n64k16(acc, adesc + 2 * k, bdesc + 2 * k, accumulate);
-            accumulate = 1u;
-          }
-        }
-      }
-      ptx::wgmma_commit();
-      ptx::wgmma_wait<1>();
-      ptx::reg_fence(acc);
-      if (prev >= 0 && lane == 0) ptx::mbar_arrive(&bempty[prev]);
-      prev = bs;
-      if (++bs == kHaloBStages) { bs = 0; bphase ^= 1u; }
+      consume_k_block<64, P, 1>(acc, &bfull[bc.stage], bc.phase, p, 405,
+                                pbase + ky * kHaloRowBytes + kx * 128, kHaloPatchBytes, kHaloRowBytes,
+                                ptx::smem_u32(bring + bc.stage * Cfg::kBStage), kHaloBBytes, tap > 0, bempty, prev, lane);
+      prev = bc.stage;
+      bc.advance();
     }
     ptx::wgmma_wait<0>();
-    ptx::reg_fence(acc);
+    ptx::reg_fence(acc[0]);
     if (lane == 0) {
       ptx::mbar_arrive(&bempty[prev]);
-      ptx::mbar_arrive(&pempty[ps]);
+      ptx::mbar_arrive(&pempty[pc.stage]);
     }
-    if (++ps == 2) { ps = 0; pphase ^= 1u; }
+    pc.advance();
 
     const int frame = w / per_frame;
     long long row[2];
@@ -699,10 +693,9 @@ conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
     const int r0 = cw * 64 + warp * 16 + (lane >> 2);
     tile_row(p, w, r0, row[0], row_ok[0]);
     tile_row(p, w, r0 + 8, row[1], row_ok[1]);
-    epilogue<64>(p, acc, row, row_ok, 0, frame, lane, 0);
+    epilogue<64>(p, acc[0], row, row_ok, 0, frame, lane, 0);
   }
 }
-
 
 // Second pass of a split-K GEMM: sums the k-slice partials in a fixed order (deterministic) and
 // applies the epilogue (bias, GELU, residual, fp32 / bf16-plane outputs).
@@ -800,29 +793,72 @@ void choose_conv_tile(int H, int W, int* tw, int* th) {
   }
 }
 
-template <int BLOCK_N, int P, bool PINGPONG = false>
-int launch(const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
-  using Cfg = TcCfg<BLOCK_N, P>;
-  void (*kernel)(TcParams);
-  if constexpr (PINGPONG) kernel = gemm_tc_pingpong_kernel<BLOCK_N, P>;
-  else kernel = gemm_tc_kernel<BLOCK_N, P>;
+// Map of a row-major operand: P planes of `rows` rows of K elements, `ld` apart, planes
+// `plane_stride` apart (0: rows * ld), read in boxes of 64 k x `box_rows` rows of one plane.
+int encode_rows_map(CUtensorMap* m, const __nv_bfloat16* base, int K, long long rows, int ld,
+                    long long plane_stride, int P, int box_rows, const char* what) {
+  const long long plane = plane_stride > 0 ? plane_stride : rows * ld;
+  const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)rows, (cuuint64_t)P};
+  const cuuint64_t str[2] = {(cuuint64_t)ld * 2, (cuuint64_t)plane * 2};
+  const cuuint32_t box[3] = {(cuuint32_t)kBlockK, (cuuint32_t)box_rows, 1};
+  return encode_bf16_map(m, base, 3, dims, str, box, what);
+}
+
+// Map of a conv GEMM's A, the NHWC activation: P planes of [frames][H][W][C] (planes
+// a_plane_stride apart, 0: M * C), read in boxes of 64 channels x box_w x box_h pixels of one
+// frame and plane.
+int encode_nhwc_map(CUtensorMap* m, const GemmArgs& g, int box_w, int box_h, const char* what) {
+  const long long plane = g.a_plane_stride > 0 ? g.a_plane_stride : (long long)g.M * g.C;
+  const cuuint64_t dims[5] = {(cuuint64_t)g.C, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.frames,
+                              (cuuint64_t)g.planes};
+  const cuuint64_t str[4] = {(cuuint64_t)g.C * 2, (cuuint64_t)g.W * g.C * 2, (cuuint64_t)g.H * g.W * g.C * 2,
+                             (cuuint64_t)plane * 2};
+  const cuuint32_t box[5] = {(cuuint32_t)kBlockK, (cuuint32_t)box_w, (cuuint32_t)box_h, 1, 1};
+  return encode_bf16_map(m, g.a, 5, dims, str, box, what);
+}
+
+// Launches a wgmma kernel on at most one CTA per SM over p's work items, timed under the GEMM's
+// profiling tag with its FLOPs and algorithmic bytes.  The kernel's shared-memory limit is
+// raised once per device.
+template <void (*KERNEL)(TcParams), int SMEM_BYTES>
+int launch(const char* name, const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
   static PerDeviceOnce configured;
   if (configured.pending()) {
-    TAPIR_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
+    TAPIR_CUDA(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES));
     configured.mark();
   }
   const double kl = g.k_logical > 0 ? g.k_logical : g.K;
   const double out_b = (g.out_f32 ? 4.0 : 0.0) + (g.out_planes ? 2.0 * g.out_P : 0.0) + (g.residual ? 4.0 : 0.0);
   const double a_elems = (g.mode == kGemmConv3x3) ? (double)g.M * g.C : (double)g.M * g.K;
   ProfileScope ps(g.tag ? g.tag : "gemm", stream, 2.0 * g.batch * g.M * g.N * kl,
-                  g.batch * (2.0 * P * (a_elems + (double)g.N * g.K) + out_b * g.M * g.N));
+                  g.batch * (2.0 * g.planes * (a_elems + (double)g.N * g.K) + out_b * g.M * g.N));
   const int sms = num_sms();
-  const int tiles = p.num_m_tiles * p.num_n_tiles * (p.split_k > 1 ? p.split_k : 1);  // work items
-  const int grid = tiles < sms ? tiles : sms;
-  kernel<<<grid, kThreads, Cfg::kSmemBytes, stream>>>(p);
+  const int work = p.num_m_tiles * p.num_n_tiles * p.split_k;
+  KERNEL<<<work < sms ? work : sms, kThreads, SMEM_BYTES, stream>>>(p);
   count_launch();
-  TAPIR_LAUNCH_CHECK(PINGPONG ? "gemm_tc_pingpong_kernel" : "gemm_tc_kernel");
+  TAPIR_LAUNCH_CHECK(name);
   return kOk;
+}
+
+template <int BLOCK_N, int P>
+int launch_gemm(bool pingpong, const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
+  using Cfg = TcCfg<BLOCK_N, P>;
+  if constexpr (P <= 2)
+    if (pingpong) return launch<gemm_tc_pingpong_kernel<BLOCK_N, P>, Cfg::kSmemBytes>("gemm_tc_pingpong_kernel", p, g, stream);
+  return launch<gemm_tc_kernel<BLOCK_N, P>, Cfg::kSmemBytes>("gemm_tc_kernel", p, g, stream);
+}
+
+// The GEMM kernel for tile width `bn` and g.planes; ping-pong only where pick_pingpong chose it.
+int launch_gemm(int bn, bool pingpong, const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
+  const int P = g.planes;
+  if (bn == 64 && P == 1) return launch_gemm<64, 1>(pingpong, p, g, stream);
+  if (bn == 64 && P == 2) return launch_gemm<64, 2>(pingpong, p, g, stream);
+  if (bn == 64 && P == 3) return launch_gemm<64, 3>(pingpong, p, g, stream);
+  if (bn == 128 && P == 1) return launch_gemm<128, 1>(pingpong, p, g, stream);
+  if (bn == 128 && P == 2) return launch_gemm<128, 2>(pingpong, p, g, stream);
+  if (bn == 128 && P == 3) return launch_gemm<128, 3>(pingpong, p, g, stream);
+  set_error("gemm_tc: no kernel for BLOCK_N=%d planes=%d", bn, P);
+  return kUnsupported;
 }
 
 // Ping-pong hides a tile's epilogue behind the other warpgroup's mainloop.  It needs at least two
@@ -856,16 +892,134 @@ bool small_problem(int m_tiles, int N) {
 
 // 64-wide tiles for N <= 64, and for small problems when that gives every SM a tile: twice the
 // CTAs, each with half the MMA work per k-block.  (The K-summation order of an output element does
-// not depend on the tile shape, so results stay bit-identical across these choices.)
-int pick_block_n(int m_tiles, int N) {
+// not depend on the tile shape, so results stay bit-identical across these choices.)  A small
+// problem that will be split over K keeps 128-wide tiles unless TAPIR_B200_BLOCK_N is set (to
+// anything): the parallelism comes from K, and wide tiles re-read the A operand half as often.
+int pick_block_n(int m_tiles, int N, bool split_k) {
   const char* force = getenv("TAPIR_B200_BLOCK_N");
   if (force != nullptr) {
     int v = atoi(force);
     if (v == 64 || v == 128) return v;
   }
   if (N <= 64) return 64;
-  if (small_problem(m_tiles, N) && m_tiles * ceil_div(N, 128) * 2 <= num_sms()) return 64;
+  if (small_problem(m_tiles, N) && m_tiles * ceil_div(N, 128) * 2 <= num_sms())
+    return split_k && force == nullptr ? 128 : 64;
   return 128;
+}
+
+// On unless the variable is set to 0; read once per process.
+bool switch_on(const char* name) {
+  const char* e = getenv(name);
+  return !(e != nullptr && atoi(e) == 0);
+}
+
+// The parameters every kernel shares: problem, epilogue, batch layout, the generic conv tiling
+// and the A map.
+int common_params(const GemmArgs& g, TcParams* p) {
+  memset(p, 0, sizeof(*p));
+  p->M = g.M;
+  p->N = g.N;
+  p->num_k_blocks = g.K / kBlockK;
+  p->frames = g.frames;
+  p->mode = g.mode;
+  p->bias = g.bias;
+  p->residual = g.residual;
+  p->ldr = g.ldr;
+  p->act = g.act;
+  p->out_f32 = g.out_f32;
+  p->ldo = g.ldo;
+  p->out_planes = g.out_planes;
+  p->ldp = g.ldp;
+  p->out_plane_stride = g.out_plane_stride;
+  p->out_P = g.out_P;
+  p->err = device_error_flag();
+  p->stats = g.stats;
+  p->rows_per_frame = g.rows_per_frame > 0 ? g.rows_per_frame : g.M;
+  p->a_batch_rows = g.a_batch_rows > 0 ? g.a_batch_rows : g.M;
+  p->b_batch_rows = g.b_batch_rows > 0 ? g.b_batch_rows : g.N;
+  p->out_batch_stride = g.out_batch_stride > 0 ? g.out_batch_stride : (long long)g.M * g.ldo;
+  p->split_k = 1;
+  if (g.mode == kGemmConv3x3) {
+    choose_conv_tile(g.H, g.W, &p->tileW, &p->tileH);
+    p->H = g.H;
+    p->W = g.W;
+    p->cblocks = g.C / kBlockK;
+    p->tiles_x = ceil_div(g.W, p->tileW);
+    p->tiles_y = ceil_div(g.H, p->tileH);
+    p->num_m_tiles = g.frames * p->tiles_x * p->tiles_y;
+    TAPIR_RETURN_IF(encode_nhwc_map(&p->tmA, g, p->tileW, p->tileH, "A/conv"));
+  } else {
+    p->num_m_tiles = ceil_div(g.M, kBlockM) * g.batch;
+    TAPIR_RETURN_IF(encode_rows_map(&p->tmA, g.a, g.K, (g.batch - 1) * p->a_batch_rows + g.M, g.lda,
+                                    g.a_plane_stride, g.planes, kBlockM, "A"));
+  }
+  p->m_tiles_per_batch = p->num_m_tiles / g.batch;
+  return kOk;
+}
+
+// Halo-patch kernel for the C = 64 -> 64 3x3 layers (first ResNet group), see conv3x3_halo_kernel.
+// TAPIR_B200_CONV_HALO=0: generic path.
+bool use_halo(const GemmArgs& g) {
+  static const bool on = switch_on("TAPIR_B200_CONV_HALO");
+  return on && g.mode == kGemmConv3x3 && g.C == 64 && g.N == 64 && g.planes <= 2 && g.out_planes == nullptr;
+}
+
+int launch_halo(TcParams p, const GemmArgs& g, cudaStream_t stream) {
+  p.tileW = kHaloTileW;
+  p.tileH = kHaloTileH;
+  p.tiles_x = ceil_div(g.W, kHaloTileW);
+  p.tiles_y = ceil_div(g.H, kHaloTileH);
+  p.num_m_tiles = g.frames * p.tiles_x * p.tiles_y;
+  p.num_n_tiles = 1;
+  TAPIR_RETURN_IF(encode_nhwc_map(&p.tmPatch, g, kHaloTileW + 2, 1, "A/patch"));
+  TAPIR_RETURN_IF(encode_rows_map(&p.tmB, g.b, g.K, g.N, g.ldb, g.b_plane_stride, g.planes, 64, "B/halo"));
+  if (g.planes == 1) return launch<conv3x3_halo_kernel<1>, HaloCfg<1>::kSmemBytes>("conv3x3_halo_kernel", p, g, stream);
+  return launch<conv3x3_halo_kernel<2>, HaloCfg<2>::kSmemBytes>("conv3x3_halo_kernel", p, g, stream);
+}
+
+// Split-K (deterministic two-pass, below) for problems that cannot half-fill the GPU: on by
+// default, TAPIR_B200_SPLITK=0 disables.  Only where the caller allows it (single-frame streaming
+// steps) and K >= 2048 (mixer `down` at ~1000 rows, the ExtraConvs of one frame).  The summation
+// order of a split GEMM depends on the row count; offline clips keep the exact chunk /
+// permutation / shard invariance (tests/test_properties_gpu.py re-chunks config 2 into 1776-row
+// chunks, tests/multi_gpu_check.py shards 1152 rows over two ranks, both demand bit-level
+// agreement).
+bool splittable(const GemmArgs& g) {
+  static const bool on = switch_on("TAPIR_B200_SPLITK");
+  return on && g.allow_splitk && g.splitk_ws != nullptr && g.stats == nullptr && g.batch == 1 &&
+         g.K / kBlockK >= 32;
+}
+
+// Row stride of the split-K partials: whole float4 groups for the reduction.
+int splitk_ld(int N) { return (N + 7) / 8 * 8; }
+
+// Number of k-slices of a splittable GEMM with `tiles` output tiles (1: no split): up to one work
+// item per SM, at most 8, at least 4 k-blocks each, and as many as the workspace holds.
+int split_k_factor(const GemmArgs& g, int tiles) {
+  const int sms = num_sms();
+  if (tiles * 2 > sms) return 1;
+  int S = sms / tiles;
+  if (S > 8) S = 8;
+  if (S > g.K / kBlockK / 4) S = g.K / kBlockK / 4;
+  while (S > 1 && (size_t)S * g.M * splitk_ld(g.N) * sizeof(float) > g.splitk_ws_bytes) --S;
+  return S;
+}
+
+int launch_split_k(const TcParams& p, int bn, int S, const GemmArgs& g, cudaStream_t stream) {
+  const int ldw = splitk_ld(g.N);
+  TcParams q = p;  // first pass: raw partial sums
+  q.split_k = S;
+  q.split_stride = (long long)g.M * ldw;
+  q.bias = nullptr; q.residual = nullptr; q.act = 0; q.out_planes = nullptr; q.stats = nullptr;
+  q.out_f32 = g.splitk_ws; q.ldo = ldw;
+  TAPIR_RETURN_IF(launch_gemm(bn, false, q, g, stream));
+  const long long total = (long long)g.M * ((g.N + 3) / 4);
+  long long blocks = (total + 255) / 256;
+  if (blocks > (long long)num_sms() * 8) blocks = (long long)num_sms() * 8;
+  splitk_reduce_kernel<<<(unsigned)blocks, 256, 0, stream>>>(g.splitk_ws, S, q.split_stride, ldw, p);
+  count_launch();
+  TAPIR_LAUNCH_CHECK("splitk_reduce_kernel");
+  return kOk;
 }
 
 }  // namespace
@@ -916,175 +1070,19 @@ int validate_gemm_args(const GemmArgs& g) {
 int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
   TAPIR_RETURN_IF(validate_gemm_args(g));
   TcParams p;
-  memset(&p, 0, sizeof(p));
-  p.M = g.M;
-  p.N = g.N;
-  p.num_k_blocks = g.K / kBlockK;
-  p.frames = g.frames;
-  p.mode = g.mode;
-  p.bias = g.bias;
-  p.residual = g.residual;
-  p.ldr = g.ldr;
-  p.act = g.act;
-  p.out_f32 = g.out_f32;
-  p.ldo = g.ldo;
-  p.out_planes = g.out_planes;
-  p.ldp = g.ldp;
-  p.out_plane_stride = g.out_plane_stride;
-  p.out_P = g.out_P;
-  p.err = device_error_flag();
-  p.stats = g.stats;
-  p.rows_per_frame = g.rows_per_frame > 0 ? g.rows_per_frame : g.M;
-  const int P = g.planes;
-  const long long a_batch_rows = g.a_batch_rows > 0 ? g.a_batch_rows : g.M;
-  const long long b_batch_rows = g.b_batch_rows > 0 ? g.b_batch_rows : g.N;
-  p.a_batch_rows = a_batch_rows;
-  p.b_batch_rows = b_batch_rows;
-  p.out_batch_stride = g.out_batch_stride > 0 ? g.out_batch_stride : (long long)g.M * g.ldo;
-
-  if (g.mode == kGemmConv3x3) {
-    choose_conv_tile(g.H, g.W, &p.tileW, &p.tileH);
-    p.H = g.H;
-    p.W = g.W;
-    p.cblocks = g.C / kBlockK;
-    p.tiles_x = ceil_div(g.W, p.tileW);
-    p.tiles_y = ceil_div(g.H, p.tileH);
-    p.num_m_tiles = g.frames * p.tiles_x * p.tiles_y;
-    const long long plane = g.a_plane_stride > 0 ? g.a_plane_stride : (long long)g.M * g.C;
-    cuuint64_t dims[5] = {(cuuint64_t)g.C, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.frames, (cuuint64_t)P};
-    cuuint64_t str[4] = {(cuuint64_t)g.C * 2, (cuuint64_t)g.W * g.C * 2, (cuuint64_t)g.H * g.W * g.C * 2,
-                         (cuuint64_t)plane * 2};
-    cuuint32_t box[5] = {(cuuint32_t)kBlockK, (cuuint32_t)p.tileW, (cuuint32_t)p.tileH, 1, 1};
-    TAPIR_RETURN_IF(encode_bf16_map(&p.tmA, g.a, 5, dims, str, box, "A/conv"));
-  } else {
-    p.num_m_tiles = ceil_div(g.M, kBlockM) * g.batch;
-    const long long a_rows = (g.batch - 1) * a_batch_rows + g.M;
-    const long long plane = g.a_plane_stride > 0 ? g.a_plane_stride : a_rows * g.lda;
-    cuuint64_t dims[3] = {(cuuint64_t)g.K, (cuuint64_t)a_rows, (cuuint64_t)P};
-    cuuint64_t str[2] = {(cuuint64_t)g.lda * 2, (cuuint64_t)plane * 2};
-    cuuint32_t box[3] = {(cuuint32_t)kBlockK, (cuuint32_t)kBlockM, 1};
-    TAPIR_RETURN_IF(encode_bf16_map(&p.tmA, g.a, 3, dims, str, box, "A"));
-  }
-  // Halo-patch kernel for the C = 64 -> 64 3x3 layers (first ResNet group), see conv3x3_halo_kernel.
-  {
-    static int halo_on = -1;
-    if (halo_on < 0) { const char* e = getenv("TAPIR_B200_CONV_HALO"); halo_on = (e != nullptr && atoi(e) == 0) ? 0 : 1; }  // TAPIR_B200_CONV_HALO=0: generic path
-    if (halo_on && g.mode == kGemmConv3x3 && g.C == 64 && g.N == 64 && P <= 2 && g.out_planes == nullptr) {
-      p.tileW = kHaloTileW;
-      p.tileH = kHaloTileH;
-      p.tiles_x = ceil_div(g.W, kHaloTileW);
-      p.tiles_y = ceil_div(g.H, kHaloTileH);
-      p.num_m_tiles = g.frames * p.tiles_x * p.tiles_y;
-      p.num_n_tiles = 1;
-      p.split_k = 1;
-      const long long aplane = g.a_plane_stride > 0 ? g.a_plane_stride : (long long)g.M * g.C;
-      cuuint64_t adims[5] = {(cuuint64_t)g.C, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)g.frames, (cuuint64_t)P};
-      cuuint64_t astr[4] = {(cuuint64_t)g.C * 2, (cuuint64_t)g.W * g.C * 2, (cuuint64_t)g.H * g.W * g.C * 2,
-                            (cuuint64_t)aplane * 2};
-      cuuint32_t abox[5] = {(cuuint32_t)kBlockK, (cuuint32_t)(kHaloTileW + 2), 1, 1, 1};
-      TAPIR_RETURN_IF(encode_bf16_map(&p.tmPatch, g.a, 5, adims, astr, abox, "A/patch"));
-      const long long bplane = g.b_plane_stride > 0 ? g.b_plane_stride : (long long)g.N * g.ldb;
-      cuuint64_t bdims[3] = {(cuuint64_t)g.K, (cuuint64_t)g.N, (cuuint64_t)P};
-      cuuint64_t bstr[2] = {(cuuint64_t)g.ldb * 2, (cuuint64_t)bplane * 2};
-      cuuint32_t bbox[3] = {(cuuint32_t)kBlockK, 64, 1};
-      TAPIR_RETURN_IF(encode_bf16_map(&p.tmB, g.b, 3, bdims, bstr, bbox, "B/halo"));
-      static PerDeviceOnce configured;
-      if (configured.pending()) {
-        TAPIR_CUDA(cudaFuncSetAttribute(conv3x3_halo_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, HaloCfg<1>::kSmemBytes));
-        TAPIR_CUDA(cudaFuncSetAttribute(conv3x3_halo_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, HaloCfg<2>::kSmemBytes));
-        configured.mark();
-      }
-      const double kl = g.k_logical > 0 ? g.k_logical : g.K;
-      const double out_b = (g.out_f32 ? 4.0 : 0.0) + (g.residual ? 4.0 : 0.0);
-      ProfileScope ps(g.tag ? g.tag : "gemm", stream, 2.0 * g.M * g.N * kl,
-                      2.0 * P * ((double)g.M * g.C + (double)g.N * g.K) + out_b * g.M * g.N);
-      const int grid = p.num_m_tiles < num_sms() ? p.num_m_tiles : num_sms();
-      if (P == 1) conv3x3_halo_kernel<1><<<grid, kThreads, HaloCfg<1>::kSmemBytes, stream>>>(p);
-      else conv3x3_halo_kernel<2><<<grid, kThreads, HaloCfg<2>::kSmemBytes, stream>>>(p);
-      count_launch();
-      TAPIR_LAUNCH_CHECK("conv3x3_halo_kernel");
-      return kOk;
-    }
-  }
-  // Split-K (deterministic two-pass, below) for problems that cannot half-fill the GPU: on by
-  // default, TAPIR_B200_SPLITK=0 disables.
-  static int splitk_on = -1;
-  if (splitk_on < 0) { const char* e = getenv("TAPIR_B200_SPLITK"); splitk_on = (e != nullptr && atoi(e) == 0) ? 0 : 1; }
-  // Only where the caller allows it (single-frame streaming steps).  The summation order of a
-  // split GEMM depends on the row count; offline clips keep the exact chunk / permutation / shard
-  // invariance (tests/test_properties_gpu.py re-chunks config 2 into 1776-row chunks,
-  // tests/multi_gpu_check.py shards 1152 rows over two ranks, both demand bit-level agreement).
-  const bool splittable = splitk_on && g.allow_splitk && g.splitk_ws != nullptr && g.stats == nullptr &&
-                          g.batch == 1 && p.num_k_blocks >= 32;
-  p.m_tiles_per_batch = p.num_m_tiles / g.batch;
-  int bn = pick_block_n(p.num_m_tiles, g.N);
-  // a small problem that will be split over K keeps 128-wide tiles: the parallelism comes from K,
-  // and wide tiles re-read the A operand half as often
-  if (splittable && bn == 64 && g.N > 64 && small_problem(p.num_m_tiles, g.N) &&
-      p.num_m_tiles * ceil_div(g.N, 128) * 2 <= num_sms() && getenv("TAPIR_B200_BLOCK_N") == nullptr)
-    bn = 128;
+  TAPIR_RETURN_IF(common_params(g, &p));
+  if (use_halo(g)) return launch_halo(p, g, stream);
+  const bool split = splittable(g);
+  const int bn = pick_block_n(p.num_m_tiles, g.N, split);
   p.num_n_tiles = ceil_div(g.N, bn);
-  {
-    const long long b_rows = (g.batch - 1) * b_batch_rows + g.N;
-    const long long plane = g.b_plane_stride > 0 ? g.b_plane_stride : b_rows * g.ldb;
-    cuuint64_t dims[3] = {(cuuint64_t)g.K, (cuuint64_t)b_rows, (cuuint64_t)P};
-    cuuint64_t str[2] = {(cuuint64_t)g.ldb * 2, (cuuint64_t)plane * 2};
-    cuuint32_t box[3] = {(cuuint32_t)kBlockK, (cuuint32_t)bn, 1};
-    TAPIR_RETURN_IF(encode_bf16_map(&p.tmB, g.b, 3, dims, str, box, "B"));
-  }
-
-  // split-K for problems that cannot fill the GPU (streaming: T = 1): deterministic two-pass
-  p.split_k = 1;
-  p.split_stride = 0;
+  TAPIR_RETURN_IF(encode_rows_map(&p.tmB, g.b, g.K, (g.batch - 1) * p.b_batch_rows + g.N, g.ldb,
+                                  g.b_plane_stride, g.planes, bn, "B"));
   const int tiles = p.num_m_tiles * p.num_n_tiles;
-  const int sms = num_sms();
-  // K >= 2048 only (mixer `down` at ~1000 rows, the ExtraConvs of one frame).  The summation order
-  // then depends on the row count; only problems that cannot half-fill the GPU split, so offline
-  // clips keep their exact chunk / permutation invariance.
-  if (splittable && tiles * 2 <= sms) {
-    int S = sms / tiles;
-    if (S > 8) S = 8;
-    if (S > p.num_k_blocks / 4) S = p.num_k_blocks / 4;
-    const int ldw = (g.N + 7) / 8 * 8;
-    while (S > 1 && (size_t)S * g.M * ldw * sizeof(float) > g.splitk_ws_bytes) --S;
-    if (S > 1) {
-      TcParams q = p;  // first pass: raw partial sums
-      q.split_k = S;
-      q.split_stride = (long long)g.M * ldw;
-      q.bias = nullptr; q.residual = nullptr; q.act = 0; q.out_planes = nullptr; q.stats = nullptr;
-      q.out_f32 = g.splitk_ws; q.ldo = ldw;
-      int rc = kUnsupported;
-#define TAPIR_TC_SPLIT(BN, PP) \
-      if (bn == BN && P == PP) rc = launch<BN, PP>(q, g, stream);
-      TAPIR_TC_SPLIT(64, 1) TAPIR_TC_SPLIT(64, 2) TAPIR_TC_SPLIT(64, 3)
-      TAPIR_TC_SPLIT(128, 1) TAPIR_TC_SPLIT(128, 2) TAPIR_TC_SPLIT(128, 3)
-#undef TAPIR_TC_SPLIT
-      TAPIR_RETURN_IF(rc);
-      const long long total = (long long)g.M * ((g.N + 3) / 4);
-      long long blocks = (total + 255) / 256;
-      if (blocks > (long long)sms * 8) blocks = (long long)sms * 8;
-      splitk_reduce_kernel<<<(unsigned)blocks, 256, 0, stream>>>(g.splitk_ws, S, q.split_stride, ldw, p);
-      count_launch();
-      TAPIR_LAUNCH_CHECK("splitk_reduce_kernel");
-      return kOk;
-    }
-  }
-
+  const int S = split ? split_k_factor(g, tiles) : 1;
+  if (S > 1) return launch_split_k(p, bn, S, g, stream);
   bool pingpong = false;
-  TAPIR_RETURN_IF(pick_pingpong(tiles, p.num_k_blocks, P, g.batch, &pingpong));
-  if (pingpong) {
-#define TAPIR_TC_PINGPONG(BN, PP) \
-    if (bn == BN && P == PP) return launch<BN, PP, true>(p, g, stream);
-    TAPIR_TC_PINGPONG(64, 1) TAPIR_TC_PINGPONG(64, 2) TAPIR_TC_PINGPONG(128, 1) TAPIR_TC_PINGPONG(128, 2)
-#undef TAPIR_TC_PINGPONG
-  }
-#define TAPIR_TC_CASE(BN, PP) \
-  if (bn == BN && P == PP) return launch<BN, PP>(p, g, stream);
-  TAPIR_TC_CASE(64, 1) TAPIR_TC_CASE(64, 2) TAPIR_TC_CASE(64, 3)
-  TAPIR_TC_CASE(128, 1) TAPIR_TC_CASE(128, 2) TAPIR_TC_CASE(128, 3)
-#undef TAPIR_TC_CASE
-  set_error("gemm_tc: no kernel for BLOCK_N=%d planes=%d", bn, P);
-  return kUnsupported;
+  TAPIR_RETURN_IF(pick_pingpong(tiles, p.num_k_blocks, g.planes, g.batch, &pingpong));
+  return launch_gemm(bn, pingpong, p, g, stream);
 }
 
 }  // namespace tapir

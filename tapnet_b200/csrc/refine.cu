@@ -618,16 +618,10 @@ size_t plan_mixer(Arena& a, long long rows, int planes, MixerPlan* m) {
   m->splitk = a.take<float>(kSplitKBytes / sizeof(float));
   return a.off;
 }
-GemmArgs lin(const tapir_linear& l) {
-  GemmArgs g;
-  g.planes = l.planes;
-  g.N = l.N;
-  g.K = l.K;
-  g.b = static_cast<const __nv_bfloat16*>(l.w);
-  g.ldb = l.K;
-  g.b_plane_stride = (long long)l.N * l.K;
-  g.bias = l.bias;
-  g.k_logical = l.k_logical;
+// A mixer GEMM: split-K only for single-frame (streaming) steps, see GemmArgs::allow_splitk.
+GemmArgs mixer_gemm_args(const tapir_linear& l, const MixerPlan& m, int T) {
+  GemmArgs g = gemm_args(l);
+  g.splitk_ws = m.splitk; g.splitk_ws_bytes = kSplitKBytes; g.allow_splitk = (T == 1);
   return g;
 }
 }  // namespace
@@ -709,9 +703,8 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
     return kWorkspaceTooSmall;
   }
   {  // nets.py:235 linear
-    GemmArgs g = lin(w->linear);
+    GemmArgs g = mixer_gemm_args(w->linear, m, T);
     g.tag = "mixer.linear_in";
-    g.splitk_ws = m.splitk; g.splitk_ws_bytes = kSplitKBytes; g.allow_splitk = (T == 1);
     g.M = (int)rows;
     g.a = static_cast<const __nv_bfloat16*>(io->x_planes);
     g.lda = io->ldx;
@@ -725,9 +718,8 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
                              io->ctx2_in ? io->ctx2_in[b] : nullptr, io->ctx1_out ? io->ctx1_out[b] : nullptr,
                              io->ctx2_out ? io->ctx2_out[b] : nullptr, m.xb, m.y, rows * 512, P, s));
     {
-      GemmArgs g = lin(blk.up);
+      GemmArgs g = mixer_gemm_args(blk.up, m, T);
       g.tag = "mixer.up";
-      g.splitk_ws = m.splitk; g.splitk_ws_bytes = kSplitKBytes; g.allow_splitk = (T == 1);
       g.M = (int)rows;
       g.a = m.y; g.lda = 512; g.a_plane_stride = rows * 512;
       g.act = 1;
@@ -735,9 +727,8 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
       TAPIR_RETURN_IF(gemm(g, s));
     }
     {
-      GemmArgs g = lin(blk.down);
+      GemmArgs g = mixer_gemm_args(blk.down, m, T);
       g.tag = "mixer.down";
-      g.splitk_ws = m.splitk; g.splitk_ws_bytes = kSplitKBytes; g.allow_splitk = (T == 1);
       g.M = (int)rows;
       g.a = m.h; g.lda = 2048; g.a_plane_stride = rows * 2048;
       g.residual = m.xb; g.ldr = 512;
@@ -747,9 +738,8 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
   }
   TAPIR_RETURN_IF(layernorm_split(m.xa, rows, 512, w->ln_w, nullptr, nullptr, m.y, rows * 512, P, s));
   {
-    GemmArgs g = lin(w->linear_1);
+    GemmArgs g = mixer_gemm_args(w->linear_1, m, T);
     g.tag = "mixer.linear_out";
-    g.splitk_ws = m.splitk; g.splitk_ws_bytes = kSplitKBytes; g.allow_splitk = (T == 1);
     g.M = (int)rows;
     g.a = m.y; g.lda = 512; g.a_plane_stride = rows * 512;
     g.out_f32 = io->out; g.ldo = io->ldo;
