@@ -6,7 +6,8 @@
 //   warpgroups 1, 2         consumers: issue wgmma.m64nBLOCK_Nk16 (bf16 operands from shared
 //                           memory, fp32 accumulators in registers) and then run the epilogue
 //                           from their registers: bias / tanh-GELU / residual, fp32 and/or
-//                           bf16-plane stores.  Cooperative schedule (gemm_tc_kernel): each owns
+//                           bf16-plane stores (whole ping-pong tiles of GELU + two planes: through
+//                           shared memory and TMA stores).  Cooperative schedule (gemm_tc_kernel): each owns
 //                           64 rows of every 128-row tile.  Ping-pong schedule
 //                           (gemm_tc_pingpong_kernel): each owns whole tiles, alternately.
 // full/empty mbarriers between producer and consumers; the producer runs ahead into the next
@@ -44,6 +45,8 @@ struct TcParams {
   CUtensorMap tmA;
   CUtensorMap tmB;
   CUtensorMap tmPatch;  // halo convolution: one patch row {64 ch, 10 px} per load
+  CUtensorMap tmPlanes;  // ping-pong, plane_tma: output planes {N, M, 2}, stored in boxes {64, 64, 1}
+  int plane_tma;         // whole ping-pong tiles write GELU + two planes through epilogue_planes_tma
   int frames;
   int M, N;
   int num_k_blocks;
@@ -69,15 +72,21 @@ struct TcParams {
   int* err;
 };
 
-template <int BLOCK_N, int P>
+// Ping-pong output staging (epilogue_planes_tma): per consumer warpgroup one 64 x 64 bf16 box
+// buffer per output plane.
+constexpr int kPlaneBoxBytes = 64 * 128;
+constexpr int kPlaneStagingBytes = kConsumers * 2 * kPlaneBoxBytes;
+
+// Shared memory: the stage ring, STAGING bytes after it, then the barriers.
+template <int BLOCK_N, int P, int STAGING = 0>
 struct TcCfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = BLOCK_N * kBlockK * 2;
   static constexpr int kStageBytes = P * (kABytes + kBBytes);
-  static constexpr int kAvail = kSmemLimit - 1024 - kBarrierBytes;
+  static constexpr int kAvail = kSmemLimit - 1024 - STAGING - kBarrierBytes;
   static constexpr int kStagesRaw = kAvail / kStageBytes;
   static constexpr int kStages = kStagesRaw > 6 ? 6 : kStagesRaw;
-  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kBarrierBytes;
+  static constexpr int kSmemBytes = 1024 + kStages * kStageBytes + STAGING + kBarrierBytes;
   static_assert(kStages >= 2, "tile does not fit in shared memory");
   static_assert(kStages * 2 <= kBarrierBytes / 8, "barrier space");
 };
@@ -301,6 +310,77 @@ __device__ __forceinline__ void tile_epilogue(const TcParams& p, const float (&a
   epilogue<BLOCK_N>(p, acc, row, row_ok, n0, frame, lane, out_off);
 }
 
+// Whether all rows and columns of output tile (m_tile, n0) exist.  Its 128 rows are consecutive
+// output rows wherever the host sets plane_tma: plain mode, or tiles of whole image rows.
+template <int BLOCK_N>
+__device__ __forceinline__ bool whole_tile(const TcParams& p, int m_tile, int n0) {
+  long long last;
+  bool ok;
+  tile_row(p, m_tile, kBlockM - 1, last, ok);
+  return ok && n0 + BLOCK_N <= p.N;
+}
+
+// The GELU + two-plane epilogue of rows [r_base, r_base + 64) of whole tile `m_tile`, with the same
+// values as epilogue_full's, written through shared memory.  Register stores write one 4-byte word
+// in each of 8 rows per warp instruction, half of every 32-byte sector, and kept the warpgroup in
+// its epilogue longer than the other warpgroup's mainloop.  Here, per 64 columns, stmatrix puts
+// each plane's 64 x 64 box into its buffer (`boxes`, then + 8 KB; 128B-swizzled as the tensor map
+// expects) and one thread writes both boxes out with TMA stores of whole 128-byte rows.  Before
+// the warpgroup overwrites the buffers, that thread waits until the previous stores have read
+// them.
+template <int BLOCK_N, bool BIAS>
+__device__ __forceinline__ void epilogue_planes_tma(const TcParams& p, float (&acc)[BLOCK_N / 2], int m_tile,
+                                                    int r_base, int n0, uint32_t boxes, uint32_t bar, int warp,
+                                                    int lane) {
+  const bool issuer = warp == 0 && lane == 0;
+  long long row0;
+  bool ok;
+  tile_row(p, m_tile, r_base, row0, ok);
+  // stmatrix: lanes 8 i .. 8 i + 7 address the rows of matrix i, rows 8 (i & 1) on, column group i >> 1
+  const uint32_t rr = lane & 7;
+  const uint32_t row_addr = (uint32_t)(16 * warp + 8 * ((lane >> 3) & 1) + rr) * 128;
+  const uint32_t chunk_hi = (uint32_t)lane >> 4;
+#pragma unroll
+  for (int cb = 0; cb < BLOCK_N / 64; ++cb) {
+    if (issuer) ptx::bulk_wait_read<0>();
+    ptx::named_bar_sync(bar, 128);  // the previous stores have read the buffers
+    // the arithmetic below stays after the barrier: with both accumulator halves live, the
+    // registers hold one stmatrix worth of plane values at a time
+    ptx::reg_fence(acc);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      uint32_t pl[2][4];  // plane q of column group 8 cb + 2 k + g, rows +0 / +8 (s): pl[q][2 g + s]
+#pragma unroll
+      for (int g = 0; g < 2; ++g) {
+        const int j = 8 * cb + 2 * k + g;
+        const int c = n0 + 8 * j + 2 * (lane & 3);
+        float b0 = 0.f, b1 = 0.f;
+        if constexpr (BIAS) { b0 = __ldg(p.bias + c); b1 = __ldg(p.bias + c + 1); }
+#pragma unroll
+        for (int s = 0; s < 2; ++s) {
+          float v0 = acc[4 * j + 2 * s], v1 = acc[4 * j + 2 * s + 1];
+          if constexpr (BIAS) { v0 += b0; v1 += b1; }
+          v0 = gelu_tanh(v0); v1 = gelu_tanh(v1);
+          pl[0][2 * g + s] = bf16x2_split(v0, v1);
+          pl[1][2 * g + s] = bf16x2_split(v0, v1);
+        }
+      }
+#pragma unroll
+      for (int q = 0; q < 2; ++q)
+        ptx::stmatrix_x4(boxes + q * kPlaneBoxBytes + row_addr + (((2 * k + chunk_hi) ^ rr) << 4), pl[q][0],
+                         pl[q][1], pl[q][2], pl[q][3]);
+    }
+    ptx::fence_proxy_async_shared();
+    ptx::named_bar_sync(bar, 128);  // both boxes are written
+    if (issuer) {
+#pragma unroll
+      for (int q = 0; q < 2; ++q)
+        ptx::tma_store_3d(&p.tmPlanes, boxes + q * kPlaneBoxBytes, n0 + 64 * cb, (int)row0, q);
+      ptx::bulk_commit();
+    }
+  }
+}
+
 // Work item w in the order (batch, m-tile, n-tile, k-slice); m_tile is the tile within its batch,
 // [kb0, kb1) its k-blocks.  Returns the k-slice.
 template <int BLOCK_N>
@@ -396,17 +476,19 @@ __device__ __forceinline__ void consume_k_block(float (&acc)[HALVES][BLOCK_N / 2
   if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
 }
 
-// Shared-memory ring of both GEMM schedules: kStages stages of P A planes then P B planes, then the
-// full and empty mbarriers.
-template <int BLOCK_N, int P>
+// Shared-memory ring of both GEMM schedules: kStages stages of P A planes then P B planes, STAGING
+// bytes (1024-aligned) for the epilogue, then the full and empty mbarriers.
+template <int BLOCK_N, int P, int STAGING = 0>
 struct Ring {
-  using Cfg = TcCfg<BLOCK_N, P>;
+  using Cfg = TcCfg<BLOCK_N, P, STAGING>;
   uint8_t* smem;
+  uint8_t* staging;
   uint64_t* full_bar;
   uint64_t* empty_bar;
   __device__ __forceinline__ Ring(uint8_t* smem_raw, const TcParams& p, uint32_t empty_arrivals)
       : smem(aligned_smem(smem_raw)),
-        full_bar(reinterpret_cast<uint64_t*>(smem + Cfg::kStages * Cfg::kStageBytes)),
+        staging(smem + Cfg::kStages * Cfg::kStageBytes),
+        full_bar(reinterpret_cast<uint64_t*>(staging + STAGING)),
         empty_bar(full_bar + Cfg::kStages) {
     init_rings(full_bar, empty_arrivals, &p.tmA, &p.tmB, Cfg::kStages);
   }
@@ -523,14 +605,16 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
 constexpr int kProducerRegs = 40;
 constexpr int kPingPongRegs = 232;  // 128 accumulators per thread at BLOCK_N = 128
 constexpr uint32_t kTurnBarrier = 1;  // named barriers 1, 2: consumer 0's, consumer 1's turn
+constexpr uint32_t kStagingBarrier = 3;  // named barriers 3, 4: consumer 0's, consumer 1's box buffers
 
 template <int BLOCK_N, int P>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
-  using Cfg = TcCfg<BLOCK_N, P>;
+  using Cfg = TcCfg<BLOCK_N, P, kPlaneStagingBytes>;
   static_assert(P <= 2, "ping-pong: P = 3 stays cooperative");
+  static_assert(Cfg::kStages == TcCfg<BLOCK_N, P>::kStages, "the output staging must not cost the ring a stage");
   extern __shared__ uint8_t smem_raw[];
-  const Ring<BLOCK_N, P> ring(smem_raw, p, 4);  // one arrive per warp of the reading warpgroup
+  const Ring<BLOCK_N, P, kPlaneStagingBytes> ring(smem_raw, p, 4);  // one arrive per warp of the reading warpgroup
 
   const int wg = threadIdx.x >> 7;
   const int warp = (threadIdx.x >> 5) & 3;
@@ -573,16 +657,27 @@ gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
     ptx::reg_fence(acc[0]);
     ptx::reg_fence(acc[1]);
     if (lane == 0) ptx::mbar_arrive(&ring.empty_bar[prev]);
+    const bool staged = p.plane_tma && whole_tile<BLOCK_N>(p, m_tile, n0);
     // one copy of the epilogue code for both halves: it runs while the other warpgroup's mainloop
     // executes from the same instruction cache
 #pragma unroll 1
     for (int h = 0; h < 2; ++h) {
-      tile_epilogue<BLOCK_N>(p, acc[0], m_tile, 64 * h, n0, warp, lane, bat * p.out_batch_stride);
+      if (!staged) {
+        tile_epilogue<BLOCK_N>(p, acc[0], m_tile, 64 * h, n0, warp, lane, bat * p.out_batch_stride);
+      } else {
+        const uint32_t boxes = ptx::smem_u32(ring.staging) + (uint32_t)(cw * 2 * kPlaneBoxBytes);
+        if (p.bias != nullptr)
+          epilogue_planes_tma<BLOCK_N, true>(p, acc[0], m_tile, 64 * h, n0, boxes, kStagingBarrier + cw, warp, lane);
+        else
+          epilogue_planes_tma<BLOCK_N, false>(p, acc[0], m_tile, 64 * h, n0, boxes, kStagingBarrier + cw, warp, lane);
+      }
       if (h == 0) {
 #pragma unroll
         for (int i = 0; i < BLOCK_N / 2; ++i) acc[0][i] = acc[1][i];
       }
     }
+    // after the warpgroup's last tile: its stores complete while the shared memory still exists
+    if (t + 2 >= my_tiles && warp == 0 && lane == 0) ptx::bulk_wait<0>();
   }
 }
 
@@ -842,10 +937,11 @@ int launch(const char* name, const TcParams& p, const GemmArgs& g, cudaStream_t 
 
 template <int BLOCK_N, int P>
 int launch_gemm(bool pingpong, const TcParams& p, const GemmArgs& g, cudaStream_t stream) {
-  using Cfg = TcCfg<BLOCK_N, P>;
   if constexpr (P <= 2)
-    if (pingpong) return launch<gemm_tc_pingpong_kernel<BLOCK_N, P>, Cfg::kSmemBytes>("gemm_tc_pingpong_kernel", p, g, stream);
-  return launch<gemm_tc_kernel<BLOCK_N, P>, Cfg::kSmemBytes>("gemm_tc_kernel", p, g, stream);
+    if (pingpong)
+      return launch<gemm_tc_pingpong_kernel<BLOCK_N, P>, TcCfg<BLOCK_N, P, kPlaneStagingBytes>::kSmemBytes>(
+          "gemm_tc_pingpong_kernel", p, g, stream);
+  return launch<gemm_tc_kernel<BLOCK_N, P>, TcCfg<BLOCK_N, P>::kSmemBytes>("gemm_tc_kernel", p, g, stream);
 }
 
 // The GEMM kernel for tile width `bn` and g.planes; ping-pong only where pick_pingpong chose it.
@@ -881,6 +977,30 @@ int pick_pingpong(int tiles, int num_k_blocks, int P, int batch, bool* pingpong)
   }
   const int sms = num_sms();
   *pingpong = tiles >= 2 * sms && (tiles >= 4 * sms || num_k_blocks >= 16);
+  return kOk;
+}
+
+// Whole ping-pong tiles with tanh-GELU and two bf16 output planes and nothing else (mixer `up`, the
+// ExtraConv expansion) write their planes with TMA stores (epilogue_planes_tma) where a tile's rows
+// are consecutive output rows and the planes meet TMA's 16-byte rules.
+// TAPIR_B200_PLANE_STORE=tma|regs (default tma) selects that path or the register stores; it is
+// read on every call and any other value is an error.
+int plane_store_params(const GemmArgs& g, bool pingpong, TcParams* p) {
+  const char* e = getenv("TAPIR_B200_PLANE_STORE");
+  if (e != nullptr && strcmp(e, "tma") != 0 && strcmp(e, "regs") != 0) {
+    set_error("TAPIR_B200_PLANE_STORE=%s: expected tma or regs", e);
+    return kBadArgument;
+  }
+  if (!pingpong || (e != nullptr && strcmp(e, "regs") == 0)) return kOk;
+  if (g.act != 1 || g.out_planes == nullptr || g.out_P != 2 || g.out_f32 != nullptr || g.residual != nullptr ||
+      g.stats != nullptr)
+    return kOk;
+  if (g.mode == kGemmConv3x3 && p->tileW != g.W) return kOk;
+  if (g.ldp % 8 != 0 || g.out_plane_stride <= 0 || g.out_plane_stride % 8 != 0 ||
+      (reinterpret_cast<uintptr_t>(g.out_planes) & 15) != 0)
+    return kOk;
+  TAPIR_RETURN_IF(encode_rows_map(&p->tmPlanes, g.out_planes, g.N, g.M, g.ldp, g.out_plane_stride, 2, 64, "planes"));
+  p->plane_tma = 1;
   return kOk;
 }
 
@@ -1082,6 +1202,7 @@ int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
   if (S > 1) return launch_split_k(p, bn, S, g, stream);
   bool pingpong = false;
   TAPIR_RETURN_IF(pick_pingpong(tiles, p.num_k_blocks, g.planes, g.batch, &pingpong));
+  TAPIR_RETURN_IF(plane_store_params(g, pingpong, &p));
   return launch_gemm(bn, pingpong, p, g, stream);
 }
 

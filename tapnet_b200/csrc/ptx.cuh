@@ -99,6 +99,36 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       "r"(c4)
       : "memory");
 }
+// Makes this thread's generic-proxy shared-memory writes visible to later TMA (async-proxy) reads.
+__device__ __forceinline__ void fence_proxy_async_shared() {
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+// Shared (address `src`) -> global tile store, tracked in this thread's bulk async-groups.
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// Waits until at most N of this thread's bulk groups have not finished reading their source.
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// Waits until at most N of this thread's bulk groups are incomplete (their writes not yet done).
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// Four 8 x 8 b16 matrices to shared memory: register i holds matrix i in the mma fragment layout
+// (lane l: row l / 4, columns 2 (l % 4) + {0, 1}); lanes 8 i .. 8 i + 7 give its eight row addresses.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
 
 // ----------------------------------------------------------------------------- wgmma
 __device__ __forceinline__ void wgmma_fence() {
