@@ -98,6 +98,28 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[BLOCK_N / 2], uint64_t ade
   else ptx::wgmma_m64n128k16(d, adesc, bdesc, accumulate);
 }
 
+// Fused InstanceNorm statistics, per tile.  Each warp sums its 16 rows of a column in fp32 (a
+// shuffle over the 8 lanes that hold the column) and puts the fp64 (sum, sum of squares) into its
+// slot of the warpgroup's [4 warps][BLOCK_N][2] buffer in shared memory; under ping-pong the
+// second 64-row half adds to the first's slots.  flush_stats then sums the four warps' slots in
+// fp64 and issues one atomic per column and value: 2 BLOCK_N atomics per warpgroup and tile where
+// every warp used to issue its own (8x fewer under ping-pong, 4x under the cooperative schedule).
+template <int BLOCK_N>
+constexpr int kStatsSlotBytes = 4 * BLOCK_N * 2 * 8;  // per consumer warpgroup
+
+// Lanes 0-3 of a warp: its partials of columns cl, cl + 1 of the tile (st: sum cl, sum cl + 1,
+// square cl, square cl + 1) into its slots `red`, added to what they hold when `add`.
+__device__ __forceinline__ void put_stats(double* red, int cl, const float (&st)[4], bool add) {
+  double2* r = reinterpret_cast<double2*>(red + 2 * cl);
+  double2 a = make_double2(st[0], st[2]), b = make_double2(st[1], st[3]);
+  if (add) {
+    const double2 x = r[0], y = r[1];
+    a.x += x.x; a.y += x.y; b.x += y.x; b.y += y.y;
+  }
+  r[0] = a;
+  r[1] = b;
+}
+
 // Epilogue of a whole 64 x BLOCK_N accumulator whose rows and columns all exist, with the
 // options fixed at compile time and vector accesses only: straight-line code without branches,
 // so the compiler interleaves the independent column groups.  Each element goes through the
@@ -105,7 +127,8 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[BLOCK_N / 2], uint64_t ade
 template <int BLOCK_N, bool BIAS, bool GELU, bool RESID, bool F32, int PLANES, bool STATS>
 __device__ __forceinline__ void epilogue_full(const TcParams& p, const float (&acc)[BLOCK_N / 2],
                                               const float* const (&res_row)[2], float* const (&out_row)[2],
-                                              __nv_bfloat16* const (&pl_row)[2], int n0, int frame, int lane) {
+                                              __nv_bfloat16* const (&pl_row)[2], int n0, int lane, double* red,
+                                              bool add) {
 #pragma unroll
   for (int j = 0; j < BLOCK_N / 8; ++j) {
     const int c = n0 + 8 * j + 2 * (lane & 3);
@@ -132,13 +155,7 @@ __device__ __forceinline__ void epilogue_full(const TcParams& p, const float (&a
       for (int s = 4; s < 32; s <<= 1)
 #pragma unroll
         for (int e = 0; e < 4; ++e) st[e] += __shfl_xor_sync(0xffffffffu, st[e], s);
-      if (lane < 4) {
-        double* dst = p.stats + ((long long)frame * p.N + c) * 2;
-        atomicAdd(dst, (double)st[0]);
-        atomicAdd(dst + 1, (double)st[2]);
-        atomicAdd(dst + 2, (double)st[1]);
-        atomicAdd(dst + 3, (double)st[3]);
-      }
+      if (lane < 4) put_stats(red, c - n0, st, add);
     }
   }
 }
@@ -146,6 +163,7 @@ __device__ __forceinline__ void epilogue_full(const TcParams& p, const float (&a
 // Epilogue of one consumer warpgroup from its 64 x BLOCK_N accumulator in the wgmma fragment
 // layout: lane l of warp w holds tile rows 16 w + l / 4 (h = 0) and + 8 (h = 1), columns
 // 8 j + 2 (l % 4) + {0, 1} in acc[4 j + 2 h + {0, 1}].  row[h] / row_ok[h]: the global rows.
+// red / add: the warp's statistics slots (put_stats), used when p.stats is set.
 //
 // Tiles inside the output with the common option sets (GELU and two bf16 planes; fp32 with or
 // without residual and fused statistics; each with or without bias) take `epilogue_full`.
@@ -156,7 +174,7 @@ __device__ __forceinline__ void epilogue_full(const TcParams& p, const float (&a
 template <int BLOCK_N>
 __device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[BLOCK_N / 2],
                                          const long long (&row)[2], const bool (&row_ok)[2], int n0,
-                                         int frame, int lane, long long out_off) {
+                                         int lane, long long out_off, double* red, bool add) {
   const bool vec_r = p.residual != nullptr && (p.ldr & 1) == 0 && (reinterpret_cast<uintptr_t>(p.residual) & 7) == 0;
   const bool vec_o = p.out_f32 != nullptr && (p.ldo & 1) == 0 && (reinterpret_cast<uintptr_t>(p.out_f32) & 7) == 0;
   const bool vec_p = p.out_planes != nullptr && (p.ldp & 1) == 0 && (p.out_plane_stride & 1) == 0 &&
@@ -184,7 +202,7 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[B
     const bool bias = p.bias != nullptr, resid = p.residual != nullptr, stats = p.stats != nullptr;
 #define TAPIR_EPI_FULL(B, G, R, F, PL, S)                                                  \
     if (bias == B && resid == R && stats == S)                                              \
-      return epilogue_full<BLOCK_N, B, G, R, F, PL, S>(p, acc, res_row, out_row, pl_row, n0, frame, lane);
+      return epilogue_full<BLOCK_N, B, G, R, F, PL, S>(p, acc, res_row, out_row, pl_row, n0, lane, red, add);
     if (p.act == 1 && !resid && !stats && p.out_f32 == nullptr && p.out_P == 2 && vec_p) {
       TAPIR_EPI_FULL(true, true, false, false, 2, false)
       TAPIR_EPI_FULL(false, true, false, false, 2, false)
@@ -265,17 +283,24 @@ __device__ __forceinline__ void epilogue(const TcParams& p, const float (&acc)[B
       for (int s = 4; s < 32; s <<= 1)
 #pragma unroll
         for (int e = 0; e < 4; ++e) st[e] += __shfl_xor_sync(0xffffffffu, st[e], s);
-      if (lane < 4 && ok0) {
-        double* dst = p.stats + ((long long)frame * p.N + c) * 2;
-        atomicAdd(dst, (double)st[0]);
-        atomicAdd(dst + 1, (double)st[2]);
-        if (ok1) {
-          atomicAdd(dst + 2, (double)st[1]);
-          atomicAdd(dst + 3, (double)st[3]);
-        }
-      }
+      // every slot is written (zeros past N or the last row); flush_stats skips columns past N
+      if (lane < 4) put_stats(red, c - n0, st, add);
     }
   }
+}
+
+// The tile's statistics from the warpgroup's slots `red` (see kStatsSlotBytes): once all four
+// warps have put theirs (named barrier `bar`), per column and value the fp64 sum over the warps,
+// one atomic each.  The second barrier keeps the warpgroup's next tile from overwriting slots
+// that are still being read.
+template <int BLOCK_N>
+__device__ __forceinline__ void flush_stats(const TcParams& p, const double* red, int n0, int frame, uint32_t bar) {
+  ptx::named_bar_sync(bar, 128);
+  double* dst = p.stats + ((long long)frame * p.N + n0) * 2;
+  for (int i = threadIdx.x & 127; i < 2 * BLOCK_N; i += 128)
+    if (n0 + i / 2 < p.N)
+      atomicAdd(dst + i, red[i] + red[2 * BLOCK_N + i] + red[4 * BLOCK_N + i] + red[6 * BLOCK_N + i]);
+  ptx::named_bar_sync(bar, 128);
 }
 
 // Global row of tile row r (0..127) of output tile `m_tile`, and whether it exists.
@@ -294,20 +319,24 @@ __device__ __forceinline__ void tile_row(const TcParams& p, int m_tile, int r, l
   }
 }
 
-// Epilogue of rows [r_base, r_base + 64) of output tile `m_tile`, held by one consumer warpgroup.
+// Epilogue of rows [r_base, r_base + 64) of output tile `m_tile`, held by one consumer warpgroup;
+// `red`: the warpgroup's statistics slots (add: the tile's other half is already in them).
 template <int BLOCK_N>
 __device__ __forceinline__ void tile_epilogue(const TcParams& p, const float (&acc)[BLOCK_N / 2], int m_tile,
-                                              int r_base, int n0, int warp, int lane, long long out_off) {
+                                              int r_base, int n0, int warp, int lane, long long out_off,
+                                              double* red, bool add) {
   const int r0 = r_base + warp * 16 + (lane >> 2);
   long long row[2];
   bool row_ok[2];
   tile_row(p, m_tile, r0, row[0], row_ok[0]);
   tile_row(p, m_tile, r0 + 8, row[1], row_ok[1]);
-  int frame = 0;
-  if (p.stats != nullptr)
-    frame = (p.mode == kGemmConv3x3) ? m_tile / (p.tiles_x * p.tiles_y)
-                                     : (int)(((long long)m_tile * kBlockM) / p.rows_per_frame);
-  epilogue<BLOCK_N>(p, acc, row, row_ok, n0, frame, lane, out_off);
+  epilogue<BLOCK_N>(p, acc, row, row_ok, n0, lane, out_off, red + warp * 2 * BLOCK_N, add);
+}
+
+// The frame of output tile `m_tile` (tiles never straddle frames where statistics are fused).
+__device__ __forceinline__ int tile_frame(const TcParams& p, int m_tile) {
+  return (p.mode == kGemmConv3x3) ? m_tile / (p.tiles_x * p.tiles_y)
+                                  : (int)(((long long)m_tile * kBlockM) / p.rows_per_frame);
 }
 
 // Whether all rows and columns of output tile (m_tile, n0) exist.  Its 128 rows are consecutive
@@ -434,8 +463,9 @@ __device__ __forceinline__ void init_rings(uint64_t* bars, uint32_t empty_arriva
 }
 
 // The MMAs of one k-block, in the order of every kernel (plane pair (i, j), then k step), into
-// HALVES m64 accumulators (A rows 64 h on, 8 KB apart).  A plane i starts at a + i * a_plane with
-// its 8-row swizzle atoms `a_sbo` bytes apart; B plane j at b + j * b_plane.
+// HALVES m64 accumulators (A rows 64 h on: eight swizzle atoms, 8 a_sbo bytes, further).  A plane i
+// starts at a + i * a_plane with its 8-row swizzle atoms `a_sbo` bytes apart; B plane j at
+// b + j * b_plane.
 template <int BLOCK_N, int P, int HALVES>
 __device__ __forceinline__ void mma_k_block(float (&acc)[HALVES][BLOCK_N / 2], uint32_t a, uint32_t a_plane,
                                             uint32_t a_sbo, uint32_t b, uint32_t b_plane, uint32_t accumulate) {
@@ -445,7 +475,7 @@ __device__ __forceinline__ void mma_k_block(float (&acc)[HALVES][BLOCK_N / 2], u
     for (int j = 0; j < P - i; ++j) {
       uint64_t adesc[HALVES];
 #pragma unroll
-      for (int h = 0; h < HALVES; ++h) adesc[h] = ptx::make_smem_desc_sw128(a + i * a_plane + h * 64 * 128, a_sbo);
+      for (int h = 0; h < HALVES; ++h) adesc[h] = ptx::make_smem_desc_sw128(a + i * a_plane + h * 8 * a_sbo, a_sbo);
       const uint64_t bdesc = ptx::make_smem_desc_sw128(b + j * b_plane);
 #pragma unroll
       for (int k = 0; k < kBlockK / kMmaK; ++k) {
@@ -540,14 +570,27 @@ struct Ring {
   }
 };
 
+// Named barriers 3, 4: consumer 0's, consumer 1's epilogue staging (output boxes or statistics).
+constexpr uint32_t kStagingBarrier = 3;
+// setmaxnreg: registers of the producer and of each consumer warpgroup thread.  The consumers of
+// the ping-pong kernels hold 128 accumulators per thread at BLOCK_N = 128; the cooperative
+// kernel's straight-line epilogue with statistics spilled at the 168 registers of an even split.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+
 // Cooperative schedule: both consumer warpgroups work on every tile, 64 rows each, and run their
-// epilogues at the same time.  Used for split-K, P = 3 and CTAs with fewer than two tiles.
+// epilogues at the same time.  Used for split-K, P = 3 and CTAs with fewer than two tiles.  Each
+// warpgroup's statistics slots follow the ring.
+template <int BLOCK_N>
+constexpr int kCoopStaging = kConsumers * kStatsSlotBytes<BLOCK_N>;
+
 template <int BLOCK_N, int P>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_tc_kernel(const __grid_constant__ TcParams p) {
-  using Cfg = TcCfg<BLOCK_N, P>;
+  using Cfg = TcCfg<BLOCK_N, P, kCoopStaging<BLOCK_N>>;
+  static_assert(Cfg::kStages == TcCfg<BLOCK_N, P>::kStages, "the statistics slots must not cost the ring a stage");
   extern __shared__ uint8_t smem_raw[];
-  const Ring<BLOCK_N, P> ring(smem_raw, p, kConsumerArrivals);
+  const Ring<BLOCK_N, P, kCoopStaging<BLOCK_N>> ring(smem_raw, p, kConsumerArrivals);
 
   const int wg = threadIdx.x >> 7;
   const int warp = (threadIdx.x >> 5) & 3;  // within the warpgroup
@@ -558,13 +601,16 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
   const int num_work = p.num_m_tiles * p.num_n_tiles * p.split_k;
 
   if (wg == 0) {
+    ptx::setmaxnreg_dec<kProducerRegs>();
     if (threadIdx.x == 0) ring.produce(p);
     return;
   }
+  ptx::setmaxnreg_inc<kConsumerRegs>();
 
   // -------------------------------------------------------------------- consumers
   const int cw = wg - 1;                        // rows [64 cw, 64 cw + 64) of the tile
   const uint32_t a_off = (uint32_t)cw * 64 * 128;  // their A rows: eight whole swizzle atoms
+  double* red = reinterpret_cast<double*>(ring.staging + cw * kStatsSlotBytes<BLOCK_N>);
   StageCursor<Cfg::kStages> cur;
   float acc[1][BLOCK_N / 2];
   for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
@@ -584,7 +630,8 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
     ptx::reg_fence(acc[0]);
     if (prev >= 0 && lane == 0) ptx::mbar_arrive(&ring.empty_bar[prev]);
     tile_epilogue<BLOCK_N>(p, acc[0], m_tile, cw * 64, n0, warp, lane,
-                           split * p.split_stride + bat * p.out_batch_stride);
+                           split * p.split_stride + bat * p.out_batch_stride, red, false);
+    if (p.stats != nullptr) flush_stats<BLOCK_N>(p, red, n0, tile_frame(p, m_tile), kStagingBarrier + cw);
   }
 }
 
@@ -600,12 +647,11 @@ gemm_tc_kernel(const __grid_constant__ TcParams p) {
 // on has completed all earlier fills and is never a whole phase behind.
 //
 // Every output element sums its K terms in the cooperative kernel's order, so the two schedules
-// give bit-identical outputs (the fused statistics keep its per-warp partials as well; only the
-// order of their fp64 atomics may differ, as it may between two runs of either kernel).
-constexpr int kProducerRegs = 40;
-constexpr int kPingPongRegs = 232;  // 128 accumulators per thread at BLOCK_N = 128
+// give bit-identical outputs (the fused statistics keep its per-warp fp32 partials as well; only
+// the order of their fp64 additions differs, as the order of the atomics may between two runs of
+// either kernel).  A tile's statistics slots share the warpgroup's output box buffers: a GEMM
+// with statistics has no plane output.
 constexpr uint32_t kTurnBarrier = 1;  // named barriers 1, 2: consumer 0's, consumer 1's turn
-constexpr uint32_t kStagingBarrier = 3;  // named barriers 3, 4: consumer 0's, consumer 1's box buffers
 
 template <int BLOCK_N, int P>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -613,6 +659,7 @@ gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
   using Cfg = TcCfg<BLOCK_N, P, kPlaneStagingBytes>;
   static_assert(P <= 2, "ping-pong: P = 3 stays cooperative");
   static_assert(Cfg::kStages == TcCfg<BLOCK_N, P>::kStages, "the output staging must not cost the ring a stage");
+  static_assert(kStatsSlotBytes<BLOCK_N> <= 2 * kPlaneBoxBytes, "statistics slots: one warpgroup's box buffers");
   extern __shared__ uint8_t smem_raw[];
   const Ring<BLOCK_N, P, kPlaneStagingBytes> ring(smem_raw, p, 4);  // one arrive per warp of the reading warpgroup
 
@@ -626,7 +673,7 @@ gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
     if (threadIdx.x == 0) ring.produce(p);
     return;
   }
-  ptx::setmaxnreg_inc<kPingPongRegs>();
+  ptx::setmaxnreg_inc<kConsumerRegs>();
 
   const int cw = wg - 1;
   const int nkb = p.num_k_blocks;
@@ -658,14 +705,16 @@ gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
     ptx::reg_fence(acc[1]);
     if (lane == 0) ptx::mbar_arrive(&ring.empty_bar[prev]);
     const bool staged = p.plane_tma && whole_tile<BLOCK_N>(p, m_tile, n0);
+    uint8_t* const staging = ring.staging + cw * 2 * kPlaneBoxBytes;
+    double* const red = reinterpret_cast<double*>(staging);
     // one copy of the epilogue code for both halves: it runs while the other warpgroup's mainloop
     // executes from the same instruction cache
 #pragma unroll 1
     for (int h = 0; h < 2; ++h) {
       if (!staged) {
-        tile_epilogue<BLOCK_N>(p, acc[0], m_tile, 64 * h, n0, warp, lane, bat * p.out_batch_stride);
+        tile_epilogue<BLOCK_N>(p, acc[0], m_tile, 64 * h, n0, warp, lane, bat * p.out_batch_stride, red, h == 1);
       } else {
-        const uint32_t boxes = ptx::smem_u32(ring.staging) + (uint32_t)(cw * 2 * kPlaneBoxBytes);
+        const uint32_t boxes = ptx::smem_u32(staging);
         if (p.bias != nullptr)
           epilogue_planes_tma<BLOCK_N, true>(p, acc[0], m_tile, 64 * h, n0, boxes, kStagingBarrier + cw, warp, lane);
         else
@@ -676,6 +725,7 @@ gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
         for (int i = 0; i < BLOCK_N / 2; ++i) acc[0][i] = acc[1][i];
       }
     }
+    if (p.stats != nullptr) flush_stats<BLOCK_N>(p, red, n0, tile_frame(p, m_tile), kStagingBarrier + cw);
     // after the warpgroup's last tile: its stores complete while the shared memory still exists
     if (t + 2 >= my_tiles && warp == 0 && lane == 0) ptx::bulk_wait<0>();
   }
@@ -686,10 +736,12 @@ gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
 // loads one shifted 128-pixel box per tap, so every input element crosses L2 -> SM nine times.
 // Here a tile of 8 x 16 output pixels stages its 10 x 18 input patch ONCE (18 TMA loads of one
 // patch row each into rows padded to 16 pixels = 2048 B, so that every 8-pixel group of every tap
-// view has the same swizzle phase) and the nine taps are nine shared-memory views of it: consumer
-// c (output rows 8c .. 8c + 7 of the tile) reads start = patch + (8c + ky) * 2048 + kx * 128, with
-// 2048 B between its 8-pixel row groups.  B (weights, 8 KB per tap and plane) streams through a
-// 4-slot ring.  Epilogue as in gemm_tc_kernel.
+// view has the same swizzle phase) and the nine taps are nine shared-memory views of it: output
+// rows 8c .. 8c + 7 of the tile (one m64 wgmma) read start = patch + (8c + ky) * 2048 + kx * 128,
+// with 2048 B between their 8-pixel row groups.  B (weights, 8 KB per tap and plane) streams
+// through a 4-slot ring.  Two schedules, as the GEMM's: conv3x3_halo_kernel (cooperative, consumer
+// c computes rows 8c .. 8c + 7 of every tile) and conv3x3_halo_pingpong_kernel (each consumer
+// whole tiles, both halves).  Epilogue as in the GEMM kernels.
 constexpr int kHaloTileW = 8, kHaloTileH = 16;
 constexpr int kHaloRowBytes = 2048;                        // 16 pixels x 128 B
 constexpr int kHaloPatchRows = kHaloTileH + 2;
@@ -698,41 +750,45 @@ constexpr int kHaloRowLoadBytes = (kHaloTileW + 2) * 128;  // what one TMA row l
 constexpr int kHaloPatchStages = 2;
 constexpr int kHaloBStages = 4;
 constexpr int kHaloBBytes = 64 * 128;                      // per plane and tap
+constexpr int kHaloStatsBytes = kConsumers * kStatsSlotBytes<64>;
 template <int P>
 struct HaloCfg {
   static constexpr int kPatchStage = P * kHaloPatchBytes;
   static constexpr int kBStage = P * kHaloBBytes;
-  static constexpr int kSmemBytes = 1024 + kHaloPatchStages * kPatchStage + kHaloBStages * kBStage + kBarrierBytes;
-  static_assert(kSmemBytes <= kSmemLimit, "halo conv: shared memory");
+  static constexpr int kSmemBytes =
+      1024 + kHaloPatchStages * kPatchStage + kHaloBStages * kBStage + kHaloStatsBytes + kBarrierBytes;
+  static_assert(kSmemBytes <= kSmemLimit, "halo conv: the rings and the statistics slots must fit as they are");
 };
 
+// Shared memory of both halo schedules: the patch ring [2][P][18][2048], the B ring [4][P][64][128],
+// the consumers' statistics slots, then the full / empty barriers of the two rings.
 template <int P>
-__global__ void __launch_bounds__(kThreads, 1)
-conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
+struct HaloRing {
   using Cfg = HaloCfg<P>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = aligned_smem(smem_raw);
-  uint8_t* patch = smem;                                           // [2][P][18][2048]
-  uint8_t* bring = smem + kHaloPatchStages * Cfg::kPatchStage;     // [4][P][64][128]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(bring + kHaloBStages * Cfg::kBStage);
-  uint64_t* pfull = bars;                    // [2]
-  uint64_t* pempty = bars + 2;               // [2]
-  uint64_t* bfull = bars + 4;                // [4]
-  uint64_t* bempty = bars + 8;               // [4]
+  uint8_t* patch;
+  uint8_t* bring;
+  double* stats;
+  uint64_t* pfull;   // [2]
+  uint64_t* pempty;  // [2]
+  uint64_t* bfull;   // [4]
+  uint64_t* bempty;  // [4]
+  __device__ __forceinline__ HaloRing(uint8_t* smem_raw, const TcParams& p, uint32_t empty_arrivals) {
+    patch = aligned_smem(smem_raw);
+    bring = patch + kHaloPatchStages * Cfg::kPatchStage;
+    stats = reinterpret_cast<double*>(bring + kHaloBStages * Cfg::kBStage);
+    pfull = reinterpret_cast<uint64_t*>(bring + kHaloBStages * Cfg::kBStage + kHaloStatsBytes);
+    pempty = pfull + kHaloPatchStages;
+    bfull = pempty + kHaloPatchStages;
+    bempty = bfull + kHaloBStages;
+    init_rings(pfull, empty_arrivals, &p.tmPatch, &p.tmB, kHaloPatchStages, kHaloBStages);
+  }
 
-  const int wg = threadIdx.x >> 7;
-  const int warp = (threadIdx.x >> 5) & 3;
-  const int lane = threadIdx.x & 31;
-  init_rings(bars, kConsumerArrivals, &p.tmPatch, &p.tmB, kHaloPatchStages, kHaloBStages);
-  __syncthreads();
-  const int num_work = p.num_m_tiles;
-  const int per_frame = p.tiles_x * p.tiles_y;
-
-  if (wg == 0) {
-    if (threadIdx.x != 0) return;
+  // TMA producer (one thread): per tile of this CTA, its patch, then its nine taps of B.
+  __device__ __forceinline__ void produce(const TcParams& p) const {
+    const int per_frame = p.tiles_x * p.tiles_y;
     StageCursor<kHaloPatchStages> pc;
     StageCursor<kHaloBStages> bc;
-    for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+    for (int w = blockIdx.x; w < p.num_m_tiles; w += gridDim.x) {
       const int frame = w / per_frame;
       const int r = w - frame * per_frame;
       const int y0 = (r / p.tiles_x) * kHaloTileH, x0 = (r % p.tiles_x) * kHaloTileW;
@@ -753,42 +809,135 @@ conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
         bc.advance();
       }
     }
+  }
+};
+
+template <int P>
+__global__ void __launch_bounds__(kThreads, 1)
+conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
+  using Cfg = HaloCfg<P>;
+  extern __shared__ uint8_t smem_raw[];
+  const HaloRing<P> ring(smem_raw, p, kConsumerArrivals);
+
+  const int wg = threadIdx.x >> 7;
+  const int warp = (threadIdx.x >> 5) & 3;
+  const int lane = threadIdx.x & 31;
+  __syncthreads();
+
+  if (wg == 0) {
+    if (threadIdx.x == 0) ring.produce(p);
     return;
   }
 
   const int cw = wg - 1;
+  double* red = ring.stats + cw * (kStatsSlotBytes<64> / 8);
   StageCursor<kHaloPatchStages> pc;
   StageCursor<kHaloBStages> bc;
   float acc[1][32];
-  for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
+  for (int w = blockIdx.x; w < p.num_m_tiles; w += gridDim.x) {
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[0][i] = 0.f;
-    ptx::mbar_wait(&pfull[pc.stage], pc.phase, p.err, 404);
-    const uint32_t pbase = ptx::smem_u32(patch + pc.stage * Cfg::kPatchStage) + (uint32_t)cw * 8 * kHaloRowBytes;
+    ptx::mbar_wait(&ring.pfull[pc.stage], pc.phase, p.err, 404);
+    const uint32_t pbase = ptx::smem_u32(ring.patch + pc.stage * Cfg::kPatchStage) + (uint32_t)cw * 8 * kHaloRowBytes;
     int prev = -1;
     for (int tap = 0; tap < 9; ++tap) {
       const int ky = tap / 3, kx = tap - ky * 3;
-      consume_k_block<64, P, 1>(acc, &bfull[bc.stage], bc.phase, p, 405,
+      consume_k_block<64, P, 1>(acc, &ring.bfull[bc.stage], bc.phase, p, 405,
                                 pbase + ky * kHaloRowBytes + kx * 128, kHaloPatchBytes, kHaloRowBytes,
-                                ptx::smem_u32(bring + bc.stage * Cfg::kBStage), kHaloBBytes, tap > 0, bempty, prev, lane);
+                                ptx::smem_u32(ring.bring + bc.stage * Cfg::kBStage), kHaloBBytes, tap > 0,
+                                ring.bempty, prev, lane);
       prev = bc.stage;
       bc.advance();
     }
     ptx::wgmma_wait<0>();
     ptx::reg_fence(acc[0]);
     if (lane == 0) {
-      ptx::mbar_arrive(&bempty[prev]);
-      ptx::mbar_arrive(&pempty[pc.stage]);
+      ptx::mbar_arrive(&ring.bempty[prev]);
+      ptx::mbar_arrive(&ring.pempty[pc.stage]);
     }
     pc.advance();
+    tile_epilogue<64>(p, acc[0], w, cw * 64, 0, warp, lane, 0, red, false);
+    if (p.stats != nullptr) flush_stats<64>(p, red, 0, tile_frame(p, w), kStagingBarrier + cw);
+  }
+}
 
-    const int frame = w / per_frame;
-    long long row[2];
-    bool row_ok[2];
-    const int r0 = cw * 64 + warp * 16 + (lane >> 2);
-    tile_row(p, w, r0, row[0], row_ok[0]);
-    tile_row(p, w, r0 + 8, row[1], row_ok[1]);
-    epilogue<64>(p, acc[0], row, row_ok, 0, frame, lane, 0);
+// Ping-pong halo convolution: as gemm_tc_pingpong_kernel, each consumer warpgroup owns whole
+// tiles, alternately, and per tap issues two m64n64 wgmma on the views of output rows 0-7 and
+// 8-15 (2 x 32 accumulators), passes the tensor pipe to the other warpgroup once its nine taps
+// are issued, and runs its epilogue while the other's MMAs execute.
+//
+// Parity waits.  The producer fills the patch stages in tile order, so local tile t of the CTA
+// uses patch stage t % 2: warpgroup c always reads stage c, and its fills alternate with no one
+// else's; it waits for fill t / 2 with parity (t / 2) & 1 and releases the stage once the tile's
+// MMAs have retired, and the producer then refills it for tile t + 2.  The B ring holds tile t's
+// nine taps at ring positions 9 t .. 9 t + 8, and each stage is read by whichever warpgroup owns
+// the tile.  A warpgroup waits on its tile's first B stage only after the other has passed the
+// turn, that is after it has waited on every B stage of tile t - 1, so every earlier fill of the
+// stage it waits on has completed and that stage is never a whole phase behind: the parity
+// (position / 4) & 1 is exact.
+template <int P>
+__global__ void __launch_bounds__(kThreads, 1)
+conv3x3_halo_pingpong_kernel(const __grid_constant__ TcParams p) {
+  using Cfg = HaloCfg<P>;
+  extern __shared__ uint8_t smem_raw[];
+  const HaloRing<P> ring(smem_raw, p, 4);  // one arrive per warp of the reading warpgroup
+
+  const int wg = threadIdx.x >> 7;
+  const int warp = (threadIdx.x >> 5) & 3;
+  const int lane = threadIdx.x & 31;
+  __syncthreads();
+
+  if (wg == 0) {
+    ptx::setmaxnreg_dec<kProducerRegs>();
+    if (threadIdx.x == 0) ring.produce(p);
+    return;
+  }
+  ptx::setmaxnreg_inc<kConsumerRegs>();
+
+  const int cw = wg - 1;
+  const int my_tiles = (p.num_m_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  double* red = ring.stats + cw * (kStatsSlotBytes<64> / 8);
+  const uint32_t pbase = ptx::smem_u32(ring.patch + cw * Cfg::kPatchStage);  // patch stage cw
+  float acc[2][32];  // output rows 0-7, rows 8-15 of the tile
+  for (int t = cw; t < my_tiles; t += 2) {
+    const int w = (int)blockIdx.x + t * (int)gridDim.x;
+    if (t > 0) ptx::named_bar_sync(kTurnBarrier + cw, 256);
+    const int pos = 9 * t;  // ring position of the tile's first tap
+    StageCursor<kHaloBStages> bc{pos % kHaloBStages, (uint32_t)(pos / kHaloBStages) & 1u};
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+    ptx::mbar_wait(&ring.pfull[cw], (uint32_t)(t >> 1) & 1u, p.err, 406);
+    int prev = -1;
+    for (int tap = 0; tap < 9; ++tap) {
+      const int ky = tap / 3, kx = tap - ky * 3;
+      consume_k_block<64, P, 2>(acc, &ring.bfull[bc.stage], bc.phase, p, 407,
+                                pbase + ky * kHaloRowBytes + kx * 128, kHaloPatchBytes, kHaloRowBytes,
+                                ptx::smem_u32(ring.bring + bc.stage * Cfg::kBStage), kHaloBBytes, tap > 0,
+                                ring.bempty, prev, lane);
+      prev = bc.stage;
+      bc.advance();
+    }
+    // every MMA of this tile is issued: the other warpgroup's tile, if it has one, may start
+    if (t + 1 < my_tiles) ptx::named_bar_arrive(kTurnBarrier + (1 - cw), 256);
+    ptx::wgmma_wait<0>();
+    ptx::reg_fence(acc[0]);
+    ptx::reg_fence(acc[1]);
+    if (lane == 0) {
+      ptx::mbar_arrive(&ring.bempty[prev]);
+      ptx::mbar_arrive(&ring.pempty[cw]);
+    }
+    // one copy of the epilogue code for both halves (see gemm_tc_pingpong_kernel)
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      tile_epilogue<64>(p, acc[0], w, 64 * h, 0, warp, lane, 0, red, h == 1);
+      if (h == 0) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i];
+      }
+    }
+    if (p.stats != nullptr) flush_stats<64>(p, red, 0, tile_frame(p, w), kStagingBarrier + cw);
   }
 }
 
@@ -941,7 +1090,8 @@ int launch_gemm(bool pingpong, const TcParams& p, const GemmArgs& g, cudaStream_
     if (pingpong)
       return launch<gemm_tc_pingpong_kernel<BLOCK_N, P>, TcCfg<BLOCK_N, P, kPlaneStagingBytes>::kSmemBytes>(
           "gemm_tc_pingpong_kernel", p, g, stream);
-  return launch<gemm_tc_kernel<BLOCK_N, P>, TcCfg<BLOCK_N, P>::kSmemBytes>("gemm_tc_kernel", p, g, stream);
+  return launch<gemm_tc_kernel<BLOCK_N, P>, TcCfg<BLOCK_N, P, kCoopStaging<BLOCK_N>>::kSmemBytes>("gemm_tc_kernel", p,
+                                                                                                 g, stream);
 }
 
 // The GEMM kernel for tile width `bn` and g.planes; ping-pong only where pick_pingpong chose it.
@@ -962,17 +1112,27 @@ int launch_gemm(int bn, bool pingpong, const TcParams& p, const GemmArgs& g, cud
 // four tiles of short (< 16 k-block) mainloops: mixer linear_in / linear_out, 2.9 tiles of 8-9
 // k-blocks, ran 10-22 % slower.  Split-K work items, P = 3 and batched GEMMs (only the P = 3 cost
 // volume is batched) stay cooperative.  TAPIR_B200_GEMM_SCHEDULE=coop|pingpong forces one schedule
-// wherever both are legal; it is read on every call and any other value is an error.
-int pick_pingpong(int tiles, int num_k_blocks, int P, int batch, bool* pingpong) {
-  *pingpong = false;
-  const char* force = getenv("TAPIR_B200_GEMM_SCHEDULE");
-  if (force != nullptr && strcmp(force, "coop") != 0 && strcmp(force, "pingpong") != 0) {
-    set_error("TAPIR_B200_GEMM_SCHEDULE=%s: expected coop or pingpong", force);
+// wherever both are legal (the GEMM kernels and the halo convolution); it is read on every call
+// and any other value is an error.  *force: 0 (not set), 1 (coop) or 2 (pingpong).
+int forced_schedule(int* force) {
+  *force = 0;
+  const char* e = getenv("TAPIR_B200_GEMM_SCHEDULE");
+  if (e == nullptr) return kOk;
+  if (strcmp(e, "coop") != 0 && strcmp(e, "pingpong") != 0) {
+    set_error("TAPIR_B200_GEMM_SCHEDULE=%s: expected coop or pingpong", e);
     return kBadArgument;
   }
+  *force = strcmp(e, "pingpong") == 0 ? 2 : 1;
+  return kOk;
+}
+
+int pick_pingpong(int tiles, int num_k_blocks, int P, int batch, bool* pingpong) {
+  *pingpong = false;
+  int force;
+  TAPIR_RETURN_IF(forced_schedule(&force));
   if (P > 2 || batch > 1) return kOk;
-  if (force != nullptr) {
-    *pingpong = strcmp(force, "pingpong") == 0;
+  if (force != 0) {
+    *pingpong = force == 2;
     return kOk;
   }
   const int sms = num_sms();
@@ -1084,6 +1244,9 @@ bool use_halo(const GemmArgs& g) {
   return on && g.mode == kGemmConv3x3 && g.C == 64 && g.N == 64 && g.planes <= 2 && g.out_planes == nullptr;
 }
 
+// Ping-pong wherever a CTA gets at least two tiles (the clip's 48 frames at 128 x 128: 6144 tiles);
+// the single-frame streaming passes (128 tiles) stay cooperative.  TAPIR_B200_GEMM_SCHEDULE forces
+// either schedule (pick_pingpong).
 int launch_halo(TcParams p, const GemmArgs& g, cudaStream_t stream) {
   p.tileW = kHaloTileW;
   p.tileH = kHaloTileH;
@@ -1091,8 +1254,16 @@ int launch_halo(TcParams p, const GemmArgs& g, cudaStream_t stream) {
   p.tiles_y = ceil_div(g.H, kHaloTileH);
   p.num_m_tiles = g.frames * p.tiles_x * p.tiles_y;
   p.num_n_tiles = 1;
+  int force;
+  TAPIR_RETURN_IF(forced_schedule(&force));
+  const bool pingpong = force != 0 ? force == 2 : p.num_m_tiles >= 2 * num_sms();
   TAPIR_RETURN_IF(encode_nhwc_map(&p.tmPatch, g, kHaloTileW + 2, 1, "A/patch"));
   TAPIR_RETURN_IF(encode_rows_map(&p.tmB, g.b, g.K, g.N, g.ldb, g.b_plane_stride, g.planes, 64, "B/halo"));
+  if (pingpong) {
+    if (g.planes == 1)
+      return launch<conv3x3_halo_pingpong_kernel<1>, HaloCfg<1>::kSmemBytes>("conv3x3_halo_pingpong_kernel", p, g, stream);
+    return launch<conv3x3_halo_pingpong_kernel<2>, HaloCfg<2>::kSmemBytes>("conv3x3_halo_pingpong_kernel", p, g, stream);
+  }
   if (g.planes == 1) return launch<conv3x3_halo_kernel<1>, HaloCfg<1>::kSmemBytes>("conv3x3_halo_kernel", p, g, stream);
   return launch<conv3x3_halo_kernel<2>, HaloCfg<2>::kSmemBytes>("conv3x3_halo_kernel", p, g, stream);
 }
