@@ -105,19 +105,6 @@ def time_us(call, reps, flush):
   return [a.elapsed_time(b) * 1e3 for a, b in evs]
 
 
-def with_env(env, fn):
-  old = {k: os.environ.get(k) for k in env}
-  os.environ.update(env)
-  try:
-    return fn()
-  finally:
-    for k, v in old.items():
-      if v is None:
-        os.environ.pop(k, None)
-      else:
-        os.environ[k] = v
-
-
 def card():
   q = 'name,power.limit,clocks.max.sm,clocks.sm'
   try:
@@ -142,7 +129,8 @@ def main():
     for i, call in enumerate(calls):
       for v, env, st in VARIANTS:
         with_stats = st and rows[i][7]
-        ts[(i, v)] += with_env(env, lambda: time_us(lambda: call(with_stats), a.reps, flush))
+        with U.switches(**env):
+          ts[(i, v)] += time_us(lambda: call(with_stats), a.reps, flush)
   names = [v for v, _, _ in VARIANTS]
   print(f'{"launch":12s} {"path":6s} {"M":>7s} {"N":>4s} {"K":>5s} {"res":>3s} {"st":>2s} '
         + ' '.join(f'{n + " us":>12s}' for n in names) + f' {"MMA us":>8s} {"HBM us":>8s}')

@@ -5,8 +5,6 @@
                                              schedules (TAPIR_B200_GEMM_SCHEDULE), alternated
   python scripts/gemm_bench.py --tile-cost   time per launch against tile count at constant MMA
                                              work, both schedules and BLOCK_N = 64 / 128
-  python scripts/gemm_bench.py --plane-store the GELU + two-plane GEMMs under both plane store
-                                             paths (TAPIR_B200_PLANE_STORE), alternated
 """
 import argparse
 import ctypes
@@ -114,17 +112,10 @@ def compare_schedules(rounds, reps):
   for name, kw in CLIP:
     call, _, _ = make(**kw)
     ts = {'coop': [], 'pingpong': []}
-    old = os.environ.get('TAPIR_B200_GEMM_SCHEDULE')
-    try:
-      for _ in range(rounds):
-        for s in ts:
-          os.environ['TAPIR_B200_GEMM_SCHEDULE'] = s
+    for _ in range(rounds):
+      for s in ts:
+        with U.switches(TAPIR_B200_GEMM_SCHEDULE=s):
           ts[s] += time_ms(call, reps, True)
-    finally:
-      if old is None:
-        os.environ.pop('TAPIR_B200_GEMM_SCHEDULE', None)
-      else:
-        os.environ['TAPIR_B200_GEMM_SCHEDULE'] = old
     med = {s: statistics.median(v) * 1e3 for s, v in ts.items()}
     cells = [f'{med[s]:8.1f} ({min(v) * 1e3:.1f}-{max(v) * 1e3:.1f})' for s, v in ts.items()]
     print(f'{name:34s} {cells[0]:>24s} {cells[1]:>24s} {1 - med["pingpong"] / med["coop"]:6.1%}', flush=True)
@@ -150,19 +141,6 @@ def _card():
     return f'{torch.cuda.get_device_name()} (nvidia-smi unavailable)'
 
 
-def _with_env(env, fn):
-  old = {k: os.environ.get(k) for k in env}
-  os.environ.update(env)
-  try:
-    return fn()
-  finally:
-    for k, v in old.items():
-      if v is None:
-        os.environ.pop(k, None)
-      else:
-        os.environ[k] = v
-
-
 def tile_cost(rounds, reps):
   """Time per launch against tile count at constant MMA work: every shape x epilogue x schedule x
   BLOCK_N, alternated `rounds` times in this process (L2 flushed before every launch), median of
@@ -179,8 +157,8 @@ def tile_cost(rounds, reps):
   for _ in range(rounds):
     for c in configs:
       shape_epi, sched, bn = c
-      env = {'TAPIR_B200_GEMM_SCHEDULE': sched, 'TAPIR_B200_BLOCK_N': str(bn)}
-      ts[c] += _with_env(env, lambda: time_ms(calls[shape_epi], reps, True))
+      with U.switches(TAPIR_B200_GEMM_SCHEDULE=sched, TAPIR_B200_BLOCK_N=bn):
+        ts[c] += time_ms(calls[shape_epi], reps, True)
   print(f'{"M x N x K":>18s} {"epilogue":>12s} {"sched":>8s} {"BN":>3s} {"tiles":>5s} {"t/CTA":>5s} '
         f'{"kb/t":>4s} {"us/launch (min-max)":>22s} {"us/tile":>8s} {"us/kblk":>8s} {"TF/s":>6s} {"out MB":>7s}')
   for c in configs:
@@ -197,37 +175,9 @@ def tile_cost(rounds, reps):
           flush=True)
 
 
-PLANE_STORE_SHAPES = [
-    ('up: gelu+planes', dict(M=12288, N=2048, K=512, gelu=True, planes_out=2, f32_out=False)),
-    ('up: f32 out, no bias', dict(M=12288, N=2048, K=512, bias=False)),
-    ('extra conv 256->1024 gelu+planes', dict(M=0, N=1024, K=0, gelu=True, planes_out=2, f32_out=False,
-                                              conv=(48, 32, 32, 256))),
-]
-
-
-def compare_plane_store(rounds, reps):
-  """The GELU + two-plane GEMMs under both plane store paths (TAPIR_B200_PLANE_STORE), ping-pong
-  schedule, alternated `rounds` times in this process (L2 flushed before every launch); the fp32
-  `up` row, which neither path touches, is the floor."""
-  print(f'card: {_card()}')
-  print(f'{"shape":34s} {"regs us (min-max)":>24s} {"tma us (min-max)":>24s} {"gain":>6s}')
-  for name, kw in PLANE_STORE_SHAPES:
-    call, _, _ = make(**kw)
-    ts = {'regs': [], 'tma': []}
-    for _ in range(rounds):
-      for s in ts:
-        env = {'TAPIR_B200_GEMM_SCHEDULE': 'pingpong', 'TAPIR_B200_PLANE_STORE': s}
-        ts[s] += _with_env(env, lambda: time_ms(call, reps, True))
-    med = {s: statistics.median(v) * 1e3 for s, v in ts.items()}
-    cells = [f'{med[s]:8.1f} ({min(v) * 1e3:.1f}-{max(v) * 1e3:.1f})' for s, v in ts.items()]
-    print(f'{name:34s} {cells[0]:>24s} {cells[1]:>24s} {1 - med["tma"] / med["regs"]:6.1%}', flush=True)
-
-
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--schedules', action='store_true', help='compare the two wgmma schedules')
-  ap.add_argument('--plane-store', action='store_true',
-                  help='compare the TMA and register plane stores of the GELU + planes GEMMs')
   ap.add_argument('--tile-cost', action='store_true',
                   help='time per launch against tile count at constant MMA work')
   ap.add_argument('--rounds', type=int, default=3)
@@ -239,9 +189,6 @@ def main():
     return
   if a.tile_cost:
     tile_cost(a.rounds, a.reps)
-    return
-  if a.plane_store:
-    compare_plane_store(a.rounds, a.reps)
     return
   print('BLOCK_N override:', os.environ.get('TAPIR_B200_BLOCK_N', 'auto'))
   print('schedule override:', os.environ.get('TAPIR_B200_GEMM_SCHEDULE', 'auto'))

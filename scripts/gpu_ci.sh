@@ -30,7 +30,6 @@ for t in $TIERS; do
     yuv)         run yuv "X=1" tests/test_yuv_gpu.py ;;
     bulk)        run bulk "X=1" tests/test_bulk_gpu.py ;;
     no_halo)     run no_halo "TAPIR_B200_CONV_HALO=0" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_exact_gpu.py tests/test_stages_gpu.py tests/test_end_to_end_gpu.py ;;
-    no_splitk)   run no_splitk "TAPIR_B200_SPLITK=0" tests/test_gemm_variants_gpu.py tests/test_gemm_exact_gpu.py tests/test_stages_gpu.py tests/test_properties_gpu.py tests/test_batched_gpu.py "tests/test_backbone_ops_gpu.py::test_backbone_vs_fp64_oracle" "tests/test_backbone_ops_gpu.py::test_backbone_frame_chunks_are_independent" ;;
     all)         run all "X=1" tests ;;
   esac
 done

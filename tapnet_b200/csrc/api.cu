@@ -77,8 +77,10 @@ int tapir_gemm_ex(const void* a_planes, int32_t lda, int64_t a_plane_stride, con
   g.splitk_ws = static_cast<float*>(splitk_workspace);
   g.splitk_ws_bytes = splitk_workspace != nullptr ? splitk_workspace_bytes : 0;
   g.allow_splitk = splitk_workspace != nullptr;
+  GemmSwitches sw;  // validated here whichever kernel `impl` names; sw.simt is not used
+  TAPIR_RETURN_IF(read_gemm_switches(&sw));
   if (impl == 1) return gemm_simt(g, S(stream));
-  if (impl == 0) return gemm_tc(g, S(stream));
+  if (impl == 0) return gemm_tc(g, sw, S(stream));
   set_error("tapir_gemm: impl must be 0 (wgmma) or 1 (simt)");
   return kBadArgument;
 }

@@ -77,12 +77,28 @@ inline GemmArgs gemm_args(const tapir_linear& l) {
   return g;
 }
 
+// Overrides of the GEMM dispatcher's choices, from environment variables.  read_gemm_switches reads
+// all four on every GEMM call, whether the call uses them or not.  Unset leaves the choice to the
+// dispatcher; any other value than those listed, the empty string included, fails the call with
+// kBadArgument before anything is launched.
+//   TAPIR_B200_GEMM           tc | simt        simt: gemm() runs the SIMT cross-check kernel
+//   TAPIR_B200_BLOCK_N        64 | 128         the wgmma kernel's tile width
+//   TAPIR_B200_GEMM_SCHEDULE  coop | pingpong  the wgmma schedule, wherever both are legal
+//   TAPIR_B200_CONV_HALO      0 | 1            0: C = 64 3x3 convolutions take the generic path
+struct GemmSwitches {
+  bool simt = false;
+  int block_n = 0;   // 0: not set
+  int schedule = 0;  // 0: not set, 1: coop, 2: pingpong
+  bool halo = true;
+};
+int read_gemm_switches(GemmSwitches* sw);
+
 int validate_gemm_args(const GemmArgs& g);
 // wgmma + TMA implementation (the product path).
-int gemm_tc(const GemmArgs& g, cudaStream_t stream);
+int gemm_tc(const GemmArgs& g, const GemmSwitches& sw, cudaStream_t stream);
 // Straightforward SIMT implementation of the same arithmetic (verification / bring-up).
 int gemm_simt(const GemmArgs& g, cudaStream_t stream);
-// Dispatches on TAPIR_B200_GEMM (default "tc").
+// gemm_simt under TAPIR_B200_GEMM=simt, else gemm_tc.
 int gemm(const GemmArgs& g, cudaStream_t stream);
 
 }  // namespace tapir

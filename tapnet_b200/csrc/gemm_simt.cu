@@ -3,9 +3,6 @@
 // switch (TAPIR_B200_GEMM=simt).  It reconstructs a = sum_i A_i, b = sum_j B_j in fp32 and
 // runs a shared-memory tiled fp32 GEMM; versus the tensor-core path it additionally contains
 // the dropped (i + j >= P) cross terms, i.e. it differs by <= 2^-16 relative for P=2.
-#include <cstdlib>
-#include <cstring>
-
 #include "gemm.cuh"
 
 namespace tapir {
@@ -133,12 +130,9 @@ int gemm_simt(const GemmArgs& g, cudaStream_t stream) {
 }
 
 int gemm(const GemmArgs& g, cudaStream_t stream) {
-  static int use_simt = -1;
-  if (use_simt < 0) {
-    const char* e = getenv("TAPIR_B200_GEMM");
-    use_simt = (e != nullptr && strcmp(e, "simt") == 0) ? 1 : 0;
-  }
-  return use_simt ? gemm_simt(g, stream) : gemm_tc(g, stream);
+  GemmSwitches sw;
+  TAPIR_RETURN_IF(read_gemm_switches(&sw));
+  return sw.simt ? gemm_simt(g, stream) : gemm_tc(g, sw, stream);
 }
 
 }  // namespace tapir

@@ -1111,47 +1111,21 @@ int launch_gemm(int bn, bool pingpong, const TcParams& p, const GemmArgs& g, cud
 // tiles per CTA, and measured on H100 it loses to the cooperative kernel when CTAs get fewer than
 // four tiles of short (< 16 k-block) mainloops: mixer linear_in / linear_out, 2.9 tiles of 8-9
 // k-blocks, ran 10-22 % slower.  Split-K work items, P = 3 and batched GEMMs (only the P = 3 cost
-// volume is batched) stay cooperative.  TAPIR_B200_GEMM_SCHEDULE=coop|pingpong forces one schedule
-// wherever both are legal (the GEMM kernels and the halo convolution); it is read on every call
-// and any other value is an error.  *force: 0 (not set), 1 (coop) or 2 (pingpong).
-int forced_schedule(int* force) {
-  *force = 0;
-  const char* e = getenv("TAPIR_B200_GEMM_SCHEDULE");
-  if (e == nullptr) return kOk;
-  if (strcmp(e, "coop") != 0 && strcmp(e, "pingpong") != 0) {
-    set_error("TAPIR_B200_GEMM_SCHEDULE=%s: expected coop or pingpong", e);
-    return kBadArgument;
-  }
-  *force = strcmp(e, "pingpong") == 0 ? 2 : 1;
-  return kOk;
-}
-
-int pick_pingpong(int tiles, int num_k_blocks, int P, int batch, bool* pingpong) {
-  *pingpong = false;
-  int force;
-  TAPIR_RETURN_IF(forced_schedule(&force));
-  if (P > 2 || batch > 1) return kOk;
-  if (force != 0) {
-    *pingpong = force == 2;
-    return kOk;
-  }
+// volume is batched) stay cooperative.  Elsewhere, and in the halo convolution (launch_halo),
+// TAPIR_B200_GEMM_SCHEDULE (sw.schedule) forces either schedule.
+bool pick_pingpong(int tiles, int num_k_blocks, int P, int batch, const GemmSwitches& sw) {
+  if (P > 2 || batch > 1) return false;
+  if (sw.schedule != 0) return sw.schedule == 2;
   const int sms = num_sms();
-  *pingpong = tiles >= 2 * sms && (tiles >= 4 * sms || num_k_blocks >= 16);
-  return kOk;
+  return tiles >= 2 * sms && (tiles >= 4 * sms || num_k_blocks >= 16);
 }
 
 // Whole ping-pong tiles with tanh-GELU and two bf16 output planes and nothing else (mixer `up`, the
 // ExtraConv expansion) write their planes with TMA stores (epilogue_planes_tma) where a tile's rows
-// are consecutive output rows and the planes meet TMA's 16-byte rules.
-// TAPIR_B200_PLANE_STORE=tma|regs (default tma) selects that path or the register stores; it is
-// read on every call and any other value is an error.
+// are consecutive output rows and the planes meet TMA's 16-byte rules.  The cooperative schedule
+// writes the same tiles with register stores (epilogue_full), the same bits.
 int plane_store_params(const GemmArgs& g, bool pingpong, TcParams* p) {
-  const char* e = getenv("TAPIR_B200_PLANE_STORE");
-  if (e != nullptr && strcmp(e, "tma") != 0 && strcmp(e, "regs") != 0) {
-    set_error("TAPIR_B200_PLANE_STORE=%s: expected tma or regs", e);
-    return kBadArgument;
-  }
-  if (!pingpong || (e != nullptr && strcmp(e, "regs") == 0)) return kOk;
+  if (!pingpong) return kOk;
   if (g.act != 1 || g.out_planes == nullptr || g.out_P != 2 || g.out_f32 != nullptr || g.residual != nullptr ||
       g.stats != nullptr)
     return kOk;
@@ -1173,24 +1147,13 @@ bool small_problem(int m_tiles, int N) {
 // 64-wide tiles for N <= 64, and for small problems when that gives every SM a tile: twice the
 // CTAs, each with half the MMA work per k-block.  (The K-summation order of an output element does
 // not depend on the tile shape, so results stay bit-identical across these choices.)  A small
-// problem that will be split over K keeps 128-wide tiles unless TAPIR_B200_BLOCK_N is set (to
-// anything): the parallelism comes from K, and wide tiles re-read the A operand half as often.
-int pick_block_n(int m_tiles, int N, bool split_k) {
-  const char* force = getenv("TAPIR_B200_BLOCK_N");
-  if (force != nullptr) {
-    int v = atoi(force);
-    if (v == 64 || v == 128) return v;
-  }
+// problem that will be split over K keeps 128-wide tiles: the parallelism comes from K, and wide
+// tiles re-read the A operand half as often.  TAPIR_B200_BLOCK_N (sw.block_n) forces the width.
+int pick_block_n(int m_tiles, int N, bool split_k, const GemmSwitches& sw) {
+  if (sw.block_n != 0) return sw.block_n;
   if (N <= 64) return 64;
-  if (small_problem(m_tiles, N) && m_tiles * ceil_div(N, 128) * 2 <= num_sms())
-    return split_k && force == nullptr ? 128 : 64;
+  if (small_problem(m_tiles, N) && m_tiles * ceil_div(N, 128) * 2 <= num_sms()) return split_k ? 128 : 64;
   return 128;
-}
-
-// On unless the variable is set to 0; read once per process.
-bool switch_on(const char* name) {
-  const char* e = getenv(name);
-  return !(e != nullptr && atoi(e) == 0);
 }
 
 // The parameters every kernel shares: problem, epilogue, batch layout, the generic conv tiling
@@ -1238,25 +1201,22 @@ int common_params(const GemmArgs& g, TcParams* p) {
 }
 
 // Halo-patch kernel for the C = 64 -> 64 3x3 layers (first ResNet group), see conv3x3_halo_kernel.
-// TAPIR_B200_CONV_HALO=0: generic path.
-bool use_halo(const GemmArgs& g) {
-  static const bool on = switch_on("TAPIR_B200_CONV_HALO");
-  return on && g.mode == kGemmConv3x3 && g.C == 64 && g.N == 64 && g.planes <= 2 && g.out_planes == nullptr;
+// TAPIR_B200_CONV_HALO=0 (sw.halo false): generic path.
+bool use_halo(const GemmArgs& g, const GemmSwitches& sw) {
+  return sw.halo && g.mode == kGemmConv3x3 && g.C == 64 && g.N == 64 && g.planes <= 2 && g.out_planes == nullptr;
 }
 
 // Ping-pong wherever a CTA gets at least two tiles (the clip's 48 frames at 128 x 128: 6144 tiles);
-// the single-frame streaming passes (128 tiles) stay cooperative.  TAPIR_B200_GEMM_SCHEDULE forces
-// either schedule (pick_pingpong).
-int launch_halo(TcParams p, const GemmArgs& g, cudaStream_t stream) {
+// the single-frame streaming passes (128 tiles) stay cooperative.  TAPIR_B200_GEMM_SCHEDULE
+// (sw.schedule) forces either schedule.
+int launch_halo(TcParams p, const GemmArgs& g, const GemmSwitches& sw, cudaStream_t stream) {
   p.tileW = kHaloTileW;
   p.tileH = kHaloTileH;
   p.tiles_x = ceil_div(g.W, kHaloTileW);
   p.tiles_y = ceil_div(g.H, kHaloTileH);
   p.num_m_tiles = g.frames * p.tiles_x * p.tiles_y;
   p.num_n_tiles = 1;
-  int force;
-  TAPIR_RETURN_IF(forced_schedule(&force));
-  const bool pingpong = force != 0 ? force == 2 : p.num_m_tiles >= 2 * num_sms();
+  const bool pingpong = sw.schedule != 0 ? sw.schedule == 2 : p.num_m_tiles >= 2 * num_sms();
   TAPIR_RETURN_IF(encode_nhwc_map(&p.tmPatch, g, kHaloTileW + 2, 1, "A/patch"));
   TAPIR_RETURN_IF(encode_rows_map(&p.tmB, g.b, g.K, g.N, g.ldb, g.b_plane_stride, g.planes, 64, "B/halo"));
   if (pingpong) {
@@ -1268,17 +1228,14 @@ int launch_halo(TcParams p, const GemmArgs& g, cudaStream_t stream) {
   return launch<conv3x3_halo_kernel<2>, HaloCfg<2>::kSmemBytes>("conv3x3_halo_kernel", p, g, stream);
 }
 
-// Split-K (deterministic two-pass, below) for problems that cannot half-fill the GPU: on by
-// default, TAPIR_B200_SPLITK=0 disables.  Only where the caller allows it (single-frame streaming
-// steps) and K >= 2048 (mixer `down` at ~1000 rows, the ExtraConvs of one frame).  The summation
-// order of a split GEMM depends on the row count; offline clips keep the exact chunk /
-// permutation / shard invariance (tests/test_properties_gpu.py re-chunks config 2 into 1776-row
-// chunks, tests/multi_gpu_check.py shards 1152 rows over two ranks, both demand bit-level
-// agreement).
+// Split-K (deterministic two-pass, below) for problems that cannot half-fill the GPU.  Only where
+// the caller allows it by passing a workspace (single-frame streaming steps) and K >= 2048 (mixer
+// `down` at ~1000 rows, the ExtraConvs of one frame).  The summation order of a split GEMM
+// depends on the row count; offline clips keep the exact chunk / permutation / shard invariance
+// (tests/test_properties_gpu.py re-chunks config 2 into 1776-row chunks,
+// tests/multi_gpu_check.py shards 1152 rows over two ranks, both demand bit-level agreement).
 bool splittable(const GemmArgs& g) {
-  static const bool on = switch_on("TAPIR_B200_SPLITK");
-  return on && g.allow_splitk && g.splitk_ws != nullptr && g.stats == nullptr && g.batch == 1 &&
-         g.K / kBlockK >= 32;
+  return g.allow_splitk && g.splitk_ws != nullptr && g.stats == nullptr && g.batch == 1 && g.K / kBlockK >= 32;
 }
 
 // Row stride of the split-K partials: whole float4 groups for the reduction.
@@ -1313,7 +1270,33 @@ int launch_split_k(const TcParams& p, int bn, int S, const GemmArgs& g, cudaStre
   return kOk;
 }
 
+// *v = -1 if the variable `name` is not set, 0 if it is `v0`, 1 if it is `v1`; any other value is
+// an error.
+int read_switch(const char* name, const char* v0, const char* v1, int* v) {
+  *v = -1;
+  const char* e = getenv(name);
+  if (e == nullptr) return kOk;
+  TAPIR_CHECK_ARG(strcmp(e, v0) == 0 || strcmp(e, v1) == 0, "%s='%s': expected %s or %s", name, e, v0, v1);
+  *v = strcmp(e, v0) == 0 ? 0 : 1;
+  return kOk;
+}
+
 }  // namespace
+
+// The one reader of the switches; the rule they follow is stated with GemmSwitches (gemm.cuh).
+int read_gemm_switches(GemmSwitches* sw) {
+  *sw = GemmSwitches();
+  int v;
+  TAPIR_RETURN_IF(read_switch("TAPIR_B200_GEMM", "tc", "simt", &v));
+  sw->simt = v == 1;
+  TAPIR_RETURN_IF(read_switch("TAPIR_B200_BLOCK_N", "64", "128", &v));
+  sw->block_n = v < 0 ? 0 : v == 0 ? 64 : 128;
+  TAPIR_RETURN_IF(read_switch("TAPIR_B200_GEMM_SCHEDULE", "coop", "pingpong", &v));
+  sw->schedule = v + 1;
+  TAPIR_RETURN_IF(read_switch("TAPIR_B200_CONV_HALO", "0", "1", &v));
+  sw->halo = v != 0;
+  return kOk;
+}
 
 int validate_gemm_args(const GemmArgs& g) {
   TAPIR_CHECK_ARG(g.planes >= 1 && g.planes <= 3, "gemm: planes must be 1..3 (got %d)", g.planes);
@@ -1358,21 +1341,20 @@ int validate_gemm_args(const GemmArgs& g) {
   return kOk;
 }
 
-int gemm_tc(const GemmArgs& g, cudaStream_t stream) {
+int gemm_tc(const GemmArgs& g, const GemmSwitches& sw, cudaStream_t stream) {
   TAPIR_RETURN_IF(validate_gemm_args(g));
   TcParams p;
   TAPIR_RETURN_IF(common_params(g, &p));
-  if (use_halo(g)) return launch_halo(p, g, stream);
+  if (use_halo(g, sw)) return launch_halo(p, g, sw, stream);
   const bool split = splittable(g);
-  const int bn = pick_block_n(p.num_m_tiles, g.N, split);
+  const int bn = pick_block_n(p.num_m_tiles, g.N, split, sw);
   p.num_n_tiles = ceil_div(g.N, bn);
   TAPIR_RETURN_IF(encode_rows_map(&p.tmB, g.b, g.K, (g.batch - 1) * p.b_batch_rows + g.N, g.ldb,
                                   g.b_plane_stride, g.planes, bn, "B"));
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int S = split ? split_k_factor(g, tiles) : 1;
   if (S > 1) return launch_split_k(p, bn, S, g, stream);
-  bool pingpong = false;
-  TAPIR_RETURN_IF(pick_pingpong(tiles, p.num_k_blocks, g.planes, g.batch, &pingpong));
+  const bool pingpong = pick_pingpong(tiles, p.num_k_blocks, g.planes, g.batch, sw);
   TAPIR_RETURN_IF(plane_store_params(g, pingpong, &p));
   return launch_gemm(bn, pingpong, p, g, stream);
 }

@@ -1,5 +1,6 @@
 """Helpers for the -m gpu tests: everything goes through the C ABI (tapnet_b200._lib)."""
 import atexit
+import contextlib
 import ctypes
 import json
 import os
@@ -124,6 +125,34 @@ def split_like_kernel(v, planes):
 
 def launch_count():
   return int(_lib.load().tapir_launch_count())
+
+
+@contextlib.contextmanager
+def switches(**kv):
+  """Sets the library's environment switches (tapnet_b200/csrc/gemm.cuh, read on every GEMM call)
+  for the body of the with block; None unsets one.  The previous values come back on exit."""
+  old = {k: os.environ.get(k) for k in kv}
+
+  def put(env):
+    for k, v in env.items():
+      if v is None:
+        os.environ.pop(k, None)
+      else:
+        os.environ[k] = str(v)
+  put(kv)
+  try:
+    yield
+  finally:
+    put(old)
+
+
+def kernels(fn, pattern):
+  """Names of the CUDA kernels that fn() runs whose names contain `pattern` (torch.profiler)."""
+  from torch.profiler import ProfilerActivity, profile  # pylint: disable=g-import-not-at-top
+  with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    fn()
+    torch.cuda.synchronize()
+  return [e.name for e in prof.events() if pattern in e.name]
 
 
 class GemmResult:

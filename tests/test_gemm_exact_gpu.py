@@ -12,9 +12,6 @@ the last GELU multiply may be fused with the residual add differently on differe
 
 tapir_split_planes, which makes the GEMM operands everywhere else, is checked bit for bit against
 torch's round-to-nearest-even split here as well."""
-import contextlib
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -26,30 +23,6 @@ from tests import gemm_exact as E  # noqa: E402
 from tests import gpu_util as U  # noqa: E402
 
 CASES = {c.cid: c for c in E.CASES}
-
-
-def _splitk_enabled():
-  e = os.environ.get('TAPIR_B200_SPLITK')  # gemm_tc.cu: set and atoi() == 0 disables split-K
-  if e is None:
-    return True
-  try:
-    return int(e.strip() or '0') != 0
-  except ValueError:
-    return False
-
-
-@contextlib.contextmanager
-def _env(**kv):
-  old = {k: os.environ.get(k) for k in kv}
-  os.environ.update({k: str(v) for k, v in kv.items()})
-  try:
-    yield
-  finally:
-    for k, v in old.items():
-      if v is None:
-        del os.environ[k]
-      else:
-        os.environ[k] = v
 
 
 def _tc_runs(P):
@@ -76,14 +49,14 @@ def _run(case, opts, impl, ld_pad=0, offset=0, env=None, splitk=False):
   ws = None
   if splitk:
     ws = torch.empty(8 * d.M * ((d.N + 7) // 8 * 8) * 4, dtype=torch.uint8, device='cuda')
-  with _env(**(env or {})):
+  with U.switches(**(env or {})):
     res = U.gemm(t['a'], t['w'], t['bias'] if bias else None, t['resid'] if resid else None, gelu,
                  f32_out, out_P, impl, conv=case.conv, stats=st,
                  rows_per_frame=d.rows_per_frame if stats and case.conv is None else 0,
                  ld_pad=ld_pad, offset=offset, splitk_ws=ws, details=True)
   assert U.untouched_padding(res), 'wrote outside the [M, N] output'
   if splitk and impl == 0:
-    assert res.launches == (2 if _splitk_enabled() else 1), res.launches
+    assert res.launches == 2, res.launches
   return res, st
 
 

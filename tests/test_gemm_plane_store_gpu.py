@@ -1,14 +1,11 @@
-"""The ping-pong GEMM's two ways of writing a GELU + two-bf16-plane output give the same bits.
+"""The two ways of writing a GELU + two-bf16-plane output give the same bits.
 
-Whole tiles whose rows are consecutive output rows (plain GEMMs, and convolutions whose tiles span
-whole image rows) stage each plane's 64 x 64 boxes in shared memory and write them with TMA stores;
-everything else keeps the register stores.  TAPIR_B200_PLANE_STORE=tma|regs, read on every call,
-selects between the two, so each case runs once per value into NaN-filled buffers, under the
-ping-pong schedule at both tile widths, and the planes must match bit for bit, padding included.
+Under the ping-pong schedule, whole tiles whose rows are consecutive output rows (plain GEMMs, and
+convolutions whose tiles span whole image rows) stage each plane's 64 x 64 boxes in shared memory
+and write them with TMA stores; everything else, and every tile of the cooperative schedule, takes
+the register stores.  So each case runs under both schedules (TAPIR_B200_GEMM_SCHEDULE) into
+NaN-filled buffers, at both tile widths, and the planes must match bit for bit, padding included.
 The operands are tests/gemm_exact.py's GELU designs, whose accumulators are exact."""
-import contextlib
-import os
-
 import pytest
 import torch
 
@@ -16,8 +13,6 @@ pytestmark = pytest.mark.gpu
 
 from tests import gemm_exact as E  # noqa: E402
 from tests import gpu_util as U  # noqa: E402
-
-SWITCH = 'TAPIR_B200_PLANE_STORE'
 
 # name: (make_design arguments, ld_pad)
 CASES = {
@@ -36,20 +31,6 @@ CASES = {
 }
 
 
-@contextlib.contextmanager
-def _env(**kv):
-  old = {k: os.environ.get(k) for k in kv}
-  os.environ.update({k: str(v) for k, v in kv.items()})
-  try:
-    yield
-  finally:
-    for k, v in old.items():
-      if v is None:
-        del os.environ[k]
-      else:
-        os.environ[k] = v
-
-
 _designs = {}
 
 
@@ -62,10 +43,10 @@ def _design(name):
   return _designs[name]
 
 
-def _run(name, store, bn, bias):
+def _run(name, schedule, bn, bias):
   d = _design(name)
   _, ld_pad = CASES[name]
-  with _env(**{SWITCH: store, 'TAPIR_B200_GEMM_SCHEDULE': 'pingpong', 'TAPIR_B200_BLOCK_N': bn}):
+  with U.switches(TAPIR_B200_GEMM_SCHEDULE=schedule, TAPIR_B200_BLOCK_N=bn):
     res = U.gemm(d.dev['a'], d.dev['w'], d.dev['bias'] if bias else None, None, True, out_f32=False,
                  out_planes=2, conv=d.conv, ld_pad=ld_pad, details=True)
   assert res.launches == 1
@@ -76,14 +57,8 @@ def _run(name, store, bn, bias):
 @pytest.mark.parametrize('bn', [128, 64])
 @pytest.mark.parametrize('name', sorted(CASES))
 def test_tma_and_register_plane_stores_agree(name, bn, bias):
-  regs = _run(name, 'regs', bn, bias)
-  tma = _run(name, 'tma', bn, bias)
+  regs = _run(name, 'coop', bn, bias)
+  tma = _run(name, 'pingpong', bn, bias)
   assert torch.equal(regs.planes_buf.view(torch.int16), tma.planes_buf.view(torch.int16)), name
   assert U.untouched_padding(tma), name
   assert not torch.isnan(tma.planes.float()).any(), name
-
-
-def test_plane_store_switch_rejects_unknown_values():
-  d = _design('ld_pad')
-  with _env(**{SWITCH: 'stmatrix'}), pytest.raises(Exception, match=SWITCH):
-    U.gemm(d.dev['a'], d.dev['w'], d.dev['bias'], None, True, out_f32=False, out_planes=2)

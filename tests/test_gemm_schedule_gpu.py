@@ -7,8 +7,7 @@ Both schedules sum every output element's K terms in the same order, so no refer
 is needed: each case runs once per schedule (TAPIR_B200_GEMM_SCHEDULE, read on every call) into
 NaN-filled buffers and the two results must match bit for bit, guard elements included.  Fused
 InstanceNorm statistics are fp64 atomic sums whose order varies between runs, so they are compared
-to fp64 rounding."""
-import os
+to fp64 rounding.  Last, every switch rejects a value outside its set, on every call."""
 import zlib
 
 import pytest
@@ -16,6 +15,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+from tapnet_b200 import _lib  # noqa: E402
 from tests import gpu_util as U  # noqa: E402
 
 SCHEDULE = 'TAPIR_B200_GEMM_SCHEDULE'
@@ -40,16 +40,9 @@ def _problem(seed, M, N, K, P, conv=None, bias=False, resid=False):
 
 
 def _run(schedule, a_pl, w_pl, stats_shape=None, **kw):
-  old = os.environ.get(SCHEDULE)
-  os.environ[SCHEDULE] = schedule
-  try:
-    stats = torch.zeros(stats_shape, dtype=torch.float64, device='cuda') if stats_shape else None
+  stats = torch.zeros(stats_shape, dtype=torch.float64, device='cuda') if stats_shape else None
+  with U.switches(**{SCHEDULE: schedule}):
     res = U.gemm(a_pl, w_pl, stats=stats, details=True, **kw)
-  finally:
-    if old is None:
-      del os.environ[SCHEDULE]
-    else:
-      os.environ[SCHEDULE] = old
   assert res.launches == 1
   return res, stats
 
@@ -134,43 +127,74 @@ def test_tc_schedules_agree_at_tile_counts(per_cta):
 
 
 def _kernels(fn):
-  from torch.profiler import ProfilerActivity, profile
-  with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    fn()
-    torch.cuda.synchronize()
-  return {e.name for e in prof.events() if 'gemm_tc' in e.name}
+  return set(U.kernels(fn, 'gemm_tc'))
 
 
 def test_tc_dispatch_picks_pingpong_for_long_clip_gemms_and_coop_otherwise():
-  if os.environ.get(SCHEDULE) is not None:
-    pytest.skip(f'{SCHEDULE} overrides the dispatcher')
-  ws = torch.empty(64 << 20, dtype=torch.uint8, device='cuda')
-  clip = ['mixer.up', 'mixer.down', 'extra_conv.up', 'resnet.g2.conv']
-  stream = {  # one frame per step, 1024 points: the split-K and small-problem paths
-      'mixer.up': dict(M=1024, N=2048, K=512, bias=True, gelu=True, out_f32=False, out_planes=2),
-      'mixer.down': dict(M=1024, N=512, K=2048, bias=True, resid=True, splitk_ws=ws),
-      'extra_conv.up': dict(M=0, N=1024, K=9 * 256, conv=(1, 32, 32, 256), bias=True, gelu=True,
-                            out_f32=False, out_planes=2),
-  }
-  for name in clip + ['mixer.linear_in', 'mixer.linear_out']:
-    c = dict(STEP[name])
-    a_pl, w_pl, b, r = _problem(1, c.pop('M'), c.pop('N'), c.pop('K'), 2, c.get('conv'),
-                                c.pop('bias', False), c.pop('resid', False))
-    c.pop('stats', None)
-    names = _kernels(lambda: U.gemm(a_pl, w_pl, bias=b, residual=r, **c))
-    if name in clip:
-      assert names and all('pingpong' in n for n in names), (name, names)
-    else:  # under four tiles per CTA of short mainloops ping-pong is slower
+  """The dispatcher's own choice: no schedule or tile width forced, the halo path allowed."""
+  with U.switches(TAPIR_B200_GEMM_SCHEDULE=None, TAPIR_B200_BLOCK_N=None, TAPIR_B200_CONV_HALO=1):
+    ws = torch.empty(64 << 20, dtype=torch.uint8, device='cuda')
+    clip = ['mixer.up', 'mixer.down', 'extra_conv.up', 'resnet.g2.conv']
+    stream = {  # one frame per step, 1024 points: the split-K and small-problem paths
+        'mixer.up': dict(M=1024, N=2048, K=512, bias=True, gelu=True, out_f32=False, out_planes=2),
+        'mixer.down': dict(M=1024, N=512, K=2048, bias=True, resid=True, splitk_ws=ws),
+        'extra_conv.up': dict(M=0, N=1024, K=9 * 256, conv=(1, 32, 32, 256), bias=True, gelu=True,
+                              out_f32=False, out_planes=2),
+    }
+    for name in clip + ['mixer.linear_in', 'mixer.linear_out']:
+      c = dict(STEP[name])
+      a_pl, w_pl, b, r = _problem(1, c.pop('M'), c.pop('N'), c.pop('K'), 2, c.get('conv'),
+                                  c.pop('bias', False), c.pop('resid', False))
+      c.pop('stats', None)
+      names = _kernels(lambda: U.gemm(a_pl, w_pl, bias=b, residual=r, **c))
+      if name in clip:
+        assert names and all('pingpong' in n for n in names), (name, names)
+      else:  # under four tiles per CTA of short mainloops ping-pong is slower
+        assert names and not any('pingpong' in n for n in names), (name, names)
+    for name, c in stream.items():
+      c = dict(c)
+      a_pl, w_pl, b, r = _problem(2, c.pop('M'), c.pop('N'), c.pop('K'), 2, c.get('conv'),
+                                  c.pop('bias', False), c.pop('resid', False))
+      names = _kernels(lambda: U.gemm(a_pl, w_pl, bias=b, residual=r, **c))
       assert names and not any('pingpong' in n for n in names), (name, names)
-  for name, c in stream.items():
-    c = dict(c)
-    a_pl, w_pl, b, r = _problem(2, c.pop('M'), c.pop('N'), c.pop('K'), 2, c.get('conv'),
-                                c.pop('bias', False), c.pop('resid', False))
-    names = _kernels(lambda: U.gemm(a_pl, w_pl, bias=b, residual=r, **c))
-    assert names and not any('pingpong' in n for n in names), (name, names)
 
 
 def test_tc_schedule_switch_rejects_unknown_values():
+  """Also on a split-K GEMM, which always runs the cooperative kernel and so never uses the switch."""
   a_pl, w_pl, _, _ = _problem(3, 256, 128, 128, 2)
-  with pytest.raises(Exception, match='TAPIR_B200_GEMM_SCHEDULE'):
+  with pytest.raises(Exception, match=SCHEDULE):
     _run('ping-pong', a_pl, w_pl)
+  a_pl, w_pl, _, _ = _problem(4, 1000, 512, 2048, 2)
+  ws = torch.empty(64 << 20, dtype=torch.uint8, device='cuda')
+  with pytest.raises(Exception, match=SCHEDULE):
+    _run('ping-pong', a_pl, w_pl, splitk_ws=ws)
+
+
+# a value outside each switch's set; the empty string is rejected as well
+BAD_VALUES = {'TAPIR_B200_GEMM': 'wgmma', 'TAPIR_B200_BLOCK_N': '96',
+              'TAPIR_B200_GEMM_SCHEDULE': 'ping-pong', 'TAPIR_B200_CONV_HALO': 'yes'}
+
+
+@pytest.mark.parametrize('value', ['bad', 'empty'])
+@pytest.mark.parametrize('switch', sorted(BAD_VALUES))
+def test_tc_switches_reject_values_outside_their_set(switch, value):
+  """Every GEMM call reads all four switches, whether it uses them or not, and fails before any
+  launch on a value outside a switch's set.  The cost volume reaches the GEMM through gemm()."""
+  a_pl, w_pl, _, _ = _problem(3, 256, 128, 128, 2)
+  with U.switches(**{switch: BAD_VALUES[switch] if value == 'bad' else ''}):
+    torch.cuda.synchronize()
+    before = U.launch_count()
+    with pytest.raises(_lib.TapirB200Error, match=switch):
+      U.gemm(a_pl, w_pl)
+    assert U.launch_count() == before
+    if value == 'bad':
+      from tests.test_stage_a_gpu import _head_weights  # pylint: disable=g-import-not-at-top
+      G, n, T = 1, 8, 2
+      qf = torch.randn(G, n, 256, device='cuda')
+      grid = torch.randn(G, T, 32, 32, 256, device='cuda')
+      pts = torch.empty(G, n, T, 2, device='cuda')
+      occ, expd = torch.empty(G, n, T, device='cuda'), torch.empty(G, n, T, device='cuda')
+      ws = torch.empty(_lib.cost_volume_workspace_bytes(qf, grid), dtype=torch.uint8, device='cuda')
+      with pytest.raises(_lib.TapirB200Error, match=switch):
+        _lib.cost_volume_tracks(_head_weights('synth'), qf, grid, None, 20.0, (256, 256), pts, occ,
+                                expd, None, ws)

@@ -6,9 +6,6 @@ fused with bias / GELU / residual), split-K with its reduction kernel, the halo-
 shapes that do not tile, the conv tile geometries, BLOCK_N and row-range invariance, and the
 host-side argument checks."""
 import ctypes
-import os
-import subprocess
-import sys
 
 import pytest
 import torch
@@ -20,16 +17,6 @@ from tapnet_b200 import _lib  # noqa: E402
 from tests import gpu_util as U  # noqa: E402
 
 IMPLS = pytest.mark.parametrize('impl', [1, 0], ids=['simt', 'tc'])
-
-
-def _splitk_enabled():
-  e = os.environ.get('TAPIR_B200_SPLITK')  # gemm_tc.cu: set and atoi() == 0 disables split-K
-  if e is None:
-    return True
-  try:
-    return int(e.strip() or '0') != 0
-  except ValueError:
-    return False
 
 
 def _problem(seed, M, N, K, P, conv=None, bias=False, resid=False):
@@ -161,7 +148,7 @@ def test_splitk(case, impl):
   ref = _model(a_pl, w_pl, conv, impl, b, gelu, r)
   name = f'splitk_{cid}_impl{impl}'
   # a split GEMM is one partial-sum launch plus the reduction (the SIMT path never splits)
-  expect = 2 if (impl == 0 and splits and _splitk_enabled()) else 1
+  expect = 2 if (impl == 0 and splits) else 1
   U.record(name + '_launches', launches=res.launches, expected=expect)
   assert res.launches == expect and runs[1].launches == expect
   assert U.untouched_padding(res), name
@@ -196,40 +183,22 @@ HALO_CASES = [
     (1, 33, 37, 2, True, False, True),
     (3, 33, 5, 2, False, False, False),
     (1, 7, 13, 1, True, True, False),
+    (3, 40, 56, 2, True, True, True),
 ]
 
-_HALO_CHILD = """
-import sys, torch
-sys.path.insert(0, {root!r})
-from tests import gpu_util as U
-from tests.test_gemm_variants_gpu import HALO_CASES, _problem
-outs = []
-for i, (Fr, H, W, P, bias, resid, stats) in enumerate(HALO_CASES):
-  M = Fr * H * W
-  a_pl, w_pl, b, r = _problem(100 + i, M, 64, 576, P, (Fr, H, W, 64), bias, resid)
-  st = torch.zeros(Fr, 64, 2, dtype=torch.float64, device='cuda') if stats else None
-  o, _ = U.gemm(a_pl, w_pl, b, r, False, True, 0, 0, conv=(Fr, H, W, 64), stats=st)
-  outs.append((o.cpu(), st.cpu() if stats else None))
-torch.save(outs, sys.argv[1])
-"""
 
-
-def test_halo_conv_shapes_tc(tmp_path):
+def test_halo_conv_shapes_tc():
   """conv3x3_halo_kernel (C = 64 -> 64, P <= 2) against the fp64 model, and bit for bit against the
-  generic implicit GEMM.  The switch is read once per process: one child per setting."""
-  root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-  results = []
-  for halo in ('1', '0'):
-    path = str(tmp_path / f'halo{halo}.pt')
-    env = dict(os.environ, TAPIR_B200_CONV_HALO=halo)
-    p = subprocess.run([sys.executable, '-c', _HALO_CHILD.format(root=root), path],
-                       capture_output=True, text=True, timeout=300, env=env)
-    assert p.returncode == 0, p.stderr[-3000:]
-    results.append(torch.load(path))
-  for i, case in enumerate(HALO_CASES):
-    Fr, H, W, P, bias, resid, stats = case
-    (o_h, st_h), (o_g, _) = results[0][i], results[1][i]
+  generic implicit GEMM (TAPIR_B200_CONV_HALO=0)."""
+  for i, (Fr, H, W, P, bias, resid, stats) in enumerate(HALO_CASES):
     a_pl, w_pl, b, r = _problem(100 + i, Fr * H * W, 64, 576, P, (Fr, H, W, 64), bias, resid)
+    outs = {}
+    for halo in (1, 0):
+      st = torch.zeros(Fr, 64, 2, dtype=torch.float64, device='cuda') if stats else None
+      with U.switches(TAPIR_B200_CONV_HALO=halo):
+        o, _ = U.gemm(a_pl, w_pl, b, r, False, True, 0, 0, conv=(Fr, H, W, 64), stats=st)
+      outs[halo] = (o, st)
+    (o_h, st_h), (o_g, _) = outs[1], outs[0]
     ref = _model(a_pl, w_pl, True, 0, b, False, r)
     name = f'halo_{Fr}x{H}x{W}_P{P}'
     _check_out(name, o_h, ref, False, 576, P)
@@ -268,18 +237,6 @@ def test_conv_tile_geometry(case, impl):
 
 
 # ------------------------------------------------------------------------------- invariance
-def _with_block_n(bn, fn):
-  old = os.environ.get('TAPIR_B200_BLOCK_N')
-  os.environ['TAPIR_B200_BLOCK_N'] = str(bn)  # pick_block_n reads it on every call
-  try:
-    return fn()
-  finally:
-    if old is None:
-      del os.environ['TAPIR_B200_BLOCK_N']
-    else:
-      os.environ['TAPIR_B200_BLOCK_N'] = old
-
-
 @pytest.mark.parametrize('mode', ['plain', 'conv'])
 @pytest.mark.parametrize('P', [1, 2, 3])
 def test_block_n_invariance_tc(P, mode):
@@ -289,7 +246,10 @@ def test_block_n_invariance_tc(P, mode):
   M, K = (2 * 20 * 24, 576) if conv else (700, 256)
   a_pl, w_pl, b, r = _problem(P + N, M, N, K, P, conv, True, True)
   run = lambda: U.gemm(a_pl, w_pl, b, r, True, True, P, 0, conv=conv, ld_pad=3, details=True)  # noqa: E731
-  r64, r128 = _with_block_n(64, run), _with_block_n(128, run)
+  with U.switches(TAPIR_B200_BLOCK_N=64):
+    r64 = run()
+  with U.switches(TAPIR_B200_BLOCK_N=128):
+    r128 = run()
   same = torch.equal(r64.out_buf.view(torch.int32), r128.out_buf.view(torch.int32)) and \
       torch.equal(r64.planes_buf.view(torch.int16), r128.planes_buf.view(torch.int16))
   U.record(f'block_n_invariance_{mode}_P{P}', identical=int(same))

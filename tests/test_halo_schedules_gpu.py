@@ -3,16 +3,11 @@ conv3x3_halo_pingpong_kernel) and the generic implicit GEMM give the same output
 fused InstanceNorm statistics are the sums of the kernel's own output.
 
 Every output element sums its nine taps' terms in the same order on all three paths, so no
-reference computation is needed for the outputs: the schedules (TAPIR_B200_GEMM_SCHEDULE, read on
-every call) run in this process into NaN-filled buffers and must match bit for bit, padding
-included; the generic path (TAPIR_B200_CONV_HALO=0, read once per process) runs in a child, which
-hands back a digest of each output.  The statistics are fp64 atomic sums whose order varies, so
-across paths and against an fp64 sum of the output they are compared to rounding; on operands
+reference computation is needed for the outputs: the schedules (TAPIR_B200_GEMM_SCHEDULE) and the
+generic path (TAPIR_B200_CONV_HALO=0), switches read on every call, run into NaN-filled buffers and
+must match bit for bit, padding included.  The statistics are fp64 atomic sums whose order varies,
+so across paths and against an fp64 sum of the output they are compared to rounding; on operands
 whose every sum is exact (tests/gemm_exact.py 'S' designs) they must equal that sum exactly."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
@@ -23,7 +18,7 @@ from tests import gemm_exact as E  # noqa: E402
 from tests import gpu_util as U  # noqa: E402
 
 SCHEDULE = 'TAPIR_B200_GEMM_SCHEDULE'
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+HALO = 'TAPIR_B200_CONV_HALO'
 
 # (frames, H, W, P): 128 x 128 is the first ResNet group of a 256 x 256 clip; the others have partial
 # tiles (W not a multiple of 8, H not a multiple of 16, W below 8); f40_33x13 has many small
@@ -51,55 +46,18 @@ def _problem(name):
   return a_pl, w_pl, r
 
 
-def _run(name, opt, schedule=None):
+def _run(name, opt, schedule=None, halo=1):
+  """One case on the halo kernel (halo=1) under `schedule` (None: the dispatcher's choice), or on
+  the generic implicit GEMM (halo=0)."""
   Fr, H, W, _ = SHAPES[name]
   resid, stats = OPTIONS[opt]
   a_pl, w_pl, r = _problem(name)
   st = torch.zeros(Fr, 64, 2, dtype=torch.float64, device='cuda') if stats else None
-  old = os.environ.get(SCHEDULE)
-  if schedule is not None:
-    os.environ[SCHEDULE] = schedule
-  try:
+  with U.switches(**{SCHEDULE: schedule, HALO: halo}):
     res = U.gemm(a_pl, w_pl, None, r if resid else None, conv=(Fr, H, W, 64), stats=st, details=True)
-  finally:
-    if old is None:
-      os.environ.pop(SCHEDULE, None)
-    else:
-      os.environ[SCHEDULE] = old
   assert res.launches == 1
-  assert U.untouched_padding(res), (name, opt, schedule)
+  assert U.untouched_padding(res), (name, opt, schedule, halo)
   return res, st
-
-
-def _digest(x):
-  b = x.contiguous().view(torch.int32).reshape(-1).long()
-  w = torch.arange(b.numel(), device=b.device) % 65521 + 1
-  return int(b.sum()), int((b * w).sum())
-
-
-_CHILD = """
-import sys, torch
-sys.path.insert(0, {root!r})
-from tests.test_halo_schedules_gpu import OPTIONS, SHAPES, _digest, _run
-out = {{}}
-for name in SHAPES:
-  for opt in OPTIONS:
-    res, st = _run(name, opt)
-    out[(name, opt)] = (_digest(res.out), None if st is None else st.cpu())
-torch.save(out, sys.argv[1])
-"""
-
-
-@pytest.fixture(scope='module')
-def generic(tmp_path_factory):
-  """Digest and statistics of every case on the generic implicit GEMM, from one child process."""
-  path = str(tmp_path_factory.mktemp('halo') / 'generic.pt')
-  env = dict(os.environ, TAPIR_B200_CONV_HALO='0')
-  env.pop(SCHEDULE, None)
-  p = subprocess.run([sys.executable, '-c', _CHILD.format(root=ROOT), path], capture_output=True,
-                     text=True, timeout=600, env=env)
-  assert p.returncode == 0, p.stderr[-3000:]
-  return torch.load(path)
 
 
 def _stats_close(got, want, what):
@@ -107,17 +65,16 @@ def _stats_close(got, want, what):
 
 
 @pytest.mark.parametrize('name', sorted(SHAPES))
-def test_halo_schedules_and_generic_conv_agree_bit_for_bit(name, generic):
-  if os.environ.get('TAPIR_B200_CONV_HALO', '1') == '0':
-    pytest.skip('TAPIR_B200_CONV_HALO=0: no halo kernel in this process')
+def test_halo_schedules_and_generic_conv_agree_bit_for_bit(name):
   Fr = SHAPES[name][0]
   for opt, (_, stats) in OPTIONS.items():
     coop, st_c = _run(name, opt, 'coop')
     pp, st_p = _run(name, opt, 'pingpong')
+    gen, st_g = _run(name, opt, halo=0)
     what = f'{name}/{opt}'
     assert torch.equal(coop.out_buf.view(torch.int32), pp.out_buf.view(torch.int32)), what
-    dig, st_g = generic[(name, opt)]
-    assert _digest(pp.out) == dig, f'{what}: halo != generic implicit GEMM'
+    assert torch.equal(gen.out_buf.view(torch.int32), pp.out_buf.view(torch.int32)), \
+        f'{what}: halo != generic implicit GEMM'
     if stats:
       # the two halo schedules share their fp32 partials (same 16-row groups): fp64 order only
       _stats_close(st_p, st_c, what)
@@ -125,7 +82,7 @@ def test_halo_schedules_and_generic_conv_agree_bit_for_bit(name, generic):
       want = torch.stack([out.sum(1), (out * out).sum(1)], -1)
       # fp32 sums over a warp's 16 rows, then fp64: rounding of the fp32 partials only.  The
       # generic path's warps hold other 16-pixel groups, so it is held to the same bound.
-      for got in (st_p, st_g.cuda()):
+      for got in (st_p, st_g):
         rel = ((got - want).abs() / want.abs().clamp(min=1.0)).max().item()
         assert rel < 5e-5, (what, rel)
 
@@ -140,15 +97,8 @@ def test_halo_stats_are_exact_sums_on_exact_operands(conv, schedule):
   Fr = conv[0]
   for resid in (False, True):
     st = torch.zeros(Fr, 64, 2, dtype=torch.float64, device='cuda')
-    old = os.environ.get(SCHEDULE)
-    os.environ[SCHEDULE] = schedule
-    try:
+    with U.switches(**{SCHEDULE: schedule, HALO: 1}):
       o, _ = U.gemm(d.a_pl.cuda(), d.w_pl.cuda(), None, d.resid.cuda() if resid else None, conv=conv, stats=st)
-    finally:
-      if old is None:
-        os.environ.pop(SCHEDULE, None)
-      else:
-        os.environ[SCHEDULE] = old
     want = E.emulate(d, False, resid, 0, True)
     assert np.array_equal(o.cpu().numpy(), want['out']), (conv, schedule, resid)
     out = o.double().cpu().reshape(Fr, -1, 64)
@@ -157,26 +107,23 @@ def test_halo_stats_are_exact_sums_on_exact_operands(conv, schedule):
     assert np.array_equal(st.cpu().numpy(), want['stats']), (conv, schedule, resid)
 
 
-def _kernels(fn):
-  from torch.profiler import ProfilerActivity, profile
-  with profile(activities=[ProfilerActivity.CUDA]) as prof:
-    fn()
-    torch.cuda.synchronize()
-  return {e.name for e in prof.events() if 'conv3x3_halo' in e.name}
-
-
 def test_halo_dispatch_and_forced_schedules():
-  if os.environ.get('TAPIR_B200_CONV_HALO', '1') == '0':
-    pytest.skip('TAPIR_B200_CONV_HALO=0: no halo kernel in this process')
-  if os.environ.get(SCHEDULE) is not None:
-    pytest.skip(f'{SCHEDULE} overrides the dispatcher')
   # 48 frames: 6144 tiles, many per CTA -> ping-pong; one frame: 128 tiles -> cooperative
   want = {('f48_128', None): True, ('f1_128', None): False,
           ('f48_128', 'coop'): False, ('f1_128', 'pingpong'): True}
-  for (name, schedule), pingpong in want.items():
-    names = _kernels(lambda: _run(name, 'plain', schedule))
-    assert len(names) == 1, (name, schedule, names)
-    assert ('pingpong' in next(iter(names))) == pingpong, (name, schedule, names)
+  with U.switches(TAPIR_B200_BLOCK_N=None):
+    for (name, schedule), pingpong in want.items():
+      names = set(U.kernels(lambda: _run(name, 'plain', schedule), 'conv3x3_halo'))
+      assert len(names) == 1, (name, schedule, names)
+      assert ('pingpong' in next(iter(names))) == pingpong, (name, schedule, names)
+
+
+def test_halo_switch_takes_effect_on_every_call():
+  """TAPIR_B200_CONV_HALO is read on every call: off, on and off again in one process (each run is
+  one launch)."""
+  for halo in (0, 1, 0):
+    names = set(U.kernels(lambda: _run('f1_128', 'plain', halo=halo), 'conv3x3_halo'))
+    assert len(names) == halo, (halo, names)
 
 
 def test_halo_schedule_switch_rejects_unknown_values():
