@@ -6,12 +6,16 @@
 //   warpgroups 1, 2         consumers: issue wgmma.m64nBLOCK_Nk16 (bf16 operands from shared
 //                           memory, fp32 accumulators in registers) and then run the epilogue
 //                           from their registers: bias / tanh-GELU / residual, fp32 and/or
-//                           bf16-plane stores (whole ping-pong tiles of GELU + two planes: through
-//                           shared memory and TMA stores).  Cooperative schedule (gemm_tc_kernel): each owns
-//                           64 rows of every 128-row tile.  Ping-pong schedule
-//                           (gemm_tc_pingpong_kernel): each owns whole tiles, alternately.
+//                           bf16-plane stores (whole ping-pong GEMM tiles of GELU + two planes:
+//                           through shared memory and TMA stores).  Cooperative schedule: each
+//                           owns 64 rows of every 128-row tile.  Ping-pong schedule: each owns
+//                           whole tiles, alternately.
 // full/empty mbarriers between producer and consumers; the producer runs ahead into the next
 // tile while the consumers are in the epilogue of the current one.
+//
+// The four kernels are one body, wgmma_kernel<operand source, schedule>: gemm_tc_kernel and
+// gemm_tc_pingpong_kernel over the stage ring (Ring), conv3x3_halo_kernel and
+// conv3x3_halo_pingpong_kernel over the halo patch ring and its B ring (HaloRing).
 //
 // A operand, plain mode: 3-D tensor map {K, M, plane}, box {64, 128, 1}.
 // A operand, conv mode : 5-D tensor map {C, W, H, frame, plane} over the NHWC activation,
@@ -303,16 +307,25 @@ __device__ __forceinline__ void flush_stats(const TcParams& p, const double* red
   ptx::named_bar_sync(bar, 128);
 }
 
+// Conv m-tile `m_tile` of p.tileW x p.tileH output pixels: its frame and top-left pixel.
+struct ConvTile {
+  int frame, y0, x0;
+};
+__device__ __forceinline__ ConvTile conv_tile(const TcParams& p, int m_tile) {
+  const int per_frame = p.tiles_x * p.tiles_y;
+  const int frame = m_tile / per_frame;
+  const int r = m_tile - frame * per_frame;
+  return {frame, (r / p.tiles_x) * p.tileH, (r % p.tiles_x) * p.tileW};
+}
+
 // Global row of tile row r (0..127) of output tile `m_tile`, and whether it exists.
 __device__ __forceinline__ void tile_row(const TcParams& p, int m_tile, int r, long long& row, bool& ok) {
   if (p.mode == kGemmConv3x3) {
-    const int per_frame = p.tiles_x * p.tiles_y;
-    const int frame = m_tile / per_frame;
-    const int rr = m_tile % per_frame;
-    const int y = (rr / p.tiles_x) * p.tileH + r / p.tileW;
-    const int x = (rr % p.tiles_x) * p.tileW + r % p.tileW;
+    const ConvTile ct = conv_tile(p, m_tile);
+    const int y = ct.y0 + r / p.tileW;
+    const int x = ct.x0 + r % p.tileW;
     ok = (y < p.H) && (x < p.W);
-    row = ((long long)frame * p.H + y) * p.W + x;
+    row = ((long long)ct.frame * p.H + y) * p.W + x;
   } else {
     row = (long long)m_tile * kBlockM + r;
     ok = row < p.M;
@@ -335,7 +348,7 @@ __device__ __forceinline__ void tile_epilogue(const TcParams& p, const float (&a
 
 // The frame of output tile `m_tile` (tiles never straddle frames where statistics are fused).
 __device__ __forceinline__ int tile_frame(const TcParams& p, int m_tile) {
-  return (p.mode == kGemmConv3x3) ? m_tile / (p.tiles_x * p.tiles_y)
+  return (p.mode == kGemmConv3x3) ? conv_tile(p, m_tile).frame
                                   : (int)(((long long)m_tile * kBlockM) / p.rows_per_frame);
 }
 
@@ -422,8 +435,10 @@ __device__ __forceinline__ int decode_work(const TcParams& p, int w, int& bat, i
   n0 = (tile - m_tile * p.num_n_tiles) * BLOCK_N;
   bat = m_tile / p.m_tiles_per_batch;
   m_tile -= bat * p.m_tiles_per_batch;
-  kb0 = (int)((long long)p.num_k_blocks * split / S);
-  kb1 = (int)((long long)p.num_k_blocks * (split + 1) / S);
+  // 32-bit: num_k_blocks < 2^25 and S <= 8.  A 64-bit division here is a subroutine call, which
+  // the ping-pong consumers would pay twice between their epilogue and their next turn.
+  kb0 = p.num_k_blocks * split / S;
+  kb1 = p.num_k_blocks * (split + 1) / S;
   return split;
 }
 
@@ -435,6 +450,19 @@ struct StageCursor {
   __device__ __forceinline__ void advance() {
     if (++stage == STAGES) { stage = 0; phase ^= 1u; }
   }
+  // past n >= 0 positions at once
+  __device__ __forceinline__ void advance(int n) {
+    stage += n;
+    phase ^= (uint32_t)(stage / STAGES) & 1u;
+    stage %= STAGES;
+  }
+};
+
+// A work item as the consumers see it: output tile (m_tile, n0), the offset of its fp32 output
+// (k-slice partial buffer and batch), and its k-blocks [kb0, kb1).
+struct Work {
+  int m_tile, n0, kb0, kb1;
+  long long out_off;
 };
 
 // The dynamic shared memory from its first 1024-byte boundary: the 128B swizzle of TMA and wgmma
@@ -506,11 +534,30 @@ __device__ __forceinline__ void consume_k_block(float (&acc)[HALVES][BLOCK_N / 2
   if (prev >= 0 && lane == 0) ptx::mbar_arrive(&empty[prev]);
 }
 
+// The operand sources of wgmma_kernel: Ring (both GEMM schedules) and HaloRing (both halo
+// convolution schedules).  Each has the same members:
+//   kBlockN, kP, kStages     tile width, operand planes, stages of the ring the k-blocks stream through
+//   kAPlane, kASbo, kBPlane  A: bytes between planes and between 8-row swizzle atoms; B: between planes
+//   kPlaneBoxes              its staging holds epilogue_planes_tma's output boxes
+//   kFullErr                 the error code of the consumers' full-barrier wait
+//   full_bar, empty_bar      that ring's barriers
+//   produce(p)               the TMA producer
+//   work(p, w)               work item w: its output tile, output offset and k-blocks
+//   kblock(t, stage, kb)     A and B of k-block kb of the CTA's local tile t, held in `stage`
+//   wait_tile, release_tile  what a tile needs beside its k-blocks (the halo patch)
+//   consumer_staging(cw)     consumer cw's statistics slots or output boxes
+
 // Shared-memory ring of both GEMM schedules: kStages stages of P A planes then P B planes, STAGING
 // bytes (1024-aligned) for the epilogue, then the full and empty mbarriers.
-template <int BLOCK_N, int P, int STAGING = 0>
+template <int BLOCK_N, int P, int STAGING>
 struct Ring {
   using Cfg = TcCfg<BLOCK_N, P, STAGING>;
+  static_assert(Cfg::kStages == TcCfg<BLOCK_N, P>::kStages, "the epilogue staging must not cost the ring a stage");
+  static_assert(kStatsSlotBytes<BLOCK_N> <= STAGING / kConsumers, "each consumer's staging holds its statistics slots");
+  static constexpr int kBlockN = BLOCK_N, kP = P, kStages = Cfg::kStages;
+  static constexpr uint32_t kAPlane = Cfg::kABytes, kASbo = 1024, kBPlane = Cfg::kBBytes;
+  static constexpr bool kPlaneBoxes = STAGING >= kPlaneStagingBytes;
+  static constexpr int kFullErr = 103;
   uint8_t* smem;
   uint8_t* staging;
   uint64_t* full_bar;
@@ -523,6 +570,21 @@ struct Ring {
     init_rings(full_bar, empty_arrivals, &p.tmA, &p.tmB, Cfg::kStages);
   }
 
+  __device__ __forceinline__ Work work(const TcParams& p, int w) const {
+    Work wk;
+    int bat;
+    const int split = decode_work<BLOCK_N>(p, w, bat, wk.m_tile, wk.n0, wk.kb0, wk.kb1);
+    wk.out_off = split * p.split_stride + bat * p.out_batch_stride;
+    return wk;
+  }
+  __device__ __forceinline__ void kblock(int, int stage, int, uint32_t& a, uint32_t& b) const {
+    a = ptx::smem_u32(smem + stage * Cfg::kStageBytes);
+    b = a + P * Cfg::kABytes;
+  }
+  __device__ __forceinline__ void wait_tile(const TcParams&, int) const {}
+  __device__ __forceinline__ void release_tile(int) const {}
+  __device__ __forceinline__ uint8_t* consumer_staging(int cw) const { return staging + cw * (STAGING / kConsumers); }
+
   // TMA producer (one thread): the k-blocks of this CTA's work items, in order, into the ring.
   __device__ __forceinline__ void produce(const TcParams& p) const {
     const int num_work = p.num_m_tiles * p.num_n_tiles * p.split_k;
@@ -534,14 +596,8 @@ struct Ring {
       // belong to the next one (or are TMA zero fill) and are masked by the epilogue
       const int a_row0 = (int)(bat * p.a_batch_rows) + m_tile * kBlockM;
       const int b_row0 = (int)(bat * p.b_batch_rows) + n0;
-      int frame = 0, y0 = 0, x0 = 0;
-      if (p.mode == kGemmConv3x3) {
-        const int per_frame = p.tiles_x * p.tiles_y;
-        frame = m_tile / per_frame;
-        const int r = m_tile % per_frame;
-        y0 = (r / p.tiles_x) * p.tileH;
-        x0 = (r % p.tiles_x) * p.tileW;
-      }
+      ConvTile ct{0, 0, 0};
+      if (p.mode == kGemmConv3x3) ct = conv_tile(p, m_tile);
       for (int kb = kb0; kb < kb1; ++kb) {
         ptx::mbar_wait(&empty_bar[cur.stage], cur.phase ^ 1u, p.err, 101);
         ptx::mbar_arrive_expect_tx(&full_bar[cur.stage], Cfg::kStageBytes);
@@ -554,7 +610,7 @@ struct Ring {
 #pragma unroll
           for (int pl = 0; pl < P; ++pl)
             ptx::tma_load_5d(sa + pl * Cfg::kABytes, &p.tmA, &full_bar[cur.stage], cb * kBlockK,
-                             x0 + kx - 1, y0 + ky - 1, frame, pl);
+                             ct.x0 + kx - 1, ct.y0 + ky - 1, ct.frame, pl);
         } else {
 #pragma unroll
           for (int pl = 0; pl < P; ++pl)
@@ -570,167 +626,6 @@ struct Ring {
   }
 };
 
-// Named barriers 3, 4: consumer 0's, consumer 1's epilogue staging (output boxes or statistics).
-constexpr uint32_t kStagingBarrier = 3;
-// setmaxnreg: registers of the producer and of each consumer warpgroup thread.  The consumers of
-// the ping-pong kernels hold 128 accumulators per thread at BLOCK_N = 128; the cooperative
-// kernel's straight-line epilogue with statistics spilled at the 168 registers of an even split.
-constexpr int kProducerRegs = 40;
-constexpr int kConsumerRegs = 232;
-
-// Cooperative schedule: both consumer warpgroups work on every tile, 64 rows each, and run their
-// epilogues at the same time.  Used for split-K, P = 3 and CTAs with fewer than two tiles.  Each
-// warpgroup's statistics slots follow the ring.
-template <int BLOCK_N>
-constexpr int kCoopStaging = kConsumers * kStatsSlotBytes<BLOCK_N>;
-
-template <int BLOCK_N, int P>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_tc_kernel(const __grid_constant__ TcParams p) {
-  using Cfg = TcCfg<BLOCK_N, P, kCoopStaging<BLOCK_N>>;
-  static_assert(Cfg::kStages == TcCfg<BLOCK_N, P>::kStages, "the statistics slots must not cost the ring a stage");
-  extern __shared__ uint8_t smem_raw[];
-  const Ring<BLOCK_N, P, kCoopStaging<BLOCK_N>> ring(smem_raw, p, kConsumerArrivals);
-
-  const int wg = threadIdx.x >> 7;
-  const int warp = (threadIdx.x >> 5) & 3;  // within the warpgroup
-  const int lane = threadIdx.x & 31;
-  __syncthreads();
-
-  // split-K (small problems that cannot fill the GPU): work item = (tile, k-slice)
-  const int num_work = p.num_m_tiles * p.num_n_tiles * p.split_k;
-
-  if (wg == 0) {
-    ptx::setmaxnreg_dec<kProducerRegs>();
-    if (threadIdx.x == 0) ring.produce(p);
-    return;
-  }
-  ptx::setmaxnreg_inc<kConsumerRegs>();
-
-  // -------------------------------------------------------------------- consumers
-  const int cw = wg - 1;                        // rows [64 cw, 64 cw + 64) of the tile
-  const uint32_t a_off = (uint32_t)cw * 64 * 128;  // their A rows: eight whole swizzle atoms
-  double* red = reinterpret_cast<double*>(ring.staging + cw * kStatsSlotBytes<BLOCK_N>);
-  StageCursor<Cfg::kStages> cur;
-  float acc[1][BLOCK_N / 2];
-  for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-    int bat, m_tile, n0, kb0, kb1;
-    const int split = decode_work<BLOCK_N>(p, w, bat, m_tile, n0, kb0, kb1);
-#pragma unroll
-    for (int i = 0; i < BLOCK_N / 2; ++i) acc[0][i] = 0.f;
-    int prev = -1;
-    for (int kb = kb0; kb < kb1; ++kb) {
-      const uint32_t sa = ptx::smem_u32(ring.smem + cur.stage * Cfg::kStageBytes);
-      consume_k_block<BLOCK_N, P, 1>(acc, &ring.full_bar[cur.stage], cur.phase, p, 103, sa + a_off, Cfg::kABytes,
-                                     1024, sa + P * Cfg::kABytes, Cfg::kBBytes, kb > kb0, ring.empty_bar, prev, lane);
-      prev = cur.stage;
-      cur.advance();
-    }
-    ptx::wgmma_wait<0>();
-    ptx::reg_fence(acc[0]);
-    if (prev >= 0 && lane == 0) ptx::mbar_arrive(&ring.empty_bar[prev]);
-    tile_epilogue<BLOCK_N>(p, acc[0], m_tile, cw * 64, n0, warp, lane,
-                           split * p.split_stride + bat * p.out_batch_stride, red, false);
-    if (p.stats != nullptr) flush_stats<BLOCK_N>(p, red, n0, tile_frame(p, m_tile), kStagingBarrier + cw);
-  }
-}
-
-// Ping-pong schedule (no split-K, P <= 2): each consumer warpgroup owns whole 128-row tiles, two
-// m64 wgmma per k step (rows 0-63 and 64-127), and the CTA's tiles alternate between the two.  The
-// warpgroups take turns on the tensor pipe: one issues its tile's whole mainloop, passes the turn
-// and runs its epilogue while the other's MMAs execute, so the epilogue costs no MMA time as long
-// as it is shorter than a mainloop.  The producer is the cooperative one: the ring holds tile t's
-// k-blocks, then tile t + 1's, and each stage is read (and released) by one warpgroup.
-//
-// The turn also keeps the full-barrier parity waits exact: a warpgroup waits on its tile's first
-// stage only after the other has waited on every stage of the tile before, so the stage it waits
-// on has completed all earlier fills and is never a whole phase behind.
-//
-// Every output element sums its K terms in the cooperative kernel's order, so the two schedules
-// give bit-identical outputs (the fused statistics keep its per-warp fp32 partials as well; only
-// the order of their fp64 additions differs, as the order of the atomics may between two runs of
-// either kernel).  A tile's statistics slots share the warpgroup's output box buffers: a GEMM
-// with statistics has no plane output.
-constexpr uint32_t kTurnBarrier = 1;  // named barriers 1, 2: consumer 0's, consumer 1's turn
-
-template <int BLOCK_N, int P>
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
-  using Cfg = TcCfg<BLOCK_N, P, kPlaneStagingBytes>;
-  static_assert(P <= 2, "ping-pong: P = 3 stays cooperative");
-  static_assert(Cfg::kStages == TcCfg<BLOCK_N, P>::kStages, "the output staging must not cost the ring a stage");
-  static_assert(kStatsSlotBytes<BLOCK_N> <= 2 * kPlaneBoxBytes, "statistics slots: one warpgroup's box buffers");
-  extern __shared__ uint8_t smem_raw[];
-  const Ring<BLOCK_N, P, kPlaneStagingBytes> ring(smem_raw, p, 4);  // one arrive per warp of the reading warpgroup
-
-  const int wg = threadIdx.x >> 7;
-  const int warp = (threadIdx.x >> 5) & 3;
-  const int lane = threadIdx.x & 31;
-  __syncthreads();
-
-  if (wg == 0) {
-    ptx::setmaxnreg_dec<kProducerRegs>();
-    if (threadIdx.x == 0) ring.produce(p);
-    return;
-  }
-  ptx::setmaxnreg_inc<kConsumerRegs>();
-
-  const int cw = wg - 1;
-  const int nkb = p.num_k_blocks;
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
-  const int my_tiles = (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  float acc[2][BLOCK_N / 2];  // rows 0-63, rows 64-127
-  for (int t = cw; t < my_tiles; t += 2) {
-    int bat, m_tile, n0, kb0, kb1;
-    decode_work<BLOCK_N>(p, (int)blockIdx.x + t * (int)gridDim.x, bat, m_tile, n0, kb0, kb1);
-    if (t > 0) ptx::named_bar_sync(kTurnBarrier + cw, 256);
-    const long long pos = (long long)t * nkb;  // ring position of the tile's first k-block
-    StageCursor<Cfg::kStages> cur{(int)(pos % Cfg::kStages), (uint32_t)(pos / Cfg::kStages) & 1u};
-#pragma unroll
-    for (int h = 0; h < 2; ++h)
-#pragma unroll
-      for (int i = 0; i < BLOCK_N / 2; ++i) acc[h][i] = 0.f;
-    int prev = -1;
-    for (int kb = 0; kb < nkb; ++kb) {
-      const uint32_t sa = ptx::smem_u32(ring.smem + cur.stage * Cfg::kStageBytes);
-      consume_k_block<BLOCK_N, P, 2>(acc, &ring.full_bar[cur.stage], cur.phase, p, 104, sa, Cfg::kABytes, 1024,
-                                     sa + P * Cfg::kABytes, Cfg::kBBytes, kb > 0, ring.empty_bar, prev, lane);
-      prev = cur.stage;
-      cur.advance();
-    }
-    // every MMA of this tile is issued: the other warpgroup's tile, if it has one, may start
-    if (t + 1 < my_tiles) ptx::named_bar_arrive(kTurnBarrier + (1 - cw), 256);
-    ptx::wgmma_wait<0>();
-    ptx::reg_fence(acc[0]);
-    ptx::reg_fence(acc[1]);
-    if (lane == 0) ptx::mbar_arrive(&ring.empty_bar[prev]);
-    const bool staged = p.plane_tma && whole_tile<BLOCK_N>(p, m_tile, n0);
-    uint8_t* const staging = ring.staging + cw * 2 * kPlaneBoxBytes;
-    double* const red = reinterpret_cast<double*>(staging);
-    // one copy of the epilogue code for both halves: it runs while the other warpgroup's mainloop
-    // executes from the same instruction cache
-#pragma unroll 1
-    for (int h = 0; h < 2; ++h) {
-      if (!staged) {
-        tile_epilogue<BLOCK_N>(p, acc[0], m_tile, 64 * h, n0, warp, lane, bat * p.out_batch_stride, red, h == 1);
-      } else {
-        const uint32_t boxes = ptx::smem_u32(staging);
-        if (p.bias != nullptr)
-          epilogue_planes_tma<BLOCK_N, true>(p, acc[0], m_tile, 64 * h, n0, boxes, kStagingBarrier + cw, warp, lane);
-        else
-          epilogue_planes_tma<BLOCK_N, false>(p, acc[0], m_tile, 64 * h, n0, boxes, kStagingBarrier + cw, warp, lane);
-      }
-      if (h == 0) {
-#pragma unroll
-        for (int i = 0; i < BLOCK_N / 2; ++i) acc[0][i] = acc[1][i];
-      }
-    }
-    if (p.stats != nullptr) flush_stats<BLOCK_N>(p, red, n0, tile_frame(p, m_tile), kStagingBarrier + cw);
-    // after the warpgroup's last tile: its stores complete while the shared memory still exists
-    if (t + 2 >= my_tiles && warp == 0 && lane == 0) ptx::bulk_wait<0>();
-  }
-}
-
 // ------------------------------------------------------------------------------ halo-patch conv
 // 3x3 convolution, C = 64 -> N = 64 (the first ResNet group, stride 1).  The generic implicit GEMM
 // loads one shifted 128-pixel box per tap, so every input element crosses L2 -> SM nine times.
@@ -739,9 +634,8 @@ gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
 // view has the same swizzle phase) and the nine taps are nine shared-memory views of it: output
 // rows 8c .. 8c + 7 of the tile (one m64 wgmma) read start = patch + (8c + ky) * 2048 + kx * 128,
 // with 2048 B between their 8-pixel row groups.  B (weights, 8 KB per tap and plane) streams
-// through a 4-slot ring.  Two schedules, as the GEMM's: conv3x3_halo_kernel (cooperative, consumer
-// c computes rows 8c .. 8c + 7 of every tile) and conv3x3_halo_pingpong_kernel (each consumer
-// whole tiles, both halves).  Epilogue as in the GEMM kernels.
+// through a 4-slot ring, one tap per k-block.  Both schedules of wgmma_kernel run it:
+// conv3x3_halo_kernel and conv3x3_halo_pingpong_kernel.
 constexpr int kHaloTileW = 8, kHaloTileH = 16;
 constexpr int kHaloRowBytes = 2048;                        // 16 pixels x 128 B
 constexpr int kHaloPatchRows = kHaloTileH + 2;
@@ -761,184 +655,231 @@ struct HaloCfg {
 };
 
 // Shared memory of both halo schedules: the patch ring [2][P][18][2048], the B ring [4][P][64][128],
-// the consumers' statistics slots, then the full / empty barriers of the two rings.
+// the consumers' statistics slots, then the full / empty barriers of the two rings.  The k-blocks
+// (full_bar, empty_bar) are the B ring's.
 template <int P>
 struct HaloRing {
   using Cfg = HaloCfg<P>;
+  static constexpr int kBlockN = 64, kP = P, kStages = kHaloBStages;
+  static constexpr uint32_t kAPlane = kHaloPatchBytes, kASbo = kHaloRowBytes, kBPlane = kHaloBBytes;
+  static constexpr bool kPlaneBoxes = false;
+  static constexpr int kFullErr = 405;
   uint8_t* patch;
   uint8_t* bring;
-  double* stats;
-  uint64_t* pfull;   // [2]
-  uint64_t* pempty;  // [2]
-  uint64_t* bfull;   // [4]
-  uint64_t* bempty;  // [4]
+  uint8_t* staging;
+  uint64_t* pfull;      // [2]
+  uint64_t* pempty;     // [2]
+  uint64_t* full_bar;   // [4]
+  uint64_t* empty_bar;  // [4]
   __device__ __forceinline__ HaloRing(uint8_t* smem_raw, const TcParams& p, uint32_t empty_arrivals) {
     patch = aligned_smem(smem_raw);
     bring = patch + kHaloPatchStages * Cfg::kPatchStage;
-    stats = reinterpret_cast<double*>(bring + kHaloBStages * Cfg::kBStage);
-    pfull = reinterpret_cast<uint64_t*>(bring + kHaloBStages * Cfg::kBStage + kHaloStatsBytes);
+    staging = bring + kHaloBStages * Cfg::kBStage;
+    pfull = reinterpret_cast<uint64_t*>(staging + kHaloStatsBytes);
     pempty = pfull + kHaloPatchStages;
-    bfull = pempty + kHaloPatchStages;
-    bempty = bfull + kHaloBStages;
+    full_bar = pempty + kHaloPatchStages;
+    empty_bar = full_bar + kHaloBStages;
     init_rings(pfull, empty_arrivals, &p.tmPatch, &p.tmB, kHaloPatchStages, kHaloBStages);
   }
 
   // TMA producer (one thread): per tile of this CTA, its patch, then its nine taps of B.
   __device__ __forceinline__ void produce(const TcParams& p) const {
-    const int per_frame = p.tiles_x * p.tiles_y;
     StageCursor<kHaloPatchStages> pc;
     StageCursor<kHaloBStages> bc;
     for (int w = blockIdx.x; w < p.num_m_tiles; w += gridDim.x) {
-      const int frame = w / per_frame;
-      const int r = w - frame * per_frame;
-      const int y0 = (r / p.tiles_x) * kHaloTileH, x0 = (r % p.tiles_x) * kHaloTileW;
+      const ConvTile ct = conv_tile(p, w);
       ptx::mbar_wait(&pempty[pc.stage], pc.phase ^ 1u, p.err, 401);
       ptx::mbar_arrive_expect_tx(&pfull[pc.stage], (uint32_t)(P * kHaloPatchRows * kHaloRowLoadBytes));
       for (int pl = 0; pl < P; ++pl)
         for (int pr = 0; pr < kHaloPatchRows; ++pr)
           ptx::tma_load_5d(patch + pc.stage * Cfg::kPatchStage + pl * kHaloPatchBytes + pr * kHaloRowBytes,
-                           &p.tmPatch, &pfull[pc.stage], 0, x0 - 1, y0 - 1 + pr, frame, pl);
+                           &p.tmPatch, &pfull[pc.stage], 0, ct.x0 - 1, ct.y0 - 1 + pr, ct.frame, pl);
       pc.advance();
       for (int tap = 0; tap < 9; ++tap) {
-        ptx::mbar_wait(&bempty[bc.stage], bc.phase ^ 1u, p.err, 402);
-        ptx::mbar_arrive_expect_tx(&bfull[bc.stage], (uint32_t)Cfg::kBStage);
+        ptx::mbar_wait(&empty_bar[bc.stage], bc.phase ^ 1u, p.err, 402);
+        ptx::mbar_arrive_expect_tx(&full_bar[bc.stage], (uint32_t)Cfg::kBStage);
 #pragma unroll
         for (int pl = 0; pl < P; ++pl)
-          ptx::tma_load_3d(bring + bc.stage * Cfg::kBStage + pl * kHaloBBytes, &p.tmB, &bfull[bc.stage],
+          ptx::tma_load_3d(bring + bc.stage * Cfg::kBStage + pl * kHaloBBytes, &p.tmB, &full_bar[bc.stage],
                            tap * kBlockK, 0, pl);
         bc.advance();
       }
     }
   }
+
+  __device__ __forceinline__ Work work(const TcParams&, int w) const { return {w, 0, 0, 9, 0}; }
+  // tap kb = 3 ky + kx: the patch view of output rows 0-7 (see above)
+  __device__ __forceinline__ void kblock(int t, int stage, int kb, uint32_t& a, uint32_t& b) const {
+    const int ky = kb / 3, kx = kb - ky * 3;
+    a = ptx::smem_u32(patch + (t % kHaloPatchStages) * Cfg::kPatchStage) + ky * kHaloRowBytes + kx * 128;
+    b = ptx::smem_u32(bring + stage * Cfg::kBStage);
+  }
+  // The producer fills the patch stages in tile order: local tile t's patch is fill t / 2 of stage t % 2.
+  __device__ __forceinline__ void wait_tile(const TcParams& p, int t) const {
+    ptx::mbar_wait(&pfull[t % kHaloPatchStages], (uint32_t)(t / kHaloPatchStages) & 1u, p.err, 404);
+  }
+  __device__ __forceinline__ void release_tile(int t) const { ptx::mbar_arrive(&pempty[t % kHaloPatchStages]); }
+  __device__ __forceinline__ uint8_t* consumer_staging(int cw) const { return staging + cw * kStatsSlotBytes<64>; }
 };
 
-template <int P>
-__global__ void __launch_bounds__(kThreads, 1)
-conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
-  using Cfg = HaloCfg<P>;
-  extern __shared__ uint8_t smem_raw[];
-  const HaloRing<P> ring(smem_raw, p, kConsumerArrivals);
+// ------------------------------------------------------------------------------ the kernels
+// Named barriers 1, 2: consumer 0's, consumer 1's turn (ping-pong).  3, 4: their epilogue staging
+// (output boxes or statistics).
+constexpr uint32_t kTurnBarrier = 1;
+constexpr uint32_t kStagingBarrier = 3;
+// setmaxnreg: registers of the producer and of each consumer warpgroup thread.  The consumers of
+// the ping-pong kernels hold 128 accumulators per thread at BLOCK_N = 128; the cooperative
+// kernel's straight-line epilogue with statistics spilled at the 168 registers of an even split.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
 
-  const int wg = threadIdx.x >> 7;
-  const int warp = (threadIdx.x >> 5) & 3;
-  const int lane = threadIdx.x & 31;
-  __syncthreads();
-
-  if (wg == 0) {
-    if (threadIdx.x == 0) ring.produce(p);
-    return;
-  }
-
-  const int cw = wg - 1;
-  double* red = ring.stats + cw * (kStatsSlotBytes<64> / 8);
-  StageCursor<kHaloPatchStages> pc;
-  StageCursor<kHaloBStages> bc;
-  float acc[1][32];
-  for (int w = blockIdx.x; w < p.num_m_tiles; w += gridDim.x) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc[0][i] = 0.f;
-    ptx::mbar_wait(&ring.pfull[pc.stage], pc.phase, p.err, 404);
-    const uint32_t pbase = ptx::smem_u32(ring.patch + pc.stage * Cfg::kPatchStage) + (uint32_t)cw * 8 * kHaloRowBytes;
-    int prev = -1;
-    for (int tap = 0; tap < 9; ++tap) {
-      const int ky = tap / 3, kx = tap - ky * 3;
-      consume_k_block<64, P, 1>(acc, &ring.bfull[bc.stage], bc.phase, p, 405,
-                                pbase + ky * kHaloRowBytes + kx * 128, kHaloPatchBytes, kHaloRowBytes,
-                                ptx::smem_u32(ring.bring + bc.stage * Cfg::kBStage), kHaloBBytes, tap > 0,
-                                ring.bempty, prev, lane);
-      prev = bc.stage;
-      bc.advance();
-    }
-    ptx::wgmma_wait<0>();
-    ptx::reg_fence(acc[0]);
-    if (lane == 0) {
-      ptx::mbar_arrive(&ring.bempty[prev]);
-      ptx::mbar_arrive(&ring.pempty[pc.stage]);
-    }
-    pc.advance();
-    tile_epilogue<64>(p, acc[0], w, cw * 64, 0, warp, lane, 0, red, false);
-    if (p.stats != nullptr) flush_stats<64>(p, red, 0, tile_frame(p, w), kStagingBarrier + cw);
-  }
-}
-
-// Ping-pong halo convolution: as gemm_tc_pingpong_kernel, each consumer warpgroup owns whole
-// tiles, alternately, and per tap issues two m64n64 wgmma on the views of output rows 0-7 and
-// 8-15 (2 x 32 accumulators), passes the tensor pipe to the other warpgroup once its nine taps
-// are issued, and runs its epilogue while the other's MMAs execute.
+// The body of every wgmma kernel, over the operand source Src (Ring or HaloRing) in one of two
+// schedules.  Warpgroup 0's first thread runs Src's producer; warpgroups 1 and 2 consume:
+//   cooperative (PINGPONG false): both consumers work on every tile, consumer cw on its rows
+//     64 cw .. 64 cw + 63 (one m64 accumulator, A from + 8 cw kASbo), and they run their epilogues
+//     at the same time.  Used for split-K, P = 3 and where a CTA gets too few tiles for
+//     ping-pong (pick_pingpong, launch_halo).
+//   ping-pong: consumer cw owns the CTA's local tiles t with t % 2 == cw, whole (two m64
+//     accumulators, rows 0-63 and 64-127).  The warpgroups take turns on the tensor pipe: one
+//     issues its tile's whole mainloop, passes the turn and runs its epilogue while the other's
+//     MMAs execute, so the epilogue costs no MMA time as long as it is shorter than a mainloop.
 //
-// Parity waits.  The producer fills the patch stages in tile order, so local tile t of the CTA
-// uses patch stage t % 2: warpgroup c always reads stage c, and its fills alternate with no one
-// else's; it waits for fill t / 2 with parity (t / 2) & 1 and releases the stage once the tile's
-// MMAs have retired, and the producer then refills it for tile t + 2.  The B ring holds tile t's
-// nine taps at ring positions 9 t .. 9 t + 8, and each stage is read by whichever warpgroup owns
-// the tile.  A warpgroup waits on its tile's first B stage only after the other has passed the
-// turn, that is after it has waited on every B stage of tile t - 1, so every earlier fill of the
-// stage it waits on has completed and that stage is never a whole phase behind: the parity
-// (position / 4) & 1 is exact.
-template <int P>
-__global__ void __launch_bounds__(kThreads, 1)
-conv3x3_halo_pingpong_kernel(const __grid_constant__ TcParams p) {
-  using Cfg = HaloCfg<P>;
+// Each consumer walks every local tile of its CTA in order, as the producer fills the ring, and
+// keeps one ring position, advanced by each tile's k-block count; under ping-pong it only
+// advances it over the other warpgroup's tiles.  A full-barrier parity wait is exact when every
+// earlier fill of the stage has completed (the producer cannot be a fill ahead: it waits for the
+// stage to be released).  The cooperative consumers wait on every position in order.  Under
+// ping-pong, a warpgroup waits on its tile's first stage only after the other has passed the
+// turn, that is after it has waited on every stage of the tile before; by induction every earlier
+// position has been waited on.  The halo patch ring holds one tile per stage and follows the same
+// argument: under ping-pong consumer cw always reads patch stage cw.
+//
+// Every output element sums its K terms in the same order in both schedules, so they give
+// bit-identical outputs (the fused statistics keep the per-warp fp32 partials as well; only the
+// order of their fp64 additions differs, as the order of the atomics may between two runs of
+// either kernel).
+template <class Src, bool PINGPONG>
+__device__ __forceinline__ void wgmma_kernel(const TcParams& p) {
+  constexpr int BLOCK_N = Src::kBlockN, HALVES = PINGPONG ? 2 : 1;
+  constexpr bool kBoxes = PINGPONG && Src::kPlaneBoxes;
   extern __shared__ uint8_t smem_raw[];
-  const HaloRing<P> ring(smem_raw, p, 4);  // one arrive per warp of the reading warpgroup
+  const Src src(smem_raw, p, PINGPONG ? 4 : kConsumerArrivals);  // one arrive per reading warp
 
   const int wg = threadIdx.x >> 7;
-  const int warp = (threadIdx.x >> 5) & 3;
+  const int warp = (threadIdx.x >> 5) & 3;  // within the warpgroup
   const int lane = threadIdx.x & 31;
   __syncthreads();
 
   if (wg == 0) {
     ptx::setmaxnreg_dec<kProducerRegs>();
-    if (threadIdx.x == 0) ring.produce(p);
+    if (threadIdx.x == 0) src.produce(p);
     return;
   }
   ptx::setmaxnreg_inc<kConsumerRegs>();
 
   const int cw = wg - 1;
-  const int my_tiles = (p.num_m_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  double* red = ring.stats + cw * (kStatsSlotBytes<64> / 8);
-  const uint32_t pbase = ptx::smem_u32(ring.patch + cw * Cfg::kPatchStage);  // patch stage cw
-  float acc[2][32];  // output rows 0-7, rows 8-15 of the tile
-  for (int t = cw; t < my_tiles; t += 2) {
-    const int w = (int)blockIdx.x + t * (int)gridDim.x;
-    if (t > 0) ptx::named_bar_sync(kTurnBarrier + cw, 256);
-    const int pos = 9 * t;  // ring position of the tile's first tap
-    StageCursor<kHaloBStages> bc{pos % kHaloBStages, (uint32_t)(pos / kHaloBStages) & 1u};
+  const uint32_t a_rows = PINGPONG ? 0u : (uint32_t)cw * 8 * Src::kASbo;
+  uint8_t* const staging = src.consumer_staging(cw);
+  double* const red = reinterpret_cast<double*>(staging);
+  // split-K (small problems that cannot fill the GPU): work item = (tile, k-slice)
+  const int num_work = p.num_m_tiles * p.num_n_tiles * p.split_k;
+  const int my_tiles = (num_work - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  StageCursor<Src::kStages> cur;
+  float acc[HALVES][BLOCK_N / 2];
+  for (int t = 0; t < my_tiles; ++t) {
+    const Work wk = src.work(p, (int)blockIdx.x + t * (int)gridDim.x);
+    if (PINGPONG && (t & 1) != cw) {
+      cur.advance(wk.kb1 - wk.kb0);
+      continue;
+    }
+    if (PINGPONG && t > 0) ptx::named_bar_sync(kTurnBarrier + cw, 256);
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+    for (int h = 0; h < HALVES; ++h)
 #pragma unroll
-      for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
-    ptx::mbar_wait(&ring.pfull[cw], (uint32_t)(t >> 1) & 1u, p.err, 406);
+      for (int i = 0; i < BLOCK_N / 2; ++i) acc[h][i] = 0.f;
+    src.wait_tile(p, t);
     int prev = -1;
-    for (int tap = 0; tap < 9; ++tap) {
-      const int ky = tap / 3, kx = tap - ky * 3;
-      consume_k_block<64, P, 2>(acc, &ring.bfull[bc.stage], bc.phase, p, 407,
-                                pbase + ky * kHaloRowBytes + kx * 128, kHaloPatchBytes, kHaloRowBytes,
-                                ptx::smem_u32(ring.bring + bc.stage * Cfg::kBStage), kHaloBBytes, tap > 0,
-                                ring.bempty, prev, lane);
-      prev = bc.stage;
-      bc.advance();
+    for (int kb = wk.kb0; kb < wk.kb1; ++kb) {
+      uint32_t a, b;
+      src.kblock(t, cur.stage, kb, a, b);
+      consume_k_block<BLOCK_N, Src::kP, HALVES>(acc, &src.full_bar[cur.stage], cur.phase, p, Src::kFullErr,
+                                                a + a_rows, Src::kAPlane, Src::kASbo, b, Src::kBPlane, kb > wk.kb0,
+                                                src.empty_bar, prev, lane);
+      prev = cur.stage;
+      cur.advance();
     }
     // every MMA of this tile is issued: the other warpgroup's tile, if it has one, may start
-    if (t + 1 < my_tiles) ptx::named_bar_arrive(kTurnBarrier + (1 - cw), 256);
+    if (PINGPONG && t + 1 < my_tiles) ptx::named_bar_arrive(kTurnBarrier + (1 - cw), 256);
     ptx::wgmma_wait<0>();
-    ptx::reg_fence(acc[0]);
-    ptx::reg_fence(acc[1]);
-    if (lane == 0) {
-      ptx::mbar_arrive(&ring.bempty[prev]);
-      ptx::mbar_arrive(&ring.pempty[cw]);
-    }
-    // one copy of the epilogue code for both halves (see gemm_tc_pingpong_kernel)
-#pragma unroll 1
-    for (int h = 0; h < 2; ++h) {
-      tile_epilogue<64>(p, acc[0], w, 64 * h, 0, warp, lane, 0, red, h == 1);
-      if (h == 0) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) acc[0][i] = acc[1][i];
+    for (int h = 0; h < HALVES; ++h) ptx::reg_fence(acc[h]);
+    if (lane == 0) {
+      if (prev >= 0) ptx::mbar_arrive(&src.empty_bar[prev]);
+      src.release_tile(t);
+    }
+    const bool staged = kBoxes && p.plane_tma && whole_tile<BLOCK_N>(p, wk.m_tile, wk.n0);
+    // one copy of the epilogue code for both ping-pong halves: it runs while the other
+    // warpgroup's mainloop executes from the same instruction cache
+#pragma unroll 1
+    for (int h = 0; h < HALVES; ++h) {
+      const int r_base = 64 * (PINGPONG ? h : cw);
+      if (staged) {
+        if constexpr (kBoxes) {  // only the ping-pong GEMM compiles this path
+          const uint32_t boxes = ptx::smem_u32(staging);
+          if (p.bias != nullptr)
+            epilogue_planes_tma<BLOCK_N, true>(p, acc[0], wk.m_tile, r_base, wk.n0, boxes, kStagingBarrier + cw,
+                                               warp, lane);
+          else
+            epilogue_planes_tma<BLOCK_N, false>(p, acc[0], wk.m_tile, r_base, wk.n0, boxes, kStagingBarrier + cw,
+                                                warp, lane);
+        }
+      } else {
+        tile_epilogue<BLOCK_N>(p, acc[0], wk.m_tile, r_base, wk.n0, warp, lane, wk.out_off, red, h == 1);
+      }
+      if constexpr (HALVES == 2) {
+        if (h == 0) {
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 2; ++i) acc[0][i] = acc[1][i];
+        }
       }
     }
-    if (p.stats != nullptr) flush_stats<64>(p, red, 0, tile_frame(p, w), kStagingBarrier + cw);
+    if (p.stats != nullptr) flush_stats<BLOCK_N>(p, red, wk.n0, tile_frame(p, wk.m_tile), kStagingBarrier + cw);
+    // after the warpgroup's last tile: its stores complete while the shared memory still exists
+    // (here rather than after the loop, where the BN = 128 instances spill)
+    if constexpr (kBoxes)
+      if (t + 2 >= my_tiles && warp == 0 && lane == 0) ptx::bulk_wait<0>();
   }
+}
+
+// Cooperative GEMM: each warpgroup's statistics slots follow the ring.
+template <int BLOCK_N>
+constexpr int kCoopStaging = kConsumers * kStatsSlotBytes<BLOCK_N>;
+
+template <int BLOCK_N, int P>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_tc_kernel(const __grid_constant__ TcParams p) {
+  wgmma_kernel<Ring<BLOCK_N, P, kCoopStaging<BLOCK_N>>, false>(p);
+}
+
+// Ping-pong GEMM (no split-K, P <= 2): each warpgroup's two output box buffers follow the ring; a
+// tile's statistics slots share them (a GEMM with statistics has no plane output).
+template <int BLOCK_N, int P>
+__global__ void __launch_bounds__(kThreads, 1)
+gemm_tc_pingpong_kernel(const __grid_constant__ TcParams p) {
+  static_assert(P <= 2, "ping-pong: P = 3 stays cooperative");
+  wgmma_kernel<Ring<BLOCK_N, P, kPlaneStagingBytes>, true>(p);
+}
+
+template <int P>
+__global__ void __launch_bounds__(kThreads, 1)
+conv3x3_halo_kernel(const __grid_constant__ TcParams p) {
+  wgmma_kernel<HaloRing<P>, false>(p);
+}
+
+template <int P>
+__global__ void __launch_bounds__(kThreads, 1)
+conv3x3_halo_pingpong_kernel(const __grid_constant__ TcParams p) {
+  wgmma_kernel<HaloRing<P>, true>(p);
 }
 
 // Second pass of a split-K GEMM: sums the k-slice partials in a fixed order (deterministic) and
