@@ -384,6 +384,36 @@ int tapir_paint_point_track(const uint8_t* frames, int32_t T, int32_t H, int32_t
                             int32_t N, const uint8_t* colors, uint8_t* out, void* workspace,
                             size_t workspace_bytes, void* stream);
 
+/* ---- f6: evaluation (the step before the path) -------------------------------------- */
+/* tapvid/evaluation_datasets.py:41-45 resize_video on uint8 RGB frames, bit for bit as PIL's
+ * Image.resize(..., LANCZOS) (what mediapy.resize_video runs per uint8 frame).  Per axis
+ * (in -> out): scale = in / out, fs = max(scale, 1), ksize = 2 ceil(3 fs) + 1; output o reads
+ * inputs xmin .. xmin + n - 1 with taps lanczos((i + xmin - c + 0.5) * (1 / fs)), c = (o + 0.5) scale,
+ * normalised in double and rounded half away from zero to 22 fraction bits; a pass is
+ * clamp((2^21 + sum src * tap) >> 22, 0, 255) in int32.
+ *
+ * tapir_lanczos_weights is host only (no GPU): for sizes in 1..TAPIR_MAX_RESIZE_SIDE it returns
+ * ksize and, unless they are NULL, fills the host arrays bounds [out_size][2] (xmin, n) and
+ * taps [out_size][ksize] int32; bad sizes return -1 with tapir_last_error() set. */
+#define TAPIR_MAX_RESIZE_SIDE 65535
+int32_t tapir_lanczos_weights(int32_t in_size, int32_t out_size, int32_t* bounds, int32_t* taps);
+/* Workspace of tapir_resize_lanczos_u8: the uint8 intermediate of the rows the vertical pass reads
+ * (0 unless both W != w and H != h); 0 for bad sizes. */
+size_t tapir_resize_lanczos_u8_workspace_bytes(int32_t frames, int32_t H, int32_t W, int32_t h,
+                                               int32_t w);
+/* src [frames][H][W][3] uint8 -> dst [frames][h][w][3] uint8: a horizontal pass (if W != w) into
+ * a uint8 intermediate, then a vertical pass (if H != h); equal sizes copy.  x_* are the device
+ * copies of tapir_lanczos_weights(W, w) (with its ksize), y_* of tapir_lanczos_weights(H, h); the
+ * tables of an axis that keeps its size are not read and may be NULL.  Workspace 16-byte aligned,
+ * at least tapir_resize_lanczos_u8_workspace_bytes (NULL when that is 0).  No allocation, no
+ * host <-> device copy, no host sync: graph-capturable.  A bad argument (size, NULL pointer, table
+ * size, workspace size or alignment, dst or workspace overlapping src) returns 1 before any CUDA
+ * call. */
+int tapir_resize_lanczos_u8(const uint8_t* src, uint8_t* dst, int32_t frames, int32_t H, int32_t W,
+                            int32_t h, int32_t w, const int32_t* x_bounds, const int32_t* x_taps,
+                            int32_t x_ksize, const int32_t* y_bounds, const int32_t* y_taps,
+                            int32_t y_ksize, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- a4: tapir_model.py:217-291 + utils.py:45-73 (trilinear, border clamp) ---------- */
 /* query_tyx [N][3] in video coordinates (vT,vH,vW) -> out [N][C] */
 int tapir_sample_query_features(const float* grid, int32_t T, int32_t gh, int32_t gw, int32_t C,

@@ -36,3 +36,9 @@ timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
     python -m pytest -q -m gpu -p no:cacheprovider tests/test_gemm_exact_gpu.py \
     2>&1 | grep -E '^=========|passed|failed' | tail -n 25
 echo "sanitizer gemm_exact memcheck rc=${PIPESTATUS[0]}"
+# then the Lanczos resize (both passes, one axis, identity, 1-pixel sides, bad arguments); the
+# readers and the model runs of the evaluation tests are left out
+timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
+    python -m pytest -q -m gpu -p no:cacheprovider tests/test_tapvid_gpu.py -k "not evaluate and not readers" \
+    2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+echo "sanitizer tapvid memcheck rc=${PIPESTATUS[0]}"

@@ -27,6 +27,7 @@ MAX_MIXER_BLOCKS = 12
 NUM_RESNET_BLOCKS = 8
 MAX_EXTRA_BLOCKS = 5
 MAX_CORR_LEVELS = 5
+MAX_RESIZE_SIDE = 65535
 
 
 class Linear(Structure):
@@ -207,6 +208,11 @@ SIGNATURES = {
     'tapir_paint_point_track': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int32,
                                                c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_size_t,
                                                c_void_p]),
+    'tapir_lanczos_weights': (c_int32, [c_int32, c_int32, c_void_p, c_void_p]),
+    'tapir_resize_lanczos_u8_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32, c_int32, c_int32]),
+    'tapir_resize_lanczos_u8': (ctypes.c_int, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
+                                               c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                               c_int32, c_void_p, c_size_t, c_void_p]),
 }
 
 _lib = None
@@ -688,3 +694,42 @@ def paint_point_track(frames, tracks, visibles, colors, out, workspace):
   check(load().tapir_paint_point_track(
       ptr(frames), T, H, W, ptr(tracks), int(fp64), ptr(visibles), N, ptr(colors), ptr(out),
       ptr(workspace), _nbytes(workspace), stream()), fn)
+
+
+# ------------------------------------------------------------------------------ evaluation
+def lanczos_weights(in_size, out_size):
+  """Host only: PIL's 8-bit Lanczos tables of one axis in_size -> out_size, as numpy int32
+  bounds [out_size, 2] (xmin, n) and taps [out_size, ksize]."""
+  import numpy as np  # pylint: disable=g-import-not-at-top
+  lib = load()
+  ksize = lib.tapir_lanczos_weights(int(in_size), int(out_size), None, None)
+  if ksize < 0:
+    raise ValueError(lib.tapir_last_error().decode())
+  bounds = np.empty((out_size, 2), np.int32)
+  taps = np.empty((out_size, ksize), np.int32)
+  lib.tapir_lanczos_weights(int(in_size), int(out_size), bounds.ctypes.data, taps.ctypes.data)
+  return bounds, taps
+
+
+def resize_lanczos_u8(src, dst, x_tables, y_tables, workspace):
+  """uint8 src [..., H, W, 3] -> dst [..., h, w, 3] with PIL's Lanczos.  x_tables / y_tables:
+  (bounds, taps) int32 device tensors of lanczos_weights(W, w) / (H, h), or None for an axis that
+  keeps its size; workspace: uint8, at least tapir_resize_lanczos_u8_workspace_bytes."""
+  fn = 'tapir_resize_lanczos_u8'
+  _frames(fn, src, (torch.uint8,))
+  _check(fn, 'dst', dst, torch.uint8, device=src.device)
+  _need(dst.dim() == src.dim() and dst.shape[:-3] == src.shape[:-3] and dst.shape[-1] == 3, fn,
+        f'dst {tuple(dst.shape)} does not match src {tuple(src.shape)}')
+  (H, W), (h, w), nf = src.shape[-3:-1], dst.shape[-3:-1], math.prod(src.shape[:-3])
+  tables = []
+  for name, t, n_out in (('x_tables', x_tables, w), ('y_tables', y_tables, h)):
+    if t is None:
+      tables += [None, None, 0]
+      continue
+    bounds, taps = t
+    _check(fn, name, bounds, torch.int32, (n_out, 2), device=src.device)
+    _check(fn, name, taps, torch.int32, device=src.device)
+    _need(taps.dim() == 2 and taps.shape[0] == n_out, fn, f'{name} taps {tuple(taps.shape)} for {n_out} outputs')
+    tables += [ptr(bounds), ptr(taps), taps.shape[1]]
+  check(load().tapir_resize_lanczos_u8(ptr(src), ptr(dst), nf, H, W, h, w, *tables, ptr(workspace),
+                                       _nbytes(workspace) if workspace is not None else 0, stream()), fn)

@@ -460,4 +460,61 @@ int tapir_paint_point_track(const uint8_t* frames, int32_t T, int32_t H, int32_t
                            S(stream));
 }
 
+namespace {
+bool resize_side_ok(int n) { return n >= 1 && n <= TAPIR_MAX_RESIZE_SIDE; }
+}  // namespace
+
+int32_t tapir_lanczos_weights(int32_t in_size, int32_t out_size, int32_t* bounds, int32_t* taps) {
+  if (!resize_side_ok(in_size) || !resize_side_ok(out_size)) {
+    set_error("tapir_lanczos_weights: sizes %d -> %d outside 1..%d", in_size, out_size,
+              TAPIR_MAX_RESIZE_SIDE);
+    return -1;
+  }
+  if (bounds != nullptr && taps != nullptr) lanczos_weights(in_size, out_size, bounds, taps);
+  return lanczos_ksize(in_size, out_size);
+}
+
+size_t tapir_resize_lanczos_u8_workspace_bytes(int32_t frames, int32_t H, int32_t W, int32_t h,
+                                               int32_t w) {
+  if (frames < 1 || !resize_side_ok(H) || !resize_side_ok(W) || !resize_side_ok(h) || !resize_side_ok(w))
+    return 0;
+  return resize_lanczos_u8_workspace_bytes(frames, H, W, h, w);
+}
+
+int tapir_resize_lanczos_u8(const uint8_t* src, uint8_t* dst, int32_t frames, int32_t H, int32_t W,
+                            int32_t h, int32_t w, const int32_t* x_bounds, const int32_t* x_taps,
+                            int32_t x_ksize, const int32_t* y_bounds, const int32_t* y_taps,
+                            int32_t y_ksize, void* workspace, size_t workspace_bytes, void* stream) {
+  Range nvtx_range("tapir_resize_lanczos_u8");
+  const char* fn = "tapir_resize_lanczos_u8";
+  TAPIR_CHECK_ARG(frames >= 1 && resize_side_ok(H) && resize_side_ok(W) && resize_side_ok(h) &&
+                      resize_side_ok(w),
+                  "%s: frames=%d %dx%d -> %dx%d (frames >= 1, sides in 1..%d)", fn, frames, H, W, h, w,
+                  TAPIR_MAX_RESIZE_SIDE);
+  TAPIR_CHECK_ARG(src && dst, "%s: null src / dst", fn);
+  const size_t src_bytes = (size_t)frames * H * W * 3, dst_bytes = (size_t)frames * h * w * 3;
+  TAPIR_CHECK_ARG(!overlap(src, src_bytes, dst, dst_bytes), "%s: dst overlaps src", fn);
+  if (W != w) {
+    TAPIR_CHECK_ARG(x_bounds && x_taps && aligned(x_bounds, 4) && aligned(x_taps, 4),
+                    "%s: width %d -> %d needs the x tables (4-byte aligned)", fn, W, w);
+    TAPIR_CHECK_ARG(x_ksize == lanczos_ksize(W, w), "%s: x_ksize=%d, the %d -> %d tables have %d taps",
+                    fn, x_ksize, W, w, lanczos_ksize(W, w));
+  }
+  if (H != h) {
+    TAPIR_CHECK_ARG(y_bounds && y_taps && aligned(y_bounds, 4) && aligned(y_taps, 4),
+                    "%s: height %d -> %d needs the y tables (4-byte aligned)", fn, H, h);
+    TAPIR_CHECK_ARG(y_ksize == lanczos_ksize(H, h), "%s: y_ksize=%d, the %d -> %d tables have %d taps",
+                    fn, y_ksize, H, h, lanczos_ksize(H, h));
+  }
+  const size_t need = resize_lanczos_u8_workspace_bytes(frames, H, W, h, w);
+  if (need > 0) {
+    TAPIR_CHECK_ARG(workspace && aligned(workspace, 16), "%s: workspace must be non-NULL and 16-byte aligned", fn);
+    TAPIR_CHECK_ARG(workspace_bytes >= need, "%s: workspace %zu bytes < %zu", fn, workspace_bytes, need);
+    TAPIR_CHECK_ARG(!overlap(workspace, need, src, src_bytes) && !overlap(workspace, need, dst, dst_bytes),
+                    "%s: workspace overlaps src or dst", fn);
+  }
+  return resize_lanczos_u8(src, dst, frames, H, W, h, w, x_bounds, x_taps, x_ksize, y_bounds, y_taps,
+                           y_ksize, static_cast<uint8_t*>(workspace), S(stream));
+}
+
 }  // extern "C"

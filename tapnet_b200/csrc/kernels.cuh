@@ -65,6 +65,17 @@ int postprocess_occlusions(const float* occ, const float* expd, long long n, uin
                            cudaStream_t s);
 int tapvid_counts(const tapir_tapvid_args* a, cudaStream_t s);
 
+// ---- Lanczos resize of uint8 RGB clips (resample.cu; PIL's 8-bit LANCZOS) -------------------
+// Host only: the per-axis kernel width, and the (xmin, n) bounds [out][2] and 22-bit fixed-point
+// taps [out][ksize] of one axis.
+int lanczos_ksize(int in_size, int out_size);
+void lanczos_weights(int in_size, int out_size, int* bounds, int* taps);
+size_t resize_lanczos_u8_workspace_bytes(int frames, int H, int W, int h, int w);
+// Arguments checked by tapir_resize_lanczos_u8.
+int resize_lanczos_u8(const uint8_t* src, uint8_t* dst, int frames, int H, int W, int h, int w,
+                      const int* x_bounds, const int* x_taps, int x_ksize, const int* y_bounds,
+                      const int* y_taps, int y_ksize, uint8_t* ws, cudaStream_t s);
+
 // ---- point-track painting (paint.cu; viz_utils.py:47-124) ---------------------------------
 int paint_radius(int H, int W);
 size_t paint_point_track_workspace_bytes(long long frames, long long points);
