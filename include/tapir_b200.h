@@ -337,6 +337,33 @@ int tapir_yuv420_to_rgb(const tapir_yuv420_frames* src, int32_t frames, uint8_t*
 int tapir_ingest_frames_yuv420(const tapir_yuv420_frames* src, int32_t frames, float* dst,
                                int32_t oH, int32_t oW, void* stream);
 
+/* One source frame of tapir_ingest_frames_multi: its own format, size, row pitch and crop window.
+ * TAPIR_INGEST_U8: pixel (r, c) of the frame is src[r * pitch + c * 3 ...] (bytes; pitch >= 3 W)
+ * and the window (y0, x0, h, w) lies inside the H x W frame.  TAPIR_INGEST_YUV420 reads frame 0 of
+ * `yuv` inside its own window (src, pitch, H, W and the window fields are then not read).  fp32
+ * frames are not covered: the blend of tapir_bilinear_resize rounds differently (its taps are
+ * contracted into FMAs in another order), so they keep one tapir_bilinear_resize call each. */
+#define TAPIR_INGEST_U8 1     /* uint8 RGB [0, 255] (tapir_ingest_frames' input) */
+#define TAPIR_INGEST_YUV420 2 /* 8-bit YUV 4:2:0 (tapir_ingest_frames_yuv420's input) */
+typedef struct tapir_ingest_desc {
+  const void* src;
+  int64_t pitch;
+  int32_t format;
+  int32_t H, W;
+  int32_t y0, x0, h, w;
+  int32_t reserved;
+  tapir_yuv420_frames yuv;
+} tapir_ingest_desc;
+
+/* Frames of different sizes and formats -> dst [frames][oH][oW][3] float in [-1,1], frame i from
+ * descs[i] (a host array).  Output frame i equals, bit for bit, what the one-format call gives for
+ * that frame alone: tapir_ingest_frames (uint8) or tapir_ingest_frames_yuv420 on its window.
+ * One launch per TAPIR_INGEST_MAX_FRAMES frames.  Every descriptor is checked before any CUDA call:
+ * a bad one returns 1. */
+#define TAPIR_INGEST_MAX_FRAMES 64
+int tapir_ingest_frames_multi(const tapir_ingest_desc* descs, int32_t frames, float* dst,
+                              int32_t oH, int32_t oW, void* stream);
+
 /* tapir_backbone_forward_ex on the crop window (h x w) of YUV 4:2:0 frames: the conversion and
  * the normalisation run inside the stem conv's loads; same launches as the uint8 reader. */
 int tapir_backbone_forward_yuv420(const tapir_backbone_weights* w, const tapir_yuv420_frames* video,
@@ -473,6 +500,13 @@ int tapir_mixer_dw(const tapir_mixer_block* blk, const float* x, int32_t n, int3
                    const float* ctx1_in, const float* ctx2_in, float* ctx1_out, float* ctx2_out, float* z,
                    void* planes_out, int64_t plane_stride, int32_t planes, void* stream);
 int tapir_refine_update(const tapir_update_args* args, void* stream);
+/* tapir_refine_update over a batch of clips of different video sizes: video_hw is a device int32
+ * table [clips][2] of (video_h, video_w), and row r (= query * num_frames + frame) belongs to
+ * clip r / rows_per_clip; tracks_out of that row is scaled to its clip's size (args->video_h /
+ * video_w are not read).  Each clip's rows equal a tapir_refine_update call with its size, bit for
+ * bit.  video_hw = NULL is tapir_refine_update. */
+int tapir_refine_update_ex(const tapir_update_args* args, const int32_t* video_hw,
+                           int32_t rows_per_clip, void* stream);
 
 #ifdef __cplusplus
 }

@@ -42,3 +42,10 @@ timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
     python -m pytest -q -m gpu -p no:cacheprovider tests/test_tapvid_gpu.py -k "not evaluate and not readers" \
     2>&1 | grep -E '^=========|passed|failed' | tail -n 25
 echo "sanitizer tapvid memcheck rc=${PIPESTATUS[0]}"
+# then the streams of different frame sizes: the multi-frame ingest (uint8, pitched, NV12 / I420
+# windows, more frames than one launch), the per-clip track update and the mixed-size tracker
+timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
+    python -m pytest -q -m gpu -p no:cacheprovider tests/test_tracker_sizes_gpu.py \
+    -k "not golden_and_eager and not isolated" \
+    2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+echo "sanitizer sizes memcheck rc=${PIPESTATUS[0]}"

@@ -120,6 +120,14 @@ class Yuv420Frames(Structure):
               ('matrix', c_int32), ('full_range', c_int32), ('reserved', c_int32)]
 
 
+class IngestDesc(Structure):
+  _fields_ = [('src', c_void_p), ('pitch', c_int64), ('format', c_int32), ('H', c_int32),
+              ('W', c_int32), ('y0', c_int32), ('x0', c_int32), ('h', c_int32), ('w', c_int32),
+              ('reserved', c_int32), ('yuv', Yuv420Frames)]
+
+
+INGEST_U8, INGEST_YUV420 = 1, 2
+INGEST_MAX_FRAMES = 64
 TAPVID_COUNTERS = 18
 
 # name -> (restype, argtypes); this table is also what tests/test_abi.py checks against
@@ -172,6 +180,8 @@ SIGNATURES = {
     'tapir_yuv420_to_rgb': (ctypes.c_int, [POINTER(Yuv420Frames), c_int32, c_void_p, c_void_p]),
     'tapir_ingest_frames_yuv420': (ctypes.c_int, [POINTER(Yuv420Frames), c_int32, c_void_p,
                                                   c_int32, c_int32, c_void_p]),
+    'tapir_ingest_frames_multi': (ctypes.c_int, [POINTER(IngestDesc), c_int32, c_void_p, c_int32,
+                                                 c_int32, c_void_p]),
     'tapir_backbone_forward_yuv420': (ctypes.c_int, [POINTER(BackboneWeights), POINTER(Yuv420Frames),
                                                      c_int32, c_void_p, c_void_p, c_void_p,
                                                      c_size_t, c_void_p, c_void_p]),
@@ -204,6 +214,7 @@ SIGNATURES = {
                                       c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int32,
                                       c_void_p]),
     'tapir_refine_update': (ctypes.c_int, [POINTER(UpdateArgs), c_void_p]),
+    'tapir_refine_update_ex': (ctypes.c_int, [POINTER(UpdateArgs), c_void_p, c_int32, c_void_p]),
     'tapir_paint_point_track_workspace_bytes': (c_size_t, [c_int32, c_int32]),
     'tapir_paint_point_track': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int32,
                                                c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_size_t,
@@ -418,6 +429,40 @@ def resample_frames(video, out):
   check(load().tapir_bilinear_resize(ptr(video), math.prod(out.shape[:-3]), video.shape[-3],
                                      video.shape[-2], 3, ptr(out), out.shape[-3], out.shape[-2],
                                      stream()), fn)
+
+
+def ingest_desc(frame):
+  """The tapir_ingest_desc of one frame: a uint8 [H, W, 3] tensor whose rows may be pitched (dense
+  pixels), or a YUV clip of one frame (read inside its own window).  Returns (desc, what the
+  descriptor points into)."""
+  fn = 'ingest_desc'
+  if _is_yuv(frame):
+    _need(math.prod(frame.shape[:-3]) == 1, fn, f'a YUV clip of one frame, got {tuple(frame.shape)}')
+    yuv = frame.c_struct()
+    return IngestDesc(format=INGEST_YUV420, yuv=yuv), frame._keep
+  if (frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[-1] != 3
+      or frame.stride(2) != 1 or frame.stride(1) != 3):
+    _bad(fn, 'frame', frame, 'uint8 [H, W, 3] with dense pixels')
+  H, W = frame.shape[:2]
+  return IngestDesc(src=frame.data_ptr(), pitch=frame.stride(0), format=INGEST_U8, H=H, W=W, y0=0,
+                    x0=0, h=H, w=W), frame
+
+
+def ingest_frames_multi(frames, out):
+  """Frames of their own sizes and formats (a list of ingest_desc's inputs: uint8 or YUV) -> float32
+  [-1, 1] out [len(frames), oh, ow, 3]: frame i resized as resample_frames resizes it alone."""
+  fn = 'tapir_ingest_frames_multi'
+  _check(fn, 'out', out, torch.float32)
+  _need(out.dim() == 4 and out.shape[0] == len(frames) and out.shape[-1] == 3, fn,
+        f'out {tuple(out.shape)} for {len(frames)} frames')
+  descs = (IngestDesc * len(frames))()
+  keep = []
+  for i, f in enumerate(frames):
+    _need(f.device == out.device, fn, f'frame {i} on {f.device}, out on {out.device}')
+    descs[i], k = ingest_desc(f)
+    keep.append(k)
+  check(load().tapir_ingest_frames_multi(descs, len(frames), ptr(out), out.shape[1], out.shape[2],
+                                         stream()), fn)
 
 
 def yuv420_to_rgb(frames, out):
@@ -638,10 +683,19 @@ def update_args(res, pos, occ_in, expd_in, feat_hi, feat_lo, occ_out, expd_out, 
   return ua
 
 
-def refine_update(*args):
-  """The track update of update_args(*args)."""
+def refine_update(*args, video_table=None):
+  """The track update of update_args(*args).  video_table: None, or int32 [G, 2] per-clip (h, w)
+  of the G clips the rows run over (the tracks of each clip scaled to its own size; video_hw is
+  then not used)."""
   ua = update_args(*args)
-  check(load().tapir_refine_update(byref(ua), stream()), 'tapir_refine_update')
+  if video_table is None:
+    return check(load().tapir_refine_update(byref(ua), stream()), 'tapir_refine_update')
+  fn = 'tapir_refine_update_ex'
+  G = video_table.shape[0]
+  _check(fn, 'video_table', video_table, torch.int32, (G, 2), device=args[0].device)
+  rows = ua.num_points * ua.num_frames
+  _need(G >= 1 and rows % G == 0, fn, f'{rows} rows over {G} clips')
+  check(load().tapir_refine_update_ex(byref(ua), ptr(video_table), rows // G, stream()), fn)
 
 
 # ------------------------------------------------------------------------------ outputs

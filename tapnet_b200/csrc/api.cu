@@ -251,6 +251,12 @@ int tapir_ingest_frames_yuv420(const tapir_yuv420_frames* src, int32_t frames, f
   return ingest_frames_yuv420(r, frames, src->h, src->w, dst, oH, oW, S(stream));
 }
 
+int tapir_ingest_frames_multi(const tapir_ingest_desc* descs, int32_t frames, float* dst,
+                              int32_t oH, int32_t oW, void* stream) {
+  Range nvtx_range("tapir_ingest_frames_multi");
+  return ingest_frames_multi(descs, frames, dst, oH, oW, S(stream));
+}
+
 int tapir_backbone_forward_yuv420(const tapir_backbone_weights* w, const tapir_yuv420_frames* video,
                                   int32_t frames, float* lowres, float* hires, void* workspace,
                                   size_t workspace_bytes, void* hires_ready_event, void* stream) {
@@ -412,21 +418,42 @@ int tapir_mixer_dw(const tapir_mixer_block* blk, const float* x, int32_t n, int3
                   static_cast<__nv_bfloat16*>(planes_out), plane_stride, planes, S(stream));
 }
 
-int tapir_refine_update(const tapir_update_args* args, void* stream) {
-  Range nvtx_range("tapir_refine_update");
-  const tapir_update_args* a = args;
+namespace {
+int check_update_args(const tapir_update_args* a, bool per_clip_video, const char* who) {
   TAPIR_CHECK_ARG(a != nullptr && a->res && a->pos && a->feat_out && a->occ_out && a->expd_out && a->feat_hi &&
                       a->feat_lo && a->occ_in && a->expd_in,
-                  "tapir_refine_update: null pointer");
+                  "%s: null pointer", who);
   const long long rows = (long long)a->num_points * a->num_frames;
   TAPIR_CHECK_ARG(a->num_points >= 1 && a->num_frames >= 1 && rows < (1ll << 31),
-                  "tapir_refine_update: num_points=%d num_frames=%d (rows must be in 1..2^31-1)", a->num_points,
+                  "%s: num_points=%d num_frames=%d (rows must be in 1..2^31-1)", who, a->num_points,
                   a->num_frames);
-  TAPIR_CHECK_ARG(a->ld_res >= 388, "tapir_refine_update: ld_res=%d < 388", a->ld_res);
+  TAPIR_CHECK_ARG(a->ld_res >= 388, "%s: ld_res=%d < 388", who, a->ld_res);
   TAPIR_CHECK_ARG(a->init_h >= 1 && a->init_w >= 1 && a->resize_h >= 1 && a->resize_w >= 1 &&
-                      (a->tracks_out == nullptr || (a->video_h >= 1 && a->video_w >= 1)),
-                  "tapir_refine_update: sizes must be positive");
+                      (a->tracks_out == nullptr || per_clip_video || (a->video_h >= 1 && a->video_w >= 1)),
+                  "%s: sizes must be positive", who);
+  return kOk;
+}
+}  // namespace
+
+int tapir_refine_update(const tapir_update_args* args, void* stream) {
+  Range nvtx_range("tapir_refine_update");
+  TAPIR_RETURN_IF(check_update_args(args, false, "tapir_refine_update"));
   return refine_update(args, S(stream));
+}
+
+int tapir_refine_update_ex(const tapir_update_args* args, const int32_t* video_hw,
+                           int32_t rows_per_clip, void* stream) {
+  Range nvtx_range("tapir_refine_update_ex");
+  if (video_hw == nullptr) return tapir_refine_update(args, stream);
+  TAPIR_RETURN_IF(check_update_args(args, true, "tapir_refine_update_ex"));
+  const long long rows = (long long)args->num_points * args->num_frames;
+  TAPIR_CHECK_ARG(args->tracks_out != nullptr, "tapir_refine_update_ex: a video size table needs tracks_out");
+  TAPIR_CHECK_ARG(rows_per_clip >= 1 && rows % rows_per_clip == 0 && rows_per_clip % args->num_frames == 0,
+                  "tapir_refine_update_ex: rows_per_clip=%d does not divide the %lld rows into clips of "
+                  "whole queries (%d frames each)", rows_per_clip, rows, args->num_frames);
+  TAPIR_CHECK_ARG((reinterpret_cast<uintptr_t>(video_hw) & 3) == 0,
+                  "tapir_refine_update_ex: video_hw not 4-byte aligned");
+  return refine_update(args, S(stream), video_hw, rows_per_clip);
 }
 
 size_t tapir_paint_point_track_workspace_bytes(int32_t frames, int32_t points) {

@@ -58,21 +58,70 @@ struct RgbWindow {
   }
 };
 
+// One ch x cw window of uint8 RGB pixels for every frame of the launch (RgbWindow or
+// Yuv420Reader), as ingest_frames_kernel reads it: each tap normalised through the table.
+template <typename Reader>
+struct U8Frames {
+  Reader r;
+  int ch, cw;
+  __device__ __forceinline__ void window(long long, int& h, int& w) const { h = ch; w = cw; }
+  __device__ __forceinline__ bool copies(long long, int oH, int oW) const { return ch == oH && cw == oW; }
+  __device__ __forceinline__ void tap(const float* lut, long long f, int y, int x, float (&v)[3]) const {
+    uint8_t p[3];
+    r.pixel(f, y, x, p);
+    v[0] = lut[p[0]];
+    v[1] = lut[p[1]];
+    v[2] = lut[p[2]];
+  }
+};
+
+// Device form of one tapir_ingest_desc (checked by the entry point).
+struct IngestFrame {
+  Yuv420Reader yuv;  // TAPIR_INGEST_YUV420: frame 0 of it
+  const uint8_t* src;  // TAPIR_INGEST_U8: pixel (y0, x0) of the window
+  long long pitch;     // TAPIR_INGEST_U8: row pitch in bytes
+  int format, h, w;  // window size
+};
+
+// Up to TAPIR_INGEST_MAX_FRAMES frames of their own format and window, one descriptor each.
+struct DescFrames {
+  IngestFrame fr[TAPIR_INGEST_MAX_FRAMES];
+  __device__ __forceinline__ void window(long long f, int& h, int& w) const { h = fr[f].h; w = fr[f].w; }
+  __device__ __forceinline__ bool copies(long long f, int oH, int oW) const {
+    return fr[f].h == oH && fr[f].w == oW;
+  }
+  __device__ __forceinline__ void tap(const float* lut, long long f, int y, int x, float (&v)[3]) const {
+    const IngestFrame& d = fr[f];
+    uint8_t p[3];
+    if (d.format == TAPIR_INGEST_U8) {
+      const uint8_t* q = d.src + (long long)y * d.pitch + (long long)x * 3;
+      p[0] = q[0];
+      p[1] = q[1];
+      p[2] = q[2];
+    } else {
+      d.yuv.pixel(0, y, x, p);
+    }
+    v[0] = lut[p[0]];
+    v[1] = lut[p[1]];
+    v[2] = lut[p[2]];
+  }
+};
+
 // crop + normalise + resize.  A CTA walks over runs of 256 consecutive output pixels: one thread
 // computes one pixel (3 channels) into shared memory, then the run's 768 floats leave as float4
 // rows (the direct 12-byte-strided stores would touch every sector three times).  The resize is
 // F.interpolate(mode='bilinear', align_corners=False) of the normalised crop, i.e. the same
-// arithmetic as bilinear_resize_kernel (backbone.cu) applied after normalise_u8.  Src gives the
-// uint8 RGB pixels of the ch x cw window (RgbWindow, or Yuv420Reader converting each tap).
+// arithmetic as bilinear_resize_kernel (backbone.cu) applied after normalise_u8.  Src gives each
+// frame's window size and its normalised pixels (U8Frames of RgbWindow or Yuv420Reader converting
+// each tap, or DescFrames with one window and format per frame).  The source is a grid constant:
+// DescFrames' table is indexed by frame without a local copy.
 template <typename Src>
-__global__ void __launch_bounds__(256) ingest_frames_kernel(const Src src, int ch, int cw,
+__global__ void __launch_bounds__(256) ingest_frames_kernel(const __grid_constant__ Src src,
                                                             float* __restrict__ dst, int oH, int oW,
                                                             long long total, bool dst_aligned16) {
   __shared__ float lut[256];
   __shared__ __align__(16) float stage[256 * 3];
   fill_lut(lut);
-  const float sy = (float)ch / (float)oH, sx = (float)cw / (float)oW;
-  const bool same = (ch == oH && cw == oW);
   for (long long i0 = blockIdx.x * 256LL; i0 < total; i0 += (long long)gridDim.x * 256) {
     const long long i = i0 + threadIdx.x;
     if (i < total) {
@@ -90,14 +139,17 @@ __global__ void __launch_bounds__(256) ingest_frames_kernel(const Src src, int c
         oy = (int)(r % oH);
         f = r / oH;
       }
+      int ch, cw;
+      src.window(f, ch, cw);
       float* o = stage + threadIdx.x * 3;
-      if (same) {
-        uint8_t p[3];
-        src.pixel(f, oy, ox, p);
-        o[0] = lut[p[0]];
-        o[1] = lut[p[1]];
-        o[2] = lut[p[2]];
+      if (src.copies(f, oH, oW)) {
+        float v[3];
+        src.tap(lut, f, oy, ox, v);
+        o[0] = v[0];
+        o[1] = v[1];
+        o[2] = v[2];
       } else {
+        const float sy = (float)ch / (float)oH, sx = (float)cw / (float)oW;
         float fy = sy * (oy + 0.5f) - 0.5f;
         float fx = sx * (ox + 0.5f) - 0.5f;
         if (fy < 0.f) fy = 0.f;
@@ -106,17 +158,14 @@ __global__ void __launch_bounds__(256) ingest_frames_kernel(const Src src, int c
         const int y1 = y0 + ((y0 < ch - 1) ? 1 : 0), x1 = x0 + ((x0 < cw - 1) ? 1 : 0);
         const float ly = fy - y0, lx = fx - x0;
         const float hy = 1.f - ly, hx = 1.f - lx;
-        uint8_t p00[3], p01[3], p10[3], p11[3];
-        src.pixel(f, y0, x0, p00);
-        src.pixel(f, y0, x1, p01);
-        src.pixel(f, y1, x0, p10);
-        src.pixel(f, y1, x1, p11);
+        float v00[3], v01[3], v10[3], v11[3];
+        src.tap(lut, f, y0, x0, v00);
+        src.tap(lut, f, y0, x1, v01);
+        src.tap(lut, f, y1, x0, v10);
+        src.tap(lut, f, y1, x1, v11);
 #pragma unroll
-        for (int c = 0; c < 3; ++c) {
-          const float v00 = lut[p00[c]], v01 = lut[p01[c]];
-          const float v10 = lut[p10[c]], v11 = lut[p11[c]];
-          o[c] = hy * (hx * v00 + lx * v01) + ly * (hx * v10 + lx * v11);
-        }
+        for (int c = 0; c < 3; ++c)
+          o[c] = hy * (hx * v00[c] + lx * v01[c]) + ly * (hx * v10[c] + lx * v11[c]);
       }
     }
     __syncthreads();
@@ -235,7 +284,7 @@ int ingest_frames(const uint8_t* src, int frames, int H, int W, int crop_y, int 
     preprocess_u8_kernel<<<grid_for(n / 4 / 4 + 1), 256, 0, s>>>(src, dst, n);
   } else {
     ingest_frames_kernel<<<grid_for(total), 256, 0, s>>>(
-        RgbWindow{src, H, W, crop_y, crop_x}, crop_h, crop_w, dst, oH, oW, total,
+        U8Frames<RgbWindow>{RgbWindow{src, H, W, crop_y, crop_x}, crop_h, crop_w}, dst, oH, oW, total,
         (reinterpret_cast<uintptr_t>(dst) & 15) == 0);
   }
   count_launch();
@@ -249,10 +298,68 @@ int ingest_frames_yuv420(const Yuv420Reader& src, int frames, int h, int w, floa
                   "ingest_frames_yuv420: bad arguments");
   const long long total = (long long)frames * oH * oW;
   ProfileScope ps("ingest_frames_yuv420", s, 0.0, (double)frames * h * w * 1.5 + (double)total * 12);
-  ingest_frames_kernel<<<grid_for(total), 256, 0, s>>>(src, h, w, dst, oH, oW, total,
-                                                       (reinterpret_cast<uintptr_t>(dst) & 15) == 0);
+  ingest_frames_kernel<<<grid_for(total), 256, 0, s>>>(U8Frames<Yuv420Reader>{src, h, w}, dst, oH, oW,
+                                                       total, (reinterpret_cast<uintptr_t>(dst) & 15) == 0);
   count_launch();
   TAPIR_LAUNCH_CHECK("ingest_frames_kernel");
+  return kOk;
+}
+
+int ingest_frames_multi(const tapir_ingest_desc* descs, int frames, float* dst, int oH, int oW,
+                        cudaStream_t s) {
+  TAPIR_CHECK_ARG(descs && dst && frames > 0 && oH > 0 && oW > 0,
+                  "ingest_frames_multi: bad arguments (descs %p, frames %d, dst %p, out %dx%d)",
+                  (const void*)descs, frames, (void*)dst, oH, oW);
+  TAPIR_CHECK_ARG((long long)frames * oH * oW * 3 < (1ll << 40), "ingest_frames_multi: output too large");
+  // every descriptor first: nothing is launched unless all of them are good
+  double in_bytes = 0;
+  for (int i = 0; i < frames; ++i) {
+    const tapir_ingest_desc& d = descs[i];
+    if (d.format == TAPIR_INGEST_YUV420) {
+      Yuv420Reader r;
+      TAPIR_RETURN_IF(make_yuv420_reader(&d.yuv, 1, "ingest_frames_multi", &r));
+      in_bytes += (double)d.yuv.h * d.yuv.w * 1.5;
+      continue;
+    }
+    TAPIR_CHECK_ARG(d.format == TAPIR_INGEST_U8,
+                    "ingest_frames_multi: frame %d: format %d is not 1 (uint8) or 2 (YUV 4:2:0)", i,
+                    d.format);
+    TAPIR_CHECK_ARG(d.src != nullptr && d.H > 0 && d.W > 0 && d.pitch >= 3ll * d.W,
+                    "ingest_frames_multi: frame %d: src %p, %dx%d frame, row pitch %lld", i, d.src, d.H,
+                    d.W, (long long)d.pitch);
+    TAPIR_CHECK_ARG(d.y0 >= 0 && d.x0 >= 0 && d.h > 0 && d.w > 0 && (long long)d.y0 + d.h <= d.H &&
+                        (long long)d.x0 + d.w <= d.W,
+                    "ingest_frames_multi: frame %d: crop (%d,%d,%d,%d) outside the %dx%d frame", i, d.y0,
+                    d.x0, d.h, d.w, d.H, d.W);
+    in_bytes += (double)d.h * d.w * 3;
+  }
+  for (int f0 = 0; f0 < frames; f0 += TAPIR_INGEST_MAX_FRAMES) {
+    const int n = frames - f0 < TAPIR_INGEST_MAX_FRAMES ? frames - f0 : TAPIR_INGEST_MAX_FRAMES;
+    DescFrames src;
+    for (int i = 0; i < n; ++i) {
+      const tapir_ingest_desc& d = descs[f0 + i];
+      IngestFrame& fr = src.fr[i];
+      fr = IngestFrame{};
+      fr.format = d.format;
+      if (d.format == TAPIR_INGEST_YUV420) {
+        make_yuv420_reader(&d.yuv, 1, "ingest_frames_multi", &fr.yuv);
+        fr.h = d.yuv.h;
+        fr.w = d.yuv.w;
+      } else {
+        fr.src = static_cast<const uint8_t*>(d.src) + (long long)d.y0 * d.pitch + (long long)d.x0 * 3;
+        fr.pitch = d.pitch;
+        fr.h = d.h;
+        fr.w = d.w;
+      }
+    }
+    float* out = dst + (long long)f0 * oH * oW * 3;
+    const long long total = (long long)n * oH * oW;
+    ProfileScope ps("ingest_frames_multi", s, 0.0, in_bytes * n / frames + (double)total * 12);
+    ingest_frames_kernel<<<grid_for(total), 256, 0, s>>>(src, out, oH, oW, total,
+                                                         (reinterpret_cast<uintptr_t>(out) & 15) == 0);
+    count_launch();
+    TAPIR_LAUNCH_CHECK("ingest_frames_kernel");
+  }
   return kOk;
 }
 

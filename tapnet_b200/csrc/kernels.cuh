@@ -61,6 +61,8 @@ int ingest_frames(const uint8_t* src, int frames, int H, int W, int crop_y, int 
 int ingest_frames_yuv420(const Yuv420Reader& src, int frames, int h, int w, float* dst, int oH,
                          int oW, cudaStream_t s);
 int yuv420_to_rgb(const Yuv420Reader& src, int frames, int h, int w, uint8_t* dst, cudaStream_t s);
+int ingest_frames_multi(const tapir_ingest_desc* descs, int frames, float* dst, int oH, int oW,
+                        cudaStream_t s);
 int postprocess_occlusions(const float* occ, const float* expd, long long n, uint8_t* visible,
                            cudaStream_t s);
 int tapvid_counts(const tapir_tapvid_args* a, cudaStream_t s);
@@ -106,6 +108,8 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
 int mixer_dw(const tapir_mixer_block& blk, const float* x, int n, int T, bool causal, const float* ctx1_in,
              const float* ctx2_in, float* ctx1_out, float* ctx2_out, float* z, __nv_bfloat16* planes_out,
              long long plane_stride, int planes, cudaStream_t s);
-int refine_update(const tapir_update_args* a, cudaStream_t s);
+// video_hw: NULL, or a device table [clips][2] of per-clip video sizes (rows_per_clip rows each)
+int refine_update(const tapir_update_args* a, cudaStream_t s, const int32_t* video_hw = nullptr,
+                  long long rows_per_clip = 0);
 
 }  // namespace tapir

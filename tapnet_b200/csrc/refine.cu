@@ -507,7 +507,10 @@ __global__ void __launch_bounds__(512, SMALL ? 1 : 2) mixer_dw_kernel(const DwPa
 }
 
 // ------------------------------------------------------------------------ a7 epilogue
-__global__ void __launch_bounds__(128) refine_update_kernel(const tapir_update_args a) {
+// video_hw (nullable): per-clip video sizes [clips][2], clip = row / rows_per_clip
+__global__ void __launch_bounds__(128) refine_update_kernel(const tapir_update_args a,
+                                                            const int32_t* __restrict__ video_hw,
+                                                            long long rows_per_clip) {
   const long long row = blockIdx.x;
   const int T = a.num_frames;
   const int n = (int)(row / T), t = (int)(row - (long long)n * T);
@@ -528,9 +531,15 @@ __global__ void __launch_bounds__(128) refine_update_kernel(const tapir_update_a
     a.occ_out[row] = res[2] + a.occ_in[row];
     a.expd_out[row] = res[3] + a.expd_in[row];
     if (a.tracks_out != nullptr) {
+      int vh = a.video_h, vw = a.video_w;
+      if (video_hw != nullptr) {
+        const long long clip = row / rows_per_clip;
+        vh = video_hw[clip * 2 + 0];
+        vw = video_hw[clip * 2 + 1];
+      }
       // train2orig (tapir_model.py:435-441)
-      a.tracks_out[row * 2 + 0] = __fdiv_rn(__fmul_rn(x, (float)a.video_w), (float)a.init_w);
-      a.tracks_out[row * 2 + 1] = __fdiv_rn(__fmul_rn(y, (float)a.video_h), (float)a.init_h);
+      a.tracks_out[row * 2 + 0] = __fdiv_rn(__fmul_rn(x, (float)vw), (float)a.init_w);
+      a.tracks_out[row * 2 + 1] = __fdiv_rn(__fmul_rn(y, (float)vh), (float)a.init_h);
     }
   }
 }
@@ -588,12 +597,13 @@ int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s) {
   return kOk;
 }
 
-int refine_update(const tapir_update_args* a, cudaStream_t s) {
+int refine_update(const tapir_update_args* a, cudaStream_t s, const int32_t* video_hw,
+                  long long rows_per_clip) {
   TAPIR_CHECK_ARG(a != nullptr && a->res && a->pos && a->feat_out && a->occ_out && a->expd_out,
                   "refine_update: null pointer");
   const long long rows = (long long)a->num_points * a->num_frames;
   ProfileScope ps("refine_update", s, 0.0, (double)rows * (388 * 4 + 384 * 8));
-  refine_update_kernel<<<(unsigned)rows, 128, 0, s>>>(*a);
+  refine_update_kernel<<<(unsigned)rows, 128, 0, s>>>(*a, video_hw, rows_per_clip);
   count_launch();
   TAPIR_LAUNCH_CHECK("refine_update_kernel");
   return kOk;

@@ -16,8 +16,15 @@ the S clips of one frame each (the reference's batch axis), all in one captured 
 With `yuv420=True` the tracker takes `live.YUV420Frames` (NV12 / I420 camera or decoder frames):
 it keeps static Y / U / V buffers of the camera frame, a step copies the 1.5 B/px planes into them
 and replays the graph, and the crop window and colour matrix are fixed at construction.
+
+Streams of different frame sizes (`height` / `width` / `window` given per stream) are each tracked
+as the reference tracks one camera of that size: the default refinement resolutions of its own
+size, tracks in its own pixels.  Streams whose backbone passes agree (`tapir_model._pass_plan`) form
+a group; one captured graph runs, per group, its passes over the group's frames (one ingest launch
+per resampled pass, whatever the frames' sizes) and one batched estimate_trajectories with per-clip
+video sizes.
 """
-from typing import Optional, Tuple
+from typing import List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import torch
 
@@ -25,26 +32,110 @@ from tapnet_b200 import live
 from tapnet_b200 import tapir_model
 
 
+class StreamSpec(NamedTuple):
+  """One camera stream: its frame size, the crop window it is tracked in (YUV trackers; None for
+  the whole frame) and the size of that window, in whose pixels its tracks are."""
+  frame_hw: Tuple[int, int]
+  window: Optional[Tuple[int, int, int, int]]
+  hw: Tuple[int, int]
+
+
+def _is_window_list(window):
+  return window is not None and len(window) > 0 and not isinstance(window[0], int)
+
+
+def stream_specs(height, width, num_streams: int, yuv420: bool = False,
+                 window=None) -> List[StreamSpec]:
+  """The StreamSpec of every stream from the constructor's size arguments: `height` and `width`
+  are ints or sequences of num_streams ints, `window` (yuv420 only) one (y0, x0, h, w) or a
+  sequence of num_streams of them (None entries: the whole frame)."""
+  S = int(num_streams)
+
+  def per_stream(v, name):
+    if isinstance(v, int):
+      return [int(v)] * S
+    v = [int(x) for x in v]
+    if len(v) != S:
+      raise ValueError(f'{name} has {len(v)} entries for {S} streams')
+    return v
+
+  if not yuv420 and window is not None:
+    raise ValueError('window is only supported with yuv420=True')
+  hs, ws = per_stream(height, 'height'), per_stream(width, 'width')
+  if _is_window_list(window):
+    windows = list(window)
+    if len(windows) != S:
+      raise ValueError(f'window has {len(windows)} entries for {S} streams')
+  else:
+    windows = [window] * S
+  specs = []
+  for s, (H, W, win) in enumerate(zip(hs, ws, windows)):
+    if H <= 0 or W <= 0:
+      raise ValueError(f'stream {s}: frame size {H}x{W}')
+    if win is not None:
+      win = tuple(int(a) for a in win)
+      y0, x0, h, w = win
+      if h <= 0 or w <= 0 or y0 < 0 or x0 < 0 or y0 + h > H or x0 + w > W:
+        raise ValueError(f'stream {s}: window {win} outside the {H}x{W} frame')
+    specs.append(StreamSpec((H, W), win, (win[2], win[3]) if win is not None else (H, W)))
+  return specs
+
+
+def group_streams(specs: Sequence[StreamSpec], initial_resolution=(256, 256)):
+  """Streams that run through one backbone pass sequence and one batched estimate_trajectories:
+  a list of (plan, [stream indices]) in order of first appearance.  Streams group by their pass
+  plan; a plan with a direct-read pass holds the tracked size, so such a stream only shares a
+  group with streams of its size (and, when cropping, of its frame size and window)."""
+  from tapnet_b200 import tapir_model as tm  # pylint: disable=g-import-not-at-top
+  groups = {}
+  for s, spec in enumerate(specs):
+    plan = tuple(tm._pass_plan(spec.hw, initial_resolution))
+    key = (plan, (spec.frame_hw, spec.window) if any(p.direct for p in plan) else None)
+    groups.setdefault(key, (list(plan), []))[1].append(s)
+  return list(groups.values())
+
+
+class _Group:
+  """Streams sharing a pass plan: their static inputs, query features and causal state."""
+
+  def __init__(self, plan, streams, specs):
+    self.plan, self.streams = plan, list(streams)
+    self.uniform = len({(specs[s].frame_hw, specs[s].window) for s in streams}) == 1
+    sizes = [specs[s].hw for s in streams]
+    # one size: the call (and launch sequence) of a same-size tracker; else per-clip sizes
+    self.video_size = sizes[0] if len(set(sizes)) == 1 else sizes
+    self.frames = None   # uniform groups: the [G, 1, ...] input of get_feature_grids
+    self.sources = None  # otherwise: one one-frame input per stream, resampled together
+    self.query_features = None
+    self.state = None
+
+
 class OnlineTracker:
   """Graph-replayed per-frame step of a causal TAPIR model (`use_casual_conv=True`) over
-  `num_streams` camera streams that share one frame size and one point count (pad a stream with
-  dummy points if it tracks fewer)."""
+  `num_streams` camera streams with one point count (pad a stream with dummy points if it tracks
+  fewer) and one frame format, of one frame size or of one size each."""
 
-  def __init__(self, model: 'tapir_model.TAPIR', height: int, width: int, num_points: int,
-               uint8_frames: bool = False, num_streams: int = 1, yuv420: bool = False,
-               window: Optional[Tuple[int, int, int, int]] = None, matrix: str = 'bt601',
+  def __init__(self, model: 'tapir_model.TAPIR', height: Union[int, Sequence[int]],
+               width: Union[int, Sequence[int]], num_points: int, uint8_frames: bool = False,
+               num_streams: int = 1, yuv420: bool = False, window=None, matrix: str = 'bt601',
                full_range: bool = False):
     """height x width: the frame size.  With yuv420=True that is the camera frame and `window`
     (y0, x0, h, w; e.g. `live.center_square_window(height, width)`) the crop that is tracked, in
-    whose pixels the tracks are; `matrix` / `full_range` describe the YUV frames."""
+    whose pixels the tracks are; `matrix` / `full_range` describe the YUV frames.  `height`,
+    `width` and `window` may also give one value per stream: init / step then take a list of
+    the streams' frames."""
     if not model.use_casual_conv:
       raise ValueError('OnlineTracker needs a causal model: TAPIR(use_casual_conv=True)')
     if int(num_streams) < 1:
       raise ValueError(f'num_streams must be >= 1, got {num_streams}')
     if yuv420 and uint8_frames:
       raise ValueError('uint8_frames and yuv420 are exclusive')
-    if not yuv420 and window is not None:
-      raise ValueError('window is only supported with yuv420=True')
+    specs = stream_specs(height, width, num_streams, yuv420, window)
+    self._groups = None
+    if len({(sp.frame_hw, sp.window) for sp in specs}) > 1:
+      self._init_mixed(model, specs, int(num_points), uint8_frames, yuv420, matrix, full_range)
+      return
+    (height, width), window = specs[0].frame_hw, specs[0].window
     self.model = model
     self.hw = (int(height), int(width))
     self.num_points = int(num_points)
@@ -75,10 +166,163 @@ class OnlineTracker:
     self.state = None
     self._out = None
 
+  def _init_mixed(self, model, specs, num_points, uint8_frames, yuv420, matrix, full_range):
+    """Streams of different sizes: static per-stream inputs, grouped by pass plan."""
+    self.model = model
+    self.specs = specs
+    self.hw = [sp.hw for sp in specs]
+    self.num_points = num_points
+    self.num_streams = len(specs)
+    self.dev = next(model.parameters()).device
+    if self.dev.type != 'cuda':
+      raise RuntimeError('OnlineTracker runs on CUDA only')
+    self._frame_dtype = torch.uint8 if uint8_frames else torch.float32
+    self._yuv = (matrix, bool(full_range)) if yuv420 else None
+    self._frame = None
+    self._groups = [_Group(plan, streams, specs)
+                    for plan, streams in group_streams(specs, model.initial_resolution)]
+    self._slot = {}  # stream -> (group, slot)
+    order = []
+    for gi, g in enumerate(self._groups):
+      G = len(g.streams)
+      H, W = specs[g.streams[0]].frame_hw
+      if g.uniform:  # one [G, 1, ...] buffer; each stream's input is its slot of it
+        g.frames = self._new_input(G, H, W, specs[g.streams[0]].window)
+        g.sources = [self._input_slot(g.frames, i) for i in range(G)]
+      else:
+        g.sources = [self._new_input(1, *specs[s].frame_hw, specs[s].window) for s in g.streams]
+      for i, s in enumerate(g.streams):
+        self._slot[s] = (gi, i)
+        order.append(s)
+    # row r of the groups' concatenated outputs is stream order[r]: gather them back in the graph
+    self._order = torch.tensor([order.index(s) for s in range(self.num_streams)], device=self.dev)
+    self._graph = None
+    self._graph_sig = None
+    self._pinned = False
+    self.query_features = None
+    self.state = None
+    self._out = None
+
+  def _new_input(self, n, H, W, window):
+    if self._yuv is None:
+      return torch.zeros(n, 1, H, W, 3, dtype=self._frame_dtype, device=self.dev)
+    ch, cw = (H + 1) // 2, (W + 1) // 2
+    planes = [torch.zeros(n, 1, *hw, dtype=torch.uint8, device=self.dev)
+              for hw in ((H, W), (ch, cw), (ch, cw))]
+    return live.YUV420Frames(*planes, matrix=self._yuv[0], full_range=self._yuv[1], window=window)
+
+  @staticmethod
+  def _input_slot(frames, i):
+    if isinstance(frames, live.YUV420Frames):
+      return live.YUV420Frames(frames.y[i:i + 1], frames.u[i:i + 1], frames.v[i:i + 1],
+                               frames.matrix, frames.full_range, frames.window)
+    return frames[i:i + 1]
+
+  def _stream_frames(self, frames, streams):
+    """Checks one frame per stream in `streams` (all before any copy): [H, W, 3] tensors (or
+    [1, H, W, 3], [1, 1, H, W, 3]) of the stream's size, or one-frame YUV420Frames of its frame
+    size and window.  Returns them as [1, 1, H, W, 3] tensors / YUV clips."""
+    if isinstance(frames, (torch.Tensor, live.YUV420Frames)) or len(frames) != len(streams):
+      got = len(frames) if isinstance(frames, (list, tuple)) else type(frames).__name__
+      raise ValueError(f'expected a list of {len(streams)} frames (one per stream), got {got}')
+    out = []
+    if self._yuv is not None:
+      for s, f in zip(streams, frames):
+        sp = self.specs[s]
+        if not isinstance(f, live.YUV420Frames):
+          raise ValueError(f'stream {s}: this tracker was built with yuv420=True: pass '
+                           'live.YUV420Frames (one frame format per tracker)')
+        if f.frame_size != sp.frame_hw or f.window != (sp.window or (0, 0) + sp.frame_hw):
+          raise ValueError(f'stream {s}: frame {f.frame_size} window {f.window}, expected '
+                           f'{sp.frame_hw} window {sp.window}')
+        if (f.matrix, f.full_range) != self._yuv:
+          raise ValueError(f'stream {s}: {f.matrix}, full_range={f.full_range}; the tracker was '
+                           f'built for {self._yuv[0]}, full_range={self._yuv[1]}')
+        if tuple(f.y.shape[:2]) != (1, 1) or f.device != self.dev:
+          raise ValueError(f'stream {s}: expected one frame on {self.dev}, got '
+                           f'{list(f.y.shape[:2])} on {f.device}')
+        out.append(f)
+      return out
+    dtypes = set()
+    for s, f in zip(streams, frames):
+      if not isinstance(f, torch.Tensor):
+        raise ValueError(f'stream {s}: expected a tensor frame, got {type(f).__name__} (one frame '
+                         'format per tracker)')
+      dtypes.add(f.dtype)
+      while f.dim() > 3 and f.shape[0] == 1:
+        f = f[0]
+      if f.dim() != 3 or tuple(f.shape) != (*self.specs[s].frame_hw, 3):
+        raise ValueError(f'stream {s}: frame {tuple(f.shape)}, expected '
+                         f'{(*self.specs[s].frame_hw, 3)}')
+      out.append(f[None, None])
+    if len(dtypes) > 1:
+      raise ValueError(f'frames of mixed formats {sorted(map(str, dtypes))}: one per tracker')
+    return out
+
+  def _copy_in(self, src, dst):
+    if isinstance(dst, live.YUV420Frames):
+      for d, p in zip((dst.y, dst.u, dst.v), (src.y, src.u, src.v)):
+        d.copy_(p)
+    else:
+      dst.copy_(src)
+
+  def _init_groups(self, frames, query_points):
+    qp = query_points.to(self.dev, torch.float32)
+    if qp.dim() != 3 or qp.shape[0] != self.num_streams or qp.shape[2] != 3:
+      raise ValueError(f'query_points must be [{self.num_streams}, N, 3], got {tuple(qp.shape)}')
+    if qp.shape[1] != self.num_points:
+      raise ValueError(f'expected {self.num_points} query points, got {qp.shape[1]}')
+    frames = [self._device_frame(f) for f in frames]
+    # each stream's query features as a one-stream tracker of its size computes them
+    per_stream = [self._query_features_one(frames[s], qp[s:s + 1]) for s in range(self.num_streams)]
+    for g in self._groups:
+      qfs = [per_stream[s] for s in g.streams]
+      g.query_features = tapir_model.QueryFeatures(
+          tuple(torch.cat([q.lowres[i] for q in qfs]) for i in range(len(qfs[0].lowres))),
+          tuple(torch.cat([q.hires[i] for q in qfs]) for i in range(len(qfs[0].hires))),
+          qfs[0].resolutions)
+      init = self.model.construct_initial_causal_state(self.num_points, len(g.plan) - 1)
+      g.state = [{k: v.to(self.dev).expand(len(g.streams), *v.shape[1:]).clone()
+                  for k, v in d.items()} for d in init]
+    self.query_features = [g.query_features for g in self._groups]
+    self.state = [g.state for g in self._groups]
+    self._graph = None
+    return self.query_features
+
+  def _device_frame(self, f):
+    return f if isinstance(f, live.YUV420Frames) else f.to(self.dev, self._frame_dtype)
+
+  def _query_features_one(self, frame, qp):
+    grids = self.model.get_feature_grids(frame, False)
+    return self.model.get_query_features(frame, False, qp, grids)
+
+  def _state_dicts(self):
+    if self._groups is None:
+      return self.state
+    return [d for g in self._groups for d in g.state]
+
+  def _group_grids(self, g):
+    if g.uniform:
+      return self.model.get_feature_grids(g.frames, False)
+    return self.model._feature_grids_of_frames(
+        [x if isinstance(x, live.YUV420Frames) else x[0, 0] for x in g.sources], g.plan)
+
+  def _step_group(self, g, state):
+    """One group's step on its static inputs: its passes and one batched estimate_trajectories
+    (B = group size, T = 1) that updates `state` in place; returns (tracks, occ, expd)."""
+    grids = self._group_grids(g)
+    r = self.model.estimate_trajectories(g.video_size, False, grids, g.query_features, None, 64,
+                                         causal_context=state, get_causal_context=True,
+                                         causal_context_out=state)
+    return r['tracks'][-1], r['occlusion'][-1], r['expected_dist'][-1]
+
   # -- pytorch_live_demo.py:44-54 online_model_init
   def init(self, frames: torch.Tensor, query_points: torch.Tensor):
     """frames: [S, H, W, 3] (or [S, 1, H, W, 3]; [H, W, 3] when S = 1) float in [-1, 1];
-    query_points [S, N, 3] ([N, 3] when S = 1) as (t, y, x), stream s's on its frame s."""
+    query_points [S, N, 3] ([N, 3] when S = 1) as (t, y, x), stream s's on its frame s.  With
+    per-stream sizes, frames is a list of the S streams' frames."""
+    if self._groups is not None:
+      return self._init_groups(self._stream_frames(frames, range(self.num_streams)), query_points)
     frame = self._as_frames(frames)
     qp = query_points.to(self.dev, torch.float32)
     if qp.dim() == 2:
@@ -139,6 +383,12 @@ class OnlineTracker:
     return frames
 
   def _step_eager(self):
+    if self._groups is not None:
+      # per group: its passes and one batched estimate_trajectories; outputs back in stream order
+      outs = [self._step_group(g, g.state) for g in self._groups]
+      tracks, occ, expd = (torch.cat([o[i] for o in outs]).index_select(0, self._order)
+                           for i in range(3))
+      return tracks, live.postprocess_occlusions(occ, expd), occ, expd
     # all streams in one backbone pass and one batched estimate_trajectories (B = S, T = 1)
     grids = self.model.get_feature_grids(self._frame, False)
     # single-frame step: the causal state is updated in place (causal_context_out = state)
@@ -153,20 +403,21 @@ class OnlineTracker:
   def _capture(self):
     # warm-up on a side stream (allocates workspaces, packs weights, fills the constant cache);
     # the state is saved and restored so that warm-up steps do not advance it
-    saved = [{k: v.clone() for k, v in d.items()} for d in self.state]
+    state = self._state_dicts()
+    saved = [{k: v.clone() for k, v in d.items()} for d in state]
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(s):
       for _ in range(2):
         self._step_eager()
     torch.cuda.current_stream().wait_stream(s)
-    for d, sv in zip(self.state, saved):
+    for d, sv in zip(state, saved):
       for k in d:
         d[k].copy_(sv[k])
     g = torch.cuda.CUDAGraph()
     with torch.cuda.graph(g):
       self._out = self._step_eager()
-    for d, sv in zip(self.state, saved):  # capture does not execute, but be explicit
+    for d, sv in zip(state, saved):  # capture does not execute, but be explicit
       for k in d:
         d[k].copy_(sv[k])
     self._graph = g
@@ -201,10 +452,16 @@ class OnlineTracker:
   def step(self, frames: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """frames: [S, H, W, 3] ([H, W, 3] when S = 1), one per stream.  Returns (tracks [S, N, 1, 2]
     in frame pixels (x, y), visibles [S, N, 1] bool).  The returned tensors are the graph's static
-    outputs: copy them if they must outlive the next step."""
+    outputs: copy them if they must outlive the next step.  With per-stream sizes, frames is a
+    list of the S streams' frames and each stream's tracks are in its own pixels."""
     if self.query_features is None:
       raise RuntimeError('call init(frame, query_points) first')
-    if self._yuv is not None:
+    if self._groups is not None:
+      frames = self._stream_frames(frames, range(self.num_streams))
+      for g in self._groups:
+        for s, dst in zip(g.streams, g.sources):
+          self._copy_in(frames[s], dst)
+    elif self._yuv is not None:
       src = self._as_frames(frames)
       for dst, plane in zip((self._yuv.y, self._yuv.u, self._yuv.v), (src.y, src.u, src.v)):
         dst.copy_(plane)
@@ -233,6 +490,17 @@ class OnlineTracker:
       raise ValueError(f'stream {stream} out of range [0, {self.num_streams})')
     if not 0 <= idx < self.num_points:
       raise ValueError(f'point {idx} out of range [0, {self.num_points})')
+    if self._groups is not None:
+      frame = self._device_frame(self._stream_frames([frame], [stream])[0])
+      new = self._query_features_one(frame, query_point.to(self.dev, torch.float32).reshape(1, 1, 3))
+      gi, slot = self._slot[stream]
+      g = self._groups[gi]
+      for dst, src in zip(g.query_features.lowres + g.query_features.hires, new.lowres + new.hires):
+        dst[slot, idx] = src[0, 0]
+      for d in g.state:
+        for v in d.values():
+          v[slot, idx] = 0
+      return
     frame = self._as_frames(frame, num=1)
     qp = query_point.to(self.dev, torch.float32).reshape(1, 1, 3)
     grids = self.model.get_feature_grids(frame, False)

@@ -68,6 +68,53 @@ def _is_same_res(r1, r2):
   return all(int(x) == int(y) for x, y in zip(r1, r2))
 
 
+class PassStep(NamedTuple):
+  """What get_feature_grids does for one required resolution: `new` starts a backbone pass of
+  h x w frames that reads the video itself (`direct`) or its bilinear resample; otherwise the
+  level reuses the previous pass's grids."""
+  h: int
+  w: int
+  direct: bool
+  new: bool
+
+
+def _pass_plan(video_hw, initial_resolution, refinement_resolutions=None):
+  """The backbone passes of get_feature_grids on a video_hw video (reference tapir_model.py:
+  330-360), one PassStep per required resolution (the initial one first); the refinement
+  resolutions default to generate_default_resolutions of the video size.  Two videos with the
+  same plan have feature grids of the same shapes; a direct-read pass's size is the video's."""
+  vh, vw = int(video_hw[0]), int(video_hw[1])
+  if refinement_resolutions is None:
+    refinement_resolutions = generate_default_resolutions((vh, vw), initial_resolution)
+  all_required = [tuple(initial_resolution)] + [tuple(r) for r in refinement_resolutions]
+  if any(r[0] % 8 != 0 or r[1] % 8 != 0 for r in all_required):
+    raise ValueError('Image resolution must be a multiple of 8.')
+  plan = []
+  curr_resolution = (-1, -1)
+  for resolution in all_required:
+    if not _is_same_res(curr_resolution, resolution):
+      # reference quirk (:337): the PREVIOUS resolution is compared with the video size
+      if _is_same_res(curr_resolution, (vh, vw)):
+        h, w = vh, vw
+      else:
+        h, w = int(resolution[0]), int(resolution[1])
+      curr_resolution = resolution
+      # align_corners=False resize to the same size is the identity: the pass reads the video
+      plan.append(PassStep(h, w, (h, w) == (vh, vw), True))
+    else:
+      plan.append(plan[-1]._replace(new=False))
+  return plan
+
+
+def _per_clip_sizes(video_size):
+  """None for one (h, w); else the list of per-clip (h, w) pairs."""
+  if len(video_size) and isinstance(video_size[0], (tuple, list, torch.Size)):
+    return [(int(h), int(w)) for h, w in video_size]
+  if isinstance(video_size, torch.Tensor) and video_size.dim() == 2:
+    return [(int(h), int(w)) for h, w in video_size.tolist()]
+  return None
+
+
 _PRECISIONS = {'bf16': 1, 'bf16x3': 2, 'bf16x6': 3}
 
 # rows (= queries x frames) processed per mixer pass; bounds the workspace to ~1.5 GB
@@ -239,12 +286,12 @@ class TAPIR(nn.Module):
       self._copy_streams[key] = torch.cuda.Stream(device=dev)
     return self._copy_streams[key]
 
-  def _const(self, values, dev):
+  def _const(self, values, dev, dtype=torch.float32):
     """Small constant vectors, cached: creating them per call costs a blocking H2D copy."""
-    key = (tuple(float(v) for v in values), str(dev))
+    key = (tuple(float(v) for v in values), str(dev), dtype)
     t = self._consts.get(key)
     if t is None:
-      t = torch.tensor(key[0], dtype=torch.float32, device=dev)
+      t = torch.tensor(key[0], dtype=dtype, device=dev)
       self._consts[key] = t
     return t
 
@@ -318,12 +365,7 @@ class TAPIR(nn.Module):
     (hires tensor, torch.cuda.Event) pair per distinct resolution; the event fires as soon as
     that hires grid is final, while ResNet groups 2-3 and the ExtraConvs are still running."""
     del is_training
-    if refinement_resolutions is None:
-      refinement_resolutions = generate_default_resolutions(video.shape[2:4],
-                                                            self.initial_resolution)
-    all_required = [tuple(self.initial_resolution)] + [tuple(r) for r in refinement_resolutions]
-    if any(r[0] % 8 != 0 or r[1] % 8 != 0 for r in all_required):
-      raise ValueError('Image resolution must be a multiple of 8.')
+    plan = _pass_plan(video.shape[2:4], self.initial_resolution, refinement_resolutions)
     # A HOST clip (ideally pinned) is accepted too (extension): its frames are copied to the
     # device in chunks on a copy stream and the stem convolution - the only reader of the video -
     # runs chunk by chunk behind them, so PCIe time hides behind compute.
@@ -344,34 +386,51 @@ class TAPIR(nn.Module):
     if host_video:
       host_src = video
       video = torch.empty(video.shape, dtype=video.dtype, device=dev)
-      if tuple(all_required[0]) != (vh, vw):
+      if not plan[0].direct:
         # the first pass resizes the clip: it needs all of it on the device up front
         video.copy_(host_src, non_blocking=True)
         host_src = None
     feature_grid, hires_feats, resize_im_shape = [], [], []
-    curr_resolution = (-1, -1)
     latent = hires = None
-    shape_hw = None
-    for resolution in all_required:
-      if not _is_same_res(curr_resolution, resolution):
-        # reference quirk (:337): the PREVIOUS resolution is compared with the video size
-        if _is_same_res(curr_resolution, video.shape[-3:-1]):
-          h, w = vh, vw
-        else:
-          h, w = int(resolution[0]), int(resolution[1])
-        frames = video  # align_corners=False resize to the same size is the identity
-        if (h, w) != (vh, vw):
+    for h, w, direct, new_pass in plan:
+      if new_pass:
+        frames = video
+        if not direct:
           frames = torch.empty(n, f, h, w, 3, dtype=torch.float32, device=dev)
           _lib.resample_frames(video, frames)
-        curr_resolution = resolution
-        shape_hw = (h, w)
         latent, hires = self._backbone_pass(pk, frames, host_src if frames is video else None,
                                             hires_ready_events, dev)
         if frames is video:
           host_src = None  # the whole clip is on the device now (later passes resize from it)
       feature_grid.append(latent)
       hires_feats.append(hires)
-      resize_im_shape.append(torch.Size(shape_hw))
+      resize_im_shape.append(torch.Size((h, w)))
+    return FeatureGrids(tuple(feature_grid), tuple(hires_feats), tuple(resize_im_shape))
+
+  def _feature_grids_of_frames(self, frames, plan):
+    """get_feature_grids of a batch of one-frame clips of different sizes or formats that share
+    `plan` (no direct-read pass): frames is a list of [H, W, 3] tensors (float32 in [-1, 1] or
+    uint8) or one-frame YUV clips.  Each pass resamples uint8 and YUV frames in one ingest launch;
+    float32 frames keep one tapir_bilinear_resize launch each (the multi-frame ingest cannot
+    reproduce its rounding bit for bit)."""
+    dev = self._device_check(*(None if isinstance(x, live.YUV420Frames) else x for x in frames))
+    pk = self._pack()
+    feature_grid, hires_feats, resize_im_shape = [], [], []
+    latent = hires = None
+    for h, w, direct, new_pass in plan:
+      if direct:
+        raise ValueError('_feature_grids_of_frames: a direct-read pass needs frames of one size')
+      if new_pass:
+        batch = torch.empty(len(frames), 1, h, w, 3, dtype=torch.float32, device=dev)
+        if any(isinstance(x, torch.Tensor) and x.dtype == torch.float32 for x in frames):
+          for x, out in zip(frames, batch):
+            _lib.resample_frames(x[None], out)
+        else:
+          _lib.ingest_frames_multi(frames, batch.view(len(frames), h, w, 3))
+        latent, hires = self._backbone_pass(pk, batch, None, None, dev)
+      feature_grid.append(latent)
+      hires_feats.append(hires)
+      resize_im_shape.append(torch.Size((h, w)))
     return FeatureGrids(tuple(feature_grid), tuple(hires_feats), tuple(resize_im_shape))
 
   def _backbone_pass(self, pk, frames, host_src, hires_ready_events, dev):
@@ -468,6 +527,10 @@ class TAPIR(nn.Module):
   ) -> Mapping[str, Any]:
     """Reference tapir_model.py:394-578.
 
+    `video_size` (extension): one (h, w) for every clip, or a sequence of B (h, w) pairs, clip b's
+    tracks (and query points) then being in its own video's pixels; each clip's results equal a
+    single-clip call with its size, bit for bit.
+
     `causal_context_out` (extension, optional): list of dicts of preallocated [B, N, 2, 512|2048]
     tensors that receive the new causal context instead of fresh allocations.  For single-frame
     steps (T == 1, the streaming case) it may be `causal_context` itself: the state is then
@@ -481,12 +544,19 @@ class TAPIR(nn.Module):
     del is_training, query_chunk_size
     dev = self._device_check(query_features.lowres[0])
     pk = self._pack()
-    video_hw = (int(video_size[0]), int(video_size[1]))
+    per_clip = _per_clip_sizes(video_size)
+    video_hw = None if per_clip is not None else (int(video_size[0]), int(video_size[1]))
     num_levels_total = len(feature_grids.lowres)
     num_iters = self.num_pips_iter * (num_levels_total - 1)
     B, N = query_features.lowres[0].shape[:2]
     T = feature_grids.lowres[0].shape[1]
     nb = pk['num_blocks']
+    video_table = None
+    if per_clip is not None:
+      if len(per_clip) != B:
+        raise ValueError(f'video_size has {len(per_clip)} (h, w) pairs for {B} clips')
+      # [B, 2] (h, w): the track update's table; the stage-A scalings broadcast per clip
+      video_table = self._const([v for hw in per_clip for v in hw], dev, torch.int32).view(B, 2)
 
     def new(*shape, dtype=torch.float32):
       return torch.empty(*shape, dtype=dtype, device=dev)
@@ -530,8 +600,9 @@ class TAPIR(nn.Module):
       # every [bs, sl] slice below is contiguous: either whole clips or a query chunk of one clip
       occ0, expd0 = occ_out[0][bs, sl], expd_out[0][bs, sl]  # outputs are written in place
       qp = query_points_in_video[bs, sl] if query_points_in_video is not None else None
+      vsize = video_hw if video_table is None else per_clip[b0:b1]
       pos = self._stage_a(pk, feature_grids.lowres[0][bs].contiguous(),
-                          query_features.lowres[0][bs, sl].contiguous(), qp, video_hw, occ0, expd0,
+                          query_features.lowres[0][bs, sl].contiguous(), qp, vsize, occ0, expd0,
                           trk_out[0][bs, sl], am_out[bs, sl] if am_out is not None else None, dev)
 
       # ---- refinement iterations
@@ -559,7 +630,8 @@ class TAPIR(nn.Module):
         fdst = feats[1] if fsrc is feats[0] else feats[0]
         occ_n, expd_n = occ_out[it + 1][bs, sl], expd_out[it + 1][bs, sl]
         self._refine(pk, levels, pos, occ, expd, feat, x_planes, res, ctx, mws, occ_n, expd_n,
-                     fdst, trk_out[it + 1][bs, sl], feature_grids.resolutions[level], video_hw)
+                     fdst, trk_out[it + 1][bs, sl], feature_grids.resolutions[level],
+                     video_hw if video_table is None else video_table[bs])
         fsrc, occ, expd = fdst, occ_n, expd_n
         if (it + 1) % self.num_pips_iter == 0:
           # level boundary (tapir_model.py:549-552): features restart from the query,
@@ -614,18 +686,23 @@ class TAPIR(nn.Module):
     G, n = qfeat.shape[:2]
     T = grid.shape[1]
     ih, iw = self.initial_resolution
-    vh, vw = video_hw
+    if isinstance(video_hw[0], tuple):  # one (h, w) per clip: [G, 1, 3] and [G, 1, 1, 2] scales
+      to_init = self._const([v for h, w in video_hw for v in (T, h, w)], dev).view(G, 1, 3)
+      to_video = self._const([v for h, w in video_hw for v in (w, h)], dev).view(G, 1, 1, 2)
+    else:
+      vh, vw = video_hw
+      to_init, to_video = self._const([T, vh, vw], dev), self._const([vw, vh], dev)
     qp = None
     if query_points is not None:
       qp = query_points.to(torch.float32)
       # utils.convert_grid_coordinates (coords * out / in), tapir_model.py:488-493
-      qp = (qp * self._const([T, ih, iw], dev) / self._const([T, vh, vw], dev)).contiguous()
+      qp = (qp * self._const([T, ih, iw], dev) / to_init).contiguous()
     pos = torch.empty(G, n, T, 2, dtype=torch.float32, device=dev)
     ws = self._workspace('cost_volume', _lib.cost_volume_workspace_bytes(qfeat, grid), dev)
     _lib.cost_volume_tracks(pk['head'], qfeat, grid, qp, self.softmax_temperature, (ih, iw), pos,
                             occ, expd, argmax, ws)
     # train2orig (tapir_model.py:435-441)
-    torch.div(pos * self._const([vw, vh], dev), self._const([iw, ih], dev), out=tracks)
+    torch.div(pos * to_video, self._const([iw, ih], dev), out=tracks)
     return pos
 
   def _refine(self, pk, levels, pos, occ, expd, feat, x_planes, res, ctx, mws, occ_out, expd_out,
@@ -633,11 +710,16 @@ class TAPIR(nn.Module):
     """One refinement iteration (the refine_pips call, reference tapir_model.py:529-542): local correlation around pos
     over the pyramid `levels`, the mixer, and the update of pos (in place), occlusion, expected
     distance, features (hi, lo views `feat` -> feat_out) and tracks.  ctx: the mixer's causal
-    context lists (ctx1_in, ctx2_in, ctx1_out, ctx2_out), None where absent."""
+    context lists (ctx1_in, ctx2_in, ctx1_out, ctx2_out), None where absent.  video_hw: one
+    (h, w), or an int32 [G, 2] table of per-clip sizes."""
     _lib.local_corr(levels, pos, occ, expd, *feat, x_planes, self.initial_resolution)
     _lib.mixer_forward(pk['mixer'], x_planes, res, self.use_casual_conv, *ctx, mws)
-    _lib.refine_update(res, pos, occ, expd, *feat, occ_out, expd_out, feat_out, tracks_out,
-                       self.initial_resolution, resize_hw, video_hw)
+    if isinstance(video_hw, torch.Tensor):
+      _lib.refine_update(res, pos, occ, expd, *feat, occ_out, expd_out, feat_out, tracks_out,
+                         self.initial_resolution, resize_hw, (0, 0), video_table=video_hw)
+    else:
+      _lib.refine_update(res, pos, occ, expd, *feat, occ_out, expd_out, feat_out, tracks_out,
+                         self.initial_resolution, resize_hw, video_hw)
 
   def construct_initial_causal_state(self, num_points, num_resolutions=1):
     """Reference tapir_model.py:763-772 (the same dict object repeated, CPU tensors)."""
