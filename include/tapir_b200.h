@@ -446,6 +446,17 @@ int tapir_resize_lanczos_u8(const uint8_t* src, uint8_t* dst, int32_t frames, in
 int tapir_sample_query_features(const float* grid, int32_t T, int32_t gh, int32_t gw, int32_t C,
                                 const float* query_tyx, int32_t N, int32_t vT, int32_t vH,
                                 int32_t vW, float* out, void* stream);
+/* The same sampling from a grid [T][gh][gw][C] that holds only some frames of a vT-frame clip:
+ * frame_slot (int32 [vT]) maps each clip frame to its slot in the grid, or -1 for a frame the grid
+ * does not hold.  The clip's vT normalises the time axis, so a query's features are bit for bit
+ * those sampled from the whole clip's grid whenever every tap of nonzero weight lands on a held
+ * frame; a query with such a tap on an absent frame gets a NaN row instead (the grid is never read
+ * outside its T slots).  frame_slot == NULL is tapir_sample_query_features: same launch, same
+ * results.  Every argument is checked first (sizes, NULL pointers, 4-byte alignment, out
+ * overlapping an input); a bad one returns 1 before any CUDA call. */
+int tapir_sample_query_features_ex(const float* grid, int32_t T, int32_t gh, int32_t gw, int32_t C,
+                                   const float* query_tyx, int32_t N, int32_t vT, int32_t vH,
+                                   int32_t vW, const int32_t* frame_slot, float* out, void* stream);
 
 /* ---- a6: tapir_model.py:687-761 + utils.py:116-193 --------------------------------- */
 size_t tapir_cost_volume_workspace_bytes(int32_t N, int32_t T, int32_t gh, int32_t gw, int32_t C);

@@ -191,6 +191,9 @@ SIGNATURES = {
     'tapir_sample_query_features': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32,
                                                    c_void_p, c_int32, c_int32, c_int32, c_int32,
                                                    c_void_p, c_void_p]),
+    'tapir_sample_query_features_ex': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32,
+                                                      c_void_p, c_int32, c_int32, c_int32, c_int32,
+                                                      c_void_p, c_void_p, c_void_p]),
     'tapir_cost_volume_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32, c_int32, c_int32]),
     'tapir_cost_volume_tracks': (ctypes.c_int, [POINTER(HeadWeights), c_void_p, c_void_p, c_int32,
                                                 c_int32, c_int32, c_int32, c_int32, c_void_p,
@@ -514,16 +517,23 @@ def backbone_forward(weights, frames, lowres, hires, workspace, ready_event=None
 
 
 # ------------------------------------------------------------------------------ stage A
-def sample_query_features(grid, query_tyx, video_shape, out):
+def sample_query_features(grid, query_tyx, video_shape, out, frame_slot=None):
   """Samples of grid [T, gh, gw, C] at query_tyx [N, 3] (coordinates of a video_shape = (T, H, W)
-  clip) into out [N, C]."""
-  fn = 'tapir_sample_query_features'
+  clip) into out [N, C].  frame_slot: None (the grid holds the whole clip), or int32 [video T]
+  mapping each clip frame to its slot among the grid's T frames, or -1; a query with a tap of
+  nonzero weight on a frame without a slot gets a NaN row."""
+  fn = 'tapir_sample_query_features' if frame_slot is None else 'tapir_sample_query_features_ex'
   _check(fn, 'grid', grid, torch.float32)
   (T, gh, gw, C), N = grid.shape, query_tyx.shape[0]
   _check(fn, 'query_tyx', query_tyx, torch.float32, (N, 3), device=grid.device)
   _check(fn, 'out', out, torch.float32, (N, C), device=grid.device)
-  check(load().tapir_sample_query_features(ptr(grid), T, gh, gw, C, ptr(query_tyx), N,
-                                           *(int(v) for v in video_shape), ptr(out), stream()), fn)
+  video_shape = tuple(int(v) for v in video_shape)
+  if frame_slot is None:
+    return check(load().tapir_sample_query_features(ptr(grid), T, gh, gw, C, ptr(query_tyx), N,
+                                                    *video_shape, ptr(out), stream()), fn)
+  _check(fn, 'frame_slot', frame_slot, torch.int32, (video_shape[0],), device=grid.device)
+  check(load().tapir_sample_query_features_ex(ptr(grid), T, gh, gw, C, ptr(query_tyx), N,
+                                              *video_shape, ptr(frame_slot), ptr(out), stream()), fn)
 
 
 def pool_pyramid(grid, out):

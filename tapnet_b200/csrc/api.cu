@@ -100,6 +100,10 @@ namespace {
 constexpr int kMaxGridFrames = 65535;  // frames run on gridDim.y / gridDim.z
 
 bool aligned(const void* p, int bytes) { return (reinterpret_cast<uintptr_t>(p) % bytes) == 0; }
+bool overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
+  const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
+  return pa < pb + b_bytes && pb < pa + a_bytes;
+}
 }  // namespace
 
 int tapir_stem_conv(const void* video, int32_t video_u8, const float* w_packed, int32_t frames,
@@ -282,7 +286,26 @@ int tapir_sample_query_features(const float* grid, int32_t T, int32_t gh, int32_
                                 const float* query_tyx, int32_t N, int32_t vT, int32_t vH,
                                 int32_t vW, float* out, void* stream) {
   Range nvtx_range("tapir_sample_query_features");
-  return sample_query_features(grid, T, gh, gw, C, query_tyx, N, vT, vH, vW, out, S(stream));
+  return sample_query_features(grid, T, gh, gw, C, query_tyx, N, vT, vH, vW, nullptr, out, S(stream));
+}
+
+int tapir_sample_query_features_ex(const float* grid, int32_t T, int32_t gh, int32_t gw, int32_t C,
+                                   const float* query_tyx, int32_t N, int32_t vT, int32_t vH,
+                                   int32_t vW, const int32_t* frame_slot, float* out, void* stream) {
+  Range nvtx_range("tapir_sample_query_features_ex");
+  const char* fn = "tapir_sample_query_features_ex";
+  TAPIR_CHECK_ARG(grid && query_tyx && out, "%s: null grid, query_tyx or out", fn);
+  TAPIR_CHECK_ARG(N >= 1 && T >= 1 && gh >= 1 && gw >= 1 && C >= 1,
+                  "%s: N=%d T=%d gh=%d gw=%d C=%d must be positive", fn, N, T, gh, gw, C);
+  TAPIR_CHECK_ARG(vT >= 1 && vH >= 1 && vW >= 1, "%s: video %d x %d x %d must be positive", fn, vT, vH, vW);
+  TAPIR_CHECK_ARG(aligned(grid, 4) && aligned(query_tyx, 4) && aligned(out, 4) && aligned(frame_slot, 4),
+                  "%s: grid, query_tyx, out and frame_slot must be 4-byte aligned", fn);
+  const size_t out_bytes = (size_t)N * C * 4;
+  TAPIR_CHECK_ARG(!overlap(out, out_bytes, grid, (size_t)T * gh * gw * C * 4) &&
+                      !overlap(out, out_bytes, query_tyx, (size_t)N * 12) &&
+                      !overlap(out, out_bytes, frame_slot, frame_slot ? (size_t)vT * 4 : 0),
+                  "%s: out overlaps grid, query_tyx or frame_slot", fn);
+  return sample_query_features(grid, T, gh, gw, C, query_tyx, N, vT, vH, vW, frame_slot, out, S(stream));
 }
 
 size_t tapir_cost_volume_workspace_bytes(int32_t N, int32_t T, int32_t gh, int32_t gw, int32_t C) {
@@ -377,13 +400,6 @@ int tapir_mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, 
   Range nvtx_range("tapir_mixer_forward");
   return mixer_forward(w, io, workspace, workspace_bytes, S(stream));
 }
-
-namespace {
-bool overlap(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
-  const uintptr_t pa = reinterpret_cast<uintptr_t>(a), pb = reinterpret_cast<uintptr_t>(b);
-  return pa < pb + b_bytes && pb < pa + a_bytes;
-}
-}  // namespace
 
 int tapir_mixer_dw(const tapir_mixer_block* blk, const float* x, int32_t n, int32_t T, int32_t causal,
                    const float* ctx1_in, const float* ctx2_in, float* ctx1_out, float* ctx2_out, float* z,

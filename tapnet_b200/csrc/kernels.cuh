@@ -87,8 +87,11 @@ int paint_point_track(const uint8_t* frames, int T, int H, int W, const void* tr
                       cudaStream_t s);
 
 // ---- stage A (stage_a.cu) ---------------------------------------------------------------
+// frame_slot: null (the grid holds all T frames of the clip) or vT entries, each frame's slot
+// among the grid's T or -1 (see sample_query_kernel)
 int sample_query_features(const float* grid, int T, int gh, int gw, int C, const float* query_tyx,
-                          int N, int vT, int vH, int vW, float* out, cudaStream_t s);
+                          int N, int vT, int vH, int vW, const int* frame_slot, float* out,
+                          cudaStream_t s);
 // B clips: qfeat [B][N][C], grid [B][T][gh][gw][C], outputs indexed by flattened query b*N + n
 size_t cost_volume_workspace_bytes(int B, int N, int T, int gh, int gw, int C);
 int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid, int B,

@@ -29,33 +29,51 @@ __device__ __forceinline__ float unnormalize_border(float c, int size) {
   return pix;
 }
 
+// Ta: the clip length the coordinates are normalised by.  frame_slot: null for a grid holding all
+// Ta frames (T == Ta), else Ta entries mapping each frame to its slot among the grid's T, or -1.  A
+// tap of nonzero weight on a frame without a slot makes the query's row NaN: the grid is never read
+// outside its T slots and a partial sum is never returned.
 __global__ void __launch_bounds__(128) sample_query_kernel(const float* __restrict__ grid, int T,
                                                            int gh, int gw, int C,
                                                            const float* __restrict__ q, int vT,
-                                                           int vH, int vW, float* __restrict__ out) {
+                                                           int vH, int vW, int Ta,
+                                                           const int* __restrict__ frame_slot,
+                                                           float* __restrict__ out) {
   const int n = blockIdx.x;
   // utils.convert_grid_coordinates: coords * out / in (tapir_model.py:266-277)
-  float t = __fdiv_rn(__fmul_rn(q[n * 3 + 0], (float)T), (float)vT);
+  float t = __fdiv_rn(__fmul_rn(q[n * 3 + 0], (float)Ta), (float)vT);
   const float y = __fdiv_rn(__fmul_rn(q[n * 3 + 1], (float)gh), (float)vH);
   const float x = __fdiv_rn(__fmul_rn(q[n * 3 + 2], (float)gw), (float)vW);
   t = __fadd_rn(t, 0.5f);
-  const float pt = unnormalize_border(t, T), py = unnormalize_border(y, gh), px = unnormalize_border(x, gw);
+  const float pt = unnormalize_border(t, Ta), py = unnormalize_border(y, gh), px = unnormalize_border(x, gw);
   const int t0 = (int)floorf(pt), y0 = (int)floorf(py), x0 = (int)floorf(px);
   const float ft = pt - t0, fy = py - y0, fx = px - x0;
+  bool in_clip[2];
+  int slot[2];
+#pragma unroll
+  for (int dt = 0; dt < 2; ++dt) {
+    const int tt = t0 + dt;
+    in_clip[dt] = tt >= 0 && tt < Ta;
+    slot[dt] = !in_clip[dt] ? -1 : frame_slot ? frame_slot[tt] : tt;
+  }
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float acc = 0.f;
+    bool missing = false;
 #pragma unroll
     for (int dt = 0; dt < 2; ++dt)
 #pragma unroll
       for (int dy = 0; dy < 2; ++dy)
 #pragma unroll
         for (int dx = 0; dx < 2; ++dx) {
-          const int tt = t0 + dt, yy = y0 + dy, xx = x0 + dx;
+          const int tt = slot[dt], yy = y0 + dy, xx = x0 + dx;
           const float wgt = (dt ? ft : 1.f - ft) * (dy ? fy : 1.f - fy) * (dx ? fx : 1.f - fx);
-          if (tt < T && yy < gh && xx < gw && tt >= 0 && yy >= 0 && xx >= 0)
+          if (!in_clip[dt] || yy >= gh || xx >= gw || yy < 0 || xx < 0) continue;
+          if (tt >= 0 && tt < T)
             acc += wgt * grid[(((long long)tt * gh + yy) * gw + xx) * C + c];
+          else if (wgt != 0.f)
+            missing = true;
         }
-    out[(long long)n * C + c] = acc;
+    out[(long long)n * C + c] = missing ? __int_as_float(0x7fc00000) : acc;
   }
 }
 
@@ -553,11 +571,15 @@ __global__ void __launch_bounds__(256) cost_volume_head_generic_kernel(
 }  // namespace
 
 int sample_query_features(const float* grid, int T, int gh, int gw, int C, const float* query_tyx,
-                          int N, int vT, int vH, int vW, float* out, cudaStream_t s) {
+                          int N, int vT, int vH, int vW, const int* frame_slot, float* out,
+                          cudaStream_t s) {
   TAPIR_CHECK_ARG(grid && query_tyx && out && N > 0 && T > 0 && gh > 0 && gw > 0 && C > 0,
                   "sample_query_features: bad arguments");
   ProfileScope ps("sample_query", s, 0.0, (double)N * C * 4 * 9);
-  sample_query_kernel<<<N, 128, 0, s>>>(grid, T, gh, gw, C, query_tyx, vT, vH, vW, out);
+  // without a frame table the grid's own T normalises the time axis (the reference's call, where
+  // the grid holds the whole clip); with one, the video's vT does
+  sample_query_kernel<<<N, 128, 0, s>>>(grid, T, gh, gw, C, query_tyx, vT, vH, vW,
+                                        frame_slot ? vT : T, frame_slot, out);
   count_launch();
   TAPIR_LAUNCH_CHECK("sample_query_kernel");
   return kOk;

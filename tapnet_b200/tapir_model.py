@@ -433,13 +433,24 @@ class TAPIR(nn.Module):
       resize_im_shape.append(torch.Size((h, w)))
     return FeatureGrids(tuple(feature_grid), tuple(hires_feats), tuple(resize_im_shape))
 
-  def _backbone_pass(self, pk, frames, host_src, hires_ready_events, dev):
+  def _backbone_pass(self, pk, frames, host_src, hires_ready_events, dev, out=None):
     """Feature grids (lowres, hires) of every frame of `frames` ([B, T, h, w, 3] on the device, or
-    a YUV clip).  host_src: the host clip whose copy `frames` is yet to be, streamed in here."""
+    a YUV clip).  host_src: the host clip whose copy `frames` is yet to be, streamed in here.
+    out: None, or the contiguous (lowres, hires) tensors to write the grids into."""
     n, f, h, w, _ = frames.shape
     nf = n * f
-    latent = torch.empty(n, f, h // 8, w // 8, self.lowres_dim, dtype=torch.float32, device=dev)
-    hires = torch.empty(n, f, h // 4, w // 4, self.highres_dim, dtype=torch.float32, device=dev)
+    lo_shape = (n, f, h // 8, w // 8, self.lowres_dim)
+    hi_shape = (n, f, h // 4, w // 4, self.highres_dim)
+    if out is None:
+      latent = torch.empty(lo_shape, dtype=torch.float32, device=dev)
+      hires = torch.empty(hi_shape, dtype=torch.float32, device=dev)
+    else:
+      latent, hires = out
+      for name, t, shape in (('lowres', latent, lo_shape), ('hires', hires, hi_shape)):
+        if (t.shape != shape or t.dtype != torch.float32 or t.device != dev
+            or not t.is_contiguous()):
+          raise ValueError(f'grids_out {name} must be a contiguous float32 {list(shape)} tensor '
+                           f'on {dev}, got {t.dtype} {tuple(t.shape)} on {t.device}')
     src = frames if isinstance(frames, live.YUV420Frames) else frames.view(nf, h, w, 3)
     flat_lo = latent.view(nf, h // 8, w // 8, self.lowres_dim)
     flat_hi = hires.view(nf, h // 4, w // 4, self.highres_dim)
@@ -605,38 +616,29 @@ class TAPIR(nn.Module):
                           query_features.lowres[0][bs, sl].contiguous(), qp, vsize, occ0, expd0,
                           trk_out[0][bs, sl], am_out[bs, sl] if am_out is not None else None, dev)
 
-      # ---- refinement iterations
-      x_planes = new(self._planes, nq * T, pk['mixer_in'], dtype=torch.bfloat16)
-      res = new(nq, T, 388)
-      feats = [new(nq, T, 384), new(nq, T, 384)]
-      mws = self._workspace('mixer', _lib.mixer_workspace_bytes(x_planes), dev)
-      occ, expd = occ0, expd0
-      fsrc = None  # the previous iteration's features; None: start from the query features
-      for it in range(num_iters):
-        level = it // self.num_pips_iter + 1
+      # ---- refinement iterations, one level at a time
+      bufs = self._refine_buffers(pk, nq, T, dev)
+      npi = self.num_pips_iter
+      for level in range(1, num_levels_total):
+        its = range((level - 1) * npi, level * npi)
         levels = ([feature_grids.hires[level][bs].contiguous(),
                    feature_grids.lowres[level][bs].contiguous()] + [g[bs] for g in pooled[level]])
-        if fsrc is not None:
-          feat = (fsrc[..., :128], fsrc[..., 128:])
-        else:
-          feat = tuple(q[bs, sl].contiguous().view(nq, 1, -1).expand(nq, T, -1)
-                       for q in (query_features.hires[level], query_features.lowres[level]))
-        ctx = [None] * 4
-        if causal_context is not None:
-          ctx[:2] = _ctx_lists(causal_context[it], nb, (bs, sl),
-                               lambda t: t.to(device=dev, dtype=torch.float32).contiguous())
-        if write_ctx:
-          ctx[2:] = _ctx_lists(new_ctx[it], nb, (bs, sl))
-        fdst = feats[1] if fsrc is feats[0] else feats[0]
-        occ_n, expd_n = occ_out[it + 1][bs, sl], expd_out[it + 1][bs, sl]
-        self._refine(pk, levels, pos, occ, expd, feat, x_planes, res, ctx, mws, occ_n, expd_n,
-                     fdst, trk_out[it + 1][bs, sl], feature_grids.resolutions[level],
-                     video_hw if video_table is None else video_table[bs])
-        fsrc, occ, expd = fdst, occ_n, expd_n
-        if (it + 1) % self.num_pips_iter == 0:
-          # level boundary (tapir_model.py:549-552): features restart from the query,
-          # occlusion / expected_dist revert to the stage-A estimate, positions carry over
-          fsrc, occ, expd = None, occ0, expd0
+        qfeat = tuple(q[bs, sl].contiguous()
+                      for q in (query_features.hires[level], query_features.lowres[level]))
+        ctxs = []
+        for it in its:
+          ctx = [None] * 4
+          if causal_context is not None:
+            ctx[:2] = _ctx_lists(causal_context[it], nb, (bs, sl),
+                                 lambda t: t.to(device=dev, dtype=torch.float32).contiguous())
+          if write_ctx:
+            ctx[2:] = _ctx_lists(new_ctx[it], nb, (bs, sl))
+          ctxs.append(ctx)
+        outs = [(occ_out[it + 1][bs, sl], expd_out[it + 1][bs, sl], trk_out[it + 1][bs, sl])
+                for it in its]
+        self._refine_level(pk, levels, qfeat, pos, occ0, expd0, outs, bufs,
+                           feature_grids.resolutions[level],
+                           video_hw if video_table is None else video_table[bs], ctxs)
     return out
 
   def _new_causal_context(self, causal_context, get_causal_context, causal_context_out, num_iters,
@@ -704,6 +706,38 @@ class TAPIR(nn.Module):
     # train2orig (tapir_model.py:435-441)
     torch.div(pos * to_video, self._const([iw, ih], dev), out=tracks)
     return pos
+
+  def _refine_buffers(self, pk, nq, T, dev):
+    """Scratch of the refinement of nq queries over T frames: (x_planes, res, feats, mixer
+    workspace)."""
+    x_planes = torch.empty(self._planes, nq * T, pk['mixer_in'], dtype=torch.bfloat16, device=dev)
+    res = torch.empty(nq, T, 388, dtype=torch.float32, device=dev)
+    feats = [torch.empty(nq, T, 384, dtype=torch.float32, device=dev) for _ in range(2)]
+    return x_planes, res, feats, self._workspace('mixer', _lib.mixer_workspace_bytes(x_planes), dev)
+
+  def _refine_level(self, pk, levels, qfeat, pos, occ0, expd0, outs, bufs, resize_hw, video_hw,
+                    ctxs=None):
+    """The num_pips_iter refinement iterations of one level (reference tapir_model.py:529-552)
+    for nq queries over T frames.  levels: the level's pyramid grids [G, T, h, w, C] (hires,
+    lowres, pooled); qfeat: the (hires, lowres) query features [nq, 128 | 256]; pos [..., T, 2] is
+    moved in place; occ0 / expd0: the stage-A estimates the level starts from; outs: one (occ, expd,
+    tracks) output view per iteration; bufs: _refine_buffers; ctxs: one mixer context list per
+    iteration (see _refine), or None.  Only pos carries over to the next level: features restart
+    from the query and occlusion / expected distance from stage A."""
+    x_planes, res, feats, mws = bufs
+    nq, T = res.shape[:2]
+    occ, expd = occ0, expd0
+    fsrc = None  # the previous iteration's features; None: start from the query features
+    for i, (occ_n, expd_n, trk_n) in enumerate(outs):
+      if fsrc is not None:
+        feat = (fsrc[..., :128], fsrc[..., 128:])
+      else:
+        feat = tuple(q.view(nq, 1, -1).expand(nq, T, -1) for q in qfeat)
+      fdst = feats[1] if fsrc is feats[0] else feats[0]
+      self._refine(pk, levels, pos, occ, expd, feat, x_planes, res,
+                   ctxs[i] if ctxs is not None else [None] * 4, mws, occ_n, expd_n, fdst, trk_n,
+                   resize_hw, video_hw)
+      fsrc, occ, expd = fdst, occ_n, expd_n
 
   def _refine(self, pk, levels, pos, occ, expd, feat, x_planes, res, ctx, mws, occ_out, expd_out,
               feat_out, tracks_out, resize_hw, video_hw):
