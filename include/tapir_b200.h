@@ -395,6 +395,43 @@ typedef struct {
 } tapir_tapvid_args;
 int tapir_tapvid_counts(const tapir_tapvid_args* args, void* stream);
 
+/* tapnextpp/metrics/aj_rd.py compute_raw_redetection_stats: the eligible reappearance events of
+ * every track (b, n) and their AJ_RD values, bit for bit.  A reappearance is a frame t >= 1 with
+ * gt_visible[t] && !gt_visible[t-1]; its duration is the length of the invisible run ending at
+ * t - 1 (t itself if the track is invisible from frame 0).  An event is eligible when its duration
+ * is strictly greater than every earlier event's of the track.  For threshold D, over frames
+ * [t, T): within = sqrt_rn(fma(dy, dy, dx * dx)) <= D (float32, a NaN distance is not within),
+ * TP = sum(within && gt && pred), FP = sum(pred && (!gt || !within)), value = float(TP) /
+ * float(sum(gt) + FP) (IEEE float32; 0 / 0 is NaN).
+ *
+ * A track has at most K(T) eligible events, K(T) the largest k with k (k + 3) / 2 <= T (their
+ * durations are at least 1 .. k, each followed by a visible frame); tapir_redetection_max_events
+ * (host only) returns K(T) (0 for T < 1).  Track i = b N + n writes its events, in t order, to
+ * slots i K(T) .. i K(T) + event_count[i] - 1 of event_t, event_duration and event_values
+ * [slot][num_thresholds]; the other slots are not written.  event_* need capacity >= B N K(T)
+ * slots (they may be NULL when K(T) = 0).  No allocation, no host copy, no host sync: graph-
+ * capturable.  A bad argument returns 1 before any CUDA call. */
+#define TAPIR_REDETECTION_MAX_THRESHOLDS 16
+typedef struct {
+  const uint8_t* gt_visible;    /* [B][N][T] bool */
+  const uint8_t* pred_visible;  /* [B][N][T] bool, or NULL to threshold the two logit arrays as
+                                   tapir_tapvid_counts does */
+  const float* pred_occ_logits; /* [B][N][T] (used when pred_visible is NULL) */
+  const float* pred_expd_logits;
+  const float* pred_tracks;     /* [B][N][T][2] (x, y) */
+  const float* gt_tracks;       /* [B][N][T][2] */
+  float thresholds[TAPIR_REDETECTION_MAX_THRESHOLDS]; /* distance thresholds D, float32 */
+  int32_t num_thresholds;       /* 1 .. TAPIR_REDETECTION_MAX_THRESHOLDS */
+  int32_t B, N, T;
+  int64_t capacity;             /* slots of event_t / event_duration / event_values */
+  int32_t* event_t;             /* [capacity] reappearance frame */
+  int32_t* event_duration;      /* [capacity] */
+  float* event_values;          /* [capacity][num_thresholds] */
+  int32_t* event_count;         /* [B][N] */
+} tapir_redetection_args;
+int32_t tapir_redetection_max_events(int32_t T);
+int tapir_redetection_events(const tapir_redetection_args* args, void* stream);
+
 /* ---- f5: visualisation (the step after the path) ------------------------------------- */
 /* tapnet/utils/viz_utils.py:47-124 paint_point_track, bit for bit: frames [T][H][W][3] uint8 ->
  * out (same shape, must not overlap frames) with a dot of radius round(min(H, W) * 0.015) at

@@ -29,7 +29,7 @@ for t in $TIERS; do
     io)          run io "X=1" tests/test_io_gpu.py ;;
     yuv)         run yuv "X=1" tests/test_yuv_gpu.py ;;
     bulk)        run bulk "X=1" tests/test_bulk_gpu.py ;;
-    eval)        run eval "X=1" tests/test_tapvid_gpu.py ;;
+    eval)        run eval "X=1" tests/test_tapvid_gpu.py tests/test_redetection_gpu.py ;;
     sizes)       run sizes "X=1" tests/test_tracker_sizes_gpu.py ;;
     no_halo)     run no_halo "TAPIR_B200_CONV_HALO=0" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_exact_gpu.py tests/test_stages_gpu.py tests/test_end_to_end_gpu.py ;;
     all)         run all "X=1" tests ;;

@@ -49,3 +49,10 @@ timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
     -k "not golden_and_eager and not isolated" \
     2>&1 | grep -E '^=========|passed|failed' | tail -n 25
 echo "sanitizer sizes memcheck rc=${PIPESTATUS[0]}"
+# then AJ_RD's event kernel (fixture cases, random clips up to 300 x 256, the maximal-event track
+# at T = 65536, graph replay); the largest clips and the model runs of evaluate are left out
+timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
+    python -m pytest -q -m gpu -p no:cacheprovider tests/test_redetection_gpu.py \
+    -k "not evaluate and not 1500" \
+    2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+echo "sanitizer redetection memcheck rc=${PIPESTATUS[0]}"

@@ -111,6 +111,18 @@ class TapvidArgs(Structure):
               ('counts', c_void_p)]
 
 
+REDETECTION_MAX_THRESHOLDS = 16
+
+
+class RedetectionArgs(Structure):
+  _fields_ = [('gt_visible', c_void_p), ('pred_visible', c_void_p), ('pred_occ_logits', c_void_p),
+              ('pred_expd_logits', c_void_p), ('pred_tracks', c_void_p), ('gt_tracks', c_void_p),
+              ('thresholds', c_float * REDETECTION_MAX_THRESHOLDS), ('num_thresholds', c_int32),
+              ('B', c_int32), ('N', c_int32), ('T', c_int32), ('capacity', c_int64),
+              ('event_t', c_void_p), ('event_duration', c_void_p), ('event_values', c_void_p),
+              ('event_count', c_void_p)]
+
+
 class Yuv420Frames(Structure):
   _fields_ = [('y', c_void_p), ('u', c_void_p), ('v', c_void_p),
               ('y_frame_stride', c_int64), ('u_frame_stride', c_int64), ('v_frame_stride', c_int64),
@@ -188,6 +200,8 @@ SIGNATURES = {
     'tapir_postprocess_occlusions': (ctypes.c_int, [c_void_p, c_void_p, c_int64, c_void_p,
                                                     c_void_p]),
     'tapir_tapvid_counts': (ctypes.c_int, [POINTER(TapvidArgs), c_void_p]),
+    'tapir_redetection_max_events': (c_int32, [c_int32]),
+    'tapir_redetection_events': (ctypes.c_int, [POINTER(RedetectionArgs), c_void_p]),
     'tapir_sample_query_features': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32,
                                                    c_void_p, c_int32, c_int32, c_int32, c_int32,
                                                    c_void_p, c_void_p]),
@@ -741,6 +755,48 @@ def tapvid_counts(query_points, gt_occluded, gt_tracks, pred_occluded, pred_trac
   args = TapvidArgs(ptr(query_points), ptr(gt_occluded), ptr(gt_tracks), ptr(pred_occluded),
                     ptr(logits[0]), ptr(logits[1]), ptr(pred_tracks), B, N, T, query_mode, ptr(counts))
   check(load().tapir_tapvid_counts(byref(args), stream()), 'tapir_tapvid_counts')
+
+
+def redetection_max_events(T):
+  """Host only: K(T), the most eligible reappearance events a track of T frames can have."""
+  return int(load().tapir_redetection_max_events(int(T)))
+
+
+def redetection_events(gt_visible, pred_visible, pred_tracks, gt_tracks, thresholds, event_t,
+                       event_duration, event_values, event_count, pred_logits=None):
+  """The eligible reappearance events of every track of gt_visible [B, N, T] (uint8) and their
+  AJ_RD values: pred_tracks / gt_tracks float32 [B, N, T, 2], pred_visible uint8 [B, N, T] or
+  pred_logits (occlusion, expected_dist float32 logits), `thresholds` a sequence of 1 ..
+  REDETECTION_MAX_THRESHOLDS distances.  Outputs: event_t / event_duration int32 [B, N, K(T)],
+  event_values float32 [B, N, K(T), D], event_count int32 [B, N]."""
+  fn = 'tapir_redetection_events'
+  thresholds = [float(d) for d in thresholds]
+  nd = len(thresholds)
+  _need(1 <= nd <= REDETECTION_MAX_THRESHOLDS, fn,
+        f'{nd} distance thresholds, 1 .. {REDETECTION_MAX_THRESHOLDS} supported')
+  (B, N, T), dev = gt_visible.shape, gt_visible.device
+  K = redetection_max_events(T)
+  logits = tuple(pred_logits) if pred_logits is not None else (None, None)
+  checks = [('gt_visible', gt_visible, torch.uint8, (B, N, T)),
+            ('pred_tracks', pred_tracks, torch.float32, (B, N, T, 2)),
+            ('gt_tracks', gt_tracks, torch.float32, (B, N, T, 2)),
+            ('event_t', event_t, torch.int32, (B, N, K)),
+            ('event_duration', event_duration, torch.int32, (B, N, K)),
+            ('event_values', event_values, torch.float32, (B, N, K, nd)),
+            ('event_count', event_count, torch.int32, (B, N))]
+  if pred_logits is None:
+    checks.append(('pred_visible', pred_visible, torch.uint8, (B, N, T)))
+  else:
+    pred_visible = None
+    checks += [(name, t, torch.float32, (B, N, T)) for name, t in zip(('occlusion', 'expected_dist'), logits)]
+  for name, t, dtype, shape in checks:
+    _need(t is not None, fn, f'{name} is missing')
+    _check(fn, name, t, dtype, shape, device=dev)
+  args = RedetectionArgs(ptr(gt_visible), ptr(pred_visible), ptr(logits[0]), ptr(logits[1]),
+                         ptr(pred_tracks), ptr(gt_tracks), (c_float * REDETECTION_MAX_THRESHOLDS)(*thresholds),
+                         nd, B, N, T, B * N * K, ptr(event_t), ptr(event_duration), ptr(event_values),
+                         ptr(event_count))
+  check(load().tapir_redetection_events(byref(args), stream()), fn)
 
 
 def paint_point_track(frames, tracks, visibles, colors, out, workspace):

@@ -282,6 +282,13 @@ int tapir_tapvid_counts(const tapir_tapvid_args* args, void* stream) {
   return tapvid_counts(args, S(stream));
 }
 
+int32_t tapir_redetection_max_events(int32_t T) { return redetection_max_events(T); }
+
+int tapir_redetection_events(const tapir_redetection_args* args, void* stream) {
+  Range nvtx_range("tapir_redetection_events");
+  return redetection_events(args, S(stream));
+}
+
 int tapir_sample_query_features(const float* grid, int32_t T, int32_t gh, int32_t gw, int32_t C,
                                 const float* query_tyx, int32_t N, int32_t vT, int32_t vH,
                                 int32_t vW, float* out, void* stream) {

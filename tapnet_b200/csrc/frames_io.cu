@@ -265,6 +265,114 @@ __global__ void __launch_bounds__(256) tapvid_counts_kernel(const tapir_tapvid_a
   }
 }
 
+// aj_rd.py calculate_jaccard_for_segment's ratio: float32(TP) / float32(gt_pos + FP), 0 / 0 -> nan
+__device__ __forceinline__ float jaccard_ratio(int tp, int den) {
+  return den == 0 ? __int_as_float(0x7fc00000) : __fdiv_rn(__int2float_rn(tp), __int2float_rn(den));
+}
+
+// tapnextpp/metrics/aj_rd.py compute_raw_redetection_stats.  One warp per track (b, n); lane i
+// holds frame c0 + i of each 32-frame chunk.
+//   pass 1, forward over gt_visible only: the reappearances, their durations (distance to the
+//     last visible frame, from a ballot), eligibility against the running maximum of the earlier
+//     durations (a max scan, only in chunks that hold a reappearance), compacted in t order into
+//     the track's slots.
+//   pass 2, backward from the last frame to the first event: suffix counts of gt-visible and of
+//     TP / FP per threshold (ballot + popc, carried across chunks), read off by the lanes that
+//     hold an event frame; the events of a chunk come back from pass 1's slots.
+// Frames before the first eligible event are read once, the others twice (gt_visible) or once.
+__global__ void __launch_bounds__(256) redetection_events_kernel(const tapir_redetection_args a, int K) {
+  constexpr unsigned kAll = 0xffffffffu;
+  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (warp >= a.B * a.N) return;
+  const int T = a.T;
+  const long long base = (long long)warp * T, slot0 = (long long)warp * K;
+  const unsigned below = (1u << lane) - 1u, from_me = ~below;
+
+  int last_vis = -1, max_d = -1, count = 0;
+  bool prev_vis = false;
+  for (int c0 = 0; c0 < T; c0 += 32) {
+    const int t = c0 + lane;
+    const bool g = t < T && a.gt_visible[base + t] != 0;
+    const unsigned vis = __ballot_sync(kAll, g);
+    const bool g_prev = lane == 0 ? prev_vis : ((vis >> (lane - 1)) & 1u) != 0;
+    const bool event = g && !g_prev && t >= 1;
+    if (__ballot_sync(kAll, event) != 0) {
+      // count_consecutive_invisibility at t: frames since the last visible one before t
+      const unsigned vb = vis & below;
+      const int d = t - 1 - (vb != 0 ? c0 + 31 - __clz(vb) : last_vis);
+      int m = event ? d : -1;  // inclusive max scan of the chunk's durations
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(kAll, m, o);
+        if (lane >= o) m = max(m, v);
+      }
+      int earlier = __shfl_up_sync(kAll, m, 1);
+      earlier = max(lane == 0 ? -1 : earlier, max_d);
+      const bool eligible = event && d > earlier;  // strictly longer than every earlier event
+      const unsigned em = __ballot_sync(kAll, eligible);
+      if (eligible) {
+        const long long s = slot0 + count + __popc(em & below);
+        a.event_t[s] = t;
+        a.event_duration[s] = d;
+      }
+      count += __popc(em);
+      max_d = max(max_d, __shfl_sync(kAll, m, 31));
+    }
+    if (vis != 0) last_vis = c0 + 31 - __clz(vis);
+    prev_vis = (vis >> 31) != 0;
+  }
+  if (lane == 0) a.event_count[warp] = count;
+  if (count == 0) return;
+  __syncwarp();  // the slots written above, visible to every lane
+
+  const int nd = a.num_thresholds;
+  int gt_pos = 0, tp[TAPIR_REDETECTION_MAX_THRESHOLDS], fp[TAPIR_REDETECTION_MAX_THRESHOLDS];
+#pragma unroll
+  for (int j = 0; j < TAPIR_REDETECTION_MAX_THRESHOLDS; ++j) tp[j] = fp[j] = 0;
+  int k = count - 1;  // the latest event not yet read off
+  int next_t = a.event_t[slot0 + k];
+  const int first_t = a.event_t[slot0];
+  for (int c0 = (T - 1) & ~31; c0 + 31 >= first_t; c0 -= 32) {
+    const int t = c0 + lane;
+    bool g = false, p = false;
+    float dx = 0.f, dy = 0.f;
+    if (t < T) {
+      const long long i = base + t;
+      g = a.gt_visible[i] != 0;
+      p = a.pred_visible != nullptr ? a.pred_visible[i] != 0
+                                    : visible_from_logits(a.pred_occ_logits[i], a.pred_expd_logits[i]);
+      dx = __fsub_rn(a.pred_tracks[2 * i], a.gt_tracks[2 * i]);
+      dy = __fsub_rn(a.pred_tracks[2 * i + 1], a.gt_tracks[2 * i + 1]);
+    }
+    // torch.linalg.norm(., dim=-1) of a float32 pair on the CPU: dx * dx rounded, one FMA, sqrt
+    const float dist = __fsqrt_rn(__fmaf_rn(dy, dy, __fmul_rn(dx, dx)));
+    unsigned ev_bits = 0;  // the chunk's event frames
+    const int k_last = k;
+    while (k >= 0 && next_t >= c0) {
+      ev_bits |= 1u << (next_t - c0);
+      --k;
+      next_t = k >= 0 ? a.event_t[slot0 + k] : -1;
+    }
+    const bool at_event = ((ev_bits >> lane) & 1u) != 0;
+    float* out = a.event_values + (slot0 + k_last - (__popc(ev_bits >> lane) - 1)) * nd;
+    const unsigned gm = __ballot_sync(kAll, g);
+    const int gt_here = gt_pos + __popc(gm & from_me);
+#pragma unroll
+    for (int j = 0; j < TAPIR_REDETECTION_MAX_THRESHOLDS; ++j) {
+      if (j < nd) {
+        const bool within = dist <= a.thresholds[j];  // false for a NaN distance
+        const unsigned tpm = __ballot_sync(kAll, within && g && p);
+        const unsigned fpm = __ballot_sync(kAll, p && (!g || !within));
+        if (at_event)
+          out[j] = jaccard_ratio(tp[j] + __popc(tpm & from_me), gt_here + fp[j] + __popc(fpm & from_me));
+        tp[j] += __popc(tpm);
+        fp[j] += __popc(fpm);
+      }
+    }
+    gt_pos += __popc(gm);
+  }
+}
+
 }  // namespace
 
 int ingest_frames(const uint8_t* src, int frames, int H, int W, int crop_y, int crop_x, int crop_h,
@@ -397,6 +505,43 @@ int tapvid_counts(const tapir_tapvid_args* a, cudaStream_t s) {
   tapvid_counts_kernel<<<(unsigned)ceil_div_ll(tracks, warps_per_block), 32 * warps_per_block, 0, s>>>(*a);
   count_launch();
   TAPIR_LAUNCH_CHECK("tapvid_counts_kernel");
+  return kOk;
+}
+
+int redetection_max_events(int T) {
+  if (T < 1) return 0;
+  long long k = (long long)((sqrt(9.0 + 8.0 * T) - 3.0) / 2.0);
+  while (k > 0 && k * (k + 3) / 2 > T) --k;
+  while ((k + 1) * (k + 4) / 2 <= T) ++k;
+  return (int)k;
+}
+
+int redetection_events(const tapir_redetection_args* a, cudaStream_t s) {
+  TAPIR_CHECK_ARG(a != nullptr, "redetection_events: null args");
+  TAPIR_CHECK_ARG(a->B > 0 && a->N > 0 && a->T > 0 && a->T <= (1 << 30) &&
+                      (long long)a->B * a->N <= (1ll << 26),
+                  "redetection_events: bad shape B=%d N=%d T=%d", a->B, a->N, a->T);
+  TAPIR_CHECK_ARG(a->num_thresholds >= 1 && a->num_thresholds <= TAPIR_REDETECTION_MAX_THRESHOLDS,
+                  "redetection_events: num_thresholds=%d outside 1..%d", a->num_thresholds,
+                  TAPIR_REDETECTION_MAX_THRESHOLDS);
+  TAPIR_CHECK_ARG(a->gt_visible && a->pred_tracks && a->gt_tracks && a->event_count,
+                  "redetection_events: null pointer");
+  TAPIR_CHECK_ARG(a->pred_visible != nullptr || (a->pred_occ_logits && a->pred_expd_logits),
+                  "redetection_events: need pred_visible or both logit arrays");
+  const long long tracks = (long long)a->B * a->N;
+  const int K = redetection_max_events(a->T);
+  TAPIR_CHECK_ARG(K == 0 || (a->event_t && a->event_duration && a->event_values),
+                  "redetection_events: null event array");
+  TAPIR_CHECK_ARG(a->capacity >= tracks * K,
+                  "redetection_events: capacity %lld < %lld slots (B N K(T), K(%d) = %d)",
+                  (long long)a->capacity, tracks * K, a->T, K);
+  const double pred_bytes = a->pred_visible != nullptr ? 1.0 : 8.0;
+  ProfileScope ps("redetection_events", s, 0.0, (double)tracks * a->T * (1.0 + pred_bytes + 16.0));
+  const int warps_per_block = 8;
+  redetection_events_kernel<<<(unsigned)ceil_div_ll(tracks, warps_per_block), 32 * warps_per_block, 0,
+                              s>>>(*a, K);
+  count_launch();
+  TAPIR_LAUNCH_CHECK("redetection_events_kernel");
   return kOk;
 }
 

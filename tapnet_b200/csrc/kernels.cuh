@@ -66,6 +66,8 @@ int ingest_frames_multi(const tapir_ingest_desc* descs, int frames, float* dst, 
 int postprocess_occlusions(const float* occ, const float* expd, long long n, uint8_t* visible,
                            cudaStream_t s);
 int tapvid_counts(const tapir_tapvid_args* a, cudaStream_t s);
+int redetection_max_events(int T);
+int redetection_events(const tapir_redetection_args* a, cudaStream_t s);
 
 // ---- Lanczos resize of uint8 RGB clips (resample.cu; PIL's 8-bit LANCZOS) -------------------
 // Host only: the per-axis kernel width, and the (xmin, n) bounds [out][2] and 22-bit fixed-point

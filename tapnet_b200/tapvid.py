@@ -12,6 +12,11 @@ are resized on the device and the metrics are reduced there (`metrics.compute_ta
 
 or `python -m tapnet_b200.tapvid --dataset davis --path tapvid_davis.pkl --checkpoint C.pt`.
 
+`evaluate(..., redetection=True)` adds AJ_RD, the re-detection Average Jaccard of
+`tapnet/tapnextpp/metrics/aj_rd.py` (`metrics.compute_redetection_metrics`), which the reference
+reports on RoboTAP (`create_robotap_dataset`); `window_frames` tracks long clips in bounded memory
+(`windowed.windowed_forward`).
+
 `resize_video` is the reference's `media.resize_video` on uint8 frames, assuming (mediapy is not
 a dependency) that mediapy sends a uint8 3-channel frame to
 `PIL.Image.fromarray(frame).resize((w, h), resample=LANCZOS)`: PIL's 8-bit Lanczos resampler,
@@ -182,6 +187,17 @@ def _scaled(points, video):
   return points * np.array([video.shape[2], video.shape[1]])
 
 
+def _davis_format_videos(path, key, query_mode, resolution, staging):
+  """Yields {key: converted} per video of one pickle in TAP-Vid-DAVIS's format (a dict of
+  videos, read in its key order)."""
+  with open(path, 'rb') as f:
+    data = pickle.load(f)
+  for name in data.keys():
+    video = _clip(data[name]['video'], resolution, staging)
+    points = _scaled(data[name]['points'], video)
+    yield {key: _sample(query_mode, data[name]['occluded'], points, video)}
+
+
 def create_davis_dataset(davis_points_path, query_mode='strided', full_resolution=False,
                          resolution=(256, 256)):
   """Yields {'davis': converted} per video of the TAP-Vid-DAVIS pickle, in its key order."""
@@ -189,13 +205,21 @@ def create_davis_dataset(davis_points_path, query_mode='strided', full_resolutio
   if full_resolution:
     raise NotImplementedError('full_resolution reads davis/full_resolution through '
                               'tensorflow_datasets, which tapnet_b200 does not use')
-  with open(davis_points_path, 'rb') as f:
-    data = pickle.load(f)
+  yield from _davis_format_videos(davis_points_path, 'davis', query_mode, resolution, _Staging())
+
+
+def create_robotap_dataset(robotap_path, query_mode='strided', resolution=(256, 256)):
+  """Yields {'robotap': converted} per video of RoboTAP.  RoboTAP ships as pickles in
+  TAP-Vid-DAVIS's dict format (the reference's tapvid/README.md), and each video is read exactly
+  as create_davis_dataset reads one.  robotap_path is one pickle, or a directory whose `*.pkl`
+  files are read in sorted order.  The reference has no RoboTAP reader; this one is the DAVIS
+  reader's loop over those files."""
+  _check_mode(query_mode)
+  paths = (sorted(glob.glob(os.path.join(robotap_path, '*.pkl'))) if os.path.isdir(robotap_path)
+           else [robotap_path])
   staging = _Staging()
-  for name in data.keys():
-    video = _clip(data[name]['video'], resolution, staging)
-    points = _scaled(data[name]['points'], video)
-    yield {'davis': _sample(query_mode, data[name]['occluded'], points, video)}
+  for path in paths:
+    yield from _davis_format_videos(path, 'robotap', query_mode, resolution, staging)
 
 
 def create_rgb_stacking_dataset(robotics_points_path, query_mode='strided', resolution=(256, 256)):
@@ -241,7 +265,7 @@ def _upload(a, dtype, dev):
   return torch.from_numpy(np.ascontiguousarray(a, dtype)).pin_memory().to(dev, non_blocking=True)
 
 
-def evaluate(model, dataset, query_mode='strided'):
+def evaluate(model, dataset, query_mode='strided', *, redetection=False, window_frames=None):
   """Runs `model(video, query_points)` on each video of a reader and its TAP-Vid metrics on the
   device; returns (mean_scalars, per_video).
 
@@ -255,26 +279,62 @@ def evaluate(model, dataset, query_mode='strided'):
   1 - (1 - sigmoid(occlusion)) (1 - sigmoid(expected_dist)) > 0.5 as occluded, which differs only
   for a visibility within one float32 ulp of 0.5.  Ground-truth tracks go to the counters as
   float32: exact at 256 x 256 for float32 pickle points (points x 256); at other sizes the float64
-  product is rounded to float32 once.  The host waits for the device once, at the end."""
+  product is rounded to float32 once.  The host waits for the device once, at the end.
+
+  redetection=True adds compute_redetection_metrics' scalar keys (AJ_RD_D{D}_dmin{d},
+  AJ_RD_dmin{d}, AJ_RD; default thresholds) to each video's dict, from the same predictions
+  (visible as above), ground-truth visibility = not occluded and the same float32 ground truth;
+  the TAP-Vid keys and the single sync are unchanged.  The reference defines no dataset mean for
+  AJ_RD, and a video without a reappearance has NaN there; so an AJ_RD key's mean is taken over
+  the videos where it is not NaN (float32, in video order, as dataset_mean), and
+  mean_scalars['<key>/videos'] counts them (NaN mean when there are none).
+
+  window_frames: None runs `model(video, query_points)`; an integer core length, or 'auto' (the
+  largest core that fits free device memory), runs windowed.windowed_forward instead, whose
+  outputs are bit for bit the whole-clip call's: for clips whose whole-clip grids would not fit."""
   _check_mode(query_mode)
-  keys, rows = None, []
+  if window_frames is not None and window_frames != 'auto' and (
+      isinstance(window_frames, bool) or not isinstance(window_frames, int) or window_frames < 1):
+    raise ValueError(f"evaluate: window_frames must be None, 'auto' or an integer >= 1, got {window_frames!r}")
+  keys, rows, events = None, [], []
   with torch.no_grad():
     for sample in dataset:
       (ex,) = sample.values()
       video = ex['video']
       dev = video.device
       qp = _upload(ex['query_points'], np.float32, dev)
-      out = model(video, qp)
-      m = metrics.compute_tapvid_metrics(
-          qp, _upload(ex['occluded'], np.uint8, dev), _upload(ex['target_points'], np.float32, dev),
-          None, out['tracks'], query_mode, pred_logits=(out['occlusion'], out['expected_dist']))
+      if window_frames is None:
+        out = model(video, qp)
+      else:
+        from tapnet_b200 import windowed  # pylint: disable=g-import-not-at-top
+        out = windowed.windowed_forward(model, video, qp, None if window_frames == 'auto' else window_frames)
+      occluded, target = _upload(ex['occluded'], np.uint8, dev), _upload(ex['target_points'], np.float32, dev)
+      logits = (out['occlusion'], out['expected_dist'])
+      m = metrics.compute_tapvid_metrics(qp, occluded, target, None, out['tracks'], query_mode,
+                                         pred_logits=logits)
       keys = keys or list(m)
       rows.append(torch.cat([m[k].reshape(1) for k in keys]))
+      if redetection:
+        ev = metrics.redetection_events(out['tracks'], None, target, occluded == 0,
+                                        metrics.DIST_THRESHOLDS, pred_logits=logits)
+        host = torch.empty(ev.shape, dtype=ev.dtype, pin_memory=True)
+        host.copy_(ev, non_blocking=True)   # stream-ordered before the table's copy below
+        events.append(host)
   if not rows:
     raise ValueError('evaluate: the dataset is empty')
   table = torch.stack([r.to(rows[0].device) for r in rows]).cpu().numpy()   # the one sync
   per_video = [{k: float(v) for k, v in zip(keys, row)} for row in table]
-  return dataset_mean(per_video), per_video
+  if not redetection:
+    return dataset_mean(per_video), per_video
+  mean = dataset_mean(per_video)
+  for m, host in zip(per_video, events):
+    m.update({k: float(v) for k, v in metrics.redetection_metrics_from_events(host.numpy(), 1).items()})
+  for k in per_video[0]:
+    if k.startswith('AJ_RD'):
+      vals = [{k: m[k]} for m in per_video if not np.isnan(m[k])]
+      mean[k] = dataset_mean(vals)[k] if vals else np.float32(np.nan)
+      mean[f'{k}/videos'] = len(vals)
+  return mean, per_video
 
 
 def dataset_mean(per_video):
@@ -303,7 +363,7 @@ def latex_table(mean_scalars):
 
 # ------------------------------------------------------------------------------ CLI
 _READERS = {'davis': create_davis_dataset, 'kinetics': create_kinetics_dataset,
-            'rgb_stacking': create_rgb_stacking_dataset}
+            'rgb_stacking': create_rgb_stacking_dataset, 'robotap': create_robotap_dataset}
 
 
 def _model_kwargs(path):
@@ -321,20 +381,35 @@ def _model_kwargs(path):
   raise ValueError(f'{path}: unexpected mixer input width {din}')
 
 
+def _window_frames(v):
+  if v == 'auto':
+    return v
+  if not v.isdigit() or int(v) < 1:
+    raise argparse.ArgumentTypeError(f"expected an integer >= 1 or 'auto', got {v!r}")
+  return int(v)
+
+
 def main(argv=None):
   p = argparse.ArgumentParser(description='TAP-Vid evaluation of a TAPIR checkpoint on the GPU')
   p.add_argument('--dataset', required=True, choices=sorted(_READERS))
-  p.add_argument('--path', required=True, help='the pickle (davis, rgb_stacking) or the shard directory (kinetics)')
+  p.add_argument('--path', required=True, help='the pickle (davis, rgb_stacking, robotap), the shard '
+                 'directory (kinetics) or a directory of pickles (robotap)')
   p.add_argument('--checkpoint', required=True, help='torch state dict (.pt) or Haiku tree (.npy)')
   p.add_argument('--query-mode', default='strided', choices=_MODES)
   p.add_argument('--resolution', type=int, nargs=2, default=(256, 256), metavar=('H', 'W'))
+  p.add_argument('--redetection', action='store_true',
+                 help='add the AJ_RD re-detection metrics and, per key, the videos its mean is over')
+  p.add_argument('--window-frames', type=_window_frames, default=None, metavar='N|auto',
+                 help='track each clip in temporal windows of N core frames (auto: fit free memory)')
   a = p.parse_args(argv)
   from tapnet_b200 import tapir_model  # pylint: disable=g-import-not-at-top
   model = tapir_model.build_model(a.checkpoint, **_model_kwargs(a.checkpoint))
   mean, per_video = evaluate(model, _READERS[a.dataset](a.path, a.query_mode, resolution=tuple(a.resolution)),
-                             a.query_mode)
+                             a.query_mode, redetection=a.redetection, window_frames=a.window_frames)
 
   def clean(v):
+    if isinstance(v, int):   # the AJ_RD means' video counts
+      return v
     return None if np.isnan(v) else float(v)
 
   print(json.dumps(dict(dataset=a.dataset, query_mode=a.query_mode, resolution=list(a.resolution),
