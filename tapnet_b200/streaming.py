@@ -9,20 +9,19 @@ a CUDA graph (fixed frame size and point count) and replays it: same kernels, sa
 bit, no per-launch host cost.  The causal state lives in static device buffers that the graph
 updates in place; `update_query` mirrors `TAPIR.update_query_features` for re-targeting a point.
 
-With `num_streams=S` one tracker follows S camera streams (same frame size, same point count): a
-step runs the backbone over the S frames in one pass and one batched estimate_trajectories over
-the S clips of one frame each (the reference's batch axis), all in one captured graph.
+With `num_streams=S` one tracker follows S camera streams with one point count.  Each stream is
+tracked as the reference tracks one camera of its frame size (`height` / `width` / `window` may be
+given per stream): the default refinement resolutions of its own size, tracks in its own pixels.
+Streams whose backbone passes agree (`tapir_model._pass_plan`) form a group; one captured graph
+runs, per group, its passes over the group's frames and one batched estimate_trajectories over its
+clips of one frame each (the reference's batch axis, with per-clip video sizes).  Streams of one
+frame size form one group whose input is one [S, 1, H, W, 3] batch, so a step is one backbone
+pass over the S frames; a group of several sizes resamples its frames in one ingest launch per
+pass, whatever their sizes.
 
 With `yuv420=True` the tracker takes `live.YUV420Frames` (NV12 / I420 camera or decoder frames):
-it keeps static Y / U / V buffers of the camera frame, a step copies the 1.5 B/px planes into them
-and replays the graph, and the crop window and colour matrix are fixed at construction.
-
-Streams of different frame sizes (`height` / `width` / `window` given per stream) are each tracked
-as the reference tracks one camera of that size: the default refinement resolutions of its own
-size, tracks in its own pixels.  Streams whose backbone passes agree (`tapir_model._pass_plan`) form
-a group; one captured graph runs, per group, its passes over the group's frames (one ingest launch
-per resampled pass, whatever the frames' sizes) and one batched estimate_trajectories with per-clip
-video sizes.
+it keeps static Y / U / V buffers of the camera frames, a step copies the 1.5 B/px planes into them
+and replays the graph, and the crop windows and colour matrix are fixed at construction.
 """
 from typing import List, NamedTuple, Optional, Sequence, Tuple, Union
 
@@ -102,7 +101,7 @@ class _Group:
     self.plan, self.streams = plan, list(streams)
     self.uniform = len({(specs[s].frame_hw, specs[s].window) for s in streams}) == 1
     sizes = [specs[s].hw for s in streams]
-    # one size: the call (and launch sequence) of a same-size tracker; else per-clip sizes
+    # one size: estimate_trajectories' one-size call and launches; else per-clip sizes
     self.video_size = sizes[0] if len(set(sizes)) == 1 else sizes
     self.frames = None   # uniform groups: the [G, 1, ...] input of get_feature_grids
     self.sources = None  # otherwise: one one-frame input per stream, resampled together
@@ -131,56 +130,22 @@ class OnlineTracker:
     if yuv420 and uint8_frames:
       raise ValueError('uint8_frames and yuv420 are exclusive')
     specs = stream_specs(height, width, num_streams, yuv420, window)
-    self._groups = None
-    if len({(sp.frame_hw, sp.window) for sp in specs}) > 1:
-      self._init_mixed(model, specs, int(num_points), uint8_frames, yuv420, matrix, full_range)
-      return
-    (height, width), window = specs[0].frame_hw, specs[0].window
     self.model = model
-    self.hw = (int(height), int(width))
+    self.specs = specs
     self.num_points = int(num_points)
-    self.num_streams = int(num_streams)
+    self.num_streams = len(specs)
     self.dev = next(model.parameters()).device
     if self.dev.type != 'cuda':
       raise RuntimeError('OnlineTracker runs on CUDA only')
     # uint8_frames: frames are raw [0, 255] camera frames (what pytorch_live_demo.py:139-141 holds
     # before preprocess_frames); the normalisation runs inside the stem conv's loads
     self._frame_dtype = torch.uint8 if uint8_frames else torch.float32
-    self._yuv = None
-    if yuv420:
-      H, W = self.hw
-      ch, cw = (H + 1) // 2, (W + 1) // 2
-      planes = [torch.zeros(self.num_streams, 1, *hw, dtype=torch.uint8, device=self.dev)
-                for hw in ((H, W), (ch, cw), (ch, cw))]
-      # the graph's input: static planes of the camera frame, fixed window and matrix
-      self._yuv = live.YUV420Frames(*planes, matrix=matrix, full_range=full_range, window=window)
-      self._frame = self._yuv
-      self.hw = tuple(self._yuv.window[2:])
-    else:
-      self._frame = torch.zeros(self.num_streams, 1, height, width, 3, dtype=self._frame_dtype,
-                                device=self.dev)
-    self._graph: Optional[torch.cuda.CUDAGraph] = None
-    self._graph_sig = None
-    self._pinned = False
-    self.query_features = None
-    self.state = None
-    self._out = None
-
-  def _init_mixed(self, model, specs, num_points, uint8_frames, yuv420, matrix, full_range):
-    """Streams of different sizes: static per-stream inputs, grouped by pass plan."""
-    self.model = model
-    self.specs = specs
-    self.hw = [sp.hw for sp in specs]
-    self.num_points = num_points
-    self.num_streams = len(specs)
-    self.dev = next(model.parameters()).device
-    if self.dev.type != 'cuda':
-      raise RuntimeError('OnlineTracker runs on CUDA only')
-    self._frame_dtype = torch.uint8 if uint8_frames else torch.float32
     self._yuv = (matrix, bool(full_range)) if yuv420 else None
-    self._frame = None
     self._groups = [_Group(plan, streams, specs)
                     for plan, streams in group_streams(specs, model.initial_resolution)]
+    # streams of one frame size (and window) are one uniform group: init / step take a batch
+    self._one_size = len(self._groups) == 1 and self._groups[0].uniform
+    self.hw = specs[0].hw if self._one_size else [sp.hw for sp in specs]
     self._slot = {}  # stream -> (group, slot)
     order = []
     for gi, g in enumerate(self._groups):
@@ -196,6 +161,8 @@ class OnlineTracker:
         order.append(s)
     # row r of the groups' concatenated outputs is stream order[r]: gather them back in the graph
     self._order = torch.tensor([order.index(s) for s in range(self.num_streams)], device=self.dev)
+    # a one-size tracker's input: its group's [S, 1, ...] buffer, into which a step copies the batch
+    self._frame = self._groups[0].frames if self._one_size else None
     self._graph = None
     self._graph_sig = None
     self._pinned = False
@@ -266,28 +233,43 @@ class OnlineTracker:
     else:
       dst.copy_(src)
 
-  def _init_groups(self, frames, query_points):
-    qp = query_points.to(self.dev, torch.float32)
-    if qp.dim() != 3 or qp.shape[0] != self.num_streams or qp.shape[2] != 3:
-      raise ValueError(f'query_points must be [{self.num_streams}, N, 3], got {tuple(qp.shape)}')
-    if qp.shape[1] != self.num_points:
-      raise ValueError(f'expected {self.num_points} query points, got {qp.shape[1]}')
-    frames = [self._device_frame(f) for f in frames]
-    # each stream's query features as a one-stream tracker of its size computes them
-    per_stream = [self._query_features_one(frames[s], qp[s:s + 1]) for s in range(self.num_streams)]
-    for g in self._groups:
-      qfs = [per_stream[s] for s in g.streams]
-      g.query_features = tapir_model.QueryFeatures(
-          tuple(torch.cat([q.lowres[i] for q in qfs]) for i in range(len(qfs[0].lowres))),
-          tuple(torch.cat([q.hires[i] for q in qfs]) for i in range(len(qfs[0].hires))),
-          qfs[0].resolutions)
-      init = self.model.construct_initial_causal_state(self.num_points, len(g.plan) - 1)
-      g.state = [{k: v.to(self.dev).expand(len(g.streams), *v.shape[1:]).clone()
-                  for k, v in d.items()} for d in init]
-    self.query_features = [g.query_features for g in self._groups]
-    self.state = [g.state for g in self._groups]
-    self._graph = None
-    return self.query_features
+  def _frames(self, frames):
+    """init / step input, all checked before any copy.  A one-size tracker takes one batch:
+    [S, H, W, 3], [S, 1, H, W, 3] or, when S = 1, [H, W, 3], returned as [S, 1, H, W, 3] on the
+    device; or YUV420Frames of [S, 1] frames of its frame size, window and matrix, returned as
+    they are.  Other trackers take a list of the streams' frames (`_stream_frames`)."""
+    if not self._one_size:
+      return self._stream_frames(frames, range(self.num_streams))
+    S = self.num_streams
+    if self._yuv is not None:
+      if not isinstance(frames, live.YUV420Frames):
+        raise ValueError('this tracker was built with yuv420=True: pass live.YUV420Frames')
+      ref = self._frame
+      if frames.frame_size != ref.frame_size:
+        raise ValueError(f'frame size {frames.frame_size} != {ref.frame_size}')
+      if (frames.window, frames.matrix, frames.full_range) != (ref.window, ref.matrix,
+                                                               ref.full_range):
+        raise ValueError(f'frames have window {frames.window}, {frames.matrix}, full_range='
+                         f'{frames.full_range}; the tracker was built for {ref.window}, '
+                         f'{ref.matrix}, full_range={ref.full_range}')
+      if frames.device != self.dev:
+        raise ValueError(f'frames on {frames.device}, tracker on {self.dev}')
+      if tuple(frames.y.shape[:2]) != (S, 1):
+        raise ValueError(f'expected YUV420Frames of [{S}, 1] frames, got '
+                         f'{list(frames.y.shape[:2])}')
+      return frames
+    frames = frames.to(self.dev, self._frame_dtype, non_blocking=True)
+    if frames.dim() == 3:
+      frames = frames[None, None]
+    elif frames.dim() == 4:
+      frames = frames[:, None]
+    if frames.dim() != 5 or frames.shape[1] != 1 or frames.shape[4] != 3:
+      raise ValueError(f'frames must be [S, H, W, 3], got {tuple(frames.shape)}')
+    if frames.shape[0] != S:
+      raise ValueError(f'expected {S} frames (one per stream), got {frames.shape[0]}')
+    if tuple(frames.shape[2:4]) != self.hw:
+      raise ValueError(f'frame size {tuple(frames.shape[2:4])} != {self.hw}')
+    return frames
 
   def _device_frame(self, f):
     return f if isinstance(f, live.YUV420Frames) else f.to(self.dev, self._frame_dtype)
@@ -295,11 +277,6 @@ class OnlineTracker:
   def _query_features_one(self, frame, qp):
     grids = self.model.get_feature_grids(frame, False)
     return self.model.get_query_features(frame, False, qp, grids)
-
-  def _state_dicts(self):
-    if self._groups is None:
-      return self.state
-    return [d for g in self._groups for d in g.state]
 
   def _group_grids(self, g):
     if g.uniform:
@@ -321,9 +298,7 @@ class OnlineTracker:
     """frames: [S, H, W, 3] (or [S, 1, H, W, 3]; [H, W, 3] when S = 1) float in [-1, 1];
     query_points [S, N, 3] ([N, 3] when S = 1) as (t, y, x), stream s's on its frame s.  With
     per-stream sizes, frames is a list of the S streams' frames."""
-    if self._groups is not None:
-      return self._init_groups(self._stream_frames(frames, range(self.num_streams)), query_points)
-    frame = self._as_frames(frames)
+    frames = self._frames(frames)
     qp = query_points.to(self.dev, torch.float32)
     if qp.dim() == 2:
       qp = qp[None]
@@ -331,79 +306,47 @@ class OnlineTracker:
       raise ValueError(f'query_points must be [{self.num_streams}, N, 3], got {tuple(qp.shape)}')
     if qp.shape[1] != self.num_points:
       raise ValueError(f'expected {self.num_points} query points, got {qp.shape[1]}')
-    grids = self.model.get_feature_grids(frame, False)
-    qf = self.model.get_query_features(frame, False, qp, grids)
-    # private copies: the graph reads these exact buffers on every replay
-    self.query_features = tapir_model.QueryFeatures(
-        tuple(t.clone() for t in qf.lowres), tuple(t.clone() for t in qf.hires), qf.resolutions)
-    n_res = len(qf.resolutions) - 1
-    init = self.model.construct_initial_causal_state(self.num_points, n_res)
-    # [S, N, 2, 512 | 2048] per block, one tensor per refinement iteration
-    self.state = [{k: v.to(self.dev).expand(self.num_streams, *v.shape[1:]).clone()
-                   for k, v in d.items()} for d in init]
+    # A one-size tracker's features are online_model_init's on its batch: one call over the S
+    # frames.  Other trackers compute each stream's as a one-stream tracker of its size does; the
+    # two differ in the last bits, as the library splits K for one-frame backbone chunks.
+    if self._one_size:
+      per_group = [[self._query_features_one(frames, qp)]]
+    else:
+      frames = [self._device_frame(f) for f in frames]
+      per_stream = [self._query_features_one(frames[s], qp[s:s + 1]) for s in range(self.num_streams)]
+      per_group = [[per_stream[s] for s in g.streams] for g in self._groups]
+    for g, qfs in zip(self._groups, per_group):
+      # private copies: the graph reads these exact buffers on every replay
+      g.query_features = tapir_model.QueryFeatures(
+          tuple(torch.cat([q.lowres[i] for q in qfs]) for i in range(len(qfs[0].lowres))),
+          tuple(torch.cat([q.hires[i] for q in qfs]) for i in range(len(qfs[0].hires))),
+          qfs[0].resolutions)
+      init = self.model.construct_initial_causal_state(self.num_points, len(g.plan) - 1)
+      # [G, N, 2, 512 | 2048] per block, one tensor per refinement iteration
+      g.state = [{k: v.to(self.dev).expand(len(g.streams), *v.shape[1:]).clone()
+                  for k, v in d.items()} for d in init]
+    if self._one_size:
+      self.query_features, self.state = self._groups[0].query_features, self._groups[0].state
+    else:
+      self.query_features = [g.query_features for g in self._groups]
+      self.state = [g.state for g in self._groups]
     self._graph = None
     return self.query_features
 
-  def _as_frames(self, frames, num=None):
-    """[num, 1, H, W, 3] on the device from [num, H, W, 3], [num, 1, H, W, 3] or, for one
-    frame, [H, W, 3].  YUV trackers: YUV420Frames [num, 1, ...] of the camera frame size, in the
-    tracker's window and matrix, returned as they are."""
-    num = self.num_streams if num is None else num
-    if self._yuv is not None:
-      return self._check_yuv(frames, num)
-    frames = frames.to(self.dev, self._frame_dtype, non_blocking=True)
-    if frames.dim() == 3:
-      frames = frames[None, None]
-    elif frames.dim() == 4:
-      frames = frames[:, None]
-    if frames.dim() != 5 or frames.shape[1] != 1 or frames.shape[4] != 3:
-      raise ValueError(f'frames must be [S, H, W, 3], got {tuple(frames.shape)}')
-    if frames.shape[0] != num:
-      raise ValueError(f'expected {num} frames (one per stream), got {frames.shape[0]}')
-    if tuple(frames.shape[2:4]) != self.hw:
-      raise ValueError(f'frame size {tuple(frames.shape[2:4])} != {self.hw}')
-    return frames
-
-  def _check_yuv(self, frames, num):
-    if not isinstance(frames, live.YUV420Frames):
-      raise ValueError('this tracker was built with yuv420=True: pass live.YUV420Frames')
-    ref = self._yuv
-    if frames.frame_size != ref.frame_size:
-      raise ValueError(f'frame size {frames.frame_size} != {ref.frame_size}')
-    if (frames.window, frames.matrix, frames.full_range) != (ref.window, ref.matrix,
-                                                             ref.full_range):
-      raise ValueError(f'frames have window {frames.window}, {frames.matrix}, full_range='
-                       f'{frames.full_range}; the tracker was built for {ref.window}, '
-                       f'{ref.matrix}, full_range={ref.full_range}')
-    if frames.device != self.dev:
-      raise ValueError(f'frames on {frames.device}, tracker on {self.dev}')
-    if tuple(frames.y.shape[:2]) != (num, 1):
-      raise ValueError(f'expected YUV420Frames of [{num}, 1] frames, got '
-                       f'{list(frames.y.shape[:2])}')
-    return frames
-
   def _step_eager(self):
-    if self._groups is not None:
-      # per group: its passes and one batched estimate_trajectories; outputs back in stream order
-      outs = [self._step_group(g, g.state) for g in self._groups]
+    outs = [self._step_group(g, g.state) for g in self._groups]
+    if len(outs) == 1:  # one group holds the streams in order
+      tracks, occ, expd = outs[0]
+    else:  # the groups' outputs back in stream order
       tracks, occ, expd = (torch.cat([o[i] for o in outs]).index_select(0, self._order)
                            for i in range(3))
-      return tracks, live.postprocess_occlusions(occ, expd), occ, expd
-    # all streams in one backbone pass and one batched estimate_trajectories (B = S, T = 1)
-    grids = self.model.get_feature_grids(self._frame, False)
-    # single-frame step: the causal state is updated in place (causal_context_out = state)
-    r = self.model.estimate_trajectories(self.hw, False, grids, self.query_features, None, 64,
-                                         causal_context=self.state, get_causal_context=True,
-                                         causal_context_out=self.state)
-    tracks = r['tracks'][-1]
-    occ, expd = r['occlusion'][-1], r['expected_dist'][-1]
     visibles = live.postprocess_occlusions(occ, expd)  # pytorch_live_demo.py:57-59
     return tracks, visibles, occ, expd
 
   def _capture(self):
     # warm-up on a side stream (allocates workspaces, packs weights, fills the constant cache);
     # the state is saved and restored so that warm-up steps do not advance it
-    state = self._state_dicts()
+    state = [d for g in self._groups for d in g.state]
     saved = [{k: v.clone() for k, v in d.items()} for d in state]
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -456,17 +399,13 @@ class OnlineTracker:
     list of the S streams' frames and each stream's tracks are in its own pixels."""
     if self.query_features is None:
       raise RuntimeError('call init(frame, query_points) first')
-    if self._groups is not None:
-      frames = self._stream_frames(frames, range(self.num_streams))
+    frames = self._frames(frames)
+    if self._one_size:  # one copy of the batch (three for YUV planes)
+      self._copy_in(frames, self._frame)
+    else:
       for g in self._groups:
         for s, dst in zip(g.streams, g.sources):
           self._copy_in(frames[s], dst)
-    elif self._yuv is not None:
-      src = self._as_frames(frames)
-      for dst, plane in zip((self._yuv.y, self._yuv.u, self._yuv.v), (src.y, src.u, src.v)):
-        dst.copy_(plane)
-    else:
-      self._frame.copy_(self._as_frames(frames))
     if self._graph is not None and self._graph_sig != self._model_sig():
       self._graph = None  # stale pointers: the model's buffers or weights changed since capture
     if self._graph is None:
@@ -490,25 +429,13 @@ class OnlineTracker:
       raise ValueError(f'stream {stream} out of range [0, {self.num_streams})')
     if not 0 <= idx < self.num_points:
       raise ValueError(f'point {idx} out of range [0, {self.num_points})')
-    if self._groups is not None:
-      frame = self._device_frame(self._stream_frames([frame], [stream])[0])
-      new = self._query_features_one(frame, query_point.to(self.dev, torch.float32).reshape(1, 1, 3))
-      gi, slot = self._slot[stream]
-      g = self._groups[gi]
-      for dst, src in zip(g.query_features.lowres + g.query_features.hires, new.lowres + new.hires):
-        dst[slot, idx] = src[0, 0]
-      for d in g.state:
-        for v in d.values():
-          v[slot, idx] = 0
-      return
-    frame = self._as_frames(frame, num=1)
-    qp = query_point.to(self.dev, torch.float32).reshape(1, 1, 3)
-    grids = self.model.get_feature_grids(frame, False)
-    new = self.model.get_query_features(frame, False, qp, grids)
-    # TAPIR.update_query_features writes [:, idx] of every stream; only [stream, idx] changes here
-    for dst, src in zip(self.query_features.lowres + self.query_features.hires,
-                        new.lowres + new.hires):
-      dst[stream, idx] = src[0, 0]
-    for d in self.state:
+    frame = self._device_frame(self._stream_frames([frame], [stream])[0])
+    new = self._query_features_one(frame, query_point.to(self.dev, torch.float32).reshape(1, 1, 3))
+    gi, slot = self._slot[stream]
+    g = self._groups[gi]
+    # TAPIR.update_query_features writes [:, idx] of every stream; only [slot, idx] changes here
+    for dst, src in zip(g.query_features.lowres + g.query_features.hires, new.lowres + new.hires):
+      dst[slot, idx] = src[0, 0]
+    for d in g.state:
       for v in d.values():
-        v[stream, idx] = 0
+        v[slot, idx] = 0
