@@ -131,9 +131,10 @@ def main():
   q = queries(N, T, S, S, dev, seed=4)
   shape = (1, T, S, S)
   C = windowed.choose_window_frames(model, shape, N, windowed._free_device_bytes(dev), None, True, 1)
-  grids_whole = sum(st.h * st.w * 48 for st in tapir_model._pass_plan((S, S), (256, 256)) if st.new) * T
+  plan = tapir_model._pass_plan((S, S), model.initial_resolution)
+  grids_whole = sum(st.h * st.w * 48 for st in plan if st.new) * T
   with torch.no_grad():
-    _, pre_ms, _ = timed(lambda: windowed._query_features(model, model._pack(), host, 0, 1, q[0], None, 64, dev))
+    _, pre_ms, _ = timed(lambda: windowed._query_features(model, model._pack(), host, 0, 1, q[0], plan, 64, dev))
     out, total_ms, p = timed(lambda: windowed.windowed_forward(model, host, q, window_frames=C))
   finite = bool(torch.isfinite(out['tracks']).all())
   print(json.dumps(dict(config='long', frames=T, size=[S, S], points=N, host_pinned_uint8=True,

@@ -348,6 +348,11 @@ def split_planes(src, dst):
                                   src.shape[1], kpad, P, stream()), fn)
 
 
+def padded_k(k):
+  """A GEMM operand's K rounded up to whole 64-wide k-blocks: the width its bf16 planes have."""
+  return (k + 63) // 64 * 64
+
+
 def pack_weights(sd, planes, extra_convs, device):
   """The backbone, head and mixer weight structs of state dict `sd` with `planes` bf16 planes:
   dict(backbone, head, mixer, keep, mixer_in, num_blocks), `keep` holding what they point into."""
@@ -359,7 +364,7 @@ def pack_weights(sd, planes, extra_convs, device):
 
   def linear(w2d, bias=None):
     n, k = w2d.shape
-    kp = (k + 63) // 64 * 64
+    kp = padded_k(k)
     keep.append(torch.empty(planes, n, kp, dtype=torch.bfloat16, device=device))
     split_planes(w2d.to(device=device, dtype=torch.float32).contiguous(), keep[-1])
     return Linear(w=keep[-1].data_ptr(), bias=f32(bias) if bias is not None else None, N=n, K=kp,
@@ -491,9 +496,8 @@ def yuv420_to_rgb(frames, out):
 
 
 # ------------------------------------------------------------------------------ backbone
-def backbone_workspace_bytes(weights, frames, h, w):
-  return load().tapir_backbone_workspace_bytes(frames, h, w, int(weights.num_extra > 0),
-                                               weights.planes)
+def backbone_workspace_bytes(frames, h, w, extra_convs, planes):
+  return load().tapir_backbone_workspace_bytes(frames, h, w, int(extra_convs), planes)
 
 
 def backbone_stem(weights, frames, pass_frames, pass_frame0, workspace):
@@ -561,7 +565,9 @@ def pool_pyramid(grid, out):
 
 
 def cost_volume_workspace_bytes(qfeat, grid):
-  return load().tapir_cost_volume_batched_workspace_bytes(*qfeat.shape[:2], *grid.shape[1:])
+  """cost_volume_tracks' workspace for qfeat [G, n, C], grid [G, T, gh, gw, C] (or their shapes)."""
+  G, n = getattr(qfeat, 'shape', qfeat)[:2]
+  return load().tapir_cost_volume_batched_workspace_bytes(G, n, *getattr(grid, 'shape', grid)[1:])
 
 
 def cost_volume_tracks(head, qfeat, grid, query_tyx, temperature, init_hw, points, occ, expd,
@@ -631,7 +637,9 @@ def local_corr(*args):
 
 
 def mixer_workspace_bytes(x_planes):
-  return load().tapir_mixer_workspace_bytes(x_planes.shape[1], x_planes.shape[0])
+  """mixer_forward's workspace for x_planes [P, rows, ldx] (or its shape)."""
+  P, rows = getattr(x_planes, 'shape', x_planes)[:2]
+  return load().tapir_mixer_workspace_bytes(rows, P)
 
 
 def _ctx_array(fn, name, ctx, nb, n, width, dev):
@@ -799,10 +807,14 @@ def redetection_events(gt_visible, pred_visible, pred_tracks, gt_tracks, thresho
   check(load().tapir_redetection_events(byref(args), stream()), fn)
 
 
+def paint_point_track_workspace_bytes(T, N):
+  return int(load().tapir_paint_point_track_workspace_bytes(T, N))
+
+
 def paint_point_track(frames, tracks, visibles, colors, out, workspace):
   """Paints tracks [N, T, 2] (x, y; float32 or float64) where visibles [N, T] (bool) onto uint8
   frames [T, H, W, 3] -> out, with colors uint8 [N, 3].  workspace: uint8, at least
-  tapir_paint_point_track_workspace_bytes(T, N) bytes."""
+  paint_point_track_workspace_bytes(T, N) bytes."""
   fn = 'tapir_paint_point_track'
   _check(fn, 'frames', frames, torch.uint8)
   (T, H, W, _), N, dev = frames.shape, tracks.shape[0], frames.device
@@ -831,10 +843,14 @@ def lanczos_weights(in_size, out_size):
   return bounds, taps
 
 
+def resize_lanczos_u8_workspace_bytes(T, H, W, h, w):
+  return int(load().tapir_resize_lanczos_u8_workspace_bytes(T, H, W, h, w))
+
+
 def resize_lanczos_u8(src, dst, x_tables, y_tables, workspace):
   """uint8 src [..., H, W, 3] -> dst [..., h, w, 3] with PIL's Lanczos.  x_tables / y_tables:
   (bounds, taps) int32 device tensors of lanczos_weights(W, w) / (H, h), or None for an axis that
-  keeps its size; workspace: uint8, at least tapir_resize_lanczos_u8_workspace_bytes."""
+  keeps its size; workspace: uint8, at least resize_lanczos_u8_workspace_bytes."""
   fn = 'tapir_resize_lanczos_u8'
   _frames(fn, src, (torch.uint8,))
   _check(fn, 'dst', dst, torch.uint8, device=src.device)

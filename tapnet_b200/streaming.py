@@ -369,21 +369,16 @@ class OnlineTracker:
     # remember which buffers / weights the capture saw: step() re-captures when another caller
     # of the same model (a larger offline clip, a second tracker, load_state_dict) replaced them.
     if not self._pinned:
-      self.model._ws_pins += 1
+      self.model._pin_workspaces()
       self._pinned = True
-    self._graph_sig = self._model_sig()
-
-  def _model_sig(self):
-    return (self.model._ws_generation, self.model._param_sig())
+    self._graph_sig = self.model._workspace_sig()
 
   def close(self):
     """Drops the graph and releases the workspace pin."""
     self._graph = None
     if self._pinned:
-      self.model._ws_pins -= 1
+      self.model._unpin_workspaces()
       self._pinned = False
-      if self.model._ws_pins == 0:
-        self.model._ws_retired.clear()
 
   def __del__(self):
     try:
@@ -406,7 +401,7 @@ class OnlineTracker:
       for g in self._groups:
         for s, dst in zip(g.streams, g.sources):
           self._copy_in(frames[s], dst)
-    if self._graph is not None and self._graph_sig != self._model_sig():
+    if self._graph is not None and self._graph_sig != self.model._workspace_sig():
       self._graph = None  # stale pointers: the model's buffers or weights changed since capture
     if self._graph is None:
       self._capture()

@@ -125,6 +125,38 @@ _MAX_BACKBONE_PIXELS = 96 * 256 * 256
 _H2D_SUBCHUNKS = 6
 
 
+def _backbone_chunk(h, w, frames):
+  """Frames per chunk of a backbone pass over `frames` frames of h x w: it bounds the workspace, as
+  the reference's feature_extractor_chunk_size (:346-360) does, and decides bits, as the ExtraConv
+  GEMMs split K (and so sum in another order) for one-frame chunks only."""
+  return min(max(1, _MAX_BACKBONE_PIXELS // (h * w)), frames)
+
+
+def _grid_shapes(h, w):
+  """Per-frame shapes of the (lowres, hires) feature grids of an h x w backbone pass."""
+  return (h // 8, w // 8, schema.LOWRES_DIM), (h // 4, w // 4, schema.HIRES_DIM)
+
+
+def _backbone_frames(video):
+  """A clip as the backbone reads it: contiguous, uint8 kept, any other dtype as float32."""
+  return video.contiguous() if video.dtype == torch.uint8 else video.to(torch.float32).contiguous()
+
+
+def _stage_a_scratch(G, n, T, grid_shape):
+  """Stage A of G clips, n queries, T frames of grid_shape lowres grids: the shapes of its float32
+  occlusion, expected distance, tracks, positions and positions scaled on their way to the tracks,
+  and the bytes of its cost-volume workspace."""
+  return (((G, n, T),) * 2 + ((G, n, T, 2),) * 3,
+          _lib.cost_volume_workspace_bytes((G, n), (G, T, *grid_shape)))
+
+
+def _new_estimates(count, G, n, T, dev):
+  """`count` estimates of G clips' n queries over T frames as three lists: occlusion [G, n, T],
+  expected distance [G, n, T] and tracks [G, n, T, 2]."""
+  return tuple([torch.empty(s, dtype=torch.float32, device=dev) for _ in range(count)]
+               for s in ((G, n, T), (G, n, T), (G, n, T, 2)))
+
+
 def _groups(B, N, T):
   """Work groups of estimate_trajectories as (b0, b1, query slice): whole clips b0..b1-1 with all
   their queries while the group's rows (clips x queries x frames) fit _MAX_ROWS_PER_CHUNK and its
@@ -297,9 +329,9 @@ class TAPIR(nn.Module):
 
   def _workspace(self, name, nbytes, dev):
     """Grow-only scratch.  A buffer that is outgrown is parked in `_ws_retired` instead of
-    being freed while `_ws_pins` > 0: a captured CUDA graph (streaming.OnlineTracker) holds raw
-    pointers into it.  `_ws_generation` changes whenever a buffer is replaced, so graph owners
-    can tell that their capture no longer describes the model's current buffers."""
+    being freed while pinned: a captured CUDA graph (streaming.OnlineTracker) holds raw pointers
+    into it.  `_ws_generation` changes whenever a buffer is replaced, so graph owners can tell
+    (_workspace_sig) that their capture no longer describes the model's current buffers."""
     ws = self._ws.get(name)
     if ws is None or ws.numel() < nbytes or ws.device != dev:
       if ws is not None and self._ws_pins > 0:
@@ -308,6 +340,20 @@ class TAPIR(nn.Module):
       self._ws[name] = ws
       self._ws_generation += 1
     return ws
+
+  def _pin_workspaces(self):
+    """Taken by a captured graph's holder: while pinned, outgrown workspaces are parked."""
+    self._ws_pins += 1
+
+  def _unpin_workspaces(self):
+    """Releases one pin; the last pin to go frees the parked workspaces."""
+    self._ws_pins -= 1
+    if self._ws_pins == 0:
+      self._ws_retired.clear()
+
+  def _workspace_sig(self):
+    """What a captured graph's raw pointers depend on: the workspaces and the packed weights."""
+    return self._ws_generation, self._param_sig()
 
   # ------------------------------------------------------------------ weight packing
   @_on_model_device
@@ -380,7 +426,7 @@ class TAPIR(nn.Module):
     # loads; a resized pass converts each bilinear tap in the ingest kernel.  Bit for bit the
     # results of the uint8 RGB frames the conversion produces.
     if not isinstance(video, live.YUV420Frames):
-      video = video.contiguous() if video.dtype == torch.uint8 else video.to(torch.float32).contiguous()
+      video = _backbone_frames(video)
     n, f, vh, vw, _ = video.shape
     host_src = None
     if host_video:
@@ -439,26 +485,20 @@ class TAPIR(nn.Module):
     out: None, or the contiguous (lowres, hires) tensors to write the grids into."""
     n, f, h, w, _ = frames.shape
     nf = n * f
-    lo_shape = (n, f, h // 8, w // 8, self.lowres_dim)
-    hi_shape = (n, f, h // 4, w // 4, self.highres_dim)
+    shapes = [(n, f) + s for s in _grid_shapes(h, w)]
     if out is None:
-      latent = torch.empty(lo_shape, dtype=torch.float32, device=dev)
-      hires = torch.empty(hi_shape, dtype=torch.float32, device=dev)
+      out = [torch.empty(s, dtype=torch.float32, device=dev) for s in shapes]
     else:
-      latent, hires = out
-      for name, t, shape in (('lowres', latent, lo_shape), ('hires', hires, hi_shape)):
+      for name, t, shape in zip(('lowres', 'hires'), out, shapes):
         if (t.shape != shape or t.dtype != torch.float32 or t.device != dev
             or not t.is_contiguous()):
           raise ValueError(f'grids_out {name} must be a contiguous float32 {list(shape)} tensor '
                            f'on {dev}, got {t.dtype} {tuple(t.shape)} on {t.device}')
+    latent, hires = out
     src = frames if isinstance(frames, live.YUV420Frames) else frames.view(nf, h, w, 3)
-    flat_lo = latent.view(nf, h // 8, w // 8, self.lowres_dim)
-    flat_hi = hires.view(nf, h // 4, w // 4, self.highres_dim)
-    # frames are independent in the backbone (InstanceNorm per frame, LayerNorm per
-    # pixel), so the frame-chunk size only bounds the workspace; the reference's
-    # feature_extractor_chunk_size (:346-360) has the same role.
-    chunk = min(max(1, _MAX_BACKBONE_PIXELS // (h * w)), nf)
-    ws = self._workspace('backbone', _lib.backbone_workspace_bytes(pk['backbone'], chunk, h, w), dev)
+    flat_lo, flat_hi = (t.view(nf, *s[2:]) for t, s in zip(out, shapes))
+    chunk = _backbone_chunk(h, w, nf)
+    ws = self._workspace('backbone', self._backbone_workspace_bytes(nf, h, w), dev)
     ev = None
     if hires_ready_events is not None:
       ev = torch.cuda.Event()
@@ -488,6 +528,11 @@ class TAPIR(nn.Module):
       _lib.backbone_forward(pk['backbone'], src, flat_lo[s0:s0 + c], flat_hi[s0:s0 + c], ws,
                             ev if s0 + c >= nf else None, frame0=s0, stem_done=streamed)
     return latent, hires
+
+  def _backbone_workspace_bytes(self, frames, h, w):
+    """Workspace bytes of a backbone pass over `frames` frames of h x w."""
+    return _lib.backbone_workspace_bytes(_backbone_chunk(h, w, frames), h, w, self._has_extra,
+                                         self._planes)
 
   @_on_model_device
   def get_query_features(
@@ -569,12 +614,7 @@ class TAPIR(nn.Module):
       # [B, 2] (h, w): the track update's table; the stage-A scalings broadcast per clip
       video_table = self._const([v for hw in per_clip for v in hw], dev, torch.int32).view(B, 2)
 
-    def new(*shape, dtype=torch.float32):
-      return torch.empty(*shape, dtype=dtype, device=dev)
-
-    occ_out = [new(B, N, T) for _ in range(num_iters + 1)]
-    expd_out = [new(B, N, T) for _ in range(num_iters + 1)]
-    trk_out = [new(B, N, T, 2) for _ in range(num_iters + 1)]
+    occ_out, expd_out, trk_out = _new_estimates(num_iters + 1, B, N, T, dev)
     new_ctx = self._new_causal_context(causal_context, get_causal_context, causal_context_out,
                                        num_iters, nb, B, N, T, dev)
     write_ctx = get_causal_context and causal_context is not None
@@ -591,19 +631,9 @@ class TAPIR(nn.Module):
       return out
 
     # pooled pyramid levels: once per resolution level over all B*T frames (the reference
-    # recomputes them every iteration of every chunk, tapir_model.py:519-527); each is the 2x2
-    # average of the one before it
-    pooled = {}
-    for level in range(1, num_levels_total):
-      g = feature_grids.lowres[level].contiguous()
-      outs = []
-      for _ in range(self.pyramid_level):
-        _, t, gh, gw, c = g.shape
-        pooled_g = new(B, t, gh // 2, gw // 2, c)
-        _lib.pool_pyramid(g, pooled_g)
-        outs.append(pooled_g)
-        g = pooled_g
-      pooled[level] = outs
+    # recomputes them every iteration of every chunk, tapir_model.py:519-527)
+    pooled = {level: self._pool_pyramid(feature_grids.lowres[level].contiguous())
+              for level in range(1, num_levels_total)}
 
     for b0, b1, sl in _groups(B, N, T):
       bs = slice(b0, b1)
@@ -617,14 +647,10 @@ class TAPIR(nn.Module):
                           trk_out[0][bs, sl], am_out[bs, sl] if am_out is not None else None, dev)
 
       # ---- refinement iterations, one level at a time
-      bufs = self._refine_buffers(pk, nq, T, dev)
+      bufs = self._refine_buffers(nq, T, dev)
       npi = self.num_pips_iter
       for level in range(1, num_levels_total):
         its = range((level - 1) * npi, level * npi)
-        levels = ([feature_grids.hires[level][bs].contiguous(),
-                   feature_grids.lowres[level][bs].contiguous()] + [g[bs] for g in pooled[level]])
-        qfeat = tuple(q[bs, sl].contiguous()
-                      for q in (query_features.hires[level], query_features.lowres[level]))
         ctxs = []
         for it in its:
           ctx = [None] * 4
@@ -636,7 +662,9 @@ class TAPIR(nn.Module):
           ctxs.append(ctx)
         outs = [(occ_out[it + 1][bs, sl], expd_out[it + 1][bs, sl], trk_out[it + 1][bs, sl])
                 for it in its]
-        self._refine_level(pk, levels, qfeat, pos, occ0, expd0, outs, bufs,
+        self._refine_level(pk, feature_grids.hires[level][bs], feature_grids.lowres[level][bs],
+                           [g[bs] for g in pooled[level]], query_features.hires[level][bs, sl],
+                           query_features.lowres[level][bs, sl], pos, occ0, expd0, outs, bufs,
                            feature_grids.resolutions[level],
                            video_hw if video_table is None else video_table[bs], ctxs)
     return out
@@ -699,31 +727,52 @@ class TAPIR(nn.Module):
       qp = query_points.to(torch.float32)
       # utils.convert_grid_coordinates (coords * out / in), tapir_model.py:488-493
       qp = (qp * self._const([T, ih, iw], dev) / to_init).contiguous()
-    pos = torch.empty(G, n, T, 2, dtype=torch.float32, device=dev)
-    ws = self._workspace('cost_volume', _lib.cost_volume_workspace_bytes(qfeat, grid), dev)
+    shapes, ws_bytes = _stage_a_scratch(G, n, T, grid.shape[2:])
+    pos = torch.empty(shapes[3], dtype=torch.float32, device=dev)
+    ws = self._workspace('cost_volume', ws_bytes, dev)
     _lib.cost_volume_tracks(pk['head'], qfeat, grid, qp, self.softmax_temperature, (ih, iw), pos,
                             occ, expd, argmax, ws)
     # train2orig (tapir_model.py:435-441)
     torch.div(pos * to_video, self._const([iw, ih], dev), out=tracks)
     return pos
 
-  def _refine_buffers(self, pk, nq, T, dev):
-    """Scratch of the refinement of nq queries over T frames: (x_planes, res, feats, mixer
-    workspace)."""
-    x_planes = torch.empty(self._planes, nq * T, pk['mixer_in'], dtype=torch.bfloat16, device=dev)
-    res = torch.empty(nq, T, 388, dtype=torch.float32, device=dev)
-    feats = [torch.empty(nq, T, 384, dtype=torch.float32, device=dev) for _ in range(2)]
-    return x_planes, res, feats, self._workspace('mixer', _lib.mixer_workspace_bytes(x_planes), dev)
+  def _refine_scratch(self, nq, T):
+    """The refinement of nq queries over T frames: the (shape, dtype) of the mixer's input planes,
+    its output rows and the two feature buffers the iterations alternate between, and the bytes of
+    the mixer workspace."""
+    x_planes = (self._planes, nq * T, _lib.padded_k(schema.mixer_input_dim(self.pyramid_level)))
+    f32 = torch.float32
+    return ([(x_planes, torch.bfloat16), ((nq, T, schema.mixer_output_dim()), f32)]
+            + [((nq, T, schema.HIRES_DIM + schema.LOWRES_DIM), f32)] * 2,
+            _lib.mixer_workspace_bytes(x_planes))
 
-  def _refine_level(self, pk, levels, qfeat, pos, occ0, expd0, outs, bufs, resize_hw, video_hw,
-                    ctxs=None):
+  def _refine_buffers(self, nq, T, dev):
+    """The _refine_scratch of nq queries over T frames: (x_planes, res, feats, mixer workspace)."""
+    specs, ws_bytes = self._refine_scratch(nq, T)
+    x_planes, res, *feats = (torch.empty(s, dtype=d, device=dev) for s, d in specs)
+    return x_planes, res, feats, self._workspace('mixer', ws_bytes, dev)
+
+  def _pool_pyramid(self, grid):
+    """The pooled levels of lowres grids [..., h, w, C], each the 2 x 2 mean of the one before."""
+    pooled = []
+    for _ in range(self.pyramid_level):
+      *lead, h, w, c = grid.shape
+      pooled.append(torch.empty(*lead, h // 2, w // 2, c, dtype=torch.float32, device=grid.device))
+      _lib.pool_pyramid(grid, pooled[-1])
+      grid = pooled[-1]
+    return pooled
+
+  def _refine_level(self, pk, hires, lowres, pooled, qf_hi, qf_lo, pos, occ0, expd0, outs, bufs,
+                    resize_hw, video_hw, ctxs=None):
     """The num_pips_iter refinement iterations of one level (reference tapir_model.py:529-552)
-    for nq queries over T frames.  levels: the level's pyramid grids [G, T, h, w, C] (hires,
-    lowres, pooled); qfeat: the (hires, lowres) query features [nq, 128 | 256]; pos [..., T, 2] is
-    moved in place; occ0 / expd0: the stage-A estimates the level starts from; outs: one (occ, expd,
-    tracks) output view per iteration; bufs: _refine_buffers; ctxs: one mixer context list per
-    iteration (see _refine), or None.  Only pos carries over to the next level: features restart
-    from the query and occlusion / expected distance from stage A."""
+    for nq queries over T frames.  hires, lowres [G, T, h, w, C]: the level's grids, pooled: the
+    _pool_pyramid of lowres; qf_hi / qf_lo: the query features [..., 128 | 256] of the nq queries;
+    pos [..., T, 2] is moved in place; occ0 / expd0: the stage-A estimates the level starts from;
+    outs: one (occ, expd, tracks) output view per iteration; bufs: _refine_buffers; ctxs: one mixer
+    context list per iteration (see _refine), or None.  Only pos carries over to the next level:
+    features restart from the query and occlusion / expected distance from stage A."""
+    levels = [hires.contiguous(), lowres.contiguous()] + pooled
+    qfeat = (qf_hi.contiguous(), qf_lo.contiguous())
     x_planes, res, feats, mws = bufs
     nq, T = res.shape[:2]
     occ, expd = occ0, expd0

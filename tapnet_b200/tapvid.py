@@ -91,7 +91,7 @@ def resize_video(video, output_size):
         dev, non_blocking=True)
     out = torch.empty(T, h, w, 3, dtype=torch.uint8, device=dev)
     if T:
-      ws_bytes = int(_lib.load().tapir_resize_lanczos_u8_workspace_bytes(T, H, W, h, w))
+      ws_bytes = _lib.resize_lanczos_u8_workspace_bytes(T, H, W, h, w)
       ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if ws_bytes else None
       _lib.resize_lanczos_u8(src, out, _tables(W, w, dev) if W != w else None,
                              _tables(H, h, dev) if H != h else None, ws)

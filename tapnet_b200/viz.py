@@ -119,7 +119,7 @@ def paint_point_track(frames, point_tracks, visibles, colormap=None):
   colors_d = _to_device(colors, dev)
   out = torch.empty_like(frames_d)
   with torch.cuda.device(dev):
-    ws_bytes = int(_lib.load().tapir_paint_point_track_workspace_bytes(T, N))
+    ws_bytes = _lib.paint_point_track_workspace_bytes(T, N)
     ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)[:ws_bytes]
     _lib.paint_point_track(frames_d, tracks_d, vis_d, colors_d, out, ws)
   return out if on_device else out.cpu().numpy()

@@ -32,6 +32,7 @@ The driver, per clip:
      iteration's outputs are copied into full-length outputs.
   3. The averages over the levels' last estimates are taken once, on the full-length outputs.
 """
+import math
 from typing import List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
@@ -85,12 +86,7 @@ class Window(NamedTuple):
 def pass_levels(plan):
   """For each backbone pass of `plan` (tapir_model._pass_plan), the lowest refinement level among
   the resolutions it serves (the initial resolution, index 0, is served over level 1's range)."""
-  first, p = [], -1
-  for i, step in enumerate(plan):
-    if step.new:
-      p += 1
-      first.append(max(i, 1))
-  return first
+  return [max(i, 1) for i, step in enumerate(plan) if step.new]
 
 
 def window_plan(num_frames, window_frames, halos, plan) -> List[Window]:
@@ -139,25 +135,8 @@ def query_frames(t, num_frames):
 
 
 # ------------------------------------------------------------------------------ byte model
-def _grid_frame_bytes(h, w):
-  return 4 * ((h // 8) * (w // 8) * schema.LOWRES_DIM + (h // 4) * (w // 4) * schema.HIRES_DIM)
-
-
-def _backbone_ws_bytes(model, frames, h, w):
-  chunk = min(max(1, tapir_model._MAX_BACKBONE_PIXELS // (h * w)), max(1, frames))
-  return _lib.load().tapir_backbone_workspace_bytes(chunk, h, w, int(model._has_extra),
-                                                    model._planes)
-
-
-def _mixer_in(model):
-  k = dict(model.named_parameters())['torch_pips_mixer.linear.weight'].shape[1]
-  return (k + 63) // 64 * 64
-
-
-def _refine_bytes(model, nq, frames):
-  rows = nq * frames
-  return (model._planes * rows * _mixer_in(model) * 2 + rows * (388 + 2 * 384) * 4
-          + _lib.load().tapir_mixer_workspace_bytes(rows, model._planes))
+def _f32_bytes(shapes):
+  return 4 * sum(math.prod(s) for s in shapes)
 
 
 def output_bytes(model, video_shape, num_points, refinement_resolutions=None):
@@ -182,11 +161,12 @@ def sweep_bytes(model, video_shape, num_points, window_frames, refinement_resolu
   span = [min(T, C + left + right) for left, right in halos]
   steps = [st for st in plan if st.new]
   owners = pass_levels(plan)
-  buffers = sum(span[l - 1] * _grid_frame_bytes(st.h, st.w) for st, l in zip(steps, owners))
+  buffers = sum(span[l - 1] * _f32_bytes(tapir_model._grid_shapes(st.h, st.w))
+                for st, l in zip(steps, owners))
   backbone = 0
   for st, l in zip(steps, owners):
     new = min(T, C + halos[l - 1][1])  # the first window computes its whole right halo
-    b = _backbone_ws_bytes(model, new, st.h, st.w)
+    b = model._backbone_workspace_bytes(new, st.h, st.w)
     if not st.direct:
       b += new * st.h * st.w * 3 * 4
     if host_video or not st.direct:
@@ -194,17 +174,19 @@ def sweep_bytes(model, video_shape, num_points, window_frames, refinement_resolu
     backbone = max(backbone, b)
   # stage A: one query group over level 1's range
   T1 = span[0]
-  gh, gw = model.initial_resolution[0] // 8, model.initial_resolution[1] // 8
   nq = _group_queries(num_points, T1)
-  stage_a = (_lib.load().tapir_cost_volume_workspace_bytes(nq, T1, gh, gw, schema.LOWRES_DIM)
-             + nq * T1 * 24)
+  shapes, stage_a = tapir_model._stage_a_scratch(
+      1, nq, T1, tapir_model._grid_shapes(*model.initial_resolution)[0])
+  stage_a += _f32_bytes(shapes)
   refine = 0
   for l, (st_i, Tl) in enumerate(zip(plan[1:], span), start=1):
-    pooled = sum(Tl * (st_i.h // 8 >> j) * (st_i.w // 8 >> j) * schema.LOWRES_DIM * 4
-                 for j in range(1, model.pyramid_level + 1))
+    gh, gw, c = tapir_model._grid_shapes(st_i.h, st_i.w)[0]
+    pooled = sum(Tl * (gh >> j) * (gw >> j) * c * 4 for j in range(1, model.pyramid_level + 1))
     level_io = nq * Tl * 16 * (model.num_pips_iter + 2)  # outputs, the cut pos / occ / expd
-    refine = max(refine, pooled + level_io + _refine_bytes(model, nq, Tl))
-  return buffers + max(backbone, stage_a + nq * T1 * 8 + refine)
+    specs, mixer_ws = model._refine_scratch(nq, Tl)
+    scratch = mixer_ws + sum(math.prod(s) * d.itemsize for s, d in specs)
+    refine = max(refine, pooled + level_io + scratch)
+  return buffers + max(backbone, stage_a + refine)
 
 
 def prepass_bytes(model, video_shape, frames, refinement_resolutions=None, host_video=False,
@@ -216,8 +198,8 @@ def prepass_bytes(model, video_shape, frames, refinement_resolutions=None, host_
   work = 0
   for st in plan:
     if st.new:
-      total += frames * _grid_frame_bytes(st.h, st.w)
-      work = max(work, _backbone_ws_bytes(model, frames, st.h, st.w)
+      total += frames * _f32_bytes(tapir_model._grid_shapes(st.h, st.w))
+      work = max(work, model._backbone_workspace_bytes(frames, st.h, st.w)
                  + (0 if st.direct else frames * st.h * st.w * 3 * 4))
   return total + work
 
@@ -271,33 +253,17 @@ def _check_inputs(model, video, query_points):
   return dev
 
 
-def _stage_frames(video, a, z, dev):
-  """Frames a..z-1 of a one-clip video [1, T, H, W, 3] on the device (uint8 or float32)."""
-  x = video[:, a:z]
-  x = x if x.dtype == torch.uint8 else x.to(torch.float32)
-  return x.to(dev, non_blocking=True).contiguous()
-
-
 def _run_pass(model, pk, video, step, a, z, out, dev):
   """Backbone pass `step` over frames a..z-1 of the one-clip video into out (lowres, hires)."""
-  host = video.device.type == 'cpu'
-  if step.direct and host:
-    src = video[:, a:z]
-    src = src.contiguous() if src.dtype == torch.uint8 else src.to(torch.float32).contiguous()
-    frames = torch.empty(src.shape, dtype=src.dtype, device=dev)
-    model._backbone_pass(pk, frames, src, None, dev, out)
-    return
-  frames = _stage_frames(video, a, z, dev)
+  src = tapir_model._backbone_frames(video[:, a:z])
+  if step.direct and video.device.type == 'cpu':  # streamed in behind the stem convolution
+    return model._backbone_pass(pk, torch.empty_like(src, device=dev), src, None, dev, out)
+  frames = src.to(dev, non_blocking=True)
   if not step.direct:
     resized = torch.empty(1, z - a, step.h, step.w, 3, dtype=torch.float32, device=dev)
     _lib.resample_frames(frames, resized)
     frames = resized
   model._backbone_pass(pk, frames, None, None, dev, out)
-
-
-def _backbone_chunk(step):
-  """Frames per backbone chunk of a pass over `step`'s frame size (TAPIR._backbone_pass)."""
-  return max(1, tapir_model._MAX_BACKBONE_PIXELS // (step.h * step.w))
 
 
 def _alone_frames(step, num_clips, T, b, frames):
@@ -307,7 +273,7 @@ def _alone_frames(step, num_clips, T, b, frames):
   whole-clip call chunks the num_clips * T frames of the batch in order: every frame is alone when
   a chunk holds one frame, otherwise only the batch's last frame, when it is left over."""
   nf = num_clips * T
-  chunk = min(_backbone_chunk(step), nf)
+  chunk = tapir_model._backbone_chunk(step.h, step.w, nf)
   g = b * T + np.asarray(frames, dtype=np.int64)
   return np.full(g.shape, chunk == 1) | ((g == nf - 1) & (nf % chunk == 1))
 
@@ -318,7 +284,7 @@ def _run_frames(model, pk, video, step, out, alone, dev):
   one chunk of frames, so that the backbone never splits K for them.  A lone unmarked frame runs as
   a two-frame call of itself twice; a short last call starts earlier and recomputes a frame."""
   n = video.shape[1]
-  P = _backbone_chunk(step)
+  P = tapir_model._backbone_chunk(step.h, step.w, n)
   i = 0
   while i < n:
     if alone[i]:
@@ -342,12 +308,11 @@ def _run_frames(model, pk, video, step, out, alone, dev):
     i = j
 
 
-def _query_features(model, pk, video, b, num_clips, qp, refinement_resolutions, max_frames, dev):
-  """Query features [N, C] of clip b (video [1, T, H, W, 3]) of num_clips at every resolution
-  (lowres list, hires list), sampled from the grids of the queries' tap frames only, in chunks of at
-  most max_frames frames that keep each query's tap pair together."""
+def _query_features(model, pk, video, b, num_clips, qp, plan, max_frames, dev):
+  """Query features [N, C] of clip b (video [1, T, H, W, 3]) of num_clips at every resolution of
+  `plan` (lowres list, hires list), sampled from the grids of the queries' tap frames only, in
+  chunks of at most max_frames frames that keep each query's tap pair together."""
   T, H, W = (int(v) for v in video.shape[1:4])
-  plan = tapir_model._pass_plan((H, W), model.initial_resolution, refinement_resolutions)
   steps = [st for st in plan if st.new]
   pass_of = np.cumsum([st.new for st in plan]) - 1
   N = qp.shape[0]
@@ -369,8 +334,8 @@ def _query_features(model, pk, video, b, num_clips, qp, refinement_resolutions, 
     F = len(frame_list)
     grids = []
     for st in steps:
-      g = (torch.empty(1, F, st.h // 8, st.w // 8, schema.LOWRES_DIM, dtype=torch.float32, device=dev),
-           torch.empty(1, F, st.h // 4, st.w // 4, schema.HIRES_DIM, dtype=torch.float32, device=dev))
+      g = tuple(torch.empty((1, F) + s, dtype=torch.float32, device=dev)
+                for s in tapir_model._grid_shapes(st.h, st.w))
       _run_frames(model, pk, sub, st, g, _alone_frames(st, num_clips, T, b, frame_list), dev)
       grids.append(g)
     slot = torch.full((T,), -1, dtype=torch.int32)
@@ -443,12 +408,7 @@ def _windowed(model, video, query_points, window_frames, refinement_resolutions,
                                           host, itemsize) <= bound):
     max_frames *= 2
 
-  def new(*s):
-    return torch.empty(*s, dtype=torch.float32, device=dev)
-
-  occ_out = [new(B, N, T) for _ in range(num_iters + 1)]
-  expd_out = [new(B, N, T) for _ in range(num_iters + 1)]
-  trk_out = [new(B, N, T, 2) for _ in range(num_iters + 1)]
+  occ_out, expd_out, trk_out = tapir_model._new_estimates(num_iters + 1, B, N, T, dev)
   qp_all = query_points.to(device=dev, dtype=torch.float32)
   if N > 0 and T > 0:
     steps = [st for st in plan if st.new]
@@ -456,8 +416,7 @@ def _windowed(model, video, query_points, window_frames, refinement_resolutions,
     for b in range(B):
       clip = video[b:b + 1]
       qp = qp_all[b].contiguous()
-      qf_lo, qf_hi = _query_features(model, pk, clip, b, B, qp, refinement_resolutions,
-                                     max_frames, dev)
+      qf_lo, qf_hi = _query_features(model, pk, clip, b, B, qp, plan, max_frames, dev)
       # stage A's query frame, resolved once over the whole clip; each window sees it relative to
       # its own range, so a query outside the range matches no frame
       qframe = torch.from_numpy(query_frames(qp[:, 0].cpu().numpy(), T).astype(np.float32))
@@ -475,7 +434,6 @@ def _windowed(model, video, query_points, window_frames, refinement_resolutions,
 
 def _sweep(model, pk, clip, qp, qframe, qf_lo, qf_hi, plan, steps, pass_of, halos, C, b, B,
            outs, dev):
-  occ_out, expd_out, trk_out = outs
   T, H, W = (int(v) for v in clip.shape[1:4])
   N = qp.shape[0]
   L = len(plan) - 1
@@ -485,10 +443,8 @@ def _sweep(model, pk, clip, qp, qframe, qf_lo, qf_hi, plan, steps, pass_of, halo
   bufs = []
   for st, l in zip(steps, owners):
     cap = max(z - a for w in windows for a, z in [w.levels[l - 1]])
-    bufs.append((torch.empty(1, cap, st.h // 8, st.w // 8, schema.LOWRES_DIM,
-                             dtype=torch.float32, device=dev),
-                 torch.empty(1, cap, st.h // 4, st.w // 4, schema.HIRES_DIM,
-                             dtype=torch.float32, device=dev)))
+    bufs.append(tuple(torch.empty((1, cap) + s, dtype=torch.float32, device=dev)
+                      for s in tapir_model._grid_shapes(st.h, st.w)))
   held = [(0, 0)] * len(steps)
   for win in windows:
     # ---- slide every pass's buffer and run the backbone on the new frames only
@@ -509,33 +465,21 @@ def _sweep(model, pk, clip, qp, qframe, qf_lo, qf_hi, plan, steps, pass_of, halo
       a = held[p][0]
       return bufs[p][1 if hires else 0][:, rng[0] - a:rng[1] - a]
 
-    # pooled pyramid levels of each level's range (2 x 2 averages, one frame at a time)
-    pooled = {}
-    for l in range(1, L + 1):
-      g, outs_l = grid(l, win.levels[l - 1]), []
-      for _ in range(model.pyramid_level):
-        pg = torch.empty(g.shape[:2] + (g.shape[2] // 2, g.shape[3] // 2, g.shape[4]),
-                         dtype=torch.float32, device=dev)
-        _lib.pool_pyramid(g, pg)
-        outs_l.append(pg)
-        g = pg
-      pooled[l] = outs_l
+    # pooled pyramid levels of each level's range
+    pooled = {l: model._pool_pyramid(grid(l, win.levels[l - 1])) for l in range(1, L + 1)}
 
     a1, z1 = win.levels[0]
     T1 = z1 - a1
     core = slice(win.start, win.stop)
     for _, _, sl in tapir_model._groups(1, N, T1):
       nq = sl.stop - sl.start
-      occ0 = torch.empty(1, nq, T1, dtype=torch.float32, device=dev)
-      expd0 = torch.empty_like(occ0)
-      trk0 = torch.empty(1, nq, T1, 2, dtype=torch.float32, device=dev)
+      shapes, _ = tapir_model._stage_a_scratch(1, nq, T1, grid(0, (a1, z1)).shape[2:])
+      occ0, expd0, trk0 = (torch.empty(s, dtype=torch.float32, device=dev) for s in shapes[:3])
       qp_w = torch.cat([(qframe[sl] - a1)[:, None], qp[sl, 1:]], dim=1)[None].contiguous()
       pos = model._stage_a(pk, grid(0, (a1, z1)), qf_lo[0][sl][None].contiguous(), qp_w, (H, W),
                            occ0, expd0, trk0, None, dev)
-      cs = slice(win.start - a1, win.stop - a1)
-      occ_out[0][b, sl, core] = occ0[0, :, cs]
-      expd_out[0][b, sl, core] = expd0[0, :, cs]
-      trk_out[0][b, sl, core] = trk0[0, :, cs]
+      for full, x in zip(outs, (occ0, expd0, trk0)):
+        full[0][b, sl, core] = x[0, :, win.start - a1:win.stop - a1]
       prev = (a1, z1)
       for l in range(1, L + 1):
         al, zl = win.levels[l - 1]
@@ -543,18 +487,12 @@ def _sweep(model, pk, clip, qp, qframe, qf_lo, qf_hi, plan, steps, pass_of, halo
         pos = pos[:, :, al - prev[0]:zl - prev[0]].contiguous()
         occ0_l = occ0[:, :, al - a1:zl - a1].contiguous()
         expd0_l = expd0[:, :, al - a1:zl - a1].contiguous()
-        levels = [grid(l, (al, zl), hires=True), grid(l, (al, zl))] + pooled[l]
-        qfeat = (qf_hi[l][sl].contiguous(), qf_lo[l][sl].contiguous())
-        level_outs = [(torch.empty(1, nq, Tl, dtype=torch.float32, device=dev),
-                       torch.empty(1, nq, Tl, dtype=torch.float32, device=dev),
-                       torch.empty(1, nq, Tl, 2, dtype=torch.float32, device=dev))
-                      for _ in range(npi)]
-        model._refine_level(pk, levels, qfeat, pos, occ0_l, expd0_l, level_outs,
-                            model._refine_buffers(pk, nq, Tl, dev), plan[l][:2], (H, W))
-        cs = slice(win.start - al, win.stop - al)
-        for i, (o, e, t) in enumerate(level_outs):
-          it = (l - 1) * npi + i + 1
-          occ_out[it][b, sl, core] = o[0, :, cs]
-          expd_out[it][b, sl, core] = e[0, :, cs]
-          trk_out[it][b, sl, core] = t[0, :, cs]
+        level_outs = tapir_model._new_estimates(npi, 1, nq, Tl, dev)
+        model._refine_level(pk, grid(l, (al, zl), hires=True), grid(l, (al, zl)), pooled[l],
+                            qf_hi[l][sl], qf_lo[l][sl], pos, occ0_l, expd0_l,
+                            list(zip(*level_outs)), model._refine_buffers(nq, Tl, dev),
+                            plan[l][:2], (H, W))
+        for full, xs in zip(outs, level_outs):
+          for i, x in enumerate(xs):
+            full[(l - 1) * npi + i + 1][b, sl, core] = x[0, :, win.start - al:win.stop - al]
         prev = (al, zl)
