@@ -3,7 +3,7 @@
 # and leaves logs + a JSON report in gpurun_out/.  Usage: gpurun -- bash scripts/gpu_ci.sh [tiers]
 cd "$(dirname "$0")/.." || exit 1
 mkdir -p gpurun_out
-TIERS=${*:-"gemm_simt gemm_tc stages_simt stages_tc e2e_simt e2e_tc"}
+TIERS=${*:-"gemm_simt gemm_tc pairs stages_simt stages_tc e2e_simt e2e_tc"}
 nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm,memory.total --format=csv > gpurun_out/gpu_info.txt 2>&1
 rc=0
 run() {  # name, env, pytest args...
@@ -21,6 +21,7 @@ for t in $TIERS; do
   case $t in
     gemm_simt)   run gemm_simt "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_exact_gpu.py -k simt ;;
     gemm_tc)     run gemm_tc "X=1" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_schedule_gpu.py tests/test_gemm_exact_gpu.py -k tc ;;
+    pairs)       run pairs "X=1" tests/test_plane_pairs_gpu.py ;;
     stages_simt) run stages_simt "TAPIR_B200_GEMM=simt" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py tests/test_backbone_ops_gpu.py tests/test_refine_ops_gpu.py ;;
     stages_tc)   run stages_tc "X=1" tests/test_stages_gpu.py tests/test_batched_gpu.py tests/test_stage_a_gpu.py tests/test_backbone_ops_gpu.py tests/test_refine_ops_gpu.py ;;
     e2e_simt)    run e2e_simt "TAPIR_B200_GEMM=simt" tests/test_end_to_end_gpu.py ;;

@@ -2,8 +2,10 @@
 mirror of gemm_tc.cu's epilogue dispatch.
 
 The exact-accumulator contract.  A is integer-valued with |a| < 2^11 (so most entries above 256
-need a second bf16 plane), B is bf16-exact (its planes 1 and 2 are zero, so the tensor cores'
-dropped i + j >= P plane pairs are zero too), and column n of B is an integer times 2^-s_n.  Every
+need a second bf16 plane, and none a third), B is bf16-exact, and column n of B is an integer
+times 2^-s_n.  B's planes 1 and 2 are zero and so is A's plane 2: only the pairs (0, 0) and (1, 0)
+are nonzero, and every kernel that sums those two gives the same accumulator whatever else it sums
+or drops.  These designs test the epilogue; tests/plane_pairs.py tests the plane pairs.  Every
 product is then an integer times 2^-s_n, and when sum_k |a||b| < 2^(22 - s_n) every partial sum in
 any order is exact in fp32 with two bits to spare for the wgmma adder.  So wgmma at either tile
 width and schedule, split-K, the halo convolution and the SIMT kernel all hold the same

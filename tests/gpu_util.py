@@ -166,7 +166,9 @@ class GemmResult:
 def gemm(a_pl, w_pl, bias=None, residual=None, gelu=False, out_f32=True, out_planes=0, impl=0,
          conv=None, stats=None, rows_per_frame=0, ld_pad=0, offset=0, splitk_ws=None,
          details=False):
-  """Runs tapir_gemm_ex. a_pl: [P, M, K] (plain) or [P, F, H, W, C] (conv=(F,H,W,C)).
+  """Runs tapir_gemm_ex. a_pl: [P, M, K] (plain) or [P, F, H, W, C] (conv=(F,H,W,C)), unit
+  stride in K (plain) or dense within a plane (conv); its plane stride and, plain, its row stride
+  are passed as they are, so a view may space its planes and rows further apart.
 
   ld_pad: the output, residual and plane leading dimensions are N + ld_pad.  offset: the fp32
   output and the residual start `offset` floats into their allocations (offset 1 gives 4-byte but
@@ -177,13 +179,15 @@ def gemm(a_pl, w_pl, bias=None, residual=None, gelu=False, out_f32=True, out_pla
   P, n, k = w_pl.shape
   dev = w_pl.device
   if conv is None:
+    assert a_pl.stride(2) == 1, a_pl.stride()
     m = a_pl.shape[1]
-    lda, aps = a_pl.shape[2], a_pl.shape[1] * a_pl.shape[2]
+    lda, aps = a_pl.stride(1), a_pl.stride(0)
     f = h = w = c = 0
   else:
+    assert a_pl[0].is_contiguous(), a_pl.stride()
     f, h, w, c = conv
     m = f * h * w
-    lda, aps = 0, m * c
+    lda, aps = 0, a_pl.stride(0)
   ld = n + ld_pad
   tail = 8  # guard elements after the last row
   lin = make_linear(w_pl, bias)

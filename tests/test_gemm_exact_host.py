@@ -14,7 +14,8 @@ CASES = {c.cid: c for c in E.CASES}
 def test_accumulator_is_exact_in_fp32(cid):
   d = CASES[cid].design()
   assert float(E.abs_sum_units(d).max()) < E.EXACT_UNITS
-  # B carries no low planes: the tensor cores' dropped i + j >= P pairs are zero
+  # B carries no low planes: only the pairs (i, 0) are nonzero (tests/plane_pairs.py tells the
+  # pair sets apart)
   assert not d.w_pl[1:].float().any()
   # acc is on its columns' grids and therefore held exactly by fp32
   scaled = d.acc * torch.exp2(d.units.double())[None, :]
