@@ -31,6 +31,11 @@ The driver, per clip:
      range starting from the positions the level before left, and the core frames of every
      iteration's outputs are copied into full-length outputs.
   3. The averages over the levels' last estimates are taken once, on the full-length outputs.
+
+`track_video` runs the same sweep (the same `_slide` and `_track_window` per window) on frames it
+asks a reader for: the pre-pass reads only the tap frames, the sweep reads each frame once into a
+device ring one window ahead, and each core's outputs are yielded as soon as they are enqueued, so
+neither the clip nor full-length outputs ever exist.
 """
 import math
 from typing import List, NamedTuple, Optional, Sequence, Tuple
@@ -39,6 +44,7 @@ import numpy as np
 import torch
 
 from tapnet_b200 import _lib
+from tapnet_b200 import live
 from tapnet_b200 import schema
 from tapnet_b200 import tapir_model
 
@@ -155,8 +161,20 @@ def sweep_bytes(model, video_shape, num_points, window_frames, refinement_resolu
   window_frames frames: the pass buffers, the largest backbone step (new frames, their resample and
   the backbone workspace), stage A over level 1's range and the largest refinement level."""
   _, T, H, W = (int(v) for v in video_shape[:4])
-  plan = tapir_model._pass_plan((H, W), model.initial_resolution, refinement_resolutions)
-  halos = halo_frames(model, (H, W), refinement_resolutions)
+
+  def staged(st, new):  # the frames staged on the device
+    return new * H * W * 3 * video_itemsize if host_video or not st.direct else 0
+  buffers, work = _sweep_terms(model, T, (H, W), num_points, window_frames,
+                               refinement_resolutions, staged)
+  return buffers + work
+
+
+def _sweep_terms(model, T, hw, num_points, window_frames, refinement_resolutions, staged):
+  """(pass buffers, larger of the largest backbone step and stage A + the largest refinement
+  level) of a sweep with cores of window_frames frames; staged(step, new) gives the bytes of the
+  frames a backbone step over `new` frames stages besides its resample and workspace."""
+  plan = tapir_model._pass_plan(hw, model.initial_resolution, refinement_resolutions)
+  halos = halo_frames(model, hw, refinement_resolutions)
   C = min(int(window_frames), T)
   span = [min(T, C + left + right) for left, right in halos]
   steps = [st for st in plan if st.new]
@@ -169,8 +187,7 @@ def sweep_bytes(model, video_shape, num_points, window_frames, refinement_resolu
     b = model._backbone_workspace_bytes(new, st.h, st.w)
     if not st.direct:
       b += new * st.h * st.w * 3 * 4
-    if host_video or not st.direct:
-      b += new * H * W * 3 * video_itemsize  # the frames staged on the device
+    b += staged(st, new)
     backbone = max(backbone, b)
   # stage A: one query group over level 1's range
   T1 = span[0]
@@ -186,7 +203,7 @@ def sweep_bytes(model, video_shape, num_points, window_frames, refinement_resolu
     specs, mixer_ws = model._refine_scratch(nq, Tl)
     scratch = mixer_ws + sum(math.prod(s) * d.itemsize for s, d in specs)
     refine = max(refine, pooled + level_io + scratch)
-  return buffers + max(backbone, stage_a + refine)
+  return buffers, max(backbone, stage_a + refine)
 
 
 def prepass_bytes(model, video_shape, frames, refinement_resolutions=None, host_video=False,
@@ -222,6 +239,11 @@ def choose_window_frames(model, video_shape, num_points, free_bytes, refinement_
     raise ValueError(f'a windowed call on a {tuple(video_shape)} clip with {num_points} queries '
                      f'needs {need(1)} bytes of device memory even with one-frame windows; '
                      f'{free_bytes} are available')
+  return _largest_core(need, free_bytes, T)
+
+
+def _largest_core(need, free_bytes, T):
+  """The largest C in 1..T with need(C) <= free_bytes, need non-decreasing and need(1) fitting."""
   lo, hi = 1, T
   while lo < hi:
     mid = (lo + hi + 1) // 2
@@ -253,12 +275,23 @@ def _check_inputs(model, video, query_points):
   return dev
 
 
+def _yuv_frames(clip, a, z, repeat=1):
+  """Frames a..z-1 of a one-clip YUV clip (each `repeat` times), with its window and matrix."""
+  y, u, v = (t[:, a:z] if repeat == 1 else t[:, a:z].repeat_interleave(repeat, 1)
+             for t in (clip.y, clip.u, clip.v))
+  return live.YUV420Frames(y, u, v, clip.matrix, clip.full_range, clip.window)
+
+
 def _run_pass(model, pk, video, step, a, z, out, dev):
-  """Backbone pass `step` over frames a..z-1 of the one-clip video into out (lowres, hires)."""
-  src = tapir_model._backbone_frames(video[:, a:z])
-  if step.direct and video.device.type == 'cpu':  # streamed in behind the stem convolution
-    return model._backbone_pass(pk, torch.empty_like(src, device=dev), src, None, dev, out)
-  frames = src.to(dev, non_blocking=True)
+  """Backbone pass `step` over frames a..z-1 of the one-clip video (or device YUV clip) into out
+  (lowres, hires)."""
+  if isinstance(video, live.YUV420Frames):
+    frames = _yuv_frames(video, a, z)
+  else:
+    src = tapir_model._backbone_frames(video[:, a:z])
+    if step.direct and video.device.type == 'cpu':  # streamed in behind the stem convolution
+      return model._backbone_pass(pk, torch.empty_like(src, device=dev), src, None, dev, out)
+    frames = src.to(dev, non_blocking=True)
   if not step.direct:
     resized = torch.empty(1, z - a, step.h, step.w, 3, dtype=torch.float32, device=dev)
     _lib.resample_frames(frames, resized)
@@ -295,7 +328,10 @@ def _run_frames(model, pk, video, step, out, alone, dev):
     while j < n and not alone[j]:
       j += 1
     if j - i == 1:
-      pair = video[:, i:i + 1].expand(1, 2, *video.shape[2:]).contiguous()
+      if isinstance(video, live.YUV420Frames):
+        pair = _yuv_frames(video, i, i + 1, repeat=2)
+      else:
+        pair = video[:, i:i + 1].expand(1, 2, *video.shape[2:]).contiguous()
       tmp = tuple(torch.empty((1, 2) + t.shape[2:], dtype=t.dtype, device=dev) for t in out)
       _run_pass(model, pk, pair, step, 0, 2, tmp, dev)
       for t, x in zip(out, tmp):
@@ -308,17 +344,9 @@ def _run_frames(model, pk, video, step, out, alone, dev):
     i = j
 
 
-def _query_features(model, pk, video, b, num_clips, qp, plan, max_frames, dev):
-  """Query features [N, C] of clip b (video [1, T, H, W, 3]) of num_clips at every resolution of
-  `plan` (lowres list, hires list), sampled from the grids of the queries' tap frames only, in
-  chunks of at most max_frames frames that keep each query's tap pair together."""
-  T, H, W = (int(v) for v in video.shape[1:4])
-  steps = [st for st in plan if st.new]
-  pass_of = np.cumsum([st.new for st in plan]) - 1
-  N = qp.shape[0]
-  feats = ([torch.empty(N, schema.LOWRES_DIM, dtype=torch.float32, device=dev) for _ in plan],
-           [torch.empty(N, schema.HIRES_DIM, dtype=torch.float32, device=dev) for _ in plan])
-  t0 = query_tap_frames(qp[:, 0].cpu().numpy(), T)
+def _prepass_chunks(t0, T, max_frames):
+  """The query pre-pass's chunks as (sorted frames, queries): the tap pairs of the first tap frames
+  t0 in frame order, at most max(2, max_frames) frames per chunk, each pair within one chunk."""
   chunks, frames, queries = [], set(), []
   for f0 in np.unique(t0):
     pair = {int(f0)} | ({int(f0) + 1} if f0 + 1 < T else set())
@@ -329,8 +357,23 @@ def _query_features(model, pk, video, b, num_clips, qp, plan, max_frames, dev):
     queries.extend(np.nonzero(t0 == f0)[0].tolist())
   if frames:
     chunks.append((sorted(frames), queries))
-  for frame_list, query_list in chunks:
-    sub = video[:, torch.tensor(frame_list)]
+  return chunks
+
+
+def _query_features(model, pk, clip_of, video_shape, b, num_clips, qp, plan, max_frames, dev):
+  """Query features [N, C] of clip b of num_clips clips of video_shape (T, H, W) at every resolution
+  of `plan` (lowres list, hires list), sampled from the grids of the queries' tap frames only, in
+  the chunks of _prepass_chunks; clip_of(i, frames) gives chunk i's frames as a one-clip video
+  [1, F, H, W, 3] (or a device YUV clip)."""
+  T, H, W = (int(v) for v in video_shape)
+  steps = [st for st in plan if st.new]
+  pass_of = np.cumsum([st.new for st in plan]) - 1
+  N = qp.shape[0]
+  feats = ([torch.empty(N, schema.LOWRES_DIM, dtype=torch.float32, device=dev) for _ in plan],
+           [torch.empty(N, schema.HIRES_DIM, dtype=torch.float32, device=dev) for _ in plan])
+  t0 = query_tap_frames(qp[:, 0].cpu().numpy(), T)
+  for i, (frame_list, query_list) in enumerate(_prepass_chunks(t0, T, max_frames)):
+    sub = clip_of(i, frame_list)
     F = len(frame_list)
     grids = []
     for st in steps:
@@ -416,7 +459,8 @@ def _windowed(model, video, query_points, window_frames, refinement_resolutions,
     for b in range(B):
       clip = video[b:b + 1]
       qp = qp_all[b].contiguous()
-      qf_lo, qf_hi = _query_features(model, pk, clip, b, B, qp, plan, max_frames, dev)
+      qf_lo, qf_hi = _query_features(model, pk, lambda _, fl: clip[:, torch.tensor(fl)],
+                                     (T, H, W), b, B, qp, plan, max_frames, dev)
       # stage A's query frame, resolved once over the whole clip; each window sees it relative to
       # its own range, so a query outside the range matches no frame
       qframe = torch.from_numpy(query_frames(qp[:, 0].cpu().numpy(), T).astype(np.float32))
@@ -432,67 +476,489 @@ def _windowed(model, video, query_points, window_frames, refinement_resolutions,
   )
 
 
-def _sweep(model, pk, clip, qp, qframe, qf_lo, qf_hi, plan, steps, pass_of, halos, C, b, B,
-           outs, dev):
-  T, H, W = (int(v) for v in clip.shape[1:4])
-  N = qp.shape[0]
-  L = len(plan) - 1
-  npi = model.num_pips_iter
-  windows = window_plan(T, C, halos, plan)
-  owners = pass_levels(plan)
+def _pass_buffers(windows, plan, dev):
+  """One (lowres, hires) buffer per backbone pass of `plan`, sized by the widest range of the level
+  it serves over `windows`."""
   bufs = []
-  for st, l in zip(steps, owners):
+  for st, l in zip([st for st in plan if st.new], pass_levels(plan)):
     cap = max(z - a for w in windows for a, z in [w.levels[l - 1]])
     bufs.append(tuple(torch.empty((1, cap) + s, dtype=torch.float32, device=dev)
                       for s in tapir_model._grid_shapes(st.h, st.w)))
+  return bufs
+
+
+def _slide(bufs, held, steps, win, run):
+  """Moves every pass's buffer to window `win`'s range and computes its new frames only:
+  run(p, step, first, z, out) writes pass p's grids of frames first..z-1 into out.  held: the
+  range each buffer holds, updated in place."""
+  for p, (st, (a, z)) in enumerate(zip(steps, win.passes)):
+    a0, z0 = held[p]
+    keep = max(0, z0 - a)
+    if keep and a > a0:
+      for t in bufs[p]:
+        _shift(t, a - a0, keep)
+    first = a + keep
+    if z > first:
+      run(p, st, first, z, tuple(t[:, first - a:z - a] for t in bufs[p]))
+    held[p] = (a, z)
+
+
+def _track_window(model, pk, win, bufs, held, plan, pass_of, qp, qframe, qf_lo, qf_hi, hw, sink,
+                  dev):
+  """Stage A over level 1's range of window `win` and each refinement level over its own range,
+  from the pass buffers.  sink(it, sl, (occ, expd, tracks), a) receives iteration it's estimates
+  ([1, n, frames, ...], frames from a on) of the queries sl; iteration 0 is stage A's."""
+  N = qp.shape[0]
+  L = len(plan) - 1
+  npi = model.num_pips_iter
+
+  def grid(i, rng, hires=False):
+    p = pass_of[i]
+    a = held[p][0]
+    return bufs[p][1 if hires else 0][:, rng[0] - a:rng[1] - a]
+
+  # pooled pyramid levels of each level's range
+  pooled = {l: model._pool_pyramid(grid(l, win.levels[l - 1])) for l in range(1, L + 1)}
+
+  a1, z1 = win.levels[0]
+  T1 = z1 - a1
+  for _, _, sl in tapir_model._groups(1, N, T1):
+    nq = sl.stop - sl.start
+    shapes, _ = tapir_model._stage_a_scratch(1, nq, T1, grid(0, (a1, z1)).shape[2:])
+    occ0, expd0, trk0 = (torch.empty(s, dtype=torch.float32, device=dev) for s in shapes[:3])
+    qp_w = torch.cat([(qframe[sl] - a1)[:, None], qp[sl, 1:]], dim=1)[None].contiguous()
+    pos = model._stage_a(pk, grid(0, (a1, z1)), qf_lo[0][sl][None].contiguous(), qp_w, hw,
+                         occ0, expd0, trk0, None, dev)
+    sink(0, sl, (occ0, expd0, trk0), a1)
+    prev = (a1, z1)
+    for l in range(1, L + 1):
+      al, zl = win.levels[l - 1]
+      Tl = zl - al
+      pos = pos[:, :, al - prev[0]:zl - prev[0]].contiguous()
+      occ0_l = occ0[:, :, al - a1:zl - a1].contiguous()
+      expd0_l = expd0[:, :, al - a1:zl - a1].contiguous()
+      level_outs = tapir_model._new_estimates(npi, 1, nq, Tl, dev)
+      model._refine_level(pk, grid(l, (al, zl), hires=True), grid(l, (al, zl)), pooled[l],
+                          qf_hi[l][sl], qf_lo[l][sl], pos, occ0_l, expd0_l,
+                          list(zip(*level_outs)), model._refine_buffers(nq, Tl, dev),
+                          plan[l][:2], hw)
+      for i, xs in enumerate(zip(*level_outs)):
+        sink((l - 1) * npi + i + 1, sl, xs, al)
+      prev = (al, zl)
+
+
+def _sweep(model, pk, clip, qp, qframe, qf_lo, qf_hi, plan, steps, pass_of, halos, C, b, B,
+           outs, dev):
+  """The sweep of clip b of B ([1, T, H, W, 3] on the host or the device): each window's core
+  outputs go into the full-length outputs `outs` (occlusion, expected distance, tracks lists)."""
+  T, H, W = (int(v) for v in clip.shape[1:4])
+  windows = window_plan(T, C, halos, plan)
+  bufs = _pass_buffers(windows, plan, dev)
   held = [(0, 0)] * len(steps)
+
+  def run(p, st, first, z, out):
+    _run_frames(model, pk, clip[:, first:z], st, out, _alone_frames(st, B, T, b, range(first, z)),
+                dev)
+
   for win in windows:
-    # ---- slide every pass's buffer and run the backbone on the new frames only
-    for p, (st, (a, z)) in enumerate(zip(steps, win.passes)):
-      a0, z0 = held[p]
-      keep = max(0, z0 - a)
-      if keep and a > a0:
-        for t in bufs[p]:
-          _shift(t, a - a0, keep)
-      first = a + keep
+    def sink(it, sl, xs, a, win=win):
+      for full, x in zip(outs, xs):
+        full[it][b, sl, win.start:win.stop] = x[0, :, win.start - a:win.stop - a]
+
+    _slide(bufs, held, steps, win, run)
+    _track_window(model, pk, win, bufs, held, plan, pass_of, qp, qframe, qf_lo, qf_hi, (H, W),
+                  sink, dev)
+
+
+# ------------------------------------------------------------------------------ frame reader
+# track_video runs the same sweep on frames it asks a reader for: each frame is read once, kept in
+# a device ring in the reader's format until the last backbone pass that needs it has its grids,
+# and every window's core outputs are handed back as soon as they are enqueued.
+def _pass_spans(windows):
+  """For each window, the frames [lo, hi) its backbone passes still need: from the first frame
+  any pass adds to its buffer to the end of the widest range."""
+  held = [0] * len(windows[0].passes)
+  spans = []
+  for win in windows:
+    lo, hi = None, 0
+    for p, (a, z) in enumerate(win.passes):
+      first = max(a, held[p])
       if z > first:
-        _run_frames(model, pk, clip[:, first:z], st, tuple(t[:, first - a:z - a] for t in bufs[p]),
-                    _alone_frames(st, B, T, b, range(first, z)), dev)
-      held[p] = (a, z)
+        lo = first if lo is None else min(lo, first)
+      hi = max(hi, z)
+      held[p] = z
+    spans.append((hi if lo is None else lo, hi))
+  return spans
 
-    def grid(i, rng, hires=False):
-      p = pass_of[i]
-      a = held[p][0]
-      return bufs[p][1 if hires else 0][:, rng[0] - a:rng[1] - a]
 
-    # pooled pyramid levels of each level's range
-    pooled = {l: model._pool_pyramid(grid(l, win.levels[l - 1])) for l in range(1, L + 1)}
+def sweep_reads(num_frames, window_frames, halos, plan) -> List[Tuple[int, int]]:
+  """The frame range track_video reads for each window of the sweep (halos from halo_frames, plan
+  from tapir_model._pass_plan): the frames its passes need that no window before has read.  The
+  ranges are consecutive and cover [0, num_frames) once; a window that needs no new frame has an
+  empty range and reads nothing."""
+  reads, end = [], 0
+  for _, hi in _pass_spans(window_plan(num_frames, window_frames, halos, plan)):
+    reads.append((end, max(end, hi)))
+    end = max(end, hi)
+  return reads
 
-    a1, z1 = win.levels[0]
-    T1 = z1 - a1
-    core = slice(win.start, win.stop)
-    for _, _, sl in tapir_model._groups(1, N, T1):
-      nq = sl.stop - sl.start
-      shapes, _ = tapir_model._stage_a_scratch(1, nq, T1, grid(0, (a1, z1)).shape[2:])
-      occ0, expd0, trk0 = (torch.empty(s, dtype=torch.float32, device=dev) for s in shapes[:3])
-      qp_w = torch.cat([(qframe[sl] - a1)[:, None], qp[sl, 1:]], dim=1)[None].contiguous()
-      pos = model._stage_a(pk, grid(0, (a1, z1)), qf_lo[0][sl][None].contiguous(), qp_w, (H, W),
-                           occ0, expd0, trk0, None, dev)
-      for full, x in zip(outs, (occ0, expd0, trk0)):
-        full[0][b, sl, core] = x[0, :, win.start - a1:win.stop - a1]
-      prev = (a1, z1)
-      for l in range(1, L + 1):
-        al, zl = win.levels[l - 1]
-        Tl = zl - al
-        pos = pos[:, :, al - prev[0]:zl - prev[0]].contiguous()
-        occ0_l = occ0[:, :, al - a1:zl - a1].contiguous()
-        expd0_l = expd0[:, :, al - a1:zl - a1].contiguous()
-        level_outs = tapir_model._new_estimates(npi, 1, nq, Tl, dev)
-        model._refine_level(pk, grid(l, (al, zl), hires=True), grid(l, (al, zl)), pooled[l],
-                            qf_hi[l][sl], qf_lo[l][sl], pos, occ0_l, expd0_l,
-                            list(zip(*level_outs)), model._refine_buffers(nq, Tl, dev),
-                            plan[l][:2], (H, W))
-        for full, xs in zip(outs, level_outs):
-          for i, x in enumerate(xs):
-            full[(l - 1) * npi + i + 1][b, sl, core] = x[0, :, win.start - al:win.stop - al]
-        prev = (al, zl)
+
+def ring_frames(num_frames, window_frames, halos, plan) -> int:
+  """Frames of track_video's device ring: the most frames any window's passes still need at once.
+  A window's new frames overwrite only frames the window before has run through every pass."""
+  return max(hi - lo for lo, hi in _pass_spans(window_plan(num_frames, window_frames, halos, plan)))
+
+
+def _prepass_reads(t0, T, max_frames):
+  """(probe, reads of each _prepass_chunks chunk): the probe is the first tap pair, read before
+  anything is sized (it fixes the frame format); each chunk then reads the runs of its frames that
+  the frames kept from before (the probe, then the last frame of the chunk before) do not hold."""
+  chunks = _prepass_chunks(t0, T, max_frames)
+  f0 = chunks[0][0][0]
+  probe = (f0, min(f0 + 2, T))
+  kept = set(range(*probe))
+  reads = []
+  for frames, _ in chunks:
+    runs = []
+    for f in frames:
+      if f in kept:
+        continue
+      if runs and runs[-1][1] == f:
+        runs[-1][1] = f + 1
+      else:
+        runs.append([f, f + 1])
+    reads.append([tuple(r) for r in runs])
+    kept = {frames[-1]}
+  return probe, reads
+
+
+def prepass_reads(t, num_frames, max_frames) -> List[Tuple[int, int]]:
+  """The frame ranges track_video's query pre-pass reads, in order, for queries at times t with
+  pre-pass chunks of at most max_frames frames: only the queries' tap frames, each once."""
+  probe, reads = _prepass_reads(query_tap_frames(t, num_frames), num_frames, max_frames)
+  return [probe] + [r for chunk in reads for r in chunk]
+
+
+def reader_sweep_bytes(model, video_shape, num_points, window_frames, refinement_resolutions=None,
+                       frame_bytes=None):
+  """Device bytes of track_video's sweep over a (1, T, H, W) video with cores of window_frames
+  frames: the frame ring (frame_bytes per frame, default uint8 RGB), the pass buffers, the larger
+  of the largest backbone step and stage A + the largest refinement level, and two windows'
+  outputs (the one the caller holds while the next is computed).  No term grows with T once the
+  windows reach their full size."""
+  _, T, H, W = (int(v) for v in video_shape[:4])
+  frame_bytes = H * W * 3 if frame_bytes is None else int(frame_bytes)
+  plan = tapir_model._pass_plan((H, W), model.initial_resolution, refinement_resolutions)
+  C = min(int(window_frames), T)
+  ring = ring_frames(T, C, halo_frames(model, (H, W), refinement_resolutions), plan) * frame_bytes
+
+  def staged(st, new):  # a lone frame's two-frame call of itself: the pair and its grids
+    return 2 * frame_bytes + 2 * _f32_bytes(tapir_model._grid_shapes(st.h, st.w))
+  buffers, work = _sweep_terms(model, T, (H, W), num_points, C, refinement_resolutions, staged)
+  outs = 2 * output_bytes(model, (1, C, H, W), num_points, refinement_resolutions)
+  return ring + buffers + work + outs
+
+
+def choose_reader_window_frames(model, video_shape, num_points, free_bytes,
+                                refinement_resolutions=None, frame_bytes=None):
+  """The largest core length whose track_video sweep (reader_sweep_bytes) fits free_bytes."""
+  def need(c):
+    return reader_sweep_bytes(model, video_shape, num_points, c, refinement_resolutions,
+                              frame_bytes)
+  if need(1) > free_bytes:
+    raise ValueError(f'tracking a {tuple(video_shape)} video with {num_points} queries needs '
+                     f'{need(1)} bytes of device memory even with one-frame windows; '
+                     f'{free_bytes} are available')
+  return _largest_core(need, free_bytes, int(video_shape[1]))
+
+
+def _describe(x):
+  """(format string, frame count) of what a reader returned; (None, 0) if it is no frame batch."""
+  if isinstance(x, live.YUV420Frames):
+    if x.y.shape[0] != 1:
+      return None, 0
+    H, W = x.frame_size
+    return (f'YUV 4:2:0 {H}x{W} frames, window {x.window}, {x.matrix}, '
+            f'{"full" if x.full_range else "limited"} range, on {x.device}'), int(x.y.shape[1])
+  if (isinstance(x, torch.Tensor) and x.dim() == 4 and x.shape[-1] == 3
+      and (x.dtype == torch.uint8 or x.dtype.is_floating_point)):
+    return f'{x.dtype} RGB {x.shape[1]}x{x.shape[2]} frames on {x.device}', int(x.shape[0])
+  return None, 0
+
+
+class _FrameSource:
+  """read_frames(start, stop), its result checked against the first call's format.  Keeps what the
+  first result looked like, not the frames."""
+
+  def __init__(self, read, dev):
+    self.read, self.dev, self.format = read, dev, None
+
+  def __call__(self, a, z):
+    x = self.read(a, z)
+    what, n = _describe(x)
+    if what is None:
+      got = tuple(x.shape) if isinstance(x, torch.Tensor) else type(x).__name__
+      raise ValueError(f'read_frames({a}, {z}) returned {got}; expected a uint8 or float '
+                       f'[{z - a}, H, W, 3] tensor or live.YUV420Frames of [1, {z - a}] frames')
+    if x.device.type != 'cpu' and x.device != self.dev:
+      raise ValueError(f'read_frames({a}, {z}) returned frames on {x.device}; the model is on '
+                       f'{self.dev}')
+    if self.format is None:
+      self.format = what
+      self.host = x.device.type == 'cpu'
+      if isinstance(x, live.YUV420Frames):
+        self.yuv = (x.matrix, x.full_range, x.window)
+        self.frame_size = x.frame_size
+        self.hw = tuple(int(v) for v in x.shape[2:4])
+        self.itemsize = 1
+      else:
+        self.yuv = None
+        self.hw = self.frame_size = (int(x.shape[1]), int(x.shape[2]))
+        self.itemsize = 1 if x.dtype == torch.uint8 else 4
+    elif what != self.format:
+      raise ValueError(f'read_frames({a}, {z}) returned {what}; the first call returned '
+                       f'{self.format}')
+    if n != z - a:
+      raise ValueError(f'read_frames({a}, {z}) returned {n} frames, expected {z - a}')
+    return x
+
+  @property
+  def frame_bytes(self):
+    """Bytes of one frame as the device stores it."""
+    H, W = self.frame_size
+    if self.yuv is not None:
+      return H * W + 2 * ((H + 1) // 2) * ((W + 1) // 2)
+    return H * W * 3 * self.itemsize
+
+
+class _FrameStore:
+  """S device frames in a _FrameSource's format: uint8 or float32 RGB [1, S, H, W, 3], or Y, U and
+  V planes [1, S, ...] (the same frames in I420 layout) with the source's window and matrix."""
+
+  def __init__(self, src, S, dev):
+    self.yuv = src.yuv
+    if src.yuv is not None:
+      H, W = src.frame_size
+      self.planes = tuple(torch.empty(1, S, h, w, dtype=torch.uint8, device=dev)
+                          for h, w in ((H, W),) + (((H + 1) // 2, (W + 1) // 2),) * 2)
+    else:
+      dtype = torch.uint8 if src.itemsize == 1 else torch.float32
+      self.planes = (torch.empty((1, S) + src.hw + (3,), dtype=dtype, device=dev),)
+
+  def view(self, s, z):
+    """Slots s..z-1 as a one-clip video or YUV clip."""
+    if self.yuv is None:
+      return self.planes[0][:, s:z]
+    return live.YUV420Frames(*(t[:, s:z] for t in self.planes), *self.yuv)
+
+  def put(self, s, x, i, n, non_blocking=True):
+    """Frames i..i+n-1 of x (a reader's result or another store) into slots s..s+n-1."""
+    if isinstance(x, _FrameStore):
+      src = [t[0, i:i + n] for t in x.planes]
+    elif isinstance(x, live.YUV420Frames):
+      src = [t[0, i:i + n] for t in (x.y, x.u, x.v)]
+    else:
+      src = [x[i:i + n]]
+    for dst, t in zip(self.planes, src):
+      dst[0, s:s + n].copy_(t, non_blocking=non_blocking)
+
+
+class _ReaderSweep:
+  """The state of one track_video call: prepare() runs the query pre-pass and sizes the sweep,
+  window(w) enqueues window w, reads window w + 1's new frames and returns w's outputs, close()
+  waits for the copies in flight."""
+
+  def __init__(self, model, read, T, query_points, window_frames, refinement_resolutions,
+               unrefined, dev):
+    self.model, self.T, self.qp_in, self.dev = model, T, query_points, dev
+    self.window_frames, self.refs, self.unrefined = window_frames, refinement_resolutions, unrefined
+    self.src = _FrameSource(read, dev)
+    self.pending = None  # (reader result, copy-done event) of the next window's frames
+    self.cs = self.main = None
+
+  def prepare(self):
+    model, T, dev, src = self.model, self.T, self.dev, self.src
+    self.pk = model._pack()
+    self.main, self.cs = torch.cuda.current_stream(dev), model._copy_stream(dev)
+    qp = self.qp_in.to(device=dev, dtype=torch.float32).contiguous()
+    times = qp[:, 0].cpu().numpy()
+    t0 = query_tap_frames(times, T)
+    probe = _prepass_reads(t0, T, 2)[0]
+    first = src(*probe)  # fixes the format and the frame size
+    H, W = src.hw
+    N = qp.shape[0]
+    self.plan = plan = tapir_model._pass_plan((H, W), model.initial_resolution, self.refs)
+    halos = halo_frames(model, (H, W), self.refs)
+    shape = (1, T, H, W)
+    budget = _free_device_bytes(dev)
+    C = self.window_frames
+    if C is None:
+      C = choose_reader_window_frames(model, shape, N, budget, self.refs, src.frame_bytes)
+    C = min(int(C), T)
+    # the pre-pass may use what the sweep will, and no more than is free; two frames at least
+    bound = min(budget, reader_sweep_bytes(model, shape, N, C, self.refs, src.frame_bytes))
+    max_frames = 2
+    while (max_frames < T and prepass_bytes(model, shape, max_frames * 2, self.refs, False,
+                                            src.itemsize) <= bound):
+      max_frames *= 2
+    _, prepass = _prepass_reads(t0, T, max_frames)
+    kept = (list(range(*probe)), _FrameStore(src, probe[1] - probe[0], dev))
+    kept[1].put(0, first, 0, probe[1] - probe[0], non_blocking=False)
+    del first
+
+    def clip_of(i, frames):
+      nonlocal kept
+      store = _FrameStore(src, len(frames), dev)
+      slot = {f: j for j, f in enumerate(frames)}
+      for j, f in enumerate(kept[0]):
+        if f in slot:
+          store.put(slot[f], kept[1], j, 1)
+      for a, z in prepass[i]:
+        # a blocking copy: the reader may refill its buffer on the next call
+        store.put(slot[a], src(a, z), 0, z - a, non_blocking=False)
+      last = _FrameStore(src, 1, dev)
+      last.put(0, store, len(frames) - 1, 1)
+      kept = (frames[-1:], last)
+      return store.view(0, len(frames))
+
+    self.qf_lo, self.qf_hi = _query_features(model, self.pk, clip_of, (T, H, W), 0, 1, qp, plan,
+                                             max_frames, dev)
+    kept = None
+    self.qp = qp
+    self.qframe = torch.from_numpy(query_frames(times, T).astype(np.float32)).to(dev)
+    self.windows = window_plan(T, C, halos, plan)
+    self.reads = sweep_reads(T, C, halos, plan)
+    self.S = ring_frames(T, C, halos, plan)
+    self.ring = _FrameStore(src, self.S, dev)
+    self.steps = [st for st in plan if st.new]
+    self.pass_of = np.cumsum([st.new for st in plan]) - 1
+    self.bufs = _pass_buffers(self.windows, plan, dev)
+    self.held = [(0, 0)] * len(self.steps)
+    self.pending = self._fetch(0, None)
+
+  def _slots(self, a, z):
+    """The ring slots of frames a..z-1 as (first frame, first slot, count) runs (the ring wraps)."""
+    f = a
+    while f < z:
+      s = f % self.S
+      n = min(z - f, self.S - s)
+      yield f, s, n
+      f += n
+
+  def _fetch(self, w, after):
+    """Reads window w's new frames and starts their copy into the ring on the copy stream, after
+    event `after` (None: after the work enqueued so far)."""
+    a, z = self.reads[w]
+    if a == z:
+      return None
+    x = self.src(a, z)
+    if after is None:
+      self.cs.wait_stream(self.main)
+    else:
+      self.cs.wait_event(after)
+    with torch.cuda.stream(self.cs):
+      for f, s, n in self._slots(a, z):
+        self.ring.put(s, x, f - a, n)
+      done = torch.cuda.Event()
+      done.record(self.cs)
+    return x, done
+
+  def _run(self, p, st, first, z, out):
+    for f, s, n in self._slots(first, z):
+      _run_frames(self.model, self.pk, self.ring.view(s, s + n), st,
+                  tuple(t[:, f - first:f - first + n] for t in out),
+                  _alone_frames(st, 1, self.T, 0, range(f, f + n)), self.dev)
+
+  def window(self, w):
+    model, dev, win = self.model, self.dev, self.windows[w]
+    if self.pending is not None:
+      self.main.wait_event(self.pending[1])
+    _slide(self.bufs, self.held, self.steps, win, self._run)
+    grids_done = torch.cuda.Event()
+    grids_done.record(self.main)  # no pass reads the ring after this
+    npi = model.num_pips_iter
+    num_iters = npi * (len(self.plan) - 1)
+    N, c = self.qp.shape[0], win.stop - win.start
+    est = [tuple(x[0] for x in tapir_model._new_estimates(1, 1, N, c, dev))
+           if self.unrefined or (it and it % npi == 0) else None for it in range(num_iters + 1)]
+
+    def sink(it, sl, xs, a):
+      if est[it] is not None:
+        for dst, x in zip(est[it], xs):
+          dst[0, sl] = x[0, :, win.start - a:win.stop - a]
+
+    _track_window(model, self.pk, win, self.bufs, self.held, self.plan, self.pass_of, self.qp,
+                  self.qframe, self.qf_lo, self.qf_hi, self.src.hw, sink, dev)
+    traj = {k: [e[i] if e is not None else None for e in est]
+            for i, k in enumerate(('occlusion', 'expected_dist', 'tracks'))}
+    out = tapir_model.refined_average(traj, npi)
+    if self.unrefined:
+      out.update({f'unrefined_{k}': v[:-1] for k, v in traj.items()})
+    # window w's frames are on the device: drop the reader's result before asking for more
+    if self.pending is not None:
+      self.pending[1].synchronize()
+      self.pending = None
+    if w + 1 < len(self.windows):
+      self.pending = self._fetch(w + 1, grids_done if self.src.host else None)
+    return out
+
+  def close(self):
+    if self.pending is not None:
+      self.pending[1].synchronize()
+      self.pending = None
+    if self.main is not None:
+      self.main.wait_stream(self.cs)  # later work may reuse the ring's memory
+
+
+def track_video(model, read_frames, num_frames: int, query_points,
+                window_frames: Optional[int] = None,
+                refinement_resolutions: Optional[Sequence[Tuple[int, int]]] = None,
+                unrefined: bool = False):
+  """Tracks query_points through a video of num_frames frames that read_frames hands over in
+  pieces; yields (start, stop, outputs) window by window in frame order.
+
+  read_frames(start, stop) returns frames start..stop-1: a uint8 or float [stop - start, H, W, 3]
+  tensor on the host (pinned or pageable) or on the model's device, or a device live.YUV420Frames
+  of [1, stop - start] frames whose window is the video.  The first call fixes the frame size and
+  format (for YUV also the window, matrix and range); a later call that returns anything else, or
+  a wrong frame count, raises ValueError naming its range.  The query pre-pass asks only for the
+  queries' tap frames, each once; the sweep then asks for consecutive ranges that cover
+  [0, num_frames) once, in order, one window ahead, so the reader decodes while the GPU works.
+
+  query_points: [N, 3] or [1, N, 3] (t, y, x), N >= 1.  outputs: 'tracks' [1, N, stop - start, 2],
+  'occlusion' and 'expected_dist' [1, N, stop - start] on the model's device, fresh tensors, and
+  with unrefined=True the unrefined_* lists cut to the same frames.  Concatenated over the frame
+  axis they equal model(video, query_points) bit for bit.  window_frames: the core length C; None
+  picks the largest C whose sweep fits the free device memory.  Host and device memory stay
+  bounded whatever num_frames is.  Arguments are checked when the call is made; frames are read
+  once the iteration starts."""
+  if isinstance(num_frames, bool) or not isinstance(num_frames, (int, np.integer)) or num_frames < 1:
+    raise ValueError(f'num_frames must be a positive integer, got {num_frames!r}')
+  if window_frames is not None and int(window_frames) < 1:
+    raise ValueError(f'window_frames must be >= 1, got {window_frames}')
+  if not callable(read_frames):
+    raise ValueError(f'read_frames must be callable, got {type(read_frames).__name__}')
+  qp = query_points
+  if (not isinstance(qp, torch.Tensor) or qp.shape[-1:] != (3,) or qp.dim() not in (2, 3)
+      or (qp.dim() == 3 and qp.shape[0] != 1) or qp.shape[-2] == 0):
+    raise ValueError('query_points must be an [N, 3] or [1, N, 3] tensor with N >= 1, got '
+                     f'{tuple(qp.shape) if isinstance(qp, torch.Tensor) else type(qp).__name__}')
+  dev = model._device_check(None if qp.device.type == 'cpu' else qp)
+  sweep = _ReaderSweep(model, read_frames, int(num_frames), qp.reshape(-1, 3), window_frames,
+                       refinement_resolutions, bool(unrefined), dev)
+  return _track_video(sweep, dev)
+
+
+def _track_video(sweep, dev):
+  # the model's device is current while the sweep works, the caller's while it holds a window
+  try:
+    with torch.cuda.device(dev):
+      sweep.prepare()
+    for w, win in enumerate(sweep.windows):
+      with torch.cuda.device(dev):
+        out = sweep.window(w)
+      yield win.start, win.stop, out
+      del out
+  finally:
+    with torch.cuda.device(dev):
+      sweep.close()
