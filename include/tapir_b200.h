@@ -29,6 +29,7 @@ extern "C" {
 #define TAPIR_NUM_RESNET_BLOCKS 8
 #define TAPIR_MAX_EXTRA_BLOCKS 5
 #define TAPIR_MAX_CORR_LEVELS 5 /* hires + lowres + up to 3 pooled levels (pyramid_level <= 3) */
+#define TAPIR_MAX_RAGGED_CLIPS 64 /* clips of one tapir_cost_volume_tracks_ragged call */
 
 /* A dense layer / convolution prepared for the split-bf16 tensor-core GEMM:
  * w = bf16 planes [planes][N][K] (K padded with zeros to a multiple of 64; for 3x3
@@ -522,6 +523,24 @@ int tapir_cost_volume_tracks_batched(const tapir_head_weights* w, const float* q
                                      float* points, float* occ, float* expd, int32_t* argmax,
                                      void* workspace, size_t workspace_bytes, void* stream);
 
+/* The same for B clips with their own query counts: points_per_clip is a HOST array of B counts
+ * N_b >= 1 (1 <= B <= TAPIR_MAX_RAGGED_CLIPS), qfeat [sum N_b][C] and query_tyx [sum N_b][3] (or
+ * NULL) hold the clips' queries one clip after the other, grid is [B][T][gh][gw][C]; outputs run
+ * over the flattened query as above.  One grouped GEMM and one head launch, no host-to-device
+ * copy (the call may be captured in a CUDA graph); clip b's results equal those of a
+ * tapir_cost_volume_tracks call on clip b alone, bit for bit.  sum N_b <= 65535 for the 32 x 32
+ * map.  Every argument is checked first; a bad one returns 1 before any CUDA call.  The workspace
+ * depends on the clip count and the total query count only. */
+size_t tapir_cost_volume_ragged_workspace_bytes(int32_t B, int32_t total_points, int32_t T,
+                                                int32_t gh, int32_t gw, int32_t C);
+int tapir_cost_volume_tracks_ragged(const tapir_head_weights* w, const float* qfeat,
+                                    const float* grid, int32_t B, const int32_t* points_per_clip,
+                                    int32_t T, int32_t gh, int32_t gw, int32_t C,
+                                    const float* query_tyx, float softmax_temperature,
+                                    int32_t init_h, int32_t init_w, float* points, float* occ,
+                                    float* expd, int32_t* argmax, void* workspace,
+                                    size_t workspace_bytes, void* stream);
+
 /* ---- a9: tapir_model.py:519-527 avg_pool3d (2,2,1) ---------------------------------- */
 int tapir_pool_pyramid(const float* grid, int32_t T, int32_t h, int32_t w, int32_t C, float* out,
                        void* stream);
@@ -532,6 +551,12 @@ int tapir_local_corr(const tapir_corr_args* args, void* stream);
  * [batch][T][h][w][C]; pos / occ / expd / features / output rows run over the flattened query
  * b*num_points + n.  Equal to one tapir_local_corr call per clip, bit for bit. */
 int tapir_local_corr_batched(const tapir_corr_args* args, int32_t batch, void* stream);
+/* `batch` clips with their own query counts: args->num_points = the queries of all clips,
+ * query_clip a device int32 table [num_points] giving each flattened query's clip (in
+ * 0..batch-1), whose level grids [batch][T][h][w][C] it reads.  Equal to one tapir_local_corr
+ * call per clip, bit for bit.  Every argument is checked first; a bad one returns 1. */
+int tapir_local_corr_ragged(const tapir_corr_args* args, int32_t batch, const int32_t* query_clip,
+                            void* stream);
 size_t tapir_mixer_workspace_bytes(int64_t rows, int32_t planes);
 int tapir_mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* workspace,
                         size_t workspace_bytes, void* stream);
@@ -555,6 +580,13 @@ int tapir_refine_update(const tapir_update_args* args, void* stream);
  * bit.  video_hw = NULL is tapir_refine_update. */
 int tapir_refine_update_ex(const tapir_update_args* args, const int32_t* video_hw,
                            int32_t rows_per_clip, void* stream);
+/* tapir_refine_update over clips with their own query counts and video sizes: row r = q *
+ * num_frames + t takes its clip's (video_h, video_w) from video_hw[query_clip[q]], where
+ * query_clip is a device int32 table [num_points] and video_hw a device int32 table [clips][2].
+ * Each clip's rows equal a tapir_refine_update call with its size, bit for bit.  Every argument is
+ * checked first; a bad one returns 1. */
+int tapir_refine_update_ragged(const tapir_update_args* args, const int32_t* video_hw,
+                               const int32_t* query_clip, void* stream);
 
 #ifdef __cplusplus
 }

@@ -27,6 +27,7 @@ MAX_MIXER_BLOCKS = 12
 NUM_RESNET_BLOCKS = 8
 MAX_EXTRA_BLOCKS = 5
 MAX_CORR_LEVELS = 5
+MAX_RAGGED_CLIPS = 64
 MAX_RESIZE_SIDE = 65535
 
 
@@ -220,10 +221,18 @@ SIGNATURES = {
                                                         c_int32, c_void_p, c_float, c_int32, c_int32,
                                                         c_void_p, c_void_p, c_void_p, c_void_p,
                                                         c_void_p, c_size_t, c_void_p]),
+    'tapir_cost_volume_ragged_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32, c_int32,
+                                                            c_int32, c_int32]),
+    'tapir_cost_volume_tracks_ragged': (ctypes.c_int, [POINTER(HeadWeights), c_void_p, c_void_p,
+                                                       c_int32, POINTER(c_int32), c_int32, c_int32,
+                                                       c_int32, c_int32, c_void_p, c_float, c_int32,
+                                                       c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                                       c_void_p, c_size_t, c_void_p]),
     'tapir_pool_pyramid': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p,
                                           c_void_p]),
     'tapir_local_corr': (ctypes.c_int, [POINTER(CorrArgs), c_void_p]),
     'tapir_local_corr_batched': (ctypes.c_int, [POINTER(CorrArgs), c_int32, c_void_p]),
+    'tapir_local_corr_ragged': (ctypes.c_int, [POINTER(CorrArgs), c_int32, c_void_p, c_void_p]),
     'tapir_mixer_workspace_bytes': (c_size_t, [c_int64, c_int32]),
     'tapir_mixer_forward': (ctypes.c_int, [POINTER(MixerWeights), POINTER(MixerIO), c_void_p,
                                            c_size_t, c_void_p]),
@@ -232,6 +241,7 @@ SIGNATURES = {
                                       c_void_p]),
     'tapir_refine_update': (ctypes.c_int, [POINTER(UpdateArgs), c_void_p]),
     'tapir_refine_update_ex': (ctypes.c_int, [POINTER(UpdateArgs), c_void_p, c_int32, c_void_p]),
+    'tapir_refine_update_ragged': (ctypes.c_int, [POINTER(UpdateArgs), c_void_p, c_void_p, c_void_p]),
     'tapir_paint_point_track_workspace_bytes': (c_size_t, [c_int32, c_int32]),
     'tapir_paint_point_track': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int32,
                                                c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_size_t,
@@ -594,13 +604,58 @@ def cost_volume_tracks(head, qfeat, grid, query_tyx, temperature, init_hw, point
       _nbytes(workspace), stream()), fn)
 
 
+def _counts(fn, counts):
+  """The per-clip query counts of a ragged call as a list of ints (1..MAX_RAGGED_CLIPS of them,
+  each >= 1)."""
+  counts = [int(c) for c in counts]
+  _need(1 <= len(counts) <= MAX_RAGGED_CLIPS, fn, f'{len(counts)} clips, 1..{MAX_RAGGED_CLIPS} supported')
+  _need(min(counts) >= 1, fn, f'every clip needs at least one query, got {counts}')
+  return counts
+
+
+def cost_volume_ragged_workspace_bytes(num_clips, total_points, grid_shape):
+  """cost_volume_tracks_ragged's workspace for num_clips clips with total_points queries in all
+  against grids of shape [num_clips, T, gh, gw, C]."""
+  return load().tapir_cost_volume_ragged_workspace_bytes(num_clips, total_points, *grid_shape[1:])
+
+
+def cost_volume_tracks_ragged(head, qfeat, counts, grid, query_tyx, temperature, init_hw, points,
+                              occ, expd, argmax, workspace):
+  """Stage A of B = len(counts) clips with counts[b] queries each: qfeat [Q, C] (the clips' queries
+  one after the other, Q = sum(counts)) against grid [B, T, gh, gw, C] -> points [Q, T, 2]
+  (initial-resolution pixels), occ, expd and (unless None) argmax [Q, T].  query_tyx: [Q, 3] in
+  initial-resolution coordinates, or None."""
+  fn = 'tapir_cost_volume_tracks_ragged'
+  counts = _counts(fn, counts)
+  B, Q = len(counts), sum(counts)
+  _check(fn, 'qfeat', qfeat, torch.float32)
+  _need(qfeat.dim() == 2 and qfeat.shape[0] == Q, fn, f'qfeat {tuple(qfeat.shape)} for {Q} queries')
+  C, dev = qfeat.shape[1], qfeat.device
+  _check(fn, 'grid', grid, torch.float32, device=dev)
+  _need(grid.dim() == 5 and grid.shape[0] == B and grid.shape[-1] == C, fn,
+        f'grid {tuple(grid.shape)} does not match {B} clips of {C}-channel queries')
+  _, T, gh, gw, _ = grid.shape
+  for name, t, dtype, shape in (('query_tyx', query_tyx, torch.float32, (Q, 3)),
+                                ('points', points, torch.float32, (Q, T, 2)),
+                                ('occ', occ, torch.float32, (Q, T)),
+                                ('expd', expd, torch.float32, (Q, T)),
+                                ('argmax', argmax, torch.int32, (Q, T))):
+    if t is not None or name in ('points', 'occ', 'expd'):
+      _check(fn, name, t, dtype, shape, device=dev)
+  check(load().tapir_cost_volume_tracks_ragged(
+      byref(head), ptr(qfeat), ptr(grid), B, (c_int32 * B)(*counts), T, gh, gw, C, ptr(query_tyx),
+      float(temperature), init_hw[0], init_hw[1], ptr(points), ptr(occ), ptr(expd), ptr(argmax),
+      ptr(workspace), _nbytes(workspace), stream()), fn)
+
+
 # ------------------------------------------------------------------------------ refinement
 # corr_args, mixer_io and update_args run once per refinement iteration on the host-bound online
 # step: one fused test per tensor (dtype, extent, contiguity), the device once per call.
-def corr_args(levels, pos, occ, expd, feat_hi, feat_lo, out_planes, init_hw):
+def corr_args(levels, pos, occ, expd, feat_hi, feat_lo, out_planes, init_hw, ragged=False):
   """CorrArgs of the local correlation of G clips.  levels: grids [G, T, h, w, C], hires first;
-  pos [..., T, 2], occ / expd [..., T] over Q = G x n queries; feat_hi / feat_lo [Q, T, 128 | 256]
-  views (stride 0 over T for per-query features); out_planes bf16 [P, Q * T, ld]."""
+  pos [..., T, 2], occ / expd [..., T] over Q = G x n queries (ragged: Q queries of the G clips in
+  all, num_points = Q); feat_hi / feat_lo [Q, T, 128 | 256] views (stride 0 over T for per-query
+  features); out_planes bf16 [P, Q * T, ld]."""
   fn, L = 'corr_args', len(levels)
   _need(1 <= L <= MAX_CORR_LEVELS, fn, f'{L} levels')
   (G, T), dev = levels[0].shape[:2], pos.device
@@ -610,7 +665,7 @@ def corr_args(levels, pos, occ, expd, feat_hi, feat_lo, out_planes, init_hw):
       _bad(fn, 'levels', g, f'contiguous float32 [{G}, {T}, h, w, C]')
   _need(levels[0].device == dev, fn, 'levels and pos on different devices')
   Q = pos.numel() // (2 * T) if T else 0
-  _need(Q % G == 0, fn, f'{Q} queries over {G} clips')
+  _need(ragged or Q % G == 0, fn, f'{Q} queries over {G} clips')
   _rows(fn, 'pos', pos, Q, T, 2)
   _rows(fn, 'occ', occ, Q, T, 0)
   _rows(fn, 'expd', expd, Q, T, 0)
@@ -618,7 +673,7 @@ def corr_args(levels, pos, occ, expd, feat_hi, feat_lo, out_planes, init_hw):
   _check(fn, 'out_planes', out_planes, torch.bfloat16, (P, Q * T, ld), False)
   _need(out_planes.stride(1) == ld and ld >= 388 + 49 * L, fn,
         f'out_planes rows must be dense and hold the {388 + 49 * L} mixer inputs')
-  ca = CorrArgs(num_levels=L, num_points=Q // G, num_frames=T, init_h=int(init_hw[0]),
+  ca = CorrArgs(num_levels=L, num_points=Q if ragged else Q // G, num_frames=T, init_h=int(init_hw[0]),
                 init_w=int(init_hw[1]), planes=P, pos=pos.data_ptr(), occ=occ.data_ptr(),
                 expd=expd.data_ptr(), out_planes=out_planes.data_ptr(),
                 out_plane_stride=out_planes.stride(0), ld=ld)
@@ -629,11 +684,17 @@ def corr_args(levels, pos, occ, expd, feat_hi, feat_lo, out_planes, init_hw):
   return ca
 
 
-def local_corr(*args):
-  """Local correlation of the G = levels[0].shape[0] clips of corr_args(*args) in one launch."""
-  ca = corr_args(*args)
-  check(load().tapir_local_corr_batched(byref(ca), args[0][0].shape[0], stream()),
-        'tapir_local_corr_batched')
+def local_corr(*args, query_clip=None):
+  """Local correlation of the G = levels[0].shape[0] clips of corr_args(*args) in one launch.
+  query_clip: None (clips of equal query counts), or int32 [Q] giving each query's clip."""
+  G = args[0][0].shape[0]
+  if query_clip is None:
+    ca = corr_args(*args)
+    return check(load().tapir_local_corr_batched(byref(ca), G, stream()), 'tapir_local_corr_batched')
+  fn = 'tapir_local_corr_ragged'
+  ca = corr_args(*args, ragged=True)
+  _check(fn, 'query_clip', query_clip, torch.int32, (ca.num_points,), device=args[1].device)
+  check(load().tapir_local_corr_ragged(byref(ca), G, ptr(query_clip), stream()), fn)
 
 
 def mixer_workspace_bytes(x_planes):
@@ -715,16 +776,22 @@ def update_args(res, pos, occ_in, expd_in, feat_hi, feat_lo, occ_out, expd_out, 
   return ua
 
 
-def refine_update(*args, video_table=None):
+def refine_update(*args, video_table=None, query_clip=None):
   """The track update of update_args(*args).  video_table: None, or int32 [G, 2] per-clip (h, w)
   of the G clips the rows run over (the tracks of each clip scaled to its own size; video_hw is
-  then not used)."""
+  then not used).  query_clip: None (clips of equal query counts), or int32 [Q] giving each
+  query's clip in video_table."""
   ua = update_args(*args)
   if video_table is None:
+    _need(query_clip is None, 'tapir_refine_update_ragged', 'query_clip needs a video_table')
     return check(load().tapir_refine_update(byref(ua), stream()), 'tapir_refine_update')
-  fn = 'tapir_refine_update_ex'
+  fn = 'tapir_refine_update_ex' if query_clip is None else 'tapir_refine_update_ragged'
   G = video_table.shape[0]
   _check(fn, 'video_table', video_table, torch.int32, (G, 2), device=args[0].device)
+  if query_clip is not None:
+    _check(fn, 'query_clip', query_clip, torch.int32, (ua.num_points,), device=args[0].device)
+    return check(load().tapir_refine_update_ragged(byref(ua), ptr(video_table), ptr(query_clip),
+                                                   stream()), fn)
   rows = ua.num_points * ua.num_frames
   _need(G >= 1 and rows % G == 0, fn, f'{rows} rows over {G} clips')
   check(load().tapir_refine_update_ex(byref(ua), ptr(video_table), rows // G, stream()), fn)

@@ -321,7 +321,7 @@ size_t tapir_cost_volume_workspace_bytes(int32_t N, int32_t T, int32_t gh, int32
 
 size_t tapir_cost_volume_batched_workspace_bytes(int32_t B, int32_t N, int32_t T, int32_t gh,
                                                  int32_t gw, int32_t C) {
-  return cost_volume_workspace_bytes(B, N, T, gh, gw, C);
+  return cost_volume_workspace_bytes(B, (long long)B * N, T, gh, gw, C);
 }
 
 int tapir_cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid,
@@ -346,6 +346,42 @@ int tapir_cost_volume_tracks_batched(const tapir_head_weights* w, const float* q
   return cost_volume_tracks(w, qfeat, grid, B, N, T, gh, gw, C, query_tyx, softmax_temperature,
                             init_h, init_w, points, occ, expd, argmax, workspace, workspace_bytes,
                             S(stream));
+}
+
+size_t tapir_cost_volume_ragged_workspace_bytes(int32_t B, int32_t total_points, int32_t T, int32_t gh,
+                                                int32_t gw, int32_t C) {
+  return cost_volume_workspace_bytes(B, total_points, T, gh, gw, C);
+}
+
+int tapir_cost_volume_tracks_ragged(const tapir_head_weights* w, const float* qfeat, const float* grid,
+                                    int32_t B, const int32_t* points_per_clip, int32_t T, int32_t gh,
+                                    int32_t gw, int32_t C, const float* query_tyx,
+                                    float softmax_temperature, int32_t init_h, int32_t init_w,
+                                    float* points, float* occ, float* expd, int32_t* argmax,
+                                    void* workspace, size_t workspace_bytes, void* stream) {
+  Range nvtx_range("tapir_cost_volume_tracks_ragged");
+  const char* fn = "tapir_cost_volume_tracks_ragged";
+  TAPIR_CHECK_ARG(w && qfeat && grid && points && occ && expd && points_per_clip && workspace,
+                  "%s: null pointer", fn);
+  TAPIR_CHECK_ARG(B >= 1 && B <= TAPIR_MAX_RAGGED_CLIPS, "%s: B=%d clips, 1..%d supported", fn, B,
+                  TAPIR_MAX_RAGGED_CLIPS);
+  long long total = 0;
+  for (int b = 0; b < B; ++b) {
+    TAPIR_CHECK_ARG(points_per_clip[b] >= 1, "%s: clip %d has %d points", fn, b, points_per_clip[b]);
+    total += points_per_clip[b];
+  }
+  TAPIR_CHECK_ARG(T >= 1 && gh >= 2 && gw >= 2 && C >= 64 && C % 64 == 0,
+                  "%s: T=%d map %d x %d C=%d (T >= 1, maps at least 2 x 2, C a multiple of 64)", fn, T, gh,
+                  gw, C);
+  TAPIR_CHECK_ARG(total < (1ll << 31) && (long long)B * T * gh * gw < (1ll << 31),
+                  "%s: %lld points over %d clips exceed one launch", fn, total, B);
+  TAPIR_CHECK_ARG(init_h >= 1 && init_w >= 1, "%s: init_h=%d init_w=%d", fn, init_h, init_w);
+  TAPIR_CHECK_ARG(aligned(qfeat, 16) && aligned(grid, 16), "%s: qfeat and grid must be 16-byte aligned", fn);
+  const size_t need = cost_volume_workspace_bytes(B, total, T, gh, gw, C);
+  TAPIR_CHECK_ARG(workspace_bytes >= need, "%s: workspace %zu bytes < %zu", fn, workspace_bytes, need);
+  return cost_volume_tracks_ragged(w, qfeat, grid, B, points_per_clip, T, gh, gw, C, query_tyx,
+                                   softmax_temperature, init_h, init_w, points, occ, expd, argmax,
+                                   workspace, workspace_bytes, S(stream));
 }
 
 int tapir_pool_pyramid(const float* grid, int32_t T, int32_t h, int32_t w, int32_t C, float* out,
@@ -396,6 +432,17 @@ int tapir_local_corr_batched(const tapir_corr_args* args, int32_t batch, void* s
   Range nvtx_range("tapir_local_corr_batched");
   TAPIR_RETURN_IF(check_corr_args(args, batch, "tapir_local_corr_batched"));
   return local_corr(args, batch, S(stream));
+}
+
+int tapir_local_corr_ragged(const tapir_corr_args* args, int32_t batch, const int32_t* query_clip,
+                            void* stream) {
+  Range nvtx_range("tapir_local_corr_ragged");
+  const char* fn = "tapir_local_corr_ragged";
+  TAPIR_RETURN_IF(check_corr_args(args, 1, fn));
+  TAPIR_CHECK_ARG(batch >= 1, "%s: bad clip count %d", fn, batch);
+  TAPIR_CHECK_ARG(query_clip != nullptr && aligned(query_clip, 4), "%s: query_clip must be a 4-byte aligned table",
+                  fn);
+  return local_corr(args, batch, S(stream), query_clip);
 }
 
 size_t tapir_mixer_workspace_bytes(int64_t rows, int32_t planes) {
@@ -477,6 +524,17 @@ int tapir_refine_update_ex(const tapir_update_args* args, const int32_t* video_h
   TAPIR_CHECK_ARG((reinterpret_cast<uintptr_t>(video_hw) & 3) == 0,
                   "tapir_refine_update_ex: video_hw not 4-byte aligned");
   return refine_update(args, S(stream), video_hw, rows_per_clip);
+}
+
+int tapir_refine_update_ragged(const tapir_update_args* args, const int32_t* video_hw,
+                               const int32_t* query_clip, void* stream) {
+  Range nvtx_range("tapir_refine_update_ragged");
+  const char* fn = "tapir_refine_update_ragged";
+  TAPIR_RETURN_IF(check_update_args(args, true, fn));
+  TAPIR_CHECK_ARG(args->tracks_out != nullptr, "%s: a video size table needs tracks_out", fn);
+  TAPIR_CHECK_ARG(video_hw != nullptr && query_clip != nullptr && aligned(video_hw, 4) && aligned(query_clip, 4),
+                  "%s: video_hw and query_clip must be 4-byte aligned device tables", fn);
+  return refine_update(args, S(stream), video_hw, 0, query_clip);
 }
 
 size_t tapir_paint_point_track_workspace_bytes(int32_t frames, int32_t points) {

@@ -18,6 +18,9 @@ namespace tapir {
 
 enum GemmMode : int { kGemmPlain = 0, kGemmConv3x3 = 1 };
 
+// Most problems of one grouped GEMM (GemmArgs::groups); TAPIR_MAX_RAGGED_CLIPS in the C ABI.
+constexpr int kGemmMaxGroups = TAPIR_MAX_RAGGED_CLIPS;
+
 struct GemmArgs {
   int mode = kGemmPlain;
   int planes = 2;  // P
@@ -59,7 +62,14 @@ struct GemmArgs {
   long long a_batch_rows = 0;      // 0 = M
   long long b_batch_rows = 0;      // 0 = N
   long long out_batch_stride = 0;  // elements; 0 = M * ldo
-  int k_logical = 0;        // un-padded K for FLOP accounting (0 = K)
+  // Grouped plain GEMM (groups > 0, batch 1): problem g owns A rows and output rows
+  // [group_row0[g], group_row0[g + 1]) and B rows [g * b_batch_rows, + N); M is the rows of all
+  // groups (group_row0[groups]).  An m-tile never crosses a group; rows of a group's last tile
+  // past its end are loaded but never stored.  The same epilogue limits as batch > 1, and K is
+  // never split.  The table travels in the kernel parameters, so a call needs no device copy.
+  int groups = 0;
+  int group_row0[kGemmMaxGroups + 1] = {};
+  int k_logical = 0;       // un-padded K for FLOP accounting (0 = K)
   const char* tag = nullptr;  // profiling class name
 };
 

@@ -3,6 +3,8 @@
 // switch (TAPIR_B200_GEMM=simt).  It reconstructs a = sum_i A_i, b = sum_j B_j in fp32 and
 // runs a shared-memory tiled fp32 GEMM; versus the tensor-core path it additionally contains
 // the dropped (i + j >= P) cross terms, i.e. it differs by <= 2^-16 relative for P=2.
+#include <algorithm>
+
 #include "gemm.cuh"
 
 namespace tapir {
@@ -14,12 +16,20 @@ constexpr int TM = 64, TN = 64, TK = 16;
 struct SimtParams {
   GemmArgs g;
   long long a_plane, b_plane;
-  long long a_batch_rows, b_batch_rows, out_batch_stride;  // batch = blockIdx.z
+  long long a_batch_rows, b_batch_rows, out_batch_stride;  // batch or group = blockIdx.z
 };
+
+// Rows of problem blockIdx.z (a batch or a group) and its first A and output row.
+__device__ __forceinline__ int problem_rows(const GemmArgs& g) {
+  return g.groups > 0 ? g.group_row0[blockIdx.z + 1] - g.group_row0[blockIdx.z] : g.M;
+}
+__device__ __forceinline__ long long problem_row0(const SimtParams& p) {
+  return p.g.groups > 0 ? p.g.group_row0[blockIdx.z] : (long long)blockIdx.z * p.a_batch_rows;
+}
 
 __device__ __forceinline__ float load_a(const SimtParams& p, int m, int k) {
   const GemmArgs& g = p.g;
-  if (m >= g.M) return 0.f;
+  if (m >= problem_rows(g)) return 0.f;
   long long off;
   if (g.mode == kGemmConv3x3) {
     const int tap = k / g.C, c = k - tap * g.C;
@@ -30,7 +40,7 @@ __device__ __forceinline__ float load_a(const SimtParams& p, int m, int k) {
     if (y < 0 || y >= g.H || x < 0 || x >= g.W) return 0.f;
     off = (((long long)f * g.H + y) * g.W + x) * g.C + c;
   } else {
-    off = ((long long)blockIdx.z * p.a_batch_rows + m) * g.lda + k;
+    off = (problem_row0(p) + m) * g.lda + k;
   }
   float v = 0.f;
   for (int i = 0; i < g.planes; ++i) v += __bfloat162float(g.a[i * p.a_plane + off]);
@@ -46,13 +56,16 @@ __device__ __forceinline__ float load_b(const SimtParams& p, int n, int k) {
   return v;
 }
 
-__global__ void __launch_bounds__(256) gemm_simt_kernel(const SimtParams p) {
+__global__ void __launch_bounds__(256) gemm_simt_kernel(const __grid_constant__ SimtParams p) {
   __shared__ float As[TK][TM + 4];
   __shared__ float Bs[TK][TN + 4];
   const GemmArgs& g = p.g;
   const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
   const int m0 = blockIdx.x * TM, n0 = blockIdx.y * TN;
-  float* out_f32 = g.out_f32 != nullptr ? g.out_f32 + blockIdx.z * p.out_batch_stride : nullptr;
+  const int rows = problem_rows(g);
+  float* out_f32 = g.out_f32 == nullptr ? nullptr
+                   : g.groups > 0       ? g.out_f32 + problem_row0(p) * g.ldo
+                                        : g.out_f32 + blockIdx.z * p.out_batch_stride;
   float acc[4][4] = {};
   for (int k0 = 0; k0 < g.K; k0 += TK) {
     for (int e = threadIdx.x; e < TM * TK; e += 256) {
@@ -77,7 +90,7 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const SimtParams p) {
   }
   for (int i = 0; i < 4; ++i) {
     const long long m = m0 + ty * 4 + i;
-    if (m >= g.M) continue;
+    if (m >= rows) continue;
     for (int j = 0; j < 4; ++j) {
       const int n = n0 + tx * 4 + j;
       if (n >= g.N) continue;
@@ -119,10 +132,17 @@ int gemm_simt(const GemmArgs& g, cudaStream_t stream) {
   } else {
     p.a_plane = g.a_plane_stride > 0 ? g.a_plane_stride : ((g.batch - 1) * p.a_batch_rows + g.M) * g.lda;
   }
-  p.b_plane = g.b_plane_stride > 0 ? g.b_plane_stride : ((g.batch - 1) * p.b_batch_rows + g.N) * g.ldb;
+  p.b_plane = g.b_plane_stride > 0 ? g.b_plane_stride
+                                   : ((std::max(g.batch, g.groups) - 1) * p.b_batch_rows + g.N) * g.ldb;
   ProfileScope ps(g.tag ? g.tag : "gemm", stream,
                   2.0 * g.batch * g.M * g.N * (g.k_logical > 0 ? g.k_logical : g.K), 0.0);
-  dim3 grid(ceil_div(g.M, TM), ceil_div(g.N, TN), g.batch);
+  int rows = g.M, problems = g.batch;
+  if (g.groups > 0) {
+    problems = g.groups;
+    rows = 0;
+    for (int i = 0; i < g.groups; ++i) rows = std::max(rows, g.group_row0[i + 1] - g.group_row0[i]);
+  }
+  dim3 grid(ceil_div(rows, TM), ceil_div(g.N, TN), problems);
   gemm_simt_kernel<<<grid, 256, 0, stream>>>(p);
   count_launch();
   TAPIR_LAUNCH_CHECK("gemm_simt_kernel");

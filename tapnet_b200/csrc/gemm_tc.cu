@@ -73,6 +73,8 @@ struct TcParams {
   long long split_stride;  // elements between partial buffers (M * ldo)
   int m_tiles_per_batch;   // batched plain GEMM: m-tiles of one batch (= num_m_tiles when batch 1)
   long long a_batch_rows, b_batch_rows, out_batch_stride;
+  int groups;  // grouped plain GEMM (GemmArgs::groups): group g's first row and first m-tile
+  int group_row0[kGemmMaxGroups + 1], group_tile0[kGemmMaxGroups + 1];
   int* err;
 };
 
@@ -318,8 +320,10 @@ __device__ __forceinline__ ConvTile conv_tile(const TcParams& p, int m_tile) {
   return {frame, (r / p.tiles_x) * p.tileH, (r % p.tiles_x) * p.tileW};
 }
 
-// Global row of tile row r (0..127) of output tile `m_tile`, and whether it exists.
-__device__ __forceinline__ void tile_row(const TcParams& p, int m_tile, int r, long long& row, bool& ok) {
+// Global row of tile row r (0..127) of output tile `m_tile`, and whether it exists; a plain tile's
+// problem has m_rows rows.
+__device__ __forceinline__ void tile_row(const TcParams& p, int m_tile, int m_rows, int r, long long& row,
+                                         bool& ok) {
   if (p.mode == kGemmConv3x3) {
     const ConvTile ct = conv_tile(p, m_tile);
     const int y = ct.y0 + r / p.tileW;
@@ -328,7 +332,7 @@ __device__ __forceinline__ void tile_row(const TcParams& p, int m_tile, int r, l
     row = ((long long)ct.frame * p.H + y) * p.W + x;
   } else {
     row = (long long)m_tile * kBlockM + r;
-    ok = row < p.M;
+    ok = row < m_rows;
   }
 }
 
@@ -336,13 +340,13 @@ __device__ __forceinline__ void tile_row(const TcParams& p, int m_tile, int r, l
 // `red`: the warpgroup's statistics slots (add: the tile's other half is already in them).
 template <int BLOCK_N>
 __device__ __forceinline__ void tile_epilogue(const TcParams& p, const float (&acc)[BLOCK_N / 2], int m_tile,
-                                              int r_base, int n0, int warp, int lane, long long out_off,
+                                              int m_rows, int r_base, int n0, int warp, int lane, long long out_off,
                                               double* red, bool add) {
   const int r0 = r_base + warp * 16 + (lane >> 2);
   long long row[2];
   bool row_ok[2];
-  tile_row(p, m_tile, r0, row[0], row_ok[0]);
-  tile_row(p, m_tile, r0 + 8, row[1], row_ok[1]);
+  tile_row(p, m_tile, m_rows, r0, row[0], row_ok[0]);
+  tile_row(p, m_tile, m_rows, r0 + 8, row[1], row_ok[1]);
   epilogue<BLOCK_N>(p, acc, row, row_ok, n0, lane, out_off, red + warp * 2 * BLOCK_N, add);
 }
 
@@ -358,7 +362,7 @@ template <int BLOCK_N>
 __device__ __forceinline__ bool whole_tile(const TcParams& p, int m_tile, int n0) {
   long long last;
   bool ok;
-  tile_row(p, m_tile, kBlockM - 1, last, ok);
+  tile_row(p, m_tile, p.M, kBlockM - 1, last, ok);
   return ok && n0 + BLOCK_N <= p.N;
 }
 
@@ -377,7 +381,7 @@ __device__ __forceinline__ void epilogue_planes_tma(const TcParams& p, float (&a
   const bool issuer = warp == 0 && lane == 0;
   long long row0;
   bool ok;
-  tile_row(p, m_tile, r_base, row0, ok);
+  tile_row(p, m_tile, p.M, r_base, row0, ok);
   // stmatrix: lanes 8 i .. 8 i + 7 address the rows of matrix i, rows 8 (i & 1) on, column group i >> 1
   const uint32_t rr = lane & 7;
   const uint32_t row_addr = (uint32_t)(16 * warp + 8 * ((lane >> 3) & 1) + rr) * 128;
@@ -423,8 +427,20 @@ __device__ __forceinline__ void epilogue_planes_tma(const TcParams& p, float (&a
   }
 }
 
-// Work item w in the order (batch, m-tile, n-tile, k-slice); m_tile is the tile within its batch,
-// [kb0, kb1) its k-blocks.  Returns the k-slice.
+// The group of linear m-tile `m_tile` of a grouped GEMM: the last g with group_tile0[g] <= m_tile
+// (every group has at least one tile).
+__device__ __forceinline__ int tile_group(const TcParams& p, int m_tile) {
+  int lo = 0, hi = p.groups - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (p.group_tile0[mid] <= m_tile) lo = mid;
+    else hi = mid - 1;
+  }
+  return lo;
+}
+
+// Work item w in the order (batch or group, m-tile, n-tile, k-slice); m_tile is the tile within its
+// batch or group, [kb0, kb1) its k-blocks.  Returns the k-slice.
 template <int BLOCK_N>
 __device__ __forceinline__ int decode_work(const TcParams& p, int w, int& bat, int& m_tile, int& n0, int& kb0,
                                            int& kb1) {
@@ -433,8 +449,13 @@ __device__ __forceinline__ int decode_work(const TcParams& p, int w, int& bat, i
   const int tile = w / S;
   m_tile = tile / p.num_n_tiles;
   n0 = (tile - m_tile * p.num_n_tiles) * BLOCK_N;
-  bat = m_tile / p.m_tiles_per_batch;
-  m_tile -= bat * p.m_tiles_per_batch;
+  if (p.groups > 0) {
+    bat = tile_group(p, m_tile);
+    m_tile -= p.group_tile0[bat];
+  } else {
+    bat = m_tile / p.m_tiles_per_batch;
+    m_tile -= bat * p.m_tiles_per_batch;
+  }
   // 32-bit: num_k_blocks < 2^25 and S <= 8.  A 64-bit division here is a subroutine call, which
   // the ping-pong consumers would pay twice between their epilogue and their next turn.
   kb0 = p.num_k_blocks * split / S;
@@ -459,10 +480,12 @@ struct StageCursor {
 };
 
 // A work item as the consumers see it: output tile (m_tile, n0), the offset of its fp32 output
-// (k-slice partial buffer and batch), and its k-blocks [kb0, kb1).
+// (k-slice partial buffer and batch or group), its k-blocks [kb0, kb1) and, in plain mode, the rows
+// of its problem.
 struct Work {
   int m_tile, n0, kb0, kb1;
   long long out_off;
+  int m_rows;
 };
 
 // The dynamic shared memory from its first 1024-byte boundary: the 128B swizzle of TMA and wgmma
@@ -574,7 +597,13 @@ struct Ring {
     Work wk;
     int bat;
     const int split = decode_work<BLOCK_N>(p, w, bat, wk.m_tile, wk.n0, wk.kb0, wk.kb1);
-    wk.out_off = split * p.split_stride + bat * p.out_batch_stride;
+    if (p.groups > 0) {
+      wk.out_off = split * p.split_stride + (long long)p.group_row0[bat] * p.ldo;
+      wk.m_rows = p.group_row0[bat + 1] - p.group_row0[bat];
+    } else {
+      wk.out_off = split * p.split_stride + bat * p.out_batch_stride;
+      wk.m_rows = p.M;
+    }
     return wk;
   }
   __device__ __forceinline__ void kblock(int, int stage, int, uint32_t& a, uint32_t& b) const {
@@ -592,9 +621,9 @@ struct Ring {
     for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
       int bat, m_tile, n0, kb0, kb1;
       decode_work<BLOCK_N>(p, w, bat, m_tile, n0, kb0, kb1);
-      // batch = row offset into the flattened operands; rows loaded past the end of a batch
-      // belong to the next one (or are TMA zero fill) and are masked by the epilogue
-      const int a_row0 = (int)(bat * p.a_batch_rows) + m_tile * kBlockM;
+      // batch or group = row offset into the flattened operands; rows loaded past the end of a
+      // batch or group belong to the next one (or are TMA zero fill) and are masked by the epilogue
+      const int a_row0 = (p.groups > 0 ? p.group_row0[bat] : (int)(bat * p.a_batch_rows)) + m_tile * kBlockM;
       const int b_row0 = (int)(bat * p.b_batch_rows) + n0;
       ConvTile ct{0, 0, 0};
       if (p.mode == kGemmConv3x3) ct = conv_tile(p, m_tile);
@@ -707,7 +736,7 @@ struct HaloRing {
     }
   }
 
-  __device__ __forceinline__ Work work(const TcParams&, int w) const { return {w, 0, 0, 9, 0}; }
+  __device__ __forceinline__ Work work(const TcParams&, int w) const { return {w, 0, 0, 9, 0, 0}; }
   // tap kb = 3 ky + kx: the patch view of output rows 0-7 (see above)
   __device__ __forceinline__ void kblock(int t, int stage, int kb, uint32_t& a, uint32_t& b) const {
     const int ky = kb / 3, kx = kb - ky * 3;
@@ -834,7 +863,8 @@ __device__ __forceinline__ void wgmma_kernel(const TcParams& p) {
                                                 warp, lane);
         }
       } else {
-        tile_epilogue<BLOCK_N>(p, acc[0], wk.m_tile, r_base, wk.n0, warp, lane, wk.out_off, red, h == 1);
+        tile_epilogue<BLOCK_N>(p, acc[0], wk.m_tile, wk.m_rows, r_base, wk.n0, warp, lane, wk.out_off, red,
+                               h == 1);
       }
       if constexpr (HALVES == 2) {
         if (h == 0) {
@@ -1052,10 +1082,10 @@ int launch_gemm(int bn, bool pingpong, const TcParams& p, const GemmArgs& g, cud
 // tiles per CTA, and measured on H100 it loses to the cooperative kernel when CTAs get fewer than
 // four tiles of short (< 16 k-block) mainloops: mixer linear_in / linear_out, 2.9 tiles of 8-9
 // k-blocks, ran 10-22 % slower.  Split-K work items, P = 3 and batched GEMMs (only the P = 3 cost
-// volume is batched) stay cooperative.  Elsewhere, and in the halo convolution (launch_halo),
+// volume is batched or grouped) stay cooperative.  Elsewhere, and in the halo convolution (launch_halo),
 // TAPIR_B200_GEMM_SCHEDULE (sw.schedule) forces either schedule.
-bool pick_pingpong(int tiles, int num_k_blocks, int P, int batch, const GemmSwitches& sw) {
-  if (P > 2 || batch > 1) return false;
+bool pick_pingpong(int tiles, int num_k_blocks, int P, bool batched, const GemmSwitches& sw) {
+  if (P > 2 || batched) return false;
   if (sw.schedule != 0) return sw.schedule == 2;
   const int sms = num_sms();
   return tiles >= 2 * sms && (tiles >= 4 * sms || num_k_blocks >= 16);
@@ -1132,6 +1162,15 @@ int common_params(const GemmArgs& g, TcParams* p) {
     p->tiles_y = ceil_div(g.H, p->tileH);
     p->num_m_tiles = g.frames * p->tiles_x * p->tiles_y;
     TAPIR_RETURN_IF(encode_nhwc_map(&p->tmA, g, p->tileW, p->tileH, "A/conv"));
+  } else if (g.groups > 0) {
+    p->groups = g.groups;
+    for (int i = 0; i < g.groups; ++i) {
+      p->group_row0[i] = g.group_row0[i];
+      p->group_tile0[i + 1] = p->group_tile0[i] + ceil_div(g.group_row0[i + 1] - g.group_row0[i], kBlockM);
+    }
+    p->group_row0[g.groups] = g.group_row0[g.groups];
+    p->num_m_tiles = p->group_tile0[g.groups];
+    TAPIR_RETURN_IF(encode_rows_map(&p->tmA, g.a, g.K, g.M, g.lda, g.a_plane_stride, g.planes, kBlockM, "A"));
   } else {
     p->num_m_tiles = ceil_div(g.M, kBlockM) * g.batch;
     TAPIR_RETURN_IF(encode_rows_map(&p->tmA, g.a, g.K, (g.batch - 1) * p->a_batch_rows + g.M, g.lda,
@@ -1176,7 +1215,8 @@ int launch_halo(TcParams p, const GemmArgs& g, const GemmSwitches& sw, cudaStrea
 // (tests/test_properties_gpu.py re-chunks config 2 into 1776-row chunks,
 // tests/multi_gpu_check.py shards 1152 rows over two ranks, both demand bit-level agreement).
 bool splittable(const GemmArgs& g) {
-  return g.allow_splitk && g.splitk_ws != nullptr && g.stats == nullptr && g.batch == 1 && g.K / kBlockK >= 32;
+  return g.allow_splitk && g.splitk_ws != nullptr && g.stats == nullptr && g.batch == 1 && g.groups == 0 &&
+         g.K / kBlockK >= 32;
 }
 
 // Row stride of the split-K partials: whole float4 groups for the reduction.
@@ -1273,6 +1313,19 @@ int validate_gemm_args(const GemmArgs& g) {
     TAPIR_CHECK_ARG(arows >= g.M && brows >= g.N && arows * g.batch < (1ll << 31) && brows * g.batch < (1ll << 31),
                     "gemm: batch strides out of range");
   }
+  if (g.groups != 0) {
+    TAPIR_CHECK_ARG(g.groups >= 1 && g.groups <= kGemmMaxGroups && g.batch == 1,
+                    "gemm: groups=%d must be 1..%d, with batch 1", g.groups, kGemmMaxGroups);
+    TAPIR_CHECK_ARG(g.mode == kGemmPlain && g.out_f32 != nullptr && g.out_planes == nullptr &&
+                        g.residual == nullptr && g.stats == nullptr,
+                    "gemm: a grouped GEMM is plain mode with an fp32 output and no residual or statistics");
+    TAPIR_CHECK_ARG(g.b_batch_rows >= 0 && (long long)(g.groups - 1) * (g.b_batch_rows > 0 ? g.b_batch_rows : g.N) +
+                                               g.N < (1ll << 31),
+                    "gemm: group B rows out of range");
+    TAPIR_CHECK_ARG(g.group_row0[0] == 0 && g.group_row0[g.groups] == g.M, "gemm: group rows must cover [0, M)");
+    for (int i = 0; i < g.groups; ++i)
+      TAPIR_CHECK_ARG(g.group_row0[i + 1] > g.group_row0[i], "gemm: group %d has no rows", i);
+  }
   if (g.stats != nullptr) {
     TAPIR_CHECK_ARG(g.out_planes == nullptr, "gemm: fused statistics need an fp32-only output");
     if (g.mode == kGemmPlain)
@@ -1290,12 +1343,13 @@ int gemm_tc(const GemmArgs& g, const GemmSwitches& sw, cudaStream_t stream) {
   const bool split = splittable(g);
   const int bn = pick_block_n(p.num_m_tiles, g.N, split, sw);
   p.num_n_tiles = ceil_div(g.N, bn);
-  TAPIR_RETURN_IF(encode_rows_map(&p.tmB, g.b, g.K, (g.batch - 1) * p.b_batch_rows + g.N, g.ldb,
+  const int b_problems = g.groups > 0 ? g.groups : g.batch;
+  TAPIR_RETURN_IF(encode_rows_map(&p.tmB, g.b, g.K, (b_problems - 1) * p.b_batch_rows + g.N, g.ldb,
                                   g.b_plane_stride, g.planes, bn, "B"));
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   const int S = split ? split_k_factor(g, tiles) : 1;
   if (S > 1) return launch_split_k(p, bn, S, g, stream);
-  const bool pingpong = pick_pingpong(tiles, p.num_k_blocks, g.planes, g.batch, sw);
+  const bool pingpong = pick_pingpong(tiles, p.num_k_blocks, g.planes, g.batch > 1 || g.groups > 0, sw);
   TAPIR_RETURN_IF(plane_store_params(g, pingpong, &p));
   return launch_gemm(bn, pingpong, p, g, stream);
 }

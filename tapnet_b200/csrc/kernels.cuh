@@ -95,16 +95,24 @@ int sample_query_features(const float* grid, int T, int gh, int gw, int C, const
                           int N, int vT, int vH, int vW, const int* frame_slot, float* out,
                           cudaStream_t s);
 // B clips: qfeat [B][N][C], grid [B][T][gh][gw][C], outputs indexed by flattened query b*N + n
-size_t cost_volume_workspace_bytes(int B, int N, int T, int gh, int gw, int C);
+// (the workspace of B clips with Q queries in all)
+size_t cost_volume_workspace_bytes(int B, long long Q, int T, int gh, int gw, int C);
 int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid, int B,
                        int N, int T, int gh, int gw, int C, const float* query_tyx, float temperature,
                        int init_h, int init_w, float* points, float* occ, float* expd, int* argmax,
                        void* ws, size_t ws_bytes, cudaStream_t s);
+// B <= kGemmMaxGroups clips of counts[b] (host) queries each, one after the other in qfeat [Q][C]
+int cost_volume_tracks_ragged(const tapir_head_weights* w, const float* qfeat, const float* grid, int B,
+                              const int* counts, int T, int gh, int gw, int C, const float* query_tyx,
+                              float temperature, int init_h, int init_w, float* points, float* occ,
+                              float* expd, int* argmax, void* ws, size_t ws_bytes, cudaStream_t s);
 
 // ---- refinement (refine.cu) -------------------------------------------------------------
 int pool_pyramid(const float* grid, int T, int h, int w, int C, float* out, cudaStream_t s);
-// a->num_points queries per clip, `batch` clips; level grids are [batch][T][h][w][C]
-int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s);
+// a->num_points queries per clip, `batch` clips; level grids are [batch][T][h][w][C].  With a
+// device table query_clip [a->num_points], a->num_points is the queries of all clips and query q
+// reads the grids of clip query_clip[q].
+int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s, const int32_t* query_clip = nullptr);
 size_t mixer_workspace_bytes(long long rows, int planes);
 int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* ws, size_t ws_bytes,
                   cudaStream_t s);
@@ -113,8 +121,9 @@ int mixer_forward(const tapir_mixer_weights* w, const tapir_mixer_io* io, void* 
 int mixer_dw(const tapir_mixer_block& blk, const float* x, int n, int T, bool causal, const float* ctx1_in,
              const float* ctx2_in, float* ctx1_out, float* ctx2_out, float* z, __nv_bfloat16* planes_out,
              long long plane_stride, int planes, cudaStream_t s);
-// video_hw: NULL, or a device table [clips][2] of per-clip video sizes (rows_per_clip rows each)
+// video_hw: NULL, or a device table [clips][2] of per-clip video sizes (rows_per_clip rows each,
+// or, with a device table query_clip [a->num_points], query q's rows are clip query_clip[q]'s)
 int refine_update(const tapir_update_args* a, cudaStream_t s, const int32_t* video_hw = nullptr,
-                  long long rows_per_clip = 0);
+                  long long rows_per_clip = 0, const int32_t* query_clip = nullptr);
 
 }  // namespace tapir

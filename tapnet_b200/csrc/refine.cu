@@ -50,6 +50,7 @@ constexpr int kBoxCells = kBoxRows * kBoxColsMax;
 struct CorrParams {
   tapir_corr_args a;
   int batch;  // clips; query q = b * a.num_points + n reads frame b * T + t of every level
+  const int32_t* query_clip;  // or: a.num_points queries in all, query q of clip query_clip[q]
 };
 
 template <int V>  // V = C / 128 float4 per lane
@@ -104,10 +105,10 @@ __global__ void __launch_bounds__(32 * TAPIR_MAX_CORR_LEVELS) local_corr_kernel(
   // frames (3.3 MB per frame at 256^2), which therefore stay in L2; the row order (n, t) of the
   // inputs / outputs would cycle through every frame's grids (all of them exceed L2) per query.
   // n is the query flattened over the clips, b its clip.
-  const unsigned nq = (unsigned)a.num_points * (unsigned)p.batch;
+  const unsigned nq = (unsigned)a.num_points * (p.query_clip != nullptr ? 1u : (unsigned)p.batch);
   const int t = (int)(blockIdx.x / nq);
   const int n = (int)(blockIdx.x - (unsigned)t * nq);
-  const int b = n / a.num_points;
+  const int b = p.query_clip != nullptr ? p.query_clip[n] : n / a.num_points;
   const long long row = (long long)n * T + t;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float px = a.pos[row * 2 + 0], py = a.pos[row * 2 + 1];
@@ -507,10 +508,12 @@ __global__ void __launch_bounds__(512, SMALL ? 1 : 2) mixer_dw_kernel(const DwPa
 }
 
 // ------------------------------------------------------------------------ a7 epilogue
-// video_hw (nullable): per-clip video sizes [clips][2], clip = row / rows_per_clip
+// video_hw (nullable): per-clip video sizes [clips][2], clip = row / rows_per_clip, or
+// query_clip[query] when query_clip is not null
 __global__ void __launch_bounds__(128) refine_update_kernel(const tapir_update_args a,
                                                             const int32_t* __restrict__ video_hw,
-                                                            long long rows_per_clip) {
+                                                            long long rows_per_clip,
+                                                            const int32_t* __restrict__ query_clip) {
   const long long row = blockIdx.x;
   const int T = a.num_frames;
   const int n = (int)(row / T), t = (int)(row - (long long)n * T);
@@ -533,7 +536,7 @@ __global__ void __launch_bounds__(128) refine_update_kernel(const tapir_update_a
     if (a.tracks_out != nullptr) {
       int vh = a.video_h, vw = a.video_w;
       if (video_hw != nullptr) {
-        const long long clip = row / rows_per_clip;
+        const long long clip = query_clip != nullptr ? query_clip[n] : row / rows_per_clip;
         vh = video_hw[clip * 2 + 0];
         vw = video_hw[clip * 2 + 1];
       }
@@ -565,7 +568,7 @@ int pool_pyramid(const float* grid, int T, int h, int w, int C, float* out, cuda
   return kOk;
 }
 
-int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s) {
+int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s, const int32_t* query_clip) {
   TAPIR_CHECK_ARG(a != nullptr && a->num_levels >= 1 && a->num_levels <= TAPIR_MAX_CORR_LEVELS,
                   "local_corr: bad level count");
   TAPIR_CHECK_ARG(batch >= 1, "local_corr: bad clip count %d", batch);
@@ -581,11 +584,12 @@ int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s) {
     // (x spacing of the 49 samples is gw/gh cells - a reference quirk; boxes wider than the
     // 16-column table take the per-sample path inside the kernel)
   }
-  const long long rows = (long long)a->num_points * batch * a->num_frames;
+  const long long rows = (long long)a->num_points * (query_clip != nullptr ? 1 : batch) * a->num_frames;
   TAPIR_CHECK_ARG(rows < (1ll << 31), "local_corr: %lld rows exceed one launch", rows);
   CorrParams p;
   p.a = *a;
   p.batch = batch;
+  p.query_clip = query_clip;
   double cell_bytes = 0;
   for (int l = 0; l < a->num_levels; ++l) cell_bytes += 64.0 * a->levels[l].C * 4;
   // SURVEY.md 8(d): N*T*(64 cells * sum C * e + 384*4 + 8 + 147*4)
@@ -598,12 +602,12 @@ int local_corr(const tapir_corr_args* a, int batch, cudaStream_t s) {
 }
 
 int refine_update(const tapir_update_args* a, cudaStream_t s, const int32_t* video_hw,
-                  long long rows_per_clip) {
+                  long long rows_per_clip, const int32_t* query_clip) {
   TAPIR_CHECK_ARG(a != nullptr && a->res && a->pos && a->feat_out && a->occ_out && a->expd_out,
                   "refine_update: null pointer");
   const long long rows = (long long)a->num_points * a->num_frames;
   ProfileScope ps("refine_update", s, 0.0, (double)rows * (388 * 4 + 384 * 8));
-  refine_update_kernel<<<(unsigned)rows, 128, 0, s>>>(*a, video_hw, rows_per_clip);
+  refine_update_kernel<<<(unsigned)rows, 128, 0, s>>>(*a, video_hw, rows_per_clip, query_clip);
   count_launch();
   TAPIR_LAUNCH_CHECK("refine_update_kernel");
   return kOk;

@@ -595,16 +595,16 @@ struct CvPlan {
   int generic_ctas;
 };
 constexpr int kGenericCtasPerSm = 4;
-// B clips of N queries and T frames each
-size_t plan_cv(Arena& a, int B, int N, int T, int gh, int gw, int C, CvPlan* p) {
+// B clips of T frames with Q queries in all
+size_t plan_cv(Arena& a, int B, long long Q, int T, int gh, int gw, int C, CvPlan* p) {
   const long long cells = (long long)T * gh * gw;
-  p->q = a.take<__nv_bfloat16>((size_t)B * N * C * kCvPlanes);
+  p->q = a.take<__nv_bfloat16>((size_t)Q * C * kCvPlanes);
   p->g = a.take<__nv_bfloat16>((size_t)B * cells * C * kCvPlanes);
-  p->cv = a.take<float>((size_t)B * N * cells);
+  p->cv = a.take<float>((size_t)Q * cells);
   p->generic_scratch = nullptr;
   p->generic_ctas = 0;
   if (gh != kG || gw != kG) {
-    const long long maps = (long long)B * N * T;
+    const long long maps = Q * T;
     const long long cap = 132ll * kGenericCtasPerSm;  // independent of the device: sizes must agree
     p->generic_ctas = (int)(maps < cap ? maps : cap);
     p->generic_scratch =
@@ -612,52 +612,62 @@ size_t plan_cv(Arena& a, int B, int N, int T, int gh, int gw, int C, CvPlan* p) 
   }
   return a.off;
 }
-}  // namespace
-
-size_t cost_volume_workspace_bytes(int B, int N, int T, int gh, int gw, int C) {
-  if (B < 1) return 0;
-  Arena a(nullptr, 0);
-  CvPlan p;
-  return plan_cv(a, B, N, T, gh, gw, C, &p) + 256;
-}
-
-int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid, int B,
-                       int N, int T, int gh, int gw, int C, const float* query_tyx, float temperature,
-                       int init_h, int init_w, float* points, float* occ, float* expd, int* argmax,
-                       void* ws, size_t ws_bytes, cudaStream_t s) {
+// B clips of N queries each (counts == nullptr) or of counts[b] queries; their T frames of
+// cost maps.  One batched or grouped GEMM, then one head launch over the flattened queries.
+int run_cost_volume(const tapir_head_weights* w, const float* qfeat, const float* grid, int B, int N,
+                    const int* counts, int T, int gh, int gw, int C, const float* query_tyx,
+                    float temperature, int init_h, int init_w, float* points, float* occ, float* expd,
+                    int* argmax, void* ws, size_t ws_bytes, cudaStream_t s) {
   TAPIR_CHECK_ARG(w && qfeat && grid && points && occ && expd, "cost_volume_tracks: null pointer");
-  TAPIR_CHECK_ARG(B > 0, "cost_volume_tracks: bad clip count B=%d", B);
-  TAPIR_CHECK_ARG(N > 0 && T > 0 && C % 64 == 0, "cost_volume_tracks: bad shape N=%d T=%d C=%d", N, T, C);
+  TAPIR_CHECK_ARG(B > 0 && (counts == nullptr || B <= kGemmMaxGroups), "cost_volume_tracks: bad clip count B=%d", B);
+  long long Q = (long long)B * N;
+  if (counts != nullptr) {
+    Q = 0;
+    for (int b = 0; b < B; ++b) {
+      TAPIR_CHECK_ARG(counts[b] > 0, "cost_volume_tracks: clip %d has %d queries", b, counts[b]);
+      Q += counts[b];
+    }
+  }
+  TAPIR_CHECK_ARG((counts != nullptr || N > 0) && T > 0 && C % 64 == 0,
+                  "cost_volume_tracks: bad shape N=%d T=%d C=%d", N, T, C);
   TAPIR_CHECK_ARG(gh >= 2 && gw >= 2, "cost_volume_tracks: map %dx%d too small", gh, gw);
   // the documented per-call query limit for 32 x 32 maps (tapir_cost_volume_tracks_batched), the
   // same as the mixer's that refines these tracks
-  TAPIR_CHECK_ARG((gh != kG || gw != kG) || (long long)B * N <= 65535,
-                  "cost_volume_tracks: at most 65535 queries per call (B*N=%lld)", (long long)B * N);
+  TAPIR_CHECK_ARG((gh != kG || gw != kG) || Q <= 65535,
+                  "cost_volume_tracks: at most 65535 queries per call (%lld)", Q);
+  TAPIR_CHECK_ARG(Q < (1ll << 31), "cost_volume_tracks: %lld queries", Q);
   Arena arena(ws, ws_bytes);
   CvPlan p;
-  plan_cv(arena, B, N, T, gh, gw, C, &p);
+  plan_cv(arena, B, Q, T, gh, gw, C, &p);
   if (!arena.ok) {
     set_error("cost_volume_tracks: workspace too small (%zu < %zu)", ws_bytes, arena.off);
     return kWorkspaceTooSmall;
   }
-  // qfeat [B][N][C] -> planes [3][B*N][C]; grid [B][T][gh][gw][C] -> planes [3][B*cells][C]
+  // qfeat [Q][C] -> planes [3][Q][C]; grid [B][T][gh][gw][C] -> planes [3][B*cells][C]
   const long long cells = (long long)T * gh * gw;
-  const int BN = B * N;
+  const int BN = (int)Q;
   TAPIR_RETURN_IF(split_planes(qfeat, C, p.q, C, (long long)BN * C, BN, C, C, kCvPlanes, s));
   TAPIR_RETURN_IF(split_planes(grid, C, p.g, C, B * cells * C, B * cells, C, C, kCvPlanes, s));
-  // one batched GEMM: cv [B*N][cells], clip b = queries b*N.. against cells b*cells..
   GemmArgs g;
   g.planes = kCvPlanes;
-  g.M = N;
   g.N = (int)cells;
   g.K = C;
   g.a = p.q; g.lda = C; g.a_plane_stride = (long long)BN * C;
   g.b = p.g; g.ldb = C; g.b_plane_stride = B * cells * C;
   g.out_f32 = p.cv; g.ldo = (int)cells;
-  g.batch = B;
-  g.a_batch_rows = N;
   g.b_batch_rows = cells;
-  g.out_batch_stride = (long long)N * cells;
+  if (counts == nullptr) {
+    // one batched GEMM: cv [B*N][cells], clip b = queries b*N.. against cells b*cells..
+    g.M = N;
+    g.batch = B;
+    g.a_batch_rows = N;
+    g.out_batch_stride = (long long)N * cells;
+  } else {
+    // one grouped GEMM: cv [Q][cells], clip b = its queries against cells b*cells..
+    g.M = BN;
+    g.groups = B;
+    for (int b = 0; b < B; ++b) g.group_row0[b + 1] = g.group_row0[b] + counts[b];
+  }
   g.tag = "cost_volume.gemm";
   TAPIR_RETURN_IF(gemm(g, s));
   // the heads index maps and query_tyx by flattened query b*N + n
@@ -687,6 +697,31 @@ int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const fl
   count_launch();
   TAPIR_LAUNCH_CHECK("cost_volume_head_generic_kernel");
   return kOk;
+}
+}  // namespace
+
+size_t cost_volume_workspace_bytes(int B, long long Q, int T, int gh, int gw, int C) {
+  if (B < 1 || Q < 0) return 0;
+  Arena a(nullptr, 0);
+  CvPlan p;
+  return plan_cv(a, B, Q, T, gh, gw, C, &p) + 256;
+}
+
+int cost_volume_tracks(const tapir_head_weights* w, const float* qfeat, const float* grid, int B,
+                       int N, int T, int gh, int gw, int C, const float* query_tyx, float temperature,
+                       int init_h, int init_w, float* points, float* occ, float* expd, int* argmax,
+                       void* ws, size_t ws_bytes, cudaStream_t s) {
+  return run_cost_volume(w, qfeat, grid, B, N, nullptr, T, gh, gw, C, query_tyx, temperature, init_h,
+                         init_w, points, occ, expd, argmax, ws, ws_bytes, s);
+}
+
+int cost_volume_tracks_ragged(const tapir_head_weights* w, const float* qfeat, const float* grid, int B,
+                              const int* counts, int T, int gh, int gw, int C, const float* query_tyx,
+                              float temperature, int init_h, int init_w, float* points, float* occ,
+                              float* expd, int* argmax, void* ws, size_t ws_bytes, cudaStream_t s) {
+  TAPIR_CHECK_ARG(counts != nullptr, "cost_volume_tracks_ragged: null counts");
+  return run_cost_volume(w, qfeat, grid, B, 0, counts, T, gh, gw, C, query_tyx, temperature, init_h,
+                         init_w, points, occ, expd, argmax, ws, ws_bytes, s);
 }
 
 }  // namespace tapir

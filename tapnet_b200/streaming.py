@@ -9,7 +9,7 @@ a CUDA graph (fixed frame size and point count) and replays it: same kernels, sa
 bit, no per-launch host cost.  The causal state lives in static device buffers that the graph
 updates in place; `update_query` mirrors `TAPIR.update_query_features` for re-targeting a point.
 
-With `num_streams=S` one tracker follows S camera streams with one point count.  Each stream is
+With `num_streams=S` one tracker follows S camera streams.  Each stream is
 tracked as the reference tracks one camera of its frame size (`height` / `width` / `window` may be
 given per stream): the default refinement resolutions of its own size, tracks in its own pixels.
 Streams whose backbone passes agree (`tapir_model._pass_plan`) form a group; one captured graph
@@ -18,6 +18,12 @@ clips of one frame each (the reference's batch axis, with per-clip video sizes).
 frame size form one group whose input is one [S, 1, H, W, 3] batch, so a step is one backbone
 pass over the S frames; a group of several sizes resamples its frames in one ingest launch per
 pass, whatever their sizes.
+
+With `num_points` a sequence of S counts each stream tracks its own number of points, without
+padding: a group packs its streams' query features, causal state and outputs along the point axis
+([1, sum N, ...]) and runs one estimate_trajectories with `points_per_clip`, so the per-query stages
+(stage A, local correlation, the mixer, the track update) run over the streams' points only.  Each
+stream's tracks, visibles and logits are slices of its group's packed outputs.
 
 With `yuv420=True` the tracker takes `live.YUV420Frames` (NV12 / I420 camera or decoder frames):
 it keeps static Y / U / V buffers of the camera frames, a step copies the 1.5 B/px planes into them
@@ -97,8 +103,12 @@ def group_streams(specs: Sequence[StreamSpec], initial_resolution=(256, 256)):
 class _Group:
   """Streams sharing a pass plan: their static inputs, query features and causal state."""
 
-  def __init__(self, plan, streams, specs):
+  def __init__(self, plan, streams, specs, counts=None):
     self.plan, self.streams = plan, list(streams)
+    # per-stream point counts (a ragged tracker; None: one count); stream streams[i]'s points are
+    # rows offsets[i] .. offsets[i] + counts[i] - 1 of the group's packed point axis
+    self.counts = None if counts is None else [counts[s] for s in streams]
+    self.offsets = None if counts is None else [sum(self.counts[:i]) for i in range(len(streams))]
     self.uniform = len({(specs[s].frame_hw, specs[s].window) for s in streams}) == 1
     sizes = [specs[s].hw for s in streams]
     # one size: estimate_trajectories' one-size call and launches; else per-clip sizes
@@ -111,28 +121,38 @@ class _Group:
 
 class OnlineTracker:
   """Graph-replayed per-frame step of a causal TAPIR model (`use_casual_conv=True`) over
-  `num_streams` camera streams with one point count (pad a stream with dummy points if it tracks
-  fewer) and one frame format, of one frame size or of one size each."""
+  `num_streams` camera streams of one frame format, of one frame size or of one size each, with
+  one point count or one per stream."""
 
   def __init__(self, model: 'tapir_model.TAPIR', height: Union[int, Sequence[int]],
-               width: Union[int, Sequence[int]], num_points: int, uint8_frames: bool = False,
-               num_streams: int = 1, yuv420: bool = False, window=None, matrix: str = 'bt601',
-               full_range: bool = False):
+               width: Union[int, Sequence[int]], num_points: Union[int, Sequence[int]],
+               uint8_frames: bool = False, num_streams: int = 1, yuv420: bool = False, window=None,
+               matrix: str = 'bt601', full_range: bool = False):
     """height x width: the frame size.  With yuv420=True that is the camera frame and `window`
     (y0, x0, h, w; e.g. `live.center_square_window(height, width)`) the crop that is tracked, in
     whose pixels the tracks are; `matrix` / `full_range` describe the YUV frames.  `height`,
     `width` and `window` may also give one value per stream: init / step then take a list of
-    the streams' frames."""
+    the streams' frames.  `num_points` may give one count per stream (each >= 1): init then takes
+    a list of the streams' [N_s, 3] query points, and step / last_logits return lists of the
+    streams' outputs."""
     if not model.use_casual_conv:
       raise ValueError('OnlineTracker needs a causal model: TAPIR(use_casual_conv=True)')
     if int(num_streams) < 1:
       raise ValueError(f'num_streams must be >= 1, got {num_streams}')
+    counts = None
+    if not isinstance(num_points, int):
+      counts = [int(n) for n in num_points]
+      if len(counts) != int(num_streams):
+        raise ValueError(f'num_points has {len(counts)} counts for {num_streams} streams')
+      if min(counts) < 1:
+        raise ValueError(f'num_points: every stream needs at least one point, got {counts}')
     if yuv420 and uint8_frames:
       raise ValueError('uint8_frames and yuv420 are exclusive')
     specs = stream_specs(height, width, num_streams, yuv420, window)
     self.model = model
     self.specs = specs
-    self.num_points = int(num_points)
+    self.num_points = int(num_points) if counts is None else counts
+    self._counts = counts
     self.num_streams = len(specs)
     self.dev = next(model.parameters()).device
     if self.dev.type != 'cuda':
@@ -141,7 +161,7 @@ class OnlineTracker:
     # before preprocess_frames); the normalisation runs inside the stem conv's loads
     self._frame_dtype = torch.uint8 if uint8_frames else torch.float32
     self._yuv = (matrix, bool(full_range)) if yuv420 else None
-    self._groups = [_Group(plan, streams, specs)
+    self._groups = [_Group(plan, streams, specs, counts)
                     for plan, streams in group_streams(specs, model.initial_resolution)]
     # streams of one frame size (and window) are one uniform group: init / step take a batch
     self._one_size = len(self._groups) == 1 and self._groups[0].uniform
@@ -161,6 +181,9 @@ class OnlineTracker:
         order.append(s)
     # row r of the groups' concatenated outputs is stream order[r]: gather them back in the graph
     self._order = torch.tensor([order.index(s) for s in range(self.num_streams)], device=self.dev)
+    if counts is not None:  # ragged: stream s's points in the groups' concatenated point axis
+      packed = [counts[s] for s in order]
+      self._rows = {s: slice(sum(packed[:r]), sum(packed[:r + 1])) for r, s in enumerate(order)}
     # a one-size tracker's input: its group's [S, 1, ...] buffer, into which a step copies the batch
     self._frame = self._groups[0].frames if self._one_size else None
     self._graph = None
@@ -290,14 +313,59 @@ class OnlineTracker:
     grids = self._group_grids(g)
     r = self.model.estimate_trajectories(g.video_size, False, grids, g.query_features, None, 64,
                                          causal_context=state, get_causal_context=True,
-                                         causal_context_out=state)
+                                         causal_context_out=state, points_per_clip=g.counts)
     return r['tracks'][-1], r['occlusion'][-1], r['expected_dist'][-1]
+
+  def _ragged_query_points(self, query_points):
+    """init's query points of a ragged tracker: a list of S [N_s, 3] tensors, on the device."""
+    S = self.num_streams
+    if isinstance(query_points, torch.Tensor) or len(query_points) != S:
+      got = len(query_points) if isinstance(query_points, (list, tuple)) else type(query_points).__name__
+      raise ValueError(f'expected a list of {S} query point tensors (one per stream), got {got}')
+    out = []
+    for s, (qp, n) in enumerate(zip(query_points, self._counts)):
+      if not isinstance(qp, torch.Tensor) or tuple(qp.shape) != (n, 3):
+        got = tuple(qp.shape) if isinstance(qp, torch.Tensor) else type(qp).__name__
+        raise ValueError(f'stream {s}: query points must be [{n}, 3], got {got}')
+      out.append(qp.to(self.dev, torch.float32))
+    return out
+
+  def _init_ragged(self, frames, query_points):
+    """init of a ragged tracker: each stream's query features as the equal-count tracker computes
+    them (one-size trackers sample every stream from one backbone pass over the batch), packed
+    along the point axis per group."""
+    qps = self._ragged_query_points(query_points)
+    frames = self._frames(frames)
+    if self._one_size:
+      grids = self.model.get_feature_grids(frames, False)
+      per_stream = [self.model.get_query_features(
+          frames, False, qps[s][None], tapir_model.FeatureGrids(
+              tuple(x[s:s + 1] for x in grids.lowres), tuple(x[s:s + 1] for x in grids.hires),
+              grids.resolutions)) for s in range(self.num_streams)]
+    else:
+      frames = [self._device_frame(f) for f in frames]
+      per_stream = [self._query_features_one(frames[s], qps[s][None])
+                    for s in range(self.num_streams)]
+    for g in self._groups:
+      qfs = [per_stream[s] for s in g.streams]
+      g.query_features = tapir_model.QueryFeatures(
+          tuple(torch.cat([q.lowres[i] for q in qfs], 1) for i in range(len(qfs[0].lowres))),
+          tuple(torch.cat([q.hires[i] for q in qfs], 1) for i in range(len(qfs[0].hires))),
+          qfs[0].resolutions)
+      init = self.model.construct_initial_causal_state(sum(g.counts), len(g.plan) - 1)
+      # [1, sum N, 2, 512 | 2048] per block, one tensor per refinement iteration
+      g.state = [{k: v.to(self.dev) for k, v in d.items()} for d in init]
 
   # -- pytorch_live_demo.py:44-54 online_model_init
   def init(self, frames: torch.Tensor, query_points: torch.Tensor):
     """frames: [S, H, W, 3] (or [S, 1, H, W, 3]; [H, W, 3] when S = 1) float in [-1, 1];
     query_points [S, N, 3] ([N, 3] when S = 1) as (t, y, x), stream s's on its frame s.  With
-    per-stream sizes, frames is a list of the S streams' frames."""
+    per-stream sizes, frames is a list of the S streams' frames; with per-stream point counts,
+    query_points is a list of the S streams' [N_s, 3] points."""
+    if self._counts is not None:
+      self._init_ragged(frames, query_points)
+      self._publish_groups()
+      return self.query_features
     frames = self._frames(frames)
     qp = query_points.to(self.dev, torch.float32)
     if qp.dim() == 2:
@@ -325,16 +393,26 @@ class OnlineTracker:
       # [G, N, 2, 512 | 2048] per block, one tensor per refinement iteration
       g.state = [{k: v.to(self.dev).expand(len(g.streams), *v.shape[1:]).clone()
                   for k, v in d.items()} for d in init]
+    self._publish_groups()
+    return self.query_features
+
+  def _publish_groups(self):
     if self._one_size:
       self.query_features, self.state = self._groups[0].query_features, self._groups[0].state
     else:
       self.query_features = [g.query_features for g in self._groups]
       self.state = [g.state for g in self._groups]
     self._graph = None
-    return self.query_features
 
   def _step_eager(self):
     outs = [self._step_group(g, g.state) for g in self._groups]
+    if self._counts is not None:
+      # the groups' packed [1, sum N, 1, ...] outputs, concatenated; each stream's a slice of them
+      tracks, occ, expd = (outs[0][i][0] if len(outs) == 1 else torch.cat([o[i][0] for o in outs])
+                           for i in range(3))
+      visibles = live.postprocess_occlusions(occ, expd)
+      return tuple([x[self._rows[s]] for s in range(self.num_streams)]
+                   for x in (tracks, visibles, occ, expd))
     if len(outs) == 1:  # one group holds the streams in order
       tracks, occ, expd = outs[0]
     else:  # the groups' outputs back in stream order
@@ -391,7 +469,9 @@ class OnlineTracker:
     """frames: [S, H, W, 3] ([H, W, 3] when S = 1), one per stream.  Returns (tracks [S, N, 1, 2]
     in frame pixels (x, y), visibles [S, N, 1] bool).  The returned tensors are the graph's static
     outputs: copy them if they must outlive the next step.  With per-stream sizes, frames is a
-    list of the S streams' frames and each stream's tracks are in its own pixels."""
+    list of the S streams' frames and each stream's tracks are in its own pixels.  With per-stream
+    point counts, tracks and visibles are lists of the S streams' [N_s, 1, 2] and [N_s, 1] views
+    into those outputs."""
     if self.query_features is None:
       raise RuntimeError('call init(frame, query_points) first')
     frames = self._frames(frames)
@@ -410,7 +490,8 @@ class OnlineTracker:
 
   @property
   def last_logits(self):
-    """(occlusion, expected_dist) logits of the last step, [S, N, 1] each."""
+    """(occlusion, expected_dist) logits of the last step, [S, N, 1] each (with per-stream point
+    counts, lists of the S streams' [N_s, 1])."""
     return self._out[2], self._out[3]
 
   def update_query(self, frame: torch.Tensor, query_point: torch.Tensor, idx: int,
@@ -422,12 +503,15 @@ class OnlineTracker:
       raise RuntimeError('call init(frame, query_points) first')
     if not 0 <= stream < self.num_streams:
       raise ValueError(f'stream {stream} out of range [0, {self.num_streams})')
-    if not 0 <= idx < self.num_points:
-      raise ValueError(f'point {idx} out of range [0, {self.num_points})')
+    n = self.num_points if self._counts is None else self._counts[stream]
+    if not 0 <= idx < n:
+      raise ValueError(f'point {idx} out of range [0, {n}) of stream {stream}')
     frame = self._device_frame(self._stream_frames([frame], [stream])[0])
     new = self._query_features_one(frame, query_point.to(self.dev, torch.float32).reshape(1, 1, 3))
     gi, slot = self._slot[stream]
     g = self._groups[gi]
+    if g.counts is not None:  # ragged: row offsets[slot] + idx of the group's one packed clip
+      slot, idx = 0, g.offsets[slot] + idx
     # TAPIR.update_query_features writes [:, idx] of every stream; only [slot, idx] changes here
     for dst, src in zip(g.query_features.lowres + g.query_features.hires, new.lowres + new.hires):
       dst[slot, idx] = src[0, 0]

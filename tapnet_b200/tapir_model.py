@@ -170,6 +170,30 @@ def _groups(B, N, T):
           for bi in range(B) for q0 in range(0, N, chunk_q)]
 
 
+def _ragged_groups(counts, T):
+  """Work groups of estimate_trajectories over clips of their own query counts, as (b0, b1, q0, q1):
+  whole clips b0..b1-1, flattened queries q0..q1-1, while the group's rows (queries x frames) fit
+  _MAX_ROWS_PER_CHUNK and its queries 65535; a clip whose rows alone exceed the bound runs on its
+  own in query chunks.  With equal counts these are the groups of _groups(B, N, T), which decide
+  bits (the mixer splits K at T = 1 by row count)."""
+  out = []
+  b0 = q0 = q = 0
+  for b, n in enumerate(counts):
+    if n * T > _MAX_ROWS_PER_CHUNK or n > 65535:
+      if b > b0:
+        out.append((b0, b, q0, q))
+      chunk_q = max(1, min(n, _MAX_ROWS_PER_CHUNK // T, 65535))
+      out += [(b, b + 1, q + c0, q + min(c0 + chunk_q, n)) for c0 in range(0, n, chunk_q)]
+      b0, q0 = b + 1, q + n
+    elif b > b0 and ((q + n - q0) * T > _MAX_ROWS_PER_CHUNK or q + n - q0 > 65535):
+      out.append((b0, b, q0, q))
+      b0, q0 = b, q
+    q += n
+  if len(counts) > b0:
+    out.append((b0, len(counts), q0, q))
+  return out
+
+
 def _ctx_lists(d, nb, index, fix=lambda t: t):
   """The [index] slices of one iteration's causal context dict as two per-block lists (causal_1,
   causal_2), each passed through `fix`."""
@@ -580,8 +604,15 @@ class TAPIR(nn.Module):
       causal_context: Optional[list] = None,
       get_causal_context: bool = False,
       causal_context_out: Optional[list] = None,
+      points_per_clip: Optional[Sequence[int]] = None,
   ) -> Mapping[str, Any]:
     """Reference tapir_model.py:394-578.
+
+    `points_per_clip` (extension): None, or the query counts of the B clips of feature_grids, each
+    >= 1.  query_features, query_points_in_video and the causal context then hold the clips'
+    queries one clip after the other along the point axis ([1, sum N, ...]; the context
+    [1, sum N, 2, 512 | 2048]) and so do the outputs ([1, sum N, T, ...]).  Each clip's results
+    equal a single-clip call with its queries, bit for bit, at T > 1.
 
     `video_size` (extension): one (h, w) for every clip, or a sequence of B (h, w) pairs, clip b's
     tracks (and query points) then being in its own video's pixels; each clip's results equal a
@@ -607,6 +638,11 @@ class TAPIR(nn.Module):
     B, N = query_features.lowres[0].shape[:2]
     T = feature_grids.lowres[0].shape[1]
     nb = pk['num_blocks']
+    counts = None
+    if points_per_clip is not None:
+      counts = self._check_points_per_clip(points_per_clip, feature_grids, query_features,
+                                           query_points_in_video)
+      B = len(counts)
     video_table = None
     if per_clip is not None:
       if len(per_clip) != B:
@@ -614,13 +650,14 @@ class TAPIR(nn.Module):
       # [B, 2] (h, w): the track update's table; the stage-A scalings broadcast per clip
       video_table = self._const([v for hw in per_clip for v in hw], dev, torch.int32).view(B, 2)
 
-    occ_out, expd_out, trk_out = _new_estimates(num_iters + 1, B, N, T, dev)
+    OB = 1 if counts is not None else B  # the outputs' leading dim: the clips, or one ragged row
+    occ_out, expd_out, trk_out = _new_estimates(num_iters + 1, OB, N, T, dev)
     new_ctx = self._new_causal_context(causal_context, get_causal_context, causal_context_out,
-                                       num_iters, nb, B, N, T, dev)
+                                       num_iters, nb, OB, N, T, dev)
     write_ctx = get_causal_context and causal_context is not None
     am_out = None
     if self.capture_stage_a_argmax:
-      am_out = torch.empty(B, N, T, dtype=torch.int32, device=dev)
+      am_out = torch.empty(OB, N, T, dtype=torch.int32, device=dev)
       self.last_stage_a_argmax = am_out
     out = dict(occlusion=occ_out, tracks=trk_out, expected_dist=expd_out)
     if get_causal_context:
@@ -635,16 +672,31 @@ class TAPIR(nn.Module):
     pooled = {level: self._pool_pyramid(feature_grids.lowres[level].contiguous())
               for level in range(1, num_levels_total)}
 
-    for b0, b1, sl in _groups(B, N, T):
+    if counts is None:
+      work = [(b0, b1, (slice(b0, b1), sl), None) for b0, b1, sl in _groups(B, N, T)]
+    else:  # ragged: a group's queries are the flattened slice q0..q1 of the one point axis
+      work = [(b0, b1, (0, slice(q0, q1)), self._group_counts(counts, b0, b1, q0, q1))
+              for b0, b1, q0, q1 in _ragged_groups(counts, T)]
+    for b0, b1, oi, gcounts in work:
       bs = slice(b0, b1)
-      nq = (b1 - b0) * (sl.stop - sl.start)  # queries of the group, flattened over its clips
-      # every [bs, sl] slice below is contiguous: either whole clips or a query chunk of one clip
-      occ0, expd0 = occ_out[0][bs, sl], expd_out[0][bs, sl]  # outputs are written in place
-      qp = query_points_in_video[bs, sl] if query_points_in_video is not None else None
+      # every [oi] slice below is contiguous: whole clips or a query chunk of one clip
+      occ0, expd0 = occ_out[0][oi], expd_out[0][oi]  # outputs are written in place
+      nq = occ0.numel() // T  # queries of the group, flattened over its clips
+      qp = query_points_in_video[oi] if query_points_in_video is not None else None
       vsize = video_hw if video_table is None else per_clip[b0:b1]
-      pos = self._stage_a(pk, feature_grids.lowres[0][bs].contiguous(),
-                          query_features.lowres[0][bs, sl].contiguous(), qp, vsize, occ0, expd0,
-                          trk_out[0][bs, sl], am_out[bs, sl] if am_out is not None else None, dev)
+      am = am_out[oi] if am_out is not None else None
+      query_clip = None
+      if gcounts is None:
+        pos = self._stage_a(pk, feature_grids.lowres[0][bs].contiguous(),
+                            query_features.lowres[0][oi].contiguous(), qp, vsize, occ0, expd0,
+                            trk_out[0][oi], am, dev)
+      else:
+        # [nq] int32 clip (within the group) of each query: cached, so a captured step uploads nothing
+        query_clip = self._const([b for b, n in enumerate(gcounts) for _ in range(n)], dev,
+                                 torch.int32)
+        pos = self._stage_a_ragged(pk, feature_grids.lowres[0][bs].contiguous(),
+                                   query_features.lowres[0][oi].contiguous(), gcounts, qp, vsize,
+                                   occ0, expd0, trk_out[0][oi], am, dev)
 
       # ---- refinement iterations, one level at a time
       bufs = self._refine_buffers(nq, T, dev)
@@ -655,19 +707,41 @@ class TAPIR(nn.Module):
         for it in its:
           ctx = [None] * 4
           if causal_context is not None:
-            ctx[:2] = _ctx_lists(causal_context[it], nb, (bs, sl),
+            ctx[:2] = _ctx_lists(causal_context[it], nb, oi,
                                  lambda t: t.to(device=dev, dtype=torch.float32).contiguous())
           if write_ctx:
-            ctx[2:] = _ctx_lists(new_ctx[it], nb, (bs, sl))
+            ctx[2:] = _ctx_lists(new_ctx[it], nb, oi)
           ctxs.append(ctx)
-        outs = [(occ_out[it + 1][bs, sl], expd_out[it + 1][bs, sl], trk_out[it + 1][bs, sl])
-                for it in its]
+        outs = [(occ_out[it + 1][oi], expd_out[it + 1][oi], trk_out[it + 1][oi]) for it in its]
         self._refine_level(pk, feature_grids.hires[level][bs], feature_grids.lowres[level][bs],
-                           [g[bs] for g in pooled[level]], query_features.hires[level][bs, sl],
-                           query_features.lowres[level][bs, sl], pos, occ0, expd0, outs, bufs,
+                           [g[bs] for g in pooled[level]], query_features.hires[level][oi],
+                           query_features.lowres[level][oi], pos, occ0, expd0, outs, bufs,
                            feature_grids.resolutions[level],
-                           video_hw if video_table is None else video_table[bs], ctxs)
+                           video_hw if video_table is None else video_table[bs], ctxs, query_clip)
     return out
+
+  @staticmethod
+  def _check_points_per_clip(points_per_clip, feature_grids, query_features, query_points):
+    """estimate_trajectories' points_per_clip as a list of ints, checked against the clips of
+    feature_grids and the [1, sum N, ...] queries (ValueError before any launch)."""
+    counts = [int(n) for n in points_per_clip]
+    B = feature_grids.lowres[0].shape[0]
+    if len(counts) != B:
+      raise ValueError(f'points_per_clip has {len(counts)} counts for {B} clips')
+    if min(counts, default=0) < 1:
+      raise ValueError(f'points_per_clip: every clip needs at least one point, got {counts}')
+    want = (1, sum(counts))
+    for name, t in [('query_features', f) for f in query_features.lowres + query_features.hires] + [
+        ('query_points_in_video', query_points)]:
+      if t is not None and tuple(t.shape[:2]) != want:
+        raise ValueError(f'{name} has shape {tuple(t.shape)}; points_per_clip {counts} needs '
+                         f'[1, {want[1]}, ...]')
+    return counts
+
+  @staticmethod
+  def _group_counts(counts, b0, b1, q0, q1):
+    """The query counts of a ragged work group's clips b0..b1-1 (one query chunk: [q1 - q0])."""
+    return [q1 - q0] if b1 - b0 == 1 else list(counts[b0:b1])
 
   def _new_causal_context(self, causal_context, get_causal_context, causal_context_out, num_iters,
                           nb, B, N, T, dev):
@@ -736,6 +810,43 @@ class TAPIR(nn.Module):
     torch.div(pos * to_video, self._const([iw, ih], dev), out=tracks)
     return pos
 
+  def _stage_a_ragged(self, pk, grid, qfeat, counts, query_points, video_hw, occ, expd, tracks,
+                      argmax, dev):
+    """_stage_a for clips with their own query counts: qfeat [nq, 256] holds the clips' queries one
+    after the other (counts[b] of clip b), grid is [G, T, h, w, 256]; occ, expd [nq, T], tracks
+    [nq, T, 2].  The scalings are per query (cached), the cost volume runs in calls of at most
+    MAX_RAGGED_CLIPS clips.  Returns the positions [nq, T, 2]."""
+    nq = qfeat.shape[0]
+    T = grid.shape[1]
+    ih, iw = self.initial_resolution
+    if isinstance(video_hw[0], tuple):  # one (h, w) per clip: [nq, 3] and [nq, 1, 2] scales
+      sizes = [hw for hw, n in zip(video_hw, counts) for _ in range(n)]
+      to_init = self._const([v for h, w in sizes for v in (T, h, w)], dev).view(nq, 3)
+      to_video = self._const([v for h, w in sizes for v in (w, h)], dev).view(nq, 1, 2)
+    else:
+      vh, vw = video_hw
+      to_init, to_video = self._const([T, vh, vw], dev), self._const([vw, vh], dev)
+    qp = None
+    if query_points is not None:
+      qp = (query_points.to(torch.float32) * self._const([T, ih, iw], dev) / to_init).contiguous()
+    pos = torch.empty(nq, T, 2, dtype=torch.float32, device=dev)
+    step = _lib.MAX_RAGGED_CLIPS
+    for c0 in range(0, len(counts), step):
+      cs = counts[c0:c0 + step]
+      r0 = sum(counts[:c0])
+      r = slice(r0, r0 + sum(cs))
+      ws = self._workspace(
+          'cost_volume',
+          _lib.cost_volume_ragged_workspace_bytes(len(cs), r.stop - r0, (len(cs),) + grid.shape[1:]),
+          dev)
+      _lib.cost_volume_tracks_ragged(pk['head'], qfeat[r], cs, grid[c0:c0 + len(cs)],
+                                     qp[r] if qp is not None else None, self.softmax_temperature,
+                                     (ih, iw), pos[r], occ[r], expd[r],
+                                     argmax[r] if argmax is not None else None, ws)
+    # train2orig (tapir_model.py:435-441)
+    torch.div(pos * to_video, self._const([iw, ih], dev), out=tracks)
+    return pos
+
   def _refine_scratch(self, nq, T):
     """The refinement of nq queries over T frames: the (shape, dtype) of the mixer's input planes,
     its output rows and the two feature buffers the iterations alternate between, and the bytes of
@@ -763,13 +874,13 @@ class TAPIR(nn.Module):
     return pooled
 
   def _refine_level(self, pk, hires, lowres, pooled, qf_hi, qf_lo, pos, occ0, expd0, outs, bufs,
-                    resize_hw, video_hw, ctxs=None):
+                    resize_hw, video_hw, ctxs=None, query_clip=None):
     """The num_pips_iter refinement iterations of one level (reference tapir_model.py:529-552)
     for nq queries over T frames.  hires, lowres [G, T, h, w, C]: the level's grids, pooled: the
     _pool_pyramid of lowres; qf_hi / qf_lo: the query features [..., 128 | 256] of the nq queries;
     pos [..., T, 2] is moved in place; occ0 / expd0: the stage-A estimates the level starts from;
     outs: one (occ, expd, tracks) output view per iteration; bufs: _refine_buffers; ctxs: one mixer
-    context list per iteration (see _refine), or None.  Only pos carries over to the next level:
+    context list per iteration (see _refine), or None; query_clip: see _refine.  Only pos carries over to the next level:
     features restart from the query and occlusion / expected distance from stage A."""
     levels = [hires.contiguous(), lowres.contiguous()] + pooled
     qfeat = (qf_hi.contiguous(), qf_lo.contiguous())
@@ -785,21 +896,24 @@ class TAPIR(nn.Module):
       fdst = feats[1] if fsrc is feats[0] else feats[0]
       self._refine(pk, levels, pos, occ, expd, feat, x_planes, res,
                    ctxs[i] if ctxs is not None else [None] * 4, mws, occ_n, expd_n, fdst, trk_n,
-                   resize_hw, video_hw)
+                   resize_hw, video_hw, query_clip)
       fsrc, occ, expd = fdst, occ_n, expd_n
 
   def _refine(self, pk, levels, pos, occ, expd, feat, x_planes, res, ctx, mws, occ_out, expd_out,
-              feat_out, tracks_out, resize_hw, video_hw):
+              feat_out, tracks_out, resize_hw, video_hw, query_clip=None):
     """One refinement iteration (the refine_pips call, reference tapir_model.py:529-542): local correlation around pos
     over the pyramid `levels`, the mixer, and the update of pos (in place), occlusion, expected
     distance, features (hi, lo views `feat` -> feat_out) and tracks.  ctx: the mixer's causal
     context lists (ctx1_in, ctx2_in, ctx1_out, ctx2_out), None where absent.  video_hw: one
-    (h, w), or an int32 [G, 2] table of per-clip sizes."""
-    _lib.local_corr(levels, pos, occ, expd, *feat, x_planes, self.initial_resolution)
+    (h, w), or an int32 [G, 2] table of per-clip sizes.  query_clip: None (clips of equal query
+    counts), or the int32 [nq] clip of each query."""
+    _lib.local_corr(levels, pos, occ, expd, *feat, x_planes, self.initial_resolution,
+                    query_clip=query_clip)
     _lib.mixer_forward(pk['mixer'], x_planes, res, self.use_casual_conv, *ctx, mws)
     if isinstance(video_hw, torch.Tensor):
       _lib.refine_update(res, pos, occ, expd, *feat, occ_out, expd_out, feat_out, tracks_out,
-                         self.initial_resolution, resize_hw, (0, 0), video_table=video_hw)
+                         self.initial_resolution, resize_hw, (0, 0), video_table=video_hw,
+                         query_clip=query_clip)
     else:
       _lib.refine_update(res, pos, occ, expd, *feat, occ_out, expd_out, feat_out, tracks_out,
                          self.initial_resolution, resize_hw, video_hw)
