@@ -20,10 +20,10 @@ pass over the S frames; a group of several sizes resamples its frames in one ing
 pass, whatever their sizes.
 
 With `num_points` a sequence of S counts each stream tracks its own number of points, without
-padding: a group packs its streams' query features, causal state and outputs along the point axis
-([1, sum N, ...]) and runs one estimate_trajectories with `points_per_clip`, so the per-query stages
-(stage A, local correlation, the mixer, the track update) run over the streams' points only.  Each
-stream's tracks, visibles and logits are slices of its group's packed outputs.
+padding.  Either way a group packs its streams' query features, causal state and outputs along the
+point axis ([1, sum N, ...]) and runs one estimate_trajectories with `points_per_clip`, so the
+per-query stages (stage A, local correlation, the mixer, the track update) run over the streams'
+points only.  Each stream's tracks, visibles and logits are slices of its group's packed outputs.
 
 With `yuv420=True` the tracker takes `live.YUV420Frames` (NV12 / I420 camera or decoder frames):
 it keeps static Y / U / V buffers of the camera frames, a step copies the 1.5 B/px planes into them
@@ -103,12 +103,12 @@ def group_streams(specs: Sequence[StreamSpec], initial_resolution=(256, 256)):
 class _Group:
   """Streams sharing a pass plan: their static inputs, query features and causal state."""
 
-  def __init__(self, plan, streams, specs, counts=None):
+  def __init__(self, plan, streams, specs, counts):
     self.plan, self.streams = plan, list(streams)
-    # per-stream point counts (a ragged tracker; None: one count); stream streams[i]'s points are
-    # rows offsets[i] .. offsets[i] + counts[i] - 1 of the group's packed point axis
-    self.counts = None if counts is None else [counts[s] for s in streams]
-    self.offsets = None if counts is None else [sum(self.counts[:i]) for i in range(len(streams))]
+    # stream streams[i]'s points are rows offsets[i] .. offsets[i] + counts[i] - 1 of the group's
+    # packed point axis
+    self.counts = [counts[s] for s in streams]
+    self.offsets = [sum(self.counts[:i]) for i in range(len(streams))]
     self.uniform = len({(specs[s].frame_hw, specs[s].window) for s in streams}) == 1
     sizes = [specs[s].hw for s in streams]
     # one size: estimate_trajectories' one-size call and launches; else per-clip sizes
@@ -139,8 +139,9 @@ class OnlineTracker:
       raise ValueError('OnlineTracker needs a causal model: TAPIR(use_casual_conv=True)')
     if int(num_streams) < 1:
       raise ValueError(f'num_streams must be >= 1, got {num_streams}')
-    counts = None
-    if not isinstance(num_points, int):
+    if isinstance(num_points, int):
+      counts = [num_points] * int(num_streams)
+    else:
       counts = [int(n) for n in num_points]
       if len(counts) != int(num_streams):
         raise ValueError(f'num_points has {len(counts)} counts for {num_streams} streams')
@@ -151,7 +152,7 @@ class OnlineTracker:
     specs = stream_specs(height, width, num_streams, yuv420, window)
     self.model = model
     self.specs = specs
-    self.num_points = int(num_points) if counts is None else counts
+    self.num_points = num_points if isinstance(num_points, int) else counts
     self._counts = counts
     self.num_streams = len(specs)
     self.dev = next(model.parameters()).device
@@ -181,9 +182,9 @@ class OnlineTracker:
         order.append(s)
     # row r of the groups' concatenated outputs is stream order[r]: gather them back in the graph
     self._order = torch.tensor([order.index(s) for s in range(self.num_streams)], device=self.dev)
-    if counts is not None:  # ragged: stream s's points in the groups' concatenated point axis
-      packed = [counts[s] for s in order]
-      self._rows = {s: slice(sum(packed[:r]), sum(packed[:r + 1])) for r, s in enumerate(order)}
+    # stream s's points in the groups' concatenated point axis
+    packed = [counts[s] for s in order]
+    self._rows = {s: slice(sum(packed[:r]), sum(packed[:r + 1])) for r, s in enumerate(order)}
     # a one-size tracker's input: its group's [S, 1, ...] buffer, into which a step copies the batch
     self._frame = self._groups[0].frames if self._one_size else None
     self._graph = None
@@ -309,16 +310,28 @@ class OnlineTracker:
 
   def _step_group(self, g, state):
     """One group's step on its static inputs: its passes and one batched estimate_trajectories
-    (B = group size, T = 1) that updates `state` in place; returns (tracks, occ, expd)."""
+    (B = group size, T = 1) that updates `state` in place; returns (tracks, occ, expd), packed
+    [1, sum N, 1, ...]."""
     grids = self._group_grids(g)
     r = self.model.estimate_trajectories(g.video_size, False, grids, g.query_features, None, 64,
                                          causal_context=state, get_causal_context=True,
                                          causal_context_out=state, points_per_clip=g.counts)
     return r['tracks'][-1], r['occlusion'][-1], r['expected_dist'][-1]
 
-  def _ragged_query_points(self, query_points):
-    """init's query points of a ragged tracker: a list of S [N_s, 3] tensors, on the device."""
+  def _query_points(self, query_points):
+    """init's query points, checked, as a list of S [N_s, 3] float32 tensors on the device: a list
+    of the streams' [N_s, 3] points or, with one point count N, a [S, N, 3] tensor ([N, 3] when
+    S = 1)."""
     S = self.num_streams
+    if isinstance(self.num_points, int) and isinstance(query_points, torch.Tensor):
+      qp = query_points.to(self.dev, torch.float32)
+      if qp.dim() == 2:
+        qp = qp[None]
+      if qp.dim() != 3 or qp.shape[0] != S or qp.shape[2] != 3:
+        raise ValueError(f'query_points must be [{S}, N, 3], got {tuple(qp.shape)}')
+      if qp.shape[1] != self.num_points:
+        raise ValueError(f'expected {self.num_points} query points, got {qp.shape[1]}')
+      return list(qp)
     if isinstance(query_points, torch.Tensor) or len(query_points) != S:
       got = len(query_points) if isinstance(query_points, (list, tuple)) else type(query_points).__name__
       raise ValueError(f'expected a list of {S} query point tensors (one per stream), got {got}')
@@ -330,12 +343,18 @@ class OnlineTracker:
       out.append(qp.to(self.dev, torch.float32))
     return out
 
-  def _init_ragged(self, frames, query_points):
-    """init of a ragged tracker: each stream's query features as the equal-count tracker computes
-    them (one-size trackers sample every stream from one backbone pass over the batch), packed
-    along the point axis per group."""
-    qps = self._ragged_query_points(query_points)
+  # -- pytorch_live_demo.py:44-54 online_model_init
+  def init(self, frames: torch.Tensor, query_points: torch.Tensor):
+    """frames: [S, H, W, 3] (or [S, 1, H, W, 3]; [H, W, 3] when S = 1) float in [-1, 1];
+    query_points [S, N, 3] ([N, 3] when S = 1) as (t, y, x), stream s's on its frame s.  With
+    per-stream sizes, frames is a list of the S streams' frames; with per-stream point counts,
+    query_points is a list of the S streams' [N_s, 3] points."""
+    qps = self._query_points(query_points)
     frames = self._frames(frames)
+    # A one-size tracker samples every stream's features from one backbone pass over its batch, as
+    # online_model_init on the batch does.  Other trackers compute each stream's as a one-stream
+    # tracker of its size does; the two differ in the last bits, as the library splits K for
+    # one-frame backbone chunks.
     if self._one_size:
       grids = self.model.get_feature_grids(frames, False)
       per_stream = [self.model.get_query_features(
@@ -348,6 +367,7 @@ class OnlineTracker:
                     for s in range(self.num_streams)]
     for g in self._groups:
       qfs = [per_stream[s] for s in g.streams]
+      # private copies: the graph reads these exact buffers on every replay
       g.query_features = tapir_model.QueryFeatures(
           tuple(torch.cat([q.lowres[i] for q in qfs], 1) for i in range(len(qfs[0].lowres))),
           tuple(torch.cat([q.hires[i] for q in qfs], 1) for i in range(len(qfs[0].hires))),
@@ -355,69 +375,40 @@ class OnlineTracker:
       init = self.model.construct_initial_causal_state(sum(g.counts), len(g.plan) - 1)
       # [1, sum N, 2, 512 | 2048] per block, one tensor per refinement iteration
       g.state = [{k: v.to(self.dev) for k, v in d.items()} for d in init]
-
-  # -- pytorch_live_demo.py:44-54 online_model_init
-  def init(self, frames: torch.Tensor, query_points: torch.Tensor):
-    """frames: [S, H, W, 3] (or [S, 1, H, W, 3]; [H, W, 3] when S = 1) float in [-1, 1];
-    query_points [S, N, 3] ([N, 3] when S = 1) as (t, y, x), stream s's on its frame s.  With
-    per-stream sizes, frames is a list of the S streams' frames; with per-stream point counts,
-    query_points is a list of the S streams' [N_s, 3] points."""
-    if self._counts is not None:
-      self._init_ragged(frames, query_points)
-      self._publish_groups()
-      return self.query_features
-    frames = self._frames(frames)
-    qp = query_points.to(self.dev, torch.float32)
-    if qp.dim() == 2:
-      qp = qp[None]
-    if qp.dim() != 3 or qp.shape[0] != self.num_streams or qp.shape[2] != 3:
-      raise ValueError(f'query_points must be [{self.num_streams}, N, 3], got {tuple(qp.shape)}')
-    if qp.shape[1] != self.num_points:
-      raise ValueError(f'expected {self.num_points} query points, got {qp.shape[1]}')
-    # A one-size tracker's features are online_model_init's on its batch: one call over the S
-    # frames.  Other trackers compute each stream's as a one-stream tracker of its size does; the
-    # two differ in the last bits, as the library splits K for one-frame backbone chunks.
+    views = [self._published(g) for g in self._groups]
     if self._one_size:
-      per_group = [[self._query_features_one(frames, qp)]]
+      self.query_features, self.state = views[0]
     else:
-      frames = [self._device_frame(f) for f in frames]
-      per_stream = [self._query_features_one(frames[s], qp[s:s + 1]) for s in range(self.num_streams)]
-      per_group = [[per_stream[s] for s in g.streams] for g in self._groups]
-    for g, qfs in zip(self._groups, per_group):
-      # private copies: the graph reads these exact buffers on every replay
-      g.query_features = tapir_model.QueryFeatures(
-          tuple(torch.cat([q.lowres[i] for q in qfs]) for i in range(len(qfs[0].lowres))),
-          tuple(torch.cat([q.hires[i] for q in qfs]) for i in range(len(qfs[0].hires))),
-          qfs[0].resolutions)
-      init = self.model.construct_initial_causal_state(self.num_points, len(g.plan) - 1)
-      # [G, N, 2, 512 | 2048] per block, one tensor per refinement iteration
-      g.state = [{k: v.to(self.dev).expand(len(g.streams), *v.shape[1:]).clone()
-                  for k, v in d.items()} for d in init]
-    self._publish_groups()
+      self.query_features, self.state = [v[0] for v in views], [v[1] for v in views]
+    self._graph = None
     return self.query_features
 
-  def _publish_groups(self):
-    if self._one_size:
-      self.query_features, self.state = self._groups[0].query_features, self._groups[0].state
-    else:
-      self.query_features = [g.query_features for g in self._groups]
-      self.state = [g.state for g in self._groups]
-    self._graph = None
+  def _published(self, g):
+    """A group's (query features, state) as `query_features` / `state` show them: packed
+    [1, sum N, ...] with per-stream point counts, else [G, N, ...] views of the packed buffers
+    (writes through them reach the graph)."""
+    if not isinstance(self.num_points, int):
+      return g.query_features, g.state
+
+    def per_stream(x):
+      return x.view(len(g.streams), self.num_points, *x.shape[2:])
+    qf = g.query_features
+    return (tapir_model.QueryFeatures(tuple(map(per_stream, qf.lowres)),
+                                      tuple(map(per_stream, qf.hires)), qf.resolutions),
+            [{k: per_stream(v) for k, v in d.items()} for d in g.state])
 
   def _step_eager(self):
     outs = [self._step_group(g, g.state) for g in self._groups]
-    if self._counts is not None:
-      # the groups' packed [1, sum N, 1, ...] outputs, concatenated; each stream's a slice of them
-      tracks, occ, expd = (outs[0][i][0] if len(outs) == 1 else torch.cat([o[i][0] for o in outs])
-                           for i in range(3))
+    # the groups' packed [1, sum N, 1, ...] outputs, concatenated along the point axis
+    tracks, occ, expd = (outs[0][i][0] if len(outs) == 1 else torch.cat([o[i][0] for o in outs])
+                         for i in range(3))
+    if not isinstance(self.num_points, int):  # each stream's outputs a slice of them
       visibles = live.postprocess_occlusions(occ, expd)
       return tuple([x[self._rows[s]] for s in range(self.num_streams)]
                    for x in (tracks, visibles, occ, expd))
-    if len(outs) == 1:  # one group holds the streams in order
-      tracks, occ, expd = outs[0]
-    else:  # the groups' outputs back in stream order
-      tracks, occ, expd = (torch.cat([o[i] for o in outs]).index_select(0, self._order)
-                           for i in range(3))
+    tracks, occ, expd = (x.view(-1, self.num_points, *x.shape[1:]) for x in (tracks, occ, expd))
+    if len(outs) > 1:  # the groups' outputs back in stream order (one group holds them in order)
+      tracks, occ, expd = (x.index_select(0, self._order) for x in (tracks, occ, expd))
     visibles = live.postprocess_occlusions(occ, expd)  # pytorch_live_demo.py:57-59
     return tracks, visibles, occ, expd
 
@@ -503,18 +494,17 @@ class OnlineTracker:
       raise RuntimeError('call init(frame, query_points) first')
     if not 0 <= stream < self.num_streams:
       raise ValueError(f'stream {stream} out of range [0, {self.num_streams})')
-    n = self.num_points if self._counts is None else self._counts[stream]
+    n = self._counts[stream]
     if not 0 <= idx < n:
       raise ValueError(f'point {idx} out of range [0, {n}) of stream {stream}')
     frame = self._device_frame(self._stream_frames([frame], [stream])[0])
     new = self._query_features_one(frame, query_point.to(self.dev, torch.float32).reshape(1, 1, 3))
     gi, slot = self._slot[stream]
     g = self._groups[gi]
-    if g.counts is not None:  # ragged: row offsets[slot] + idx of the group's one packed clip
-      slot, idx = 0, g.offsets[slot] + idx
-    # TAPIR.update_query_features writes [:, idx] of every stream; only [slot, idx] changes here
+    row = g.offsets[slot] + idx  # the point's row in the group's packed point axis
+    # TAPIR.update_query_features writes [:, idx] of every stream; only this row changes here
     for dst, src in zip(g.query_features.lowres + g.query_features.hires, new.lowres + new.hires):
-      dst[slot, idx] = src[0, 0]
+      dst[0, row] = src[0, 0]
     for d in g.state:
       for v in d.values():
-        v[slot, idx] = 0
+        v[0, row] = 0

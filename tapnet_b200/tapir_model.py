@@ -142,40 +142,27 @@ def _backbone_frames(video):
   return video.contiguous() if video.dtype == torch.uint8 else video.to(torch.float32).contiguous()
 
 
-def _stage_a_scratch(G, n, T, grid_shape):
-  """Stage A of G clips, n queries, T frames of grid_shape lowres grids: the shapes of its float32
-  occlusion, expected distance, tracks, positions and positions scaled on their way to the tracks,
-  and the bytes of its cost-volume workspace."""
-  return (((G, n, T),) * 2 + ((G, n, T, 2),) * 3,
-          _lib.cost_volume_workspace_bytes((G, n), (G, T, *grid_shape)))
+def _stage_a_scratch(G, nq, T, grid_shape):
+  """Stage A of G clips with nq queries in all, T frames of grid_shape lowres grids: the shapes of
+  its float32 occlusion, expected distance, tracks, positions and positions scaled on their way to
+  the tracks, and the bytes of its cost-volume workspace."""
+  return (((nq, T),) * 2 + ((nq, T, 2),) * 3,
+          _lib.cost_volume_ragged_workspace_bytes(G, nq, (G, T, *grid_shape)))
 
 
-def _new_estimates(count, G, n, T, dev):
-  """`count` estimates of G clips' n queries over T frames as three lists: occlusion [G, n, T],
-  expected distance [G, n, T] and tracks [G, n, T, 2]."""
+def _new_estimates(count, shape, dev):
+  """`count` estimates of queries over T frames as three lists: occlusion and expected distance of
+  `shape` (the query dims, then T) and tracks of shape + (2,)."""
   return tuple([torch.empty(s, dtype=torch.float32, device=dev) for _ in range(count)]
-               for s in ((G, n, T), (G, n, T), (G, n, T, 2)))
+               for s in (shape, shape, (*shape, 2)))
 
 
-def _groups(B, N, T):
-  """Work groups of estimate_trajectories as (b0, b1, query slice): whole clips b0..b1-1 with all
-  their queries while the group's rows (clips x queries x frames) fit _MAX_ROWS_PER_CHUNK and its
-  queries fit one head / mixer launch (65535); a clip whose rows alone exceed the bound runs on its
-  own in query chunks.  Each group is one launch sequence over its clips."""
-  if N * T <= _MAX_ROWS_PER_CHUNK and N <= 65535:
-    g = max(1, min(B, _MAX_ROWS_PER_CHUNK // (N * T), 65535 // N))
-    return [(b0, min(b0 + g, B), slice(0, N)) for b0 in range(0, B, g)]
-  chunk_q = max(1, min(N, _MAX_ROWS_PER_CHUNK // T, 65535))
-  return [(bi, bi + 1, slice(q0, min(q0 + chunk_q, N)))
-          for bi in range(B) for q0 in range(0, N, chunk_q)]
-
-
-def _ragged_groups(counts, T):
-  """Work groups of estimate_trajectories over clips of their own query counts, as (b0, b1, q0, q1):
+def _work_groups(counts, T):
+  """Work groups of estimate_trajectories over clips of counts[b] queries, as (b0, b1, q0, q1):
   whole clips b0..b1-1, flattened queries q0..q1-1, while the group's rows (queries x frames) fit
-  _MAX_ROWS_PER_CHUNK and its queries 65535; a clip whose rows alone exceed the bound runs on its
-  own in query chunks.  With equal counts these are the groups of _groups(B, N, T), which decide
-  bits (the mixer splits K at T = 1 by row count)."""
+  _MAX_ROWS_PER_CHUNK and its queries one head / mixer launch (65535); a clip whose rows alone
+  exceed the bound runs on its own in query chunks.  Each group is one launch sequence over its
+  clips.  The groups decide bits: the mixer splits K at T = 1 by row count."""
   out = []
   b0 = q0 = q = 0
   for b, n in enumerate(counts):
@@ -194,11 +181,22 @@ def _ragged_groups(counts, T):
   return out
 
 
-def _ctx_lists(d, nb, index, fix=lambda t: t):
-  """The [index] slices of one iteration's causal context dict as two per-block lists (causal_1,
+def _query_rows(t, q0, q1):
+  """Queries q0..q1-1 of t [B, N, ...], counted along its flattened (B, N) point axis: whole clips
+  or a range within one clip, as a work group holds them.  One index per tensor, as a group reads
+  2 x num_blocks context tensors per iteration and each op costs host time on the online step."""
+  n = t.shape[1]
+  b, r = divmod(q0, n)
+  if r == 0 and (q1 - q0) % n == 0:
+    return t[b:b + (q1 - q0) // n]
+  return t[b, r:r + q1 - q0]
+
+
+def _ctx_lists(d, nb, q0, q1, fix=lambda t: t):
+  """Queries q0..q1-1 of one iteration's causal context dict as two per-block lists (causal_1,
   causal_2), each passed through `fix`."""
-  return ([fix(d[f'block_{i}_causal_1'][index]) for i in range(nb)],
-          [fix(d[f'block_{i}_causal_2'][index]) for i in range(nb)])
+  return ([fix(_query_rows(d[f'block_{i}_causal_1'], q0, q1)) for i in range(nb)],
+          [fix(_query_rows(d[f'block_{i}_causal_2'], q0, q1)) for i in range(nb)])
 
 
 def refined_average(trajectories, num_pips_iter):
@@ -635,29 +633,29 @@ class TAPIR(nn.Module):
     video_hw = None if per_clip is not None else (int(video_size[0]), int(video_size[1]))
     num_levels_total = len(feature_grids.lowres)
     num_iters = self.num_pips_iter * (num_levels_total - 1)
-    B, N = query_features.lowres[0].shape[:2]
+    B, N = query_features.lowres[0].shape[:2]  # [1, sum N] with points_per_clip
     T = feature_grids.lowres[0].shape[1]
     nb = pk['num_blocks']
-    counts = None
-    if points_per_clip is not None:
+    if points_per_clip is None:
+      counts = [N] * B
+    else:
       counts = self._check_points_per_clip(points_per_clip, feature_grids, query_features,
                                            query_points_in_video)
-      B = len(counts)
     video_table = None
     if per_clip is not None:
-      if len(per_clip) != B:
-        raise ValueError(f'video_size has {len(per_clip)} (h, w) pairs for {B} clips')
-      # [B, 2] (h, w): the track update's table; the stage-A scalings broadcast per clip
-      video_table = self._const([v for hw in per_clip for v in hw], dev, torch.int32).view(B, 2)
+      if len(per_clip) != len(counts):
+        raise ValueError(f'video_size has {len(per_clip)} (h, w) pairs for {len(counts)} clips')
+      # [clips, 2] (h, w): the track update's table
+      video_table = self._const([v for hw in per_clip for v in hw], dev,
+                                torch.int32).view(len(counts), 2)
 
-    OB = 1 if counts is not None else B  # the outputs' leading dim: the clips, or one ragged row
-    occ_out, expd_out, trk_out = _new_estimates(num_iters + 1, OB, N, T, dev)
+    occ_out, expd_out, trk_out = _new_estimates(num_iters + 1, (B, N, T), dev)
     new_ctx = self._new_causal_context(causal_context, get_causal_context, causal_context_out,
-                                       num_iters, nb, OB, N, T, dev)
+                                       num_iters, nb, B, N, T, dev)
     write_ctx = get_causal_context and causal_context is not None
     am_out = None
     if self.capture_stage_a_argmax:
-      am_out = torch.empty(OB, N, T, dtype=torch.int32, device=dev)
+      am_out = torch.empty(B, N, T, dtype=torch.int32, device=dev)
       self.last_stage_a_argmax = am_out
     out = dict(occlusion=occ_out, tracks=trk_out, expected_dist=expd_out)
     if get_causal_context:
@@ -672,34 +670,27 @@ class TAPIR(nn.Module):
     pooled = {level: self._pool_pyramid(feature_grids.lowres[level].contiguous())
               for level in range(1, num_levels_total)}
 
-    if counts is None:
-      work = [(b0, b1, (slice(b0, b1), sl), None) for b0, b1, sl in _groups(B, N, T)]
-    else:  # ragged: a group's queries are the flattened slice q0..q1 of the one point axis
-      work = [(b0, b1, (0, slice(q0, q1)), self._group_counts(counts, b0, b1, q0, q1))
-              for b0, b1, q0, q1 in _ragged_groups(counts, T)]
-    for b0, b1, oi, gcounts in work:
+    for b0, b1, q0, q1 in _work_groups(counts, T):
       bs = slice(b0, b1)
-      # every [oi] slice below is contiguous: whole clips or a query chunk of one clip
-      occ0, expd0 = occ_out[0][oi], expd_out[0][oi]  # outputs are written in place
-      nq = occ0.numel() // T  # queries of the group, flattened over its clips
-      qp = query_points_in_video[oi] if query_points_in_video is not None else None
-      vsize = video_hw if video_table is None else per_clip[b0:b1]
-      am = am_out[oi] if am_out is not None else None
+      gcounts = [q1 - q0] if b1 - b0 == 1 else counts[b0:b1]
       query_clip = None
-      if gcounts is None:
-        pos = self._stage_a(pk, feature_grids.lowres[0][bs].contiguous(),
-                            query_features.lowres[0][oi].contiguous(), qp, vsize, occ0, expd0,
-                            trk_out[0][oi], am, dev)
-      else:
+      if len(set(gcounts)) > 1:
         # [nq] int32 clip (within the group) of each query: cached, so a captured step uploads nothing
         query_clip = self._const([b for b, n in enumerate(gcounts) for _ in range(n)], dev,
                                  torch.int32)
-        pos = self._stage_a_ragged(pk, feature_grids.lowres[0][bs].contiguous(),
-                                   query_features.lowres[0][oi].contiguous(), gcounts, qp, vsize,
-                                   occ0, expd0, trk_out[0][oi], am, dev)
+
+      def rows(t):  # the group's queries of a per-query tensor; outputs are written in place
+        return _query_rows(t, q0, q1)
+
+      occ0, expd0 = rows(occ_out[0]), rows(expd_out[0])
+      pos = self._stage_a(pk, feature_grids.lowres[0][bs].contiguous(),
+                          rows(query_features.lowres[0]).contiguous(), gcounts, query_clip,
+                          rows(query_points_in_video) if query_points_in_video is not None else None,
+                          video_hw if video_table is None else per_clip[b0:b1], occ0, expd0,
+                          rows(trk_out[0]), rows(am_out) if am_out is not None else None, dev)
 
       # ---- refinement iterations, one level at a time
-      bufs = self._refine_buffers(nq, T, dev)
+      bufs = self._refine_buffers(q1 - q0, T, dev)
       npi = self.num_pips_iter
       for level in range(1, num_levels_total):
         its = range((level - 1) * npi, level * npi)
@@ -707,15 +698,15 @@ class TAPIR(nn.Module):
         for it in its:
           ctx = [None] * 4
           if causal_context is not None:
-            ctx[:2] = _ctx_lists(causal_context[it], nb, oi,
+            ctx[:2] = _ctx_lists(causal_context[it], nb, q0, q1,
                                  lambda t: t.to(device=dev, dtype=torch.float32).contiguous())
           if write_ctx:
-            ctx[2:] = _ctx_lists(new_ctx[it], nb, oi)
+            ctx[2:] = _ctx_lists(new_ctx[it], nb, q0, q1)
           ctxs.append(ctx)
-        outs = [(occ_out[it + 1][oi], expd_out[it + 1][oi], trk_out[it + 1][oi]) for it in its]
+        outs = [(rows(occ_out[it + 1]), rows(expd_out[it + 1]), rows(trk_out[it + 1])) for it in its]
         self._refine_level(pk, feature_grids.hires[level][bs], feature_grids.lowres[level][bs],
-                           [g[bs] for g in pooled[level]], query_features.hires[level][oi],
-                           query_features.lowres[level][oi], pos, occ0, expd0, outs, bufs,
+                           [g[bs] for g in pooled[level]], rows(query_features.hires[level]),
+                           rows(query_features.lowres[level]), pos, occ0, expd0, outs, bufs,
                            feature_grids.resolutions[level],
                            video_hw if video_table is None else video_table[bs], ctxs, query_clip)
     return out
@@ -737,11 +728,6 @@ class TAPIR(nn.Module):
         raise ValueError(f'{name} has shape {tuple(t.shape)}; points_per_clip {counts} needs '
                          f'[1, {want[1]}, ...]')
     return counts
-
-  @staticmethod
-  def _group_counts(counts, b0, b1, q0, q1):
-    """The query counts of a ragged work group's clips b0..b1-1 (one query chunk: [q1 - q0])."""
-    return [q1 - q0] if b1 - b0 == 1 else list(counts[b0:b1])
 
   def _new_causal_context(self, causal_context, get_causal_context, causal_context_out, num_iters,
                           nb, B, N, T, dev):
@@ -782,70 +768,55 @@ class TAPIR(nn.Module):
           d[f'block_{i}_causal_2'] = torch.empty(B, N, 2, 2048, dtype=torch.float32, device=dev)
     return new_ctx
 
-  def _stage_a(self, pk, grid, qfeat, query_points, video_hw, occ, expd, tracks, argmax, dev):
+  def _stage_a(self, pk, grid, qfeat, counts, query_clip, query_points, video_hw, occ, expd,
+               tracks, argmax, dev):
     """Stage A for one group of clips: the global cost volume and the track / occlusion head of
-    qfeat [G, n, 256] against grid [G, T, h, w, 256].  Writes occ, expd [G, n, T], tracks
-    [G, n, T, 2] (video pixels) and, unless None, argmax; returns the positions [G, n, T, 2] in
-    initial-resolution pixels."""
-    G, n = qfeat.shape[:2]
-    T = grid.shape[1]
+    the group's nq queries, counts[b] of clip b one clip after the other, against grid
+    [G, T, h, w, 256].  qfeat [.., 256] (contiguous), query_points [.., 3] or None, occ, expd
+    [.., T], tracks [.., T, 2] (video pixels) and argmax (or None) hold the nq queries in any
+    leading dims.  query_clip (see _refine) None: one batched call on [G, n, ...] views, the
+    scalings broadcast per clip; else calls of at most MAX_RAGGED_CLIPS clips on [nq, ...], the
+    scalings per query.  Returns the positions [nq, T, 2] in initial-resolution pixels."""
+    G, T = grid.shape[:2]
+    nq = occ.numel() // T
     ih, iw = self.initial_resolution
-    if isinstance(video_hw[0], tuple):  # one (h, w) per clip: [G, 1, 3] and [G, 1, 1, 2] scales
-      to_init = self._const([v for h, w in video_hw for v in (T, h, w)], dev).view(G, 1, 3)
-      to_video = self._const([v for h, w in video_hw for v in (w, h)], dev).view(G, 1, 1, 2)
+    lead = (G, nq // G) if query_clip is None else (nq,)
+    if isinstance(video_hw[0], tuple):  # one (h, w) per clip: per-clip or per-query scales
+      if query_clip is not None:
+        video_hw = [hw for hw, n in zip(video_hw, counts) for _ in range(n)]
+      dims = (len(video_hw),) + (1,) * (len(lead) - 1)
+      to_init = self._const([v for h, w in video_hw for v in (T, h, w)], dev).view(*dims, 3)
+      to_video = self._const([v for h, w in video_hw for v in (w, h)], dev).view(*dims, 1, 2)
     else:
       vh, vw = video_hw
       to_init, to_video = self._const([T, vh, vw], dev), self._const([vw, vh], dev)
     qp = None
     if query_points is not None:
-      qp = query_points.to(torch.float32)
+      qp = query_points.to(torch.float32).reshape(*lead, 3)
       # utils.convert_grid_coordinates (coords * out / in), tapir_model.py:488-493
       qp = (qp * self._const([T, ih, iw], dev) / to_init).contiguous()
-    shapes, ws_bytes = _stage_a_scratch(G, n, T, grid.shape[2:])
-    pos = torch.empty(shapes[3], dtype=torch.float32, device=dev)
-    ws = self._workspace('cost_volume', ws_bytes, dev)
-    _lib.cost_volume_tracks(pk['head'], qfeat, grid, qp, self.softmax_temperature, (ih, iw), pos,
-                            occ, expd, argmax, ws)
-    # train2orig (tapir_model.py:435-441)
-    torch.div(pos * to_video, self._const([iw, ih], dev), out=tracks)
-    return pos
-
-  def _stage_a_ragged(self, pk, grid, qfeat, counts, query_points, video_hw, occ, expd, tracks,
-                      argmax, dev):
-    """_stage_a for clips with their own query counts: qfeat [nq, 256] holds the clips' queries one
-    after the other (counts[b] of clip b), grid is [G, T, h, w, 256]; occ, expd [nq, T], tracks
-    [nq, T, 2].  The scalings are per query (cached), the cost volume runs in calls of at most
-    MAX_RAGGED_CLIPS clips.  Returns the positions [nq, T, 2]."""
-    nq = qfeat.shape[0]
-    T = grid.shape[1]
-    ih, iw = self.initial_resolution
-    if isinstance(video_hw[0], tuple):  # one (h, w) per clip: [nq, 3] and [nq, 1, 2] scales
-      sizes = [hw for hw, n in zip(video_hw, counts) for _ in range(n)]
-      to_init = self._const([v for h, w in sizes for v in (T, h, w)], dev).view(nq, 3)
-      to_video = self._const([v for h, w in sizes for v in (w, h)], dev).view(nq, 1, 2)
+    qfeat, occ, expd = qfeat.view(*lead, -1), occ.view(*lead, T), expd.view(*lead, T)
+    argmax = argmax.view(*lead, T) if argmax is not None else None
+    pos = torch.empty(*lead, T, 2, dtype=torch.float32, device=dev)
+    if query_clip is None:
+      ws = self._workspace('cost_volume', _stage_a_scratch(G, nq, T, grid.shape[2:])[1], dev)
+      _lib.cost_volume_tracks(pk['head'], qfeat, grid, qp, self.softmax_temperature, (ih, iw), pos,
+                              occ, expd, argmax, ws)
     else:
-      vh, vw = video_hw
-      to_init, to_video = self._const([T, vh, vw], dev), self._const([vw, vh], dev)
-    qp = None
-    if query_points is not None:
-      qp = (query_points.to(torch.float32) * self._const([T, ih, iw], dev) / to_init).contiguous()
-    pos = torch.empty(nq, T, 2, dtype=torch.float32, device=dev)
-    step = _lib.MAX_RAGGED_CLIPS
-    for c0 in range(0, len(counts), step):
-      cs = counts[c0:c0 + step]
-      r0 = sum(counts[:c0])
-      r = slice(r0, r0 + sum(cs))
-      ws = self._workspace(
-          'cost_volume',
-          _lib.cost_volume_ragged_workspace_bytes(len(cs), r.stop - r0, (len(cs),) + grid.shape[1:]),
-          dev)
-      _lib.cost_volume_tracks_ragged(pk['head'], qfeat[r], cs, grid[c0:c0 + len(cs)],
-                                     qp[r] if qp is not None else None, self.softmax_temperature,
-                                     (ih, iw), pos[r], occ[r], expd[r],
-                                     argmax[r] if argmax is not None else None, ws)
+      step = _lib.MAX_RAGGED_CLIPS
+      for c0 in range(0, G, step):
+        cs = counts[c0:c0 + step]
+        r0 = sum(counts[:c0])
+        r = slice(r0, r0 + sum(cs))
+        ws = self._workspace('cost_volume',
+                             _stage_a_scratch(len(cs), r.stop - r0, T, grid.shape[2:])[1], dev)
+        _lib.cost_volume_tracks_ragged(pk['head'], qfeat[r], cs, grid[c0:c0 + len(cs)],
+                                       qp[r] if qp is not None else None, self.softmax_temperature,
+                                       (ih, iw), pos[r], occ[r], expd[r],
+                                       argmax[r] if argmax is not None else None, ws)
     # train2orig (tapir_model.py:435-441)
-    torch.div(pos * to_video, self._const([iw, ih], dev), out=tracks)
-    return pos
+    torch.div(pos * to_video, self._const([iw, ih], dev), out=tracks.view(*lead, T, 2))
+    return pos.view(nq, T, 2)
 
   def _refine_scratch(self, nq, T):
     """The refinement of nq queries over T frames: the (shape, dtype) of the mixer's input planes,

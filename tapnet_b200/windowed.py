@@ -223,7 +223,7 @@ def prepass_bytes(model, video_shape, frames, refinement_resolutions=None, host_
 
 def _group_queries(num_points, frames):
   """Queries per refinement group of one clip over `frames` frames (as estimate_trajectories)."""
-  return tapir_model._groups(1, max(1, num_points), max(1, frames))[0][2].stop
+  return tapir_model._work_groups([max(1, num_points)], max(1, frames))[0][3]
 
 
 def choose_window_frames(model, video_shape, num_points, free_bytes, refinement_resolutions=None,
@@ -451,7 +451,7 @@ def _windowed(model, video, query_points, window_frames, refinement_resolutions,
                                           host, itemsize) <= bound):
     max_frames *= 2
 
-  occ_out, expd_out, trk_out = tapir_model._new_estimates(num_iters + 1, B, N, T, dev)
+  occ_out, expd_out, trk_out = tapir_model._new_estimates(num_iters + 1, (B, N, T), dev)
   qp_all = query_points.to(device=dev, dtype=torch.float32)
   if N > 0 and T > 0:
     steps = [st for st in plan if st.new]
@@ -507,7 +507,7 @@ def _track_window(model, pk, win, bufs, held, plan, pass_of, qp, qframe, qf_lo, 
                   dev):
   """Stage A over level 1's range of window `win` and each refinement level over its own range,
   from the pass buffers.  sink(it, sl, (occ, expd, tracks), a) receives iteration it's estimates
-  ([1, n, frames, ...], frames from a on) of the queries sl; iteration 0 is stage A's."""
+  ([n, frames, ...], frames from a on) of the queries sl; iteration 0 is stage A's."""
   N = qp.shape[0]
   L = len(plan) - 1
   npi = model.num_pips_iter
@@ -522,22 +522,22 @@ def _track_window(model, pk, win, bufs, held, plan, pass_of, qp, qframe, qf_lo, 
 
   a1, z1 = win.levels[0]
   T1 = z1 - a1
-  for _, _, sl in tapir_model._groups(1, N, T1):
-    nq = sl.stop - sl.start
+  for _, _, q0, q1 in tapir_model._work_groups([N], T1):
+    sl, nq = slice(q0, q1), q1 - q0
     shapes, _ = tapir_model._stage_a_scratch(1, nq, T1, grid(0, (a1, z1)).shape[2:])
     occ0, expd0, trk0 = (torch.empty(s, dtype=torch.float32, device=dev) for s in shapes[:3])
-    qp_w = torch.cat([(qframe[sl] - a1)[:, None], qp[sl, 1:]], dim=1)[None].contiguous()
-    pos = model._stage_a(pk, grid(0, (a1, z1)), qf_lo[0][sl][None].contiguous(), qp_w, hw,
+    qp_w = torch.cat([(qframe[sl] - a1)[:, None], qp[sl, 1:]], dim=1)
+    pos = model._stage_a(pk, grid(0, (a1, z1)), qf_lo[0][sl].contiguous(), [nq], None, qp_w, hw,
                          occ0, expd0, trk0, None, dev)
     sink(0, sl, (occ0, expd0, trk0), a1)
     prev = (a1, z1)
     for l in range(1, L + 1):
       al, zl = win.levels[l - 1]
       Tl = zl - al
-      pos = pos[:, :, al - prev[0]:zl - prev[0]].contiguous()
-      occ0_l = occ0[:, :, al - a1:zl - a1].contiguous()
-      expd0_l = expd0[:, :, al - a1:zl - a1].contiguous()
-      level_outs = tapir_model._new_estimates(npi, 1, nq, Tl, dev)
+      pos = pos[:, al - prev[0]:zl - prev[0]].contiguous()
+      occ0_l = occ0[:, al - a1:zl - a1].contiguous()
+      expd0_l = expd0[:, al - a1:zl - a1].contiguous()
+      level_outs = tapir_model._new_estimates(npi, (nq, Tl), dev)
       model._refine_level(pk, grid(l, (al, zl), hires=True), grid(l, (al, zl)), pooled[l],
                           qf_hi[l][sl], qf_lo[l][sl], pos, occ0_l, expd0_l,
                           list(zip(*level_outs)), model._refine_buffers(nq, Tl, dev),
@@ -563,7 +563,7 @@ def _sweep(model, pk, clip, qp, qframe, qf_lo, qf_hi, plan, steps, pass_of, halo
   for win in windows:
     def sink(it, sl, xs, a, win=win):
       for full, x in zip(outs, xs):
-        full[it][b, sl, win.start:win.stop] = x[0, :, win.start - a:win.stop - a]
+        full[it][b, sl, win.start:win.stop] = x[:, win.start - a:win.stop - a]
 
     _slide(bufs, held, steps, win, run)
     _track_window(model, pk, win, bufs, held, plan, pass_of, qp, qframe, qf_lo, qf_hi, (H, W),
@@ -879,13 +879,13 @@ class _ReaderSweep:
     npi = model.num_pips_iter
     num_iters = npi * (len(self.plan) - 1)
     N, c = self.qp.shape[0], win.stop - win.start
-    est = [tuple(x[0] for x in tapir_model._new_estimates(1, 1, N, c, dev))
+    est = [tuple(x[0] for x in tapir_model._new_estimates(1, (1, N, c), dev))
            if self.unrefined or (it and it % npi == 0) else None for it in range(num_iters + 1)]
 
     def sink(it, sl, xs, a):
       if est[it] is not None:
         for dst, x in zip(est[it], xs):
-          dst[0, sl] = x[0, :, win.start - a:win.stop - a]
+          dst[0, sl] = x[:, win.start - a:win.stop - a]
 
     _track_window(model, self.pk, win, self.bufs, self.held, self.plan, self.pass_of, self.qp,
                   self.qframe, self.qf_lo, self.qf_hi, self.src.hw, sink, dev)

@@ -141,7 +141,7 @@ def _compare(both, one, b, exact):
 
 
 @pytest.mark.parametrize('rows_bound', [None, 'two_clips', 'query_chunks'])
-def test_forward_batch_of_three_equals_per_clip_calls(rows_bound):
+def test_forward_batch_of_three_in_work_groups_equals_per_clip_calls(rows_bound):
   """Non-causal: bit for bit, with all clips in one group, with groups of two clips, and with
   every clip split into query chunks (the same bound applied to the per-clip calls)."""
   model, _, _ = get_model()
@@ -151,15 +151,15 @@ def test_forward_batch_of_three_equals_per_clip_calls(rows_bound):
   old = tapir_model._MAX_ROWS_PER_CHUNK
   tapir_model._MAX_ROWS_PER_CHUNK = bound
   try:
-    groups = tapir_model._groups(B, N, T)
+    groups = tapir_model._work_groups([N] * B, T)
     both = model(v, q)
     ones = [model(v[b:b + 1], q[b:b + 1]) for b in range(B)]
   finally:
     tapir_model._MAX_ROWS_PER_CHUNK = old
   if rows_bound is None:
-    assert groups == [(0, 3, slice(0, N))]
+    assert groups == [(0, 3, 0, 3 * N)]
   elif rows_bound == 'two_clips':
-    assert groups == [(0, 2, slice(0, N)), (2, 3, slice(0, N))]
+    assert groups == [(0, 2, 0, 2 * N), (2, 3, 2 * N, 3 * N)]
   else:
     assert len(groups) == 3 * 3 and all(g[1] - g[0] == 1 for g in groups)
   for b in range(B):

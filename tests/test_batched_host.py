@@ -68,20 +68,19 @@ def test_tracker_rejects_a_stream_count_below_one():
 @pytest.mark.parametrize('B,N,T,bound', [(1, 16, 24, 98304), (8, 64, 24, 98304), (3, 21, 4, 168),
                                          (3, 21, 4, 32), (2, 5000, 48, 98304), (40, 4000, 1, 98304),
                                          (5, 70000, 1, 10 ** 9)])
-def test_groups_cover_every_clip_and_query_within_bounds(B, N, T, bound, monkeypatch):
+def test_work_groups_of_equal_counts_cover_every_clip_and_query_within_bounds(B, N, T, bound, monkeypatch):
   monkeypatch.setattr(tapir_model, '_MAX_ROWS_PER_CHUNK', bound)
-  groups = tapir_model._groups(B, N, T)
+  groups = tapir_model._work_groups([N] * B, T)
   seen = [[0] * N for _ in range(B)]
-  for b0, b1, sl in groups:
-    n = sl.stop - sl.start
-    assert b1 > b0 and n > 0 and (b1 - b0) * n <= 65535
+  for b0, b1, q0, q1 in groups:  # queries q0..q1-1 of the flattened [B * N] point axis
+    assert b1 > b0 and q1 > q0 and q1 - q0 <= 65535
     if b1 - b0 > 1:  # several clips: whole clips within the row bound
-      assert sl == slice(0, N) and (b1 - b0) * N * T <= bound
-    for b in range(b0, b1):
-      for i in range(sl.start, sl.stop):
-        seen[b][i] += 1
+      assert (q0, q1) == (b0 * N, b1 * N) and (b1 - b0) * N * T <= bound
+    for q in range(q0, q1):
+      assert b0 <= q // N < b1
+      seen[q // N][q % N] += 1
   assert all(c == 1 for row in seen for c in row)
   if N * T <= bound and N <= 65535:
-    assert all(sl == slice(0, N) for _, _, sl in groups)
+    assert all((q0, q1) == (b0 * N, b1 * N) for b0, b1, q0, q1 in groups)
   if B == 1 and N * T <= bound:
-    assert groups == [(0, 1, slice(0, N))]
+    assert groups == [(0, 1, 0, N)]

@@ -1,4 +1,4 @@
-"""Per-stream point counts without a GPU: the ragged work groups, the grouped GEMM's m-tile tables,
+"""Per-stream point counts without a GPU: the work groups, the grouped GEMM's m-tile tables,
 and the argument checks of the tracker, estimate_trajectories and the new C-ABI calls."""
 import ctypes
 import random
@@ -12,20 +12,31 @@ kBlockM = 128  # the wgmma GEMM's m-tile (gemm_tc.cu)
 
 
 # ------------------------------------------------------------------------- work groups
+def _uniform_groups(B, N, T):
+  """The work groups of B clips of N queries each as (b0, b1, query slice): whole clips while the
+  group's rows fit _MAX_ROWS_PER_CHUNK and its queries 65535, else query chunks of one clip."""
+  if N * T <= tapir_model._MAX_ROWS_PER_CHUNK and N <= 65535:
+    g = max(1, min(B, tapir_model._MAX_ROWS_PER_CHUNK // (N * T), 65535 // N))
+    return [(b0, min(b0 + g, B), slice(0, N)) for b0 in range(0, B, g)]
+  chunk_q = max(1, min(N, tapir_model._MAX_ROWS_PER_CHUNK // T, 65535))
+  return [(bi, bi + 1, slice(q0, min(q0 + chunk_q, N)))
+          for bi in range(B) for q0 in range(0, N, chunk_q)]
+
+
 def _flat(groups, N):
-  """_groups' (b0, b1, query slice) as flattened (b0, b1, q0, q1)."""
+  """(b0, b1, query slice) groups as flattened (b0, b1, q0, q1)."""
   return [(b0, b1, b0 * N + sl.start, (b1 - 1) * N + sl.stop) for b0, b1, sl in groups]
 
 
 @pytest.mark.parametrize('B,N,T', [(1, 1, 1), (8, 64, 1), (5, 1024, 1), (3, 7, 48), (200, 1, 1),
                                    (4, 65535, 1), (2, 70000, 1), (3, 5000, 24), (2, 98304, 2),
                                    (70, 1500, 1)])
-def test_equal_counts_give_the_uniform_groups(B, N, T):
-  assert tapir_model._ragged_groups([N] * B, T) == _flat(tapir_model._groups(B, N, T), N)
+def test_equal_counts_work_groups_are_the_uniform_groups(B, N, T):
+  assert tapir_model._work_groups([N] * B, T) == _flat(_uniform_groups(B, N, T), N)
 
 
 def _check_cover(counts, T):
-  groups = tapir_model._ragged_groups(counts, T)
+  groups = tapir_model._work_groups(counts, T)
   offs = [sum(counts[:b]) for b in range(len(counts) + 1)]
   q = 0
   for b0, b1, q0, q1 in groups:
@@ -42,7 +53,7 @@ def _check_cover(counts, T):
   assert q == offs[-1]
 
 
-def test_ragged_groups_cover_every_query_once_within_the_bounds():
+def test_work_groups_cover_every_query_once_within_the_bounds():
   rng = random.Random(7)
   for _ in range(300):
     counts = [rng.choice([1, 2, 63, 64, 65, 200, 1024, 5000, 65535, 70000])
@@ -110,24 +121,40 @@ def test_tracker_rejects_bad_counts():
     streaming.OnlineTracker(m, 256, 256, [4, 0], num_streams=2)
 
 
-def _cpu_tracker(counts):
-  """A ragged tracker's argument handling without a device: construction stops at the CUDA check,
-  so the checks under test are run on a bare instance."""
+def _cpu_tracker(counts, num_streams=None):
+  """A tracker's argument handling without a device: construction stops at the CUDA check, so the
+  checks under test are run on a bare instance.  counts: one int (num_streams streams) or a list."""
   trk = object.__new__(streaming.OnlineTracker)
-  trk.num_streams, trk._counts, trk.num_points, trk.dev = len(counts), counts, counts, torch.device('cpu')
+  trk.num_streams = num_streams if isinstance(counts, int) else len(counts)
+  trk._counts = [counts] * trk.num_streams if isinstance(counts, int) else counts
+  trk.num_points, trk.dev = counts, torch.device('cpu')
   return trk
 
 
-def test_tracker_query_point_lists_are_checked():
+def test_tracker_query_points_are_checked():
+  """The list form of a tracker of per-stream counts, and the tensor forms of one count."""
   trk = _cpu_tracker([3, 1])
   with pytest.raises(ValueError, match='list of 2 query point tensors'):
-    trk._ragged_query_points(torch.zeros(2, 3, 3))
+    trk._query_points(torch.zeros(2, 3, 3))
   with pytest.raises(ValueError, match='list of 2 query point tensors'):
-    trk._ragged_query_points([torch.zeros(3, 3)])
+    trk._query_points([torch.zeros(3, 3)])
   with pytest.raises(ValueError, match=r'stream 1: query points must be \[1, 3\]'):
-    trk._ragged_query_points([torch.zeros(3, 3), torch.zeros(2, 3)])
-  assert [tuple(q.shape) for q in trk._ragged_query_points([torch.zeros(3, 3), torch.zeros(1, 3)])] == [
+    trk._query_points([torch.zeros(3, 3), torch.zeros(2, 3)])
+  assert [tuple(q.shape) for q in trk._query_points([torch.zeros(3, 3), torch.zeros(1, 3)])] == [
       (3, 3), (1, 3)]
+  trk = _cpu_tracker(4, num_streams=2)
+  assert [tuple(q.shape) for q in trk._query_points(torch.zeros(2, 4, 3))] == [(4, 3), (4, 3)]
+  with pytest.raises(ValueError, match=r'query_points must be \[2, N, 3\], got \(1, 4, 3\)'):
+    trk._query_points(torch.zeros(4, 3))
+  with pytest.raises(ValueError, match=r'query_points must be \[2, N, 3\]'):
+    trk._query_points(torch.zeros(2, 4, 2))
+  with pytest.raises(ValueError, match='expected 4 query points, got 5'):
+    trk._query_points(torch.zeros(2, 5, 3))
+  one = _cpu_tracker(4, num_streams=1)
+  assert [tuple(q.shape) for q in one._query_points(torch.zeros(4, 3))] == [(4, 3)]
+  assert [tuple(q.shape) for q in one._query_points(torch.zeros(1, 4, 3))] == [(4, 3)]
+  with pytest.raises(ValueError, match='expected 4 query points, got 3'):
+    one._query_points(torch.zeros(3, 3))
 
 
 def test_update_query_checks_the_streams_own_count():

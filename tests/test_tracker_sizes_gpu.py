@@ -163,7 +163,7 @@ def _vis_prob(occ, expd):
   return (1 - torch.sigmoid(occ)) * (1 - torch.sigmoid(expd))
 
 
-def test_mixed_size_tracker_against_single_streams_golden_and_eager():
+def test_mixed_size_packed_tracker_against_single_streams_golden_and_eager():
   g = load_golden('causal_480x3_n8')
   meta = g['meta']
   assert (meta['H'], meta['W']) == SIZES[GOLDEN_SLOT]
@@ -193,8 +193,9 @@ def test_mixed_size_tracker_against_single_streams_golden_and_eager():
     for grp, st in zip(trk._groups, saved):
       et, eo, ee = trk._step_group(grp, st)
       for i, s in enumerate(grp.streams):
-        assert torch.equal(tracks[s], et[i]), f'frame {t} stream {s}: replay != eager'
-        assert torch.equal(occ[s], eo[i]) and torch.equal(expd[s], ee[i])
+        r = slice(grp.offsets[i], grp.offsets[i] + N)
+        assert torch.equal(tracks[s], et[0, r]), f'frame {t} stream {s}: replay != eager'
+        assert torch.equal(occ[s], eo[0, r]) and torch.equal(expd[s], ee[0, r])
       for d, de in zip(grp.state, st):
         for k in d:
           assert torch.equal(d[k], de[k]), f'frame {t}: state {k}'
@@ -220,7 +221,7 @@ def test_mixed_size_tracker_against_single_streams_golden_and_eager():
   assert g_t < TRACK_TOL and g_o < LOGIT_TOL and g_e < LOGIT_TOL
 
 
-def test_mixed_size_streams_are_isolated():
+def test_mixed_size_packed_streams_are_isolated():
   """Changing stream 2's frames (200^2, grouped with 240^2) and re-targeting one of its points
   leaves every other stream's outputs and causal state bit for bit unchanged."""
   model, _, _ = get_model(causal=True)
@@ -239,8 +240,12 @@ def test_mixed_size_streams_are_isolated():
         trk.update_query(fr[2][1], torch.tensor([0.0, 40.5, 150.25]), 9, stream=2)
       trk.step([f[t] for f in fr])
       outs.append([x.clone() for x in (*trk._out[:2], *trk.last_logits)])
-    state = {s: [{k: v[trk._slot[s][1]].clone() for k, v in d.items()}
-                 for d in trk._groups[trk._slot[s][0]].state] for s in range(S)}
+    state = {}
+    for s in range(S):
+      gi, slot = trk._slot[s]
+      grp = trk._groups[gi]
+      r = slice(grp.offsets[slot], grp.offsets[slot] + N)
+      state[s] = [{k: v[:, r].clone() for k, v in d.items()} for d in grp.state]
     trk.close()
     return outs, state
 
