@@ -10,7 +10,7 @@ run() {  # name, env, pytest args...
   local name=$1; shift
   local envs=$1; shift
   echo "=== tier $name"
-  env $envs timeout 600 python -m pytest "$@" -q -m gpu --timeout 300 -p no:cacheprovider \
+  env $envs timeout 1500 python -m pytest "$@" -q -m gpu --timeout 300 --durations=15 -p no:cacheprovider \
       > "gpurun_out/$name.log" 2>&1
   local r=$?
   tail -n 25 "gpurun_out/$name.log"
@@ -33,7 +33,8 @@ for t in $TIERS; do
     bulk)        run bulk "X=1" tests/test_bulk_gpu.py ;;
     eval)        run eval "X=1" tests/test_tapvid_gpu.py tests/test_redetection_gpu.py ;;
     sizes)       run sizes "X=1" tests/test_tracker_sizes_gpu.py ;;
-    points)      run points "X=1" tests/test_stream_points_gpu.py ;;
+    points)      run points "X=1" tests/test_stream_points_gpu.py tests/test_refine_ops_gpu.py::test_local_corr_ragged \
+                     tests/test_refine_ops_gpu.py::test_refine_update_bit_exact ;;
     no_halo)     run no_halo "TAPIR_B200_CONV_HALO=0" tests/test_gemm_gpu.py tests/test_gemm_variants_gpu.py tests/test_gemm_exact_gpu.py tests/test_stages_gpu.py tests/test_end_to_end_gpu.py ;;
     all)         run all "X=1" tests ;;
   esac

@@ -56,3 +56,13 @@ timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
     -k "not evaluate and not 1500" \
     2>&1 | grep -E '^=========|passed|failed' | tail -n 25
 echo "sanitizer redetection memcheck rc=${PIPESTATUS[0]}"
+# then the per-clip point-count path: the grouped cost-volume GEMM on its designed maps (tail
+# guard past the workspace), the ragged stage A, local correlation and track update against
+# per-clip calls and the float64 references, and estimate_trajectories over more than 64 clips;
+# the 65535-query call and the 70-stream tracker are left out
+timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
+    python -m pytest -q -m gpu -p no:cacheprovider tests/test_plane_pairs_gpu.py tests/test_stream_points_gpu.py \
+    tests/test_refine_ops_gpu.py \
+    -k "(cost_volume_pairs or ragged or points_per_clip or more_than_64) and not query_limit and not 70_streams" \
+    2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+echo "sanitizer ragged memcheck rc=${PIPESTATUS[0]}"

@@ -18,8 +18,9 @@ A's planes are laid out plane_stride = rows * lda + GAP elements apart, with lda
 every element between the planes and past column K (gapped_a).  A kernel that reads A with a wrong
 plane stride, plane offset or row length sees NaN, not a small error.
 
-The second half of this module designs cost maps for the stage-A cost volume, the one batched GEMM,
-whose planes tapir_split_planes makes from fp32 queries and grids (see cost-volume designs)."""
+The second half of this module designs cost maps for the stage-A cost volume, the one batched and
+the one grouped GEMM, whose planes tapir_split_planes makes from fp32 queries and grids (see
+cost-volume designs)."""
 import numpy as np
 import torch
 
@@ -276,61 +277,114 @@ def cv_offsets(kind):
   return pl.float()[:, 0]
 
 
-class CvDesign:
-  """Query features qf [B, N, C] and grids [B, T, gh, gw, C] (fp32) of the designed maps, and per
-  map (b, n, t) its kind (index into CV_KINDS) and candidate cells a, b."""
+CV_GROUPS = 64  # channel groups of C = 256: query n of a clip reads group n mod 64
 
-  def __init__(self, B, N, T, gh, gw, C=256, seed=0):
-    assert N * CV_CHANNELS <= C
-    self.B, self.N, self.T, self.gh, self.gw, self.C = B, N, T, gh, gw, C
+
+class CvDesign:
+  """The designed maps of B = len(counts) clips, counts[b] queries in clip b: query features qf
+  [sum counts, C] (the clips' queries one after the other; the batched form is counts = [N] * B)
+  and grids [B, T, gh, gw, C] (fp32), and per map (query q, frame t) its kind (index into
+  CV_KINDS) and candidate cells a, b, [Q, T].
+
+  Query n of a clip reads channel group n mod 64: queries n >= 64 repeat query n mod 64's map and
+  so its outputs, bit for bit.  Each clip draws its own candidate cells, and its channels outside
+  the groups its queries read hold random values: a query that reads another clip's grid rows
+  finds another arg-max.  clip [Q] and rank [Q] are each query's clip and index within it."""
+
+  def __init__(self, counts, T, gh, gw, C=256, seed=0):
+    assert C == CV_CHANNELS * CV_GROUPS
+    self.counts = [int(n) for n in counts]
+    B = len(self.counts)
+    self.B, self.T, self.gh, self.gw, self.C = B, T, gh, gw, C
+    self.Q = sum(self.counts)
+    self.clip = torch.tensor([b for b, n in enumerate(self.counts) for _ in range(n)])
+    self.rank = torch.cat([torch.arange(n) for n in self.counts])
+    self.group = self.rank % CV_GROUPS
     cells = gh * gw
     g = torch.Generator().manual_seed(seed + 1000 * gh + gw)
-    self.qf = torch.zeros(B, N, C)
-    for n in range(N):
-      self.qf[:, n, CV_CHANNELS * n] = Q_PROBE
-      self.qf[:, n, CV_CHANNELS * n + 1:CV_CHANNELS * n + CV_CHANNELS] = 1.0
-    # channels no query reads: any finite values (a query is zero there)
+    self.qf = _probe_rows(C)[self.group].contiguous()
+    # channels no query of the clip reads: any finite values (a query is zero there)
     self.grid = torch.randn(B, T, gh, gw, C, generator=g)
-    self.grid[..., :CV_CHANNELS * N] = 0
-    self.kind = torch.zeros(B, N, T, dtype=torch.int64)
-    self.cell_a = torch.zeros(B, N, T, dtype=torch.int64)
-    self.cell_b = torch.zeros(B, N, T, dtype=torch.int64)
+    # per (clip, group, frame); a query's map is that of (its clip, its group)
+    kind = torch.zeros(B, CV_GROUPS, T, dtype=torch.int64)
+    cell_a, cell_b = torch.zeros_like(kind), torch.zeros_like(kind)
     flat = self.grid.view(B, T, cells, C)
     k = 0
     for b in range(B):
-      for n in range(N):
+      used = min(self.counts[b], CV_GROUPS)
+      flat[b, :, :, :CV_CHANNELS * used] = 0
+      for n in range(used):
         for t in range(T):
-          kind = CV_KINDS[k % len(CV_KINDS)]
+          kd = CV_KINDS[k % len(CV_KINDS)]
           ca, cb = torch.randperm(cells, generator=g)[:2].tolist()
           c0 = CV_CHANNELS * n
           flat[b, t, ca, c0] = G_A
-          if kind == 'drop (0, 0)':
+          if kd == 'drop (0, 0)':
             flat[b, t, cb, c0] = G_B
           else:
-            flat[b, t, cb, c0 + 1:c0 + CV_CHANNELS] = cv_offsets(kind)
-          self.kind[b, n, t], self.cell_a[b, n, t], self.cell_b[b, n, t] = k % len(CV_KINDS), ca, cb
+            flat[b, t, cb, c0 + 1:c0 + CV_CHANNELS] = cv_offsets(kd)
+          kind[b, n, t], cell_a[b, n, t], cell_b[b, n, t] = k % len(CV_KINDS), ca, cb
           k += 1
+    self.kind = kind[self.clip, self.group]
+    self.cell_a = cell_a[self.clip, self.group]
+    self.cell_b = cell_b[self.clip, self.group]
 
   def winner(self):
-    """[B, N, T] the cell each map's design makes the arg-max."""
+    """[Q, T] the cell each map's design makes the arg-max."""
     gain = self.kind == CV_KINDS.index('gain')
     return torch.where(gain, self.cell_b, self.cell_a)
 
+  def _maps(self, acc):
+    """[B, 64, T, cells] per (clip, channel group) -> [Q, T, cells] per query."""
+    return acc[self.clip, self.group]
+
   def heat(self, pairs, dtype=torch.float32):
-    """The identity head's heat (temperature 1) of every map, [B, N, T, cells]: the cost volume
+    """The identity head's heat (temperature 1) of every map, [Q, T, cells]: the cost volume
     summed over `pairs` (repeats counted) in fp32, pair by pair in order and channel by channel, as
     the GEMM orders its terms, then fp32(fp32(v + 64) - 64).  dtype float64: the same sums exact."""
-    B, N, T, C = self.B, self.N, self.T, self.C
+    B, T, C = self.B, self.T, self.C
     cells = self.gh * self.gw
-    qp = split_like_kernel(self.qf.reshape(-1, C), 3).to(dtype).view(3, B, N, C)
-    gp = split_like_kernel(self.grid.reshape(-1, C), 3).to(dtype).view(3, B, T, cells, C)
-    acc = torch.zeros(B, N, T, cells, dtype=dtype)
+    qp = split_like_kernel(_probe_rows(C), 3).to(dtype)
+    gp = split_like_kernel(self.grid.reshape(-1, C), 3).to(dtype).view(3, B, T, cells, CV_GROUPS, CV_CHANNELS)
+    # [3, 64, 4]: the planes of the channels each group's queries read
+    qg = torch.stack([qp[:, n, CV_CHANNELS * n:CV_CHANNELS * (n + 1)] for n in range(CV_GROUPS)], 1)
+    acc = torch.zeros(B, T, cells, CV_GROUPS, dtype=dtype)
     for i, j in pairs:
-      for n in range(N):
-        for c in range(CV_CHANNELS * n, CV_CHANNELS * (n + 1)):
-          # fp32 products of two bf16 values are exact; each add rounds as the accumulator does
-          acc[:, n] += qp[i, :, n, c][:, None, None] * gp[j, :, :, :, c]
-    return (acc + 64.0) - 64.0
+      for c in range(CV_CHANNELS):
+        # fp32 products of two bf16 values are exact; each add rounds as the accumulator does
+        acc += qg[i, :, c] * gp[j, ..., c]
+    return self._maps(((acc + 64.0) - 64.0).permute(0, 3, 1, 2))
+
+  def heat_simt(self):
+    """The identity head's heat as the SIMT kernel makes it, [Q, T, cells]: a = sum of the query's
+    planes and b = sum of the grid's (both exact: the planes split an fp32 value), then one fp32
+    FMA per channel, acc = fp32(a b + acc), channel by channel from 0.  a b + acc is exact in
+    float64 here (at most 48 + 2 significant bits), so rounding it once to fp32 is the FMA."""
+    B, T, C = self.B, self.T, self.C
+    cells = self.gh * self.gw
+    q = _probe_rows(C).view(CV_GROUPS, CV_GROUPS, CV_CHANNELS).double()
+    qg = torch.stack([q[n, n] for n in range(CV_GROUPS)])  # [64, 4]: the channels each group reads
+    gr = self.grid.view(B, T, cells, CV_GROUPS, CV_CHANNELS).double()
+    acc = torch.zeros(B, T, cells, CV_GROUPS, dtype=torch.float32)
+    for c in range(CV_CHANNELS):
+      acc = (qg[:, c] * gr[..., c] + acc.double()).float()
+    return self._maps(((acc + 64.0) - 64.0).permute(0, 3, 1, 2))
+
+  @staticmethod
+  def argmax(heat):
+    """Arg-max over the last dimension, the lowest index winning ties (as the heads)."""
+    m = heat.max(-1, keepdim=True).values
+    idx = torch.arange(heat.shape[-1]).expand_as(heat)
+    return torch.where(heat == m, idx, heat.shape[-1]).min(-1).values
+
+
+def _probe_rows(C):
+  """[64, C] the query feature of each channel group."""
+  probe = torch.zeros(CV_GROUPS, C)
+  for n in range(CV_GROUPS):
+    probe[n, CV_CHANNELS * n] = Q_PROBE
+    probe[n, CV_CHANNELS * n + 1:CV_CHANNELS * n + CV_CHANNELS] = 1.0
+  return probe
 
   @staticmethod
   def argmax(heat):

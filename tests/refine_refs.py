@@ -76,9 +76,10 @@ def _lookup(table, y, x):
   return torch.gather(table.reshape(Q, -1), 1, yy * Wp + xx)
 
 
-def local_corr_ref(levels, pos, feats, init_hw, batch, planes=3):
+def local_corr_ref(levels, pos, feats, init_hw, batch, planes=3, query_clip=None):
   """levels: fp32 [batch, T, h, w, C] per level (C 128 for level 0, 256 after); pos [Q, T, 2]
-  fp32 (x, y) with Q = batch * N queries (query q reads clip q // N); feats = (hi [Q, T, 128],
+  fp32 (x, y) with Q = batch * N queries (query q reads clip q // N), or, given query_clip
+  (int [Q]), any Q queries, query q reading clip query_clip[q]; feats = (hi [Q, T, 128],
   lo [Q, T, 256]) per row.  Returns (corr [Q, T, 49 L], bound), corr in float64.
 
   The samples are taken at pix_exact's positions (the 7 x 7 offsets in grid cells, zero padding)
@@ -95,8 +96,7 @@ def local_corr_ref(levels, pos, feats, init_hw, batch, planes=3):
   The fp64 reference's own rounding adds gamma_64(C + 8) sum |f q|."""
   ih, iw = init_hw
   Q, T, _ = pos.shape
-  N = Q // batch
-  clip = torch.arange(Q) // N
+  clip = torch.arange(Q) // (Q // batch) if query_clip is None else torch.as_tensor(query_clip).long().cpu()
   dy = torch.from_numpy(np.repeat(OFFSETS, 7)).double()
   dx = torch.from_numpy(np.tile(OFFSETS, 7)).double()
   corr = torch.zeros(Q, T, 49 * len(levels), dtype=torch.float64)
@@ -304,17 +304,19 @@ def pool_emulate(grid):
 
 def update_emulate(res, pos, occ, expd, feats, init_hw, resize_hw, video_hw):
   """tapir_model.py:674-685 and train2orig :435-441 in fp32, in the reference's order: res
-  [Q, T, >= 388], pos [Q, T, 2] (x, y), occ, expd [Q, T], feats [Q, T, 384].  Returns (pos,
-  occ, expd, feats, tracks): delta = res[:2] * init / resize (multiply, then divide), pos + delta,
+  [Q, T, >= 388], pos [Q, T, 2] (x, y), occ, expd [Q, T], feats [Q, T, 384]; video_hw (h, w), or
+  one (h, w) per query [Q, 2] (a ragged call's size of each query's clip).  Returns (pos, occ,
+  expd, feats, tracks): delta = res[:2] * init / resize (multiply, then divide), pos + delta,
   res[2] + occ, res[3] + expd, res[4:388] + feats, tracks = pos * video / init."""
   r = res.numpy().astype(f32)
   p = pos.numpy().astype(f32)
   ih, iw = init_hw
   rh, rw = resize_hw
-  vh, vw = video_hw
+  v = np.asarray(video_hw, f32)
+  vh, vw = (v[0], v[1]) if v.ndim == 1 else (v[:, None, 0], v[:, None, 1])
   d = np.stack([(r[..., 0] * f32(iw)).astype(f32) / f32(rw), (r[..., 1] * f32(ih)).astype(f32) / f32(rh)], -1)
   newp = (d.astype(f32) + p).astype(f32)
-  trk = np.stack([(newp[..., 0] * f32(vw)).astype(f32) / f32(iw), (newp[..., 1] * f32(vh)).astype(f32) / f32(ih)], -1)
+  trk = np.stack([(newp[..., 0] * vw).astype(f32) / f32(iw), (newp[..., 1] * vh).astype(f32) / f32(ih)], -1)
   t = torch.from_numpy
   return (t(newp), t((r[..., 2] + occ.numpy()).astype(f32)), t((r[..., 3] + expd.numpy()).astype(f32)),
           t((r[..., 4:388] + feats.numpy()).astype(f32)), t(trk.astype(f32)))

@@ -11,9 +11,9 @@ Runs: the plain GEMM under the cooperative schedule (P = 1, 2, 3) and the ping-p
 at BLOCK_N 64 and 128; the generic 3 x 3 convolution (TAPIR_B200_CONV_HALO=0, P = 1, 2, 3, C = 64
 and 128); the halo convolution under both schedules (P = 1, 2, C = 64); split-K (P = 2, 3, K >=
 2048, the partial-sum kernel then splitk_reduce_kernel); the SIMT kernel (P = 1, 2, 3); one run per
-kernel with three bf16 output planes.  Last, the stage-A cost volume, the one batched P = 3 GEMM,
-through tapir_cost_volume_tracks_batched: its designed maps must pick the cells
-plane_pairs.CvDesign emulates."""
+kernel with three bf16 output planes.  Last, the stage-A cost volume, the one batched and the one
+grouped P = 3 GEMM, through tapir_cost_volume_tracks_batched and tapir_cost_volume_tracks_ragged
+(tensor cores and SIMT): its designed maps must pick the cells plane_pairs.CvDesign emulates."""
 import numpy as np
 import pytest
 import torch
@@ -165,34 +165,97 @@ def test_switches_reach_the_kernels_under_test():
 
 
 # ------------------------------------------------------------------------------ cost volume
-CV_CASES = [(2, 40, 2, 32, 32), (2, 40, 3, 25, 39)]  # (B, N, T, gh, gw)
+COUNTS_64 = [(1, 63, 64, 65, 129)[b % 5] for b in range(64)]  # one grouped call of 64 clips
+# id: (entry, counts, T, gh, gw).  Batched: N = 40 queries per clip, so an m-tile reads the next
+# clip's rows; 2925 cells (25 x 39 x 3) are no multiple of either tile width.  Ragged: counts around
+# the 128-row m-tile (a clip's last tile holds 1, 40, 127, 0 or 1 rows), a one-query clip between
+# two of more than 128, and 64 clips, at T = 1 and 3 on the tensor-core head's 32 x 32 maps and the
+# generic head's 25 x 39.
+CV_CASES = {'32x32': ('batched', [40] * 2, 2, 32, 32), '25x39': ('batched', [40] * 2, 3, 25, 39)}
+for _name, _counts in (('5', [1, 40, 127, 128, 129]), ('3', [200, 1, 129]), ('64', COUNTS_64)):
+  for _T in (1, 3):
+    for _gh, _gw in ((32, 32), (25, 39)):
+      CV_CASES[f'ragged{_name}_T{_T}_{_gh}x{_gw}'] = ('ragged', _counts, _T, _gh, _gw)
+_DESIGNS_CV = {}
+
+
+def _cv_design(case):
+  if case not in _DESIGNS_CV:
+    _DESIGNS_CV[case] = PP.CvDesign(*CV_CASES[case][1:])
+  return _DESIGNS_CV[case]
+
+
+def _run_cost_volume(cv, entry, gemm, bn=None):
+  """One stage-A call on the design's maps with the identity head at temperature 1 (the heat is
+  the map, exactly); every output between NaN guards.  The workspace has one m-tile of cost-volume
+  rows (128 T gh gw floats) past what the call asks for, filled with a sentinel that must survive:
+  for 32 x 32 maps cv is the workspace's last buffer, so a store of the rows of the last clip's last
+  m-tile past its count lands there (other maps: past the generic head's scratch, which follows
+  cv).  It does not see such stores for inner clips, whose extra rows land on the next clip's rows;
+  there the designs and the repeated queries n >= 64 may see them."""
+  B, T, gh, gw, Q = cv.B, cv.T, cv.gh, cv.gw, cv.Q
+  qf, grid = cv.qf.cuda(), cv.grid.cuda()
+  outs = {k: U.guarded(Q * T * (2 if k == 'pts' else 1), torch.int32 if k == 'am' else torch.float32)
+          for k in ('pts', 'occ', 'expd', 'am')}
+  if entry == 'batched':
+    N = cv.counts[0]
+    assert cv.counts == [N] * B
+    need = _lib.cost_volume_workspace_bytes((B, N), grid.shape)
+    view = lambda k: outs[k][1].view((B, N, T, 2) if k == 'pts' else (B, N, T))  # noqa: E731
+  else:
+    need = _lib.cost_volume_ragged_workspace_bytes(B, Q, grid.shape)
+    view = lambda k: outs[k][1].view((Q, T, 2) if k == 'pts' else (Q, T))  # noqa: E731
+  tail = 128 * T * gh * gw * 4
+  ws = torch.full((need + tail,), 0xA5, dtype=torch.uint8, device='cuda')
+  with U.switches(TAPIR_B200_GEMM=gemm, TAPIR_B200_BLOCK_N=bn):
+    if entry == 'batched':
+      _lib.cost_volume_tracks(_head_weights('identity'), qf.view(B, N, -1), grid, None, 1.0,
+                              (gh * 8, gw * 8), view('pts'), view('occ'), view('expd'), view('am'), ws)
+    else:
+      _lib.cost_volume_tracks_ragged(_head_weights('identity'), qf, cv.counts, grid, None, 1.0,
+                                     (gh * 8, gw * 8), view('pts'), view('occ'), view('expd'),
+                                     view('am'), ws)
+  torch.cuda.synchronize()
+  for k, (buf, body) in outs.items():
+    assert U.guards_intact(buf), f'{k}: wrote outside the output'
+    assert not (body.isnan().any() if body.is_floating_point() else (body == -7).any()), f'{k}: not written'
+  changed = int((ws[need:] != 0xA5).sum())
+  assert changed == 0, f'{changed} workspace bytes past the cost-volume arena were written'
+  return {k: outs[k][1].cpu().view((Q, T, 2) if k == 'pts' else (Q, T)) for k in outs}
+
+
+def _check_cost_volume(cv, got, simt):
+  """The arg-max cells are the design's winners, and each query n >= 64 of a clip repeats every
+  output of query n mod 64 bit for bit."""
+  for k, x in got.items():
+    same = x.view(torch.int32)[cv.rank >= PP.CV_GROUPS]
+    src = x.view(torch.int32)[(torch.arange(cv.Q) - cv.rank + cv.group)[cv.rank >= PP.CV_GROUPS]]
+    assert torch.equal(same, src), f'{k}: a query n >= 64 differs from query n mod 64'
+  am, want = got['am'].long(), cv.winner()
+  heat = cv.heat_simt() if simt else cv.heat(PP.tc_pairs(3))
+  assert torch.equal(PP.CvDesign.argmax(heat), want)
+  bad = am != want
+  if bad.any():
+    same = [] if simt else [name for name, pairs in PP.wrong_sets(3).items()
+                            if torch.equal(PP.CvDesign.argmax(cv.heat(pairs)), am)]
+    kinds = sorted({PP.CV_KINDS[k] for k in cv.kind[bad].tolist()})
+    clips = sorted(set(cv.clip[bad.any(-1)].tolist()))
+    pytest.fail(f'{int(bad.sum())} of {bad.numel()} arg-max cells differ (kinds {kinds}, clips '
+                f'{clips[:16]}); they are those of: {same or "no listed wrong set"}')
 
 
 @pytest.mark.parametrize('bn', [64, 128])
-@pytest.mark.parametrize('shape', CV_CASES, ids=[f'{c[3]}x{c[4]}' for c in CV_CASES])
-def test_cost_volume_pairs(shape, bn):
-  """N = 40 queries per clip: an m-tile reads the next clip's rows; 2925 cells (25 x 39 x 3) are
-  no multiple of either tile width.  Temperature 1: the heat is the map, exactly."""
-  B, N, T, gh, gw = shape
-  cv = PP.CvDesign(B, N, T, gh, gw)
-  qf, grid = cv.qf.cuda(), cv.grid.cuda()
-  outs = {k: U.guarded(B * N * T * (2 if k == 'pts' else 1), torch.int32 if k == 'am' else torch.float32)
-          for k in ('pts', 'occ', 'expd', 'am')}
-  view = lambda k: outs[k][1].view((B, N, T, 2) if k == 'pts' else (B, N, T))  # noqa: E731
-  ws = torch.empty(_lib.cost_volume_workspace_bytes(qf, grid), dtype=torch.uint8, device='cuda')
-  with U.switches(TAPIR_B200_GEMM='tc', TAPIR_B200_BLOCK_N=bn):
-    _lib.cost_volume_tracks(_head_weights('identity'), qf, grid, None, 1.0, (gh * 8, gw * 8), view('pts'),
-                            view('occ'), view('expd'), view('am'), ws)
-  torch.cuda.synchronize()
-  for k, (buf, _) in outs.items():
-    assert U.guards_intact(buf), f'{k}: wrote outside the output'
-  got = view('am').cpu().long()
-  want = cv.winner()
-  assert torch.equal(PP.CvDesign.argmax(cv.heat(PP.tc_pairs(3))), want)
-  bad = got != want
-  if bad.any():
-    same = [name for name, pairs in PP.wrong_sets(3).items()
-            if torch.equal(PP.CvDesign.argmax(cv.heat(pairs)), got)]
-    kinds = sorted({PP.CV_KINDS[k] for k in cv.kind[bad].tolist()})
-    pytest.fail(f'{int(bad.sum())} of {bad.numel()} arg-max cells differ (kinds {kinds}); they are '
-                f'those of: {same or "no listed wrong set"}')
+@pytest.mark.parametrize('case', list(CV_CASES))
+def test_cost_volume_pairs(case, bn):
+  """The stage-A cost volume, the one batched and the one grouped P = 3 GEMM, through
+  tapir_cost_volume_tracks_batched or tapir_cost_volume_tracks_ragged."""
+  cv = _cv_design(case)
+  _check_cost_volume(cv, _run_cost_volume(cv, CV_CASES[case][0], 'tc', bn), simt=False)
+
+
+@pytest.mark.parametrize('case', [c for c in CV_CASES if c.endswith('32x32')])
+def test_cost_volume_pairs_simt(case):
+  """The SIMT kernel's batched and grouped modes (blockIdx.z the clip): its all-pairs sum with
+  rounded products keeps every designed winner (tests/test_plane_pairs_host.py)."""
+  cv = _cv_design(case)
+  _check_cost_volume(cv, _run_cost_volume(cv, CV_CASES[case][0], 'simt'), simt=True)

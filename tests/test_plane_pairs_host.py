@@ -3,6 +3,8 @@ fp32 whatever the summation order, and every plausible wrong pair set changes a 
 the outputs and every output tile, so a kernel that sums one of them cannot pass
 tests/test_plane_pairs_gpu.py by luck.  The cost-volume designs flip their arg-max as designed.
 CPU only."""
+import copy
+
 import pytest
 import torch
 
@@ -129,12 +131,22 @@ def test_gapped_layout_holds_nan_outside_the_planes(conv):
 
 
 # ------------------------------------------------------------------------------ cost volume
-CV_SHAPES = [(2, 40, 2, 32, 32), (2, 40, 3, 25, 39)]  # (B, N, T, gh, gw)
+# (counts, T, gh, gw): the batched form (counts = [N] * B) and ragged ones: counts around the
+# 128-row m-tile, a clip of one query between two of more than 128, and 64 clips (one grouped call
+# of TAPIR_MAX_RAGGED_CLIPS) mixing 1, 63, 64, 65 and 129
+COUNTS_64 = [(1, 63, 64, 65, 129)[b % 5] for b in range(64)]
+CV_DESIGNS = {
+    '32x32': ([40, 40], 2, 32, 32),
+    '25x39': ([40, 40], 3, 25, 39),
+    'ragged5_32x32': ([1, 40, 127, 128, 129], 3, 32, 32),
+    'ragged3_25x39': ([200, 1, 129], 1, 25, 39),
+    'ragged64_32x32': (COUNTS_64, 1, 32, 32),
+}
 
 
-@pytest.fixture(scope='module', params=CV_SHAPES, ids=lambda s: f'{s[3]}x{s[4]}')
+@pytest.fixture(scope='module', params=sorted(CV_DESIGNS))
 def cv(request):
-  return PP.CvDesign(*request.param)
+  return PP.CvDesign(*CV_DESIGNS[request.param])
 
 
 def test_cv_values_split_as_designed():
@@ -162,11 +174,13 @@ def test_cv_design_picks_its_winner(cv):
   for c in (cv.cell_a, cv.cell_b):
     rest.scatter_(-1, c[..., None], float('-inf'))
   assert rest.max() <= 0 and top[..., 1].min() >= 28
-  # every kind is on every clip, at both index orders of its candidates
+  # every kind is on every clip of at least one map per kind, at both index orders of its
+  # candidates
   for k in range(len(PP.CV_KINDS)):
     m = cv.kind == k
-    for b in range(cv.B):
-      assert m[b].any()
+    for b, n in enumerate(cv.counts):
+      if min(n, PP.CV_GROUPS) * cv.T >= len(PP.CV_KINDS):
+        assert m[cv.clip == b].any(), (b, PP.CV_KINDS[k])
     assert (cv.cell_a[m] < cv.cell_b[m]).any() and (cv.cell_a[m] > cv.cell_b[m]).any()
 
 
@@ -192,3 +206,36 @@ def test_cv_designs_see_every_wrong_set_but_the_added_pairs(cv):
       assert flipped == 0, name
     else:
       assert flipped >= 2 * cv.B, (name, flipped)
+
+
+def test_cv_queries_past_64_repeat_their_map(cv):
+  """Query n of a clip reads channel group n mod 64: its features and map are query n mod 64's."""
+  heat = cv.heat(PP.tc_pairs(3))
+  q0 = 0
+  for n in cv.counts:
+    for r in range(PP.CV_GROUPS, n):
+      src = q0 + r % PP.CV_GROUPS
+      assert torch.equal(cv.qf[q0 + r], cv.qf[src]) and torch.equal(heat[q0 + r], heat[src])
+    q0 += n
+
+
+def test_cv_another_clips_grid_moves_maps_of_every_clip(cv):
+  """A clip whose queries read the next clip's grid rows (a wrong B offset in the grouped GEMM)
+  picks another cell on at least one map of every clip: each clip has its own candidate cells."""
+  if cv.B < 2:
+    pytest.skip('one clip')
+  other = copy.copy(cv)
+  other.grid = cv.grid.roll(-1, 0)
+  moved = PP.CvDesign.argmax(other.heat(PP.tc_pairs(3))) != cv.winner()
+  for b in range(cv.B):
+    assert moved[cv.clip == b].any(), b
+
+
+def test_cv_simt_all_pairs_keep_the_winner(cv):
+  """The SIMT kernel sums a b with a, b the planes' fp32 sums: its products round (by at most
+  2^-19 near 32, half an ulp there) and it adds the pairs the tensor cores leave out (at most
+  2^-22).  Every kind's margin of 2^-16 holds through both, on the host model of its FMA chain."""
+  heat = cv.heat_simt()
+  assert torch.equal(PP.CvDesign.argmax(heat), cv.winner())
+  top = heat.topk(2, -1).values
+  assert ((top[..., 0] - top[..., 1]) >= PP.CV_MARGIN).all()

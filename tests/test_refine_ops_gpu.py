@@ -17,7 +17,7 @@ from tests import gpu_util as U  # noqa: E402
 from tests import refine_refs as R  # noqa: E402
 from tests.test_backbone_ops_gpu import Guarded, ratio  # noqa: E402
 from tests.test_refine_refs_host import (corr_design, corr_feats, corr_positions, mixer_input,  # noqa: E402
-                                         pyramid)
+                                         pyramid, ragged_corr_design)
 from tests.test_stages_gpu import MIXER_QB_CASES  # noqa: E402  every queries-per-CTA count on 132 SMs
 
 
@@ -30,10 +30,11 @@ def _ld(L, extra):
 
 
 # ------------------------------------------------------------------------------- local corr
-def run_local_corr(levels, pos, feats, init_hw, batch, P, ld, per_row):
+def run_local_corr(levels, pos, feats, init_hw, batch, P, ld, per_row, query_clip=None):
   """Returns the planes [P, Q, T, ld] (bf16, cpu).  per_row: the features are [Q, T, 384] rows
   read at stride 384 with the low half 128 floats in (what the refinement loop passes after its
-  first iteration); else per-query vectors at stride_t 0 (feats must then be constant over t)."""
+  first iteration); else per-query vectors at stride_t 0 (feats must then be constant over t).
+  query_clip: None, or int32 [Q] (tapir_local_corr_ragged: query q reads clip query_clip[q])."""
   Q, T, _ = pos.shape
   rows = Q * T
   grids = [g.cuda().contiguous() for g in levels]
@@ -47,7 +48,9 @@ def run_local_corr(levels, pos, feats, init_hw, batch, P, ld, per_row):
     fh, fl = (f[:, 0].cuda().contiguous()[:, None].expand(Q, T, -1) for f in feats)
   out = Guarded(rows * ld, torch.bfloat16, P)
   args = (grids, pos_d, occ_d, expd_d, fh, fl, out.body().view(P, rows, ld), init_hw)
-  if batch == 1:
+  if query_clip is not None:
+    _lib.local_corr(*args, query_clip=query_clip.cuda())
+  elif batch == 1:
     _lib.check(lib().tapir_local_corr(ctypes.byref(_lib.corr_args(*args)), U.stream()), 'tapir_local_corr')
   else:
     _lib.local_corr(*args)
@@ -56,14 +59,14 @@ def run_local_corr(levels, pos, feats, init_hw, batch, P, ld, per_row):
   return out.body().cpu().view(P, Q, T, ld), occ, expd
 
 
-def check_corr(name, levels, pos, feats, init_hw, batch, P, ld_extra, per_row):
+def check_corr(name, levels, pos, feats, init_hw, batch, P, ld_extra, per_row, query_clip=None):
   L = len(levels)
   ld = _ld(L, ld_extra)
   if not per_row:  # per-query features: the same vector in every frame
     feats = tuple(f[:, :1].expand_as(f).contiguous() for f in feats)
-  pl3, occ, expd = run_local_corr(levels, pos, feats, init_hw, batch, 3, ld, per_row)
+  pl3, occ, expd = run_local_corr(levels, pos, feats, init_hw, batch, 3, ld, per_row, query_clip)
   if P < 3:
-    plp, _, _ = run_local_corr(levels, pos, feats, init_hw, batch, P, ld, per_row)
+    plp, _, _ = run_local_corr(levels, pos, feats, init_hw, batch, P, ld, per_row, query_clip)
     assert torch.equal(plp.view(torch.int16), pl3[:P].view(torch.int16))
   # three planes carry the kernel's fp32 value exactly; every column is that value's split
   v32 = pl3.double().sum(0).float()
@@ -77,7 +80,8 @@ def check_corr(name, levels, pos, feats, init_hw, batch, P, ld_extra, per_row):
   bound = torch.empty_like(ref)
   for t0 in range(0, T, 8):  # the fp64 reference frame chunk by chunk
     r, b = R.local_corr_ref([g[:, t0:t0 + 8] for g in levels], pos[:, t0:t0 + 8],
-                            tuple(f[:, t0:t0 + 8] for f in feats), init_hw, batch, planes=P)
+                            tuple(f[:, t0:t0 + 8] for f in feats), init_hw, batch, planes=P,
+                            query_clip=query_clip)
     ref[:, t0:t0 + 8], bound[:, t0:t0 + 8] = r, b
   err, rr = ratio(pl3[:P].double().sum(0)[..., 388:kin], ref, bound)
   U.record(f'refine_corr_{name}_P{P}_ld+{ld_extra}_{"rows" if per_row else "query"}', err=err, ratio=rr)
@@ -95,6 +99,21 @@ CORR_GPU_CASES = [(name, P, extra, per_row) for name, P, extra, per_row in (
 def test_local_corr(name, P, ld_extra, per_row):
   levels, pos, feats, init_hw, B = corr_design(name)
   check_corr(name, levels, pos, feats, init_hw, B, P, ld_extra, per_row)
+
+
+# the designs split over 3 to 5 clips by a shuffled query_clip table, at T = 1 and T = 2
+RAGGED_CORR_CASES = [c for c in CORR_GPU_CASES if c[0] in ('tiny_4x8', 'box17_12x29', 'pl3_32x32')]
+RAGGED_CLIPS = {'tiny_4x8': 3, 'box17_12x29': 4, 'pl3_32x32': 5}
+
+
+@pytest.mark.parametrize('T', [1, 2])
+@pytest.mark.parametrize('name,P,ld_extra,per_row', RAGGED_CORR_CASES, ids=[c[0] for c in RAGGED_CORR_CASES])
+def test_local_corr_ragged(name, P, ld_extra, per_row, T):
+  """tapir_local_corr_ragged: each query reads the grids of the clip its table entry names; the
+  clips' grids differ, so a query that reads another clip's is far outside the bound."""
+  clips = RAGGED_CLIPS[name]
+  levels, pos, feats, init_hw, table = ragged_corr_design(name, clips, T)
+  check_corr(f'{name}_ragged{clips}_T{T}', levels, pos, feats, init_hw, clips, P, ld_extra, per_row, table)
 
 
 def test_local_corr_production_shape():
@@ -127,11 +146,15 @@ UPDATE_CASES = [  # (n, T, per_row, alias_occ, tracks, init, resize, video)
     (7, 3, False, True, True, (192, 320), (384, 640), (1080, 1920)),
     (9, 2, True, True, False, (256, 256), (256, 256), (256, 256)),
     (700, 100, True, False, True, (320, 384), (512, 640), (720, 1280)),   # 70000 rows > 65535
+    # tapir_refine_update_ragged: one (h, w) per clip, a shuffled query_clip table, T = 1
+    (11, 1, True, False, True, (256, 256), (320, 384), [(480, 640), (200, 200), (1080, 1920)]),
+    (13, 1, False, True, True, (192, 320), (384, 640), [(1080, 1920), (480, 640), (200, 200)]),
 ]
 
 
 @pytest.mark.parametrize('n,T,per_row,alias,tracks,init,resize,video', UPDATE_CASES,
-                         ids=['5x4_rows', '7x3_query_alias', '9x2_alias_no_tracks', '700x100_rows'])
+                         ids=['5x4_rows', '7x3_query_alias', '9x2_alias_no_tracks', '700x100_rows',
+                              '11x1_ragged_rows', '13x1_ragged_query_alias'])
 def test_refine_update_bit_exact(n, T, per_row, alias, tracks, init, resize, video):
   g = torch.Generator().manual_seed(n * T)
   ld = 392
@@ -152,12 +175,21 @@ def test_refine_update_bit_exact(n, T, per_row, alias, tracks, init, resize, vid
   occ_o = None if alias else Guarded(rows, torch.float32)
   expd_o, feat_o = Guarded(rows, torch.float32), Guarded(rows * 384, torch.float32)
   trk = Guarded(rows * 2, torch.float32) if tracks else None
+  kw = {}
+  if isinstance(video, list):  # per-clip sizes; each query's clip from a shuffled table
+    table = (torch.arange(n) % len(video))[torch.randperm(n, generator=g)]
+    kw = dict(video_table=torch.tensor(video, dtype=torch.int32, device='cuda'),
+              query_clip=table.to(torch.int32).cuda())
   _lib.refine_update(res_d, pos_d, occ_d, expd_d, fh, fl, occ_d if alias else occ_o.body().view(n, T),
                      expd_o.body().view(n, T), feat_o.body().view(n, T, 384),
-                     trk.body().view(n, T, 2) if tracks else None, init, resize, video)
+                     trk.body().view(n, T, 2) if tracks else None, init, resize,
+                     (0, 0) if kw else video, **kw)
   torch.cuda.synchronize()
   for o in (occ_o, expd_o, feat_o, trk):
     assert o is None or o.guards_untouched()
+  if kw:
+    assert not bool((table[1:] >= table[:-1]).all())
+    video = torch.tensor(video)[table].numpy()
   p, o, e, f, t = R.update_emulate(res, pos, occ, expd, feat, init, resize, video)
   eq = lambda a, b: torch.equal(a.cpu().reshape(-1).view(torch.int32), b.reshape(-1).view(torch.int32))  # noqa: E731
   assert eq(pos_d, p)

@@ -118,6 +118,21 @@ def corr_design(name, seed=0):
   return levels, pos, feats, init_hw, B
 
 
+def ragged_corr_design(name, clips, T, seed=0):
+  """corr_design(name)'s queries split over `clips` clips by a shuffled query_clip table (not in
+  clip order; every clip has queries), the clips' grids the design's and seeded variants of it,
+  frames 0..T-1.  Returns (levels [clips, T, ...], pos, feats, init_hw, query_clip int32 [Q])."""
+  levels, pos, feats, init_hw, B = corr_design(name)
+  assert B == 1 and T <= pos.shape[1]
+  variants = [levels] + [corr_design(name, seed=100 * seed + c)[0] for c in range(1, clips)]
+  levels = [torch.cat([v[li][:, :T] for v in variants]) for li in range(len(levels))]
+  Q = pos.shape[0]
+  g = torch.Generator().manual_seed(seed)
+  table = (torch.arange(Q) % clips)[torch.randperm(Q, generator=g)].to(torch.int32)
+  assert not bool((table[1:] >= table[:-1]).all())
+  return levels, pos[:, :T].contiguous(), tuple(f[:, :T].contiguous() for f in feats), init_hw, table
+
+
 # ------------------------------------------------------------------------------- emulations
 def _fma_chain(f, q):
   """f [..., K], q [..., K] fp32 -> fp32 sum by sequential FMAs from 0 (each one rounding)."""
@@ -357,6 +372,31 @@ def test_mixer_dw_bound_rejects_slips(slip, key):
   assert r > 1.5, r
 
 
+def test_corr_ref_clip_table_in_order_equals_batched():
+  levels, pos, feats, init_hw, B = corr_design('batched_b3')
+  want = R.local_corr_ref(levels, pos, feats, init_hw, B)
+  table = torch.arange(pos.shape[0]) // (pos.shape[0] // B)
+  got = R.local_corr_ref(levels, pos, feats, init_hw, B, query_clip=table)
+  assert all(torch.equal(x, y) for x, y in zip(got, want))
+  # a shuffled table reads each query's own clip: the batched result, permuted with the queries
+  perm = torch.randperm(pos.shape[0], generator=torch.Generator().manual_seed(1))
+  got = R.local_corr_ref(levels, pos[perm], tuple(f[perm] for f in feats), init_hw, B, query_clip=table[perm])
+  assert all(torch.equal(x, y[perm]) for x, y in zip(got, want))
+
+
+@pytest.mark.parametrize('T', [1, 2])
+@pytest.mark.parametrize('name,clips', [('tiny_4x8', 3), ('box17_12x29', 4), ('pl3_32x32', 5)])
+def test_corr_ref_sees_a_wrong_clip_table(name, clips, T):
+  """On the ragged designs of tests/test_refine_ops_gpu.py, the correlations of a kernel that read
+  clip 0 (or the clip in query order) for every query break the bound of the right table."""
+  levels, pos, feats, init_hw, table = ragged_corr_design(name, clips, T)
+  ref, bound = R.local_corr_ref(levels, pos, feats, init_hw, clips, query_clip=table)
+  for wrong in (torch.zeros_like(table), table.sort().values):
+    got, _ = R.local_corr_ref(levels, pos, feats, init_hw, clips, query_clip=wrong)
+    r, _ = _ratio(got.float(), ref, bound)
+    assert r > 100, r
+
+
 # ------------------------------------------------------------------------------- vs the oracle
 @pytest.mark.parametrize('name', HOST_DESIGNS)
 def test_corr_ref_matches_oracle(name):
@@ -421,6 +461,27 @@ def test_update_emulation_matches_refine_pips_update_lines():
   assert torch.equal(o, res[..., 2] + occ) and torch.equal(e, res[..., 3] + expd)
   assert torch.equal(f, res[..., 4:] + feats)
   assert torch.equal(trk, O.scale_coords(p, init_hw[::-1], video_hw[::-1]))
+
+
+def test_update_emulation_per_query_sizes_equal_per_clip_calls():
+  """update_emulate with one (h, w) per query, from an in-order clip table, equals the batched form
+  clip by clip; with a shuffled table, each query is scaled to its own clip's size."""
+  g = torch.Generator().manual_seed(5)
+  counts, T = [4, 1, 6], 2
+  Q = sum(counts)
+  res = torch.randn(Q, T, 392, generator=g)
+  pos = torch.rand(Q, T, 2, generator=g) * 300
+  occ, expd = torch.randn(Q, T, generator=g), torch.randn(Q, T, generator=g)
+  feats = torch.randn(Q, T, 384, generator=g)
+  sizes = [(480, 640), (200, 200), (1080, 1920)]
+  args = ((256, 256), (320, 384))
+  for table in (torch.tensor([b for b, n in enumerate(counts) for _ in range(n)]),
+                torch.tensor([2, 0, 1, 2, 2, 0, 2, 0, 2, 0, 2])):
+    got = R.update_emulate(res, pos, occ, expd, feats, *args, np.array(sizes)[table.numpy()])
+    for b in range(len(sizes)):
+      m = table == b
+      want = R.update_emulate(res[m], pos[m], occ[m], expd[m], feats[m], *args, sizes[b])
+      assert all(torch.equal(x[m], y) for x, y in zip(got, want)), b
 
 
 # ------------------------------------------------------------------------------- bad arguments
