@@ -541,6 +541,36 @@ int tapir_cost_volume_tracks_ragged(const tapir_head_weights* w, const float* qf
                                     float* expd, int32_t* argmax, void* workspace,
                                     size_t workspace_bytes, void* stream);
 
+/* ---- point edits of a one-frame step (pytorch_live_demo.py:180-206 re-targets a point) ----
+ * tapir_sample_query_rows applies a request table to a group of `clips` one-frame clips whose
+ * queries are packed along one point axis of `rows` rows.  Request r < *count (count is read on
+ * the device, so one captured launch serves any number of requests; at most `rows` are read):
+ *  - samples, for every grid i, grids[i].grid of clip `clip` at (t, y, x) into row `row` of
+ *    grids[i].out, exactly as tapir_sample_query_features on that clip alone with vT = T = 1;
+ *    the clip's video size is video_hw[clip] (a device int32 table [clips][2]) or, when video_hw
+ *    is NULL, video_h x video_w;
+ *  - zeroes row `row` of every causal-state tensor: `state` is a device table of num_state
+ *    pointers, entry 2k a [rows][2][512] tensor (ctx1) and entry 2k + 1 a [rows][2][2048] tensor
+ *    (ctx2), each 16-byte aligned.
+ * A request whose row or clip is out of range is skipped.  Rows without a request are not
+ * touched.  `grids` is a HOST array; nothing is allocated or copied, so the call may be captured
+ * in a CUDA graph.  Every argument is checked first; a bad one returns 1 before any CUDA call. */
+#define TAPIR_MAX_QUERY_GRIDS 16 /* a lowres and a hires grid per resolution level */
+typedef struct tapir_query_grid {
+  const float* grid;   /* [clips][h][w][C]: clip c's one-frame grid at grid + c * clip_stride */
+  int64_t clip_stride; /* in floats, >= h * w * C */
+  float* out;          /* [rows][C] packed query features */
+  int32_t h, w, C, reserved;
+} tapir_query_grid;
+typedef struct tapir_query_request {
+  int32_t row, clip; /* the point's row in the packed point axis, its clip in the group */
+  float t, y, x;     /* the query point in the clip's video pixels */
+} tapir_query_request;
+int tapir_sample_query_rows(const tapir_query_grid* grids, int32_t num_grids, int32_t clips,
+                            int32_t rows, int32_t video_h, int32_t video_w, const int32_t* video_hw,
+                            const int32_t* count, const tapir_query_request* requests,
+                            float* const* state, int32_t num_state, void* stream);
+
 /* ---- a9: tapir_model.py:519-527 avg_pool3d (2,2,1) ---------------------------------- */
 int tapir_pool_pyramid(const float* grid, int32_t T, int32_t h, int32_t w, int32_t C, float* out,
                        void* stream);

@@ -66,3 +66,11 @@ timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
     -k "(cost_volume_pairs or ragged or points_per_clip or more_than_64) and not query_limit and not 70_streams" \
     2>&1 | grep -E '^=========|passed|failed' | tail -n 25
 echo "sanitizer ragged memcheck rc=${PIPESTATUS[0]}"
+# then the point edits of the online tracker: tapir_sample_query_rows on sentinel rows (one and
+# per-clip sizes, 1 and 4 levels, out-of-range requests, graph replay) and the one-stream edited
+# tracker; the multi-stream trackers are left out
+timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
+    python -m pytest -q -m gpu -p no:cacheprovider tests/test_stream_edit_gpu.py \
+    -k "sample_query_rows or retarget_equals" \
+    2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+echo "sanitizer stream_edit memcheck rc=${PIPESTATUS[0]}"

@@ -28,6 +28,7 @@ NUM_RESNET_BLOCKS = 8
 MAX_EXTRA_BLOCKS = 5
 MAX_CORR_LEVELS = 5
 MAX_RAGGED_CLIPS = 64
+MAX_QUERY_GRIDS = 16
 MAX_RESIZE_SIDE = 65535
 
 
@@ -90,6 +91,11 @@ class CorrArgs(Structure):
               ('feat_lo', c_void_p), ('feat_lo_stride_n', c_int64), ('feat_lo_stride_t', c_int64),
               ('out_planes', c_void_p), ('out_plane_stride', c_int64), ('ld', c_int32),
               ('reserved', c_int32)]
+
+
+class QueryGrid(Structure):
+  _fields_ = [('grid', c_void_p), ('clip_stride', c_int64), ('out', c_void_p), ('h', c_int32),
+              ('w', c_int32), ('C', c_int32), ('reserved', c_int32)]
 
 
 class UpdateArgs(Structure):
@@ -209,6 +215,9 @@ SIGNATURES = {
     'tapir_sample_query_features_ex': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_int32,
                                                       c_void_p, c_int32, c_int32, c_int32, c_int32,
                                                       c_void_p, c_void_p, c_void_p]),
+    'tapir_sample_query_rows': (ctypes.c_int, [POINTER(QueryGrid), c_int32, c_int32, c_int32, c_int32,
+                                               c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                               c_int32, c_void_p]),
     'tapir_cost_volume_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32, c_int32, c_int32]),
     'tapir_cost_volume_tracks': (ctypes.c_int, [POINTER(HeadWeights), c_void_p, c_void_p, c_int32,
                                                 c_int32, c_int32, c_int32, c_int32, c_void_p,
@@ -562,6 +571,88 @@ def sample_query_features(grid, query_tyx, video_shape, out, frame_slot=None):
   _check(fn, 'frame_slot', frame_slot, torch.int32, (video_shape[0],), device=grid.device)
   check(load().tapir_sample_query_features_ex(ptr(grid), T, gh, gw, C, ptr(query_tyx), N,
                                               *video_shape, ptr(frame_slot), ptr(out), stream()), fn)
+
+
+REQUEST_WORDS = 5  # tapir_query_request: row, clip and the float32 bits of t, y, x
+
+
+def query_request_table(capacity, device, pin_memory=False):
+  """An empty request table of sample_query_rows: int32 [1 + 5 capacity], the count first, then
+  one (row, clip, t, y, x) request per 5 words."""
+  return torch.zeros(1 + REQUEST_WORDS * capacity, dtype=torch.int32, device=device,
+                     pin_memory=pin_memory)
+
+
+def write_query_requests(table, requests):
+  """Writes `requests`, a sequence of (row, clip, t, y, x), and their count into a host table of
+  query_request_table."""
+  n = len(requests)
+  _need(table.device.type == 'cpu' and 1 + REQUEST_WORDS * n <= table.numel(), 'write_query_requests',
+        f'{n} requests do not fit a host table of {table.numel()} words')
+  a = table.numpy()
+  a[0] = n
+  if n:
+    body = a[1:1 + REQUEST_WORDS * n].reshape(n, REQUEST_WORDS)
+    body[:, :2] = [(r[0], r[1]) for r in requests]
+    body[:, 2:].view('float32')[:] = [tuple(r[2:5]) for r in requests]
+
+
+def state_pointer_table(state, rows):
+  """The device pointer table of sample_query_rows over a causal state (a list of dicts of
+  block_{i}_causal_1 [.., rows, 2, 512] and block_{i}_causal_2 [.., rows, 2, 2048] tensors),
+  ctx1 and ctx2 of each block in turn."""
+  fn = 'state_pointer_table'
+  ptrs = []
+  for d in state:
+    for i in range(len(d) // 2):
+      for k, width in ((f'block_{i}_causal_1', 512), (f'block_{i}_causal_2', 2048)):
+        _need(k in d, fn, f'state entry without {k}')
+        _check(fn, k, d[k], torch.float32, device=state[0][k].device)
+        _need(d[k].numel() == rows * 2 * width and d[k].shape[-2:] == (2, width), fn,
+              f'{k} {tuple(d[k].shape)} is not [.., {rows}, 2, {width}]')
+        ptrs.append(d[k].data_ptr())
+  dev = state[0]['block_0_causal_1'].device if state else 'cpu'
+  return torch.tensor(ptrs, dtype=torch.int64).to(dev)
+
+
+def sample_query_rows(grids, outs, video_hw, requests, state_table=None):
+  """Applies the request table `requests` (query_request_table on the device) to a group of G
+  one-frame clips whose queries are packed along R rows: each request's row of every outs[i]
+  ([R, C] or [1, R, C]) is sampled from grids[i] ([G, 1, h, w, C] or [G, h, w, C]; each clip's
+  grid dense) of its clip, and that row of every state tensor of state_table (state_pointer_table
+  of R rows, or None) is zeroed.  video_hw: one (h, w) for every clip, or an int32 [G, 2] device
+  table."""
+  fn = 'tapir_sample_query_rows'
+  _need(1 <= len(grids) == len(outs) <= MAX_QUERY_GRIDS, fn,
+        f'{len(grids)} grids and {len(outs)} outputs (1..{MAX_QUERY_GRIDS}, one per grid)')
+  dev = grids[0].device
+  G = grids[0].shape[0]
+  R = outs[0].shape[-2]
+  table = (QueryGrid * len(grids))()
+  for i, (g, o) in enumerate(zip(grids, outs)):
+    _need(g.dim() in (4, 5) and (g.dim() == 4 or g.shape[1] == 1) and g.shape[0] == G, fn,
+          f'grid {i} {tuple(g.shape)} is not [{G}, 1, h, w, C]')
+    h, w, C = g.shape[-3:]
+    _need(g.dtype == torch.float32 and g.device == dev and g[0].is_contiguous()
+          and g.stride(0) >= h * w * C, fn, f'grid {i} must be float32 on {dev}, each clip dense')
+    _check(fn, f'outs[{i}]', o, torch.float32, device=dev)
+    _need(o.shape[-2:] == (R, C) and o.numel() == R * C, fn,
+          f'outs[{i}] {tuple(o.shape)} is not [{R}, {C}]')
+    table[i] = QueryGrid(grid=g.data_ptr(), clip_stride=g.stride(0), out=o.data_ptr(), h=h, w=w, C=C)
+  _check(fn, 'requests', requests, torch.int32, (1 + REQUEST_WORDS * R,), device=dev)
+  vh = vw = 0
+  if isinstance(video_hw, torch.Tensor):
+    _check(fn, 'video_hw', video_hw, torch.int32, (G, 2), device=dev)
+  else:
+    vh, vw = (int(v) for v in video_hw)
+  K = 0
+  if state_table is not None:
+    _check(fn, 'state_table', state_table, torch.int64, device=dev)
+    K = state_table.numel()
+  words = ptr(requests).value
+  check(load().tapir_sample_query_rows(
+      table, len(grids), G, R, vh, vw, ptr(video_hw) if isinstance(video_hw, torch.Tensor) else None,
+      c_void_p(words), c_void_p(words + 4), ptr(state_table), K, stream()), fn)
 
 
 def pool_pyramid(grid, out):

@@ -315,6 +315,35 @@ int tapir_sample_query_features_ex(const float* grid, int32_t T, int32_t gh, int
   return sample_query_features(grid, T, gh, gw, C, query_tyx, N, vT, vH, vW, frame_slot, out, S(stream));
 }
 
+int tapir_sample_query_rows(const tapir_query_grid* grids, int32_t num_grids, int32_t clips,
+                            int32_t rows, int32_t video_h, int32_t video_w, const int32_t* video_hw,
+                            const int32_t* count, const tapir_query_request* requests,
+                            float* const* state, int32_t num_state, void* stream) {
+  Range nvtx_range("tapir_sample_query_rows");
+  const char* fn = "tapir_sample_query_rows";
+  TAPIR_CHECK_ARG(grids && num_grids >= 1 && num_grids <= TAPIR_MAX_QUERY_GRIDS,
+                  "%s: %d grids, 1..%d supported", fn, num_grids, TAPIR_MAX_QUERY_GRIDS);
+  TAPIR_CHECK_ARG(clips >= 1 && rows >= 1, "%s: clips=%d rows=%d must be positive", fn, clips, rows);
+  TAPIR_CHECK_ARG(video_hw != nullptr || (video_h >= 1 && video_w >= 1), "%s: video %d x %d", fn, video_h,
+                  video_w);
+  TAPIR_CHECK_ARG(count && requests && aligned(count, 4) && aligned(requests, 4) && aligned(video_hw, 4),
+                  "%s: count, requests and video_hw must be 4-byte aligned device pointers", fn);
+  TAPIR_CHECK_ARG(num_state >= 0 && num_state % 2 == 0 && num_state < 65535 &&
+                      (num_state == 0 || (state != nullptr && aligned(state, 8))),
+                  "%s: num_state=%d must be even with an 8-byte aligned table", fn, num_state);
+  for (int i = 0; i < num_grids; ++i) {
+    const tapir_query_grid& g = grids[i];
+    TAPIR_CHECK_ARG(g.grid && g.out && g.h >= 1 && g.w >= 1 && g.C >= 1 &&
+                        g.clip_stride >= (int64_t)g.h * g.w * g.C && aligned(g.grid, 4) && aligned(g.out, 4),
+                    "%s: grid %d (%d x %d x %d, clip stride %lld) needs 4-byte aligned grid and out", fn, i,
+                    g.h, g.w, g.C, (long long)g.clip_stride);
+    TAPIR_CHECK_ARG(!overlap(g.out, (size_t)rows * g.C * 4, g.grid, (size_t)g.clip_stride * clips * 4),
+                    "%s: grid %d's out overlaps its grid", fn, i);
+  }
+  return sample_query_rows(grids, num_grids, clips, rows, video_h, video_w, video_hw, count, requests,
+                           state, num_state, S(stream));
+}
+
 size_t tapir_cost_volume_workspace_bytes(int32_t N, int32_t T, int32_t gh, int32_t gw, int32_t C) {
   return cost_volume_workspace_bytes(1, N, T, gh, gw, C);
 }

@@ -94,6 +94,12 @@ int paint_point_track(const uint8_t* frames, int T, int H, int W, const void* tr
 int sample_query_features(const float* grid, int T, int gh, int gw, int C, const float* query_tyx,
                           int N, int vT, int vH, int vW, const int* frame_slot, float* out,
                           cudaStream_t s);
+// Arguments checked by tapir_sample_query_rows: num_grids in 1..TAPIR_MAX_QUERY_GRIDS, state a
+// device table of num_state (even) row-aligned tensors.
+int sample_query_rows(const tapir_query_grid* grids, int num_grids, int clips, int rows, int video_h,
+                      int video_w, const int32_t* video_hw, const int32_t* count,
+                      const tapir_query_request* requests, float* const* state, int num_state,
+                      cudaStream_t s);
 // B clips: qfeat [B][N][C], grid [B][T][gh][gw][C], outputs indexed by flattened query b*N + n
 // (the workspace of B clips with Q queries in all)
 size_t cost_volume_workspace_bytes(int B, long long Q, int T, int gh, int gw, int C);

@@ -29,21 +29,19 @@ __device__ __forceinline__ float unnormalize_border(float c, int size) {
   return pix;
 }
 
+// One query's features: the block's threads sample `grid` at (qt, qy, qx) into out[0 .. C).
 // Ta: the clip length the coordinates are normalised by.  frame_slot: null for a grid holding all
 // Ta frames (T == Ta), else Ta entries mapping each frame to its slot among the grid's T, or -1.  A
 // tap of nonzero weight on a frame without a slot makes the query's row NaN: the grid is never read
 // outside its T slots and a partial sum is never returned.
-__global__ void __launch_bounds__(128) sample_query_kernel(const float* __restrict__ grid, int T,
-                                                           int gh, int gw, int C,
-                                                           const float* __restrict__ q, int vT,
-                                                           int vH, int vW, int Ta,
-                                                           const int* __restrict__ frame_slot,
-                                                           float* __restrict__ out) {
-  const int n = blockIdx.x;
+__device__ __forceinline__ void sample_query_row(const float* __restrict__ grid, int T, int gh, int gw,
+                                                 int C, float qt, float qy, float qx, int vT, int vH,
+                                                 int vW, int Ta, const int* __restrict__ frame_slot,
+                                                 float* __restrict__ out) {
   // utils.convert_grid_coordinates: coords * out / in (tapir_model.py:266-277)
-  float t = __fdiv_rn(__fmul_rn(q[n * 3 + 0], (float)Ta), (float)vT);
-  const float y = __fdiv_rn(__fmul_rn(q[n * 3 + 1], (float)gh), (float)vH);
-  const float x = __fdiv_rn(__fmul_rn(q[n * 3 + 2], (float)gw), (float)vW);
+  float t = __fdiv_rn(__fmul_rn(qt, (float)Ta), (float)vT);
+  const float y = __fdiv_rn(__fmul_rn(qy, (float)gh), (float)vH);
+  const float x = __fdiv_rn(__fmul_rn(qx, (float)gw), (float)vW);
   t = __fadd_rn(t, 0.5f);
   const float pt = unnormalize_border(t, Ta), py = unnormalize_border(y, gh), px = unnormalize_border(x, gw);
   const int t0 = (int)floorf(pt), y0 = (int)floorf(py), x0 = (int)floorf(px);
@@ -73,7 +71,58 @@ __global__ void __launch_bounds__(128) sample_query_kernel(const float* __restri
           else if (wgt != 0.f)
             missing = true;
         }
-    out[(long long)n * C + c] = missing ? __int_as_float(0x7fc00000) : acc;
+    out[c] = missing ? __int_as_float(0x7fc00000) : acc;
+  }
+}
+
+__global__ void __launch_bounds__(128) sample_query_kernel(const float* __restrict__ grid, int T,
+                                                           int gh, int gw, int C,
+                                                           const float* __restrict__ q, int vT,
+                                                           int vH, int vW, int Ta,
+                                                           const int* __restrict__ frame_slot,
+                                                           float* __restrict__ out) {
+  const int n = blockIdx.x;
+  sample_query_row(grid, T, gh, gw, C, q[n * 3 + 0], q[n * 3 + 1], q[n * 3 + 2], vT, vH, vW, Ta,
+                   frame_slot, out + (long long)n * C);
+}
+
+// Point edits of a one-frame step (OnlineTracker.retarget / add_points): request r < *count
+// re-samples row req[r].row of every query-feature grid from clip req[r].clip's grids, as
+// sample_query_kernel does for a one-frame clip (T = vT = Ta = 1), and zeroes that row of every
+// causal-state tensor.  blockIdx.y == 0 samples, blockIdx.y == 1 + k zeroes state tensor k (even
+// k: [rows][2][512], odd k: [rows][2][2048]).  CTAs stride over the requests; with no request every
+// CTA exits after one load.
+struct QueryRowsParams {
+  tapir_query_grid grids[TAPIR_MAX_QUERY_GRIDS];
+  int num_grids, clips, rows, video_h, video_w;
+  const int32_t* video_hw;  // [clips][2] or null (video_h x video_w for every clip)
+  const int32_t* count;
+  const tapir_query_request* req;
+  float* const* state;
+};
+
+__global__ void __launch_bounds__(128) sample_query_rows_kernel(const QueryRowsParams p) {
+  const int count = min(*p.count, p.rows);
+  for (int r = blockIdx.x; r < count; r += gridDim.x) {
+    const tapir_query_request q = p.req[r];
+    if (q.row < 0 || q.row >= p.rows || q.clip < 0 || q.clip >= p.clips) continue;
+    if (blockIdx.y == 0) {
+      const int vh = p.video_hw ? p.video_hw[q.clip * 2 + 0] : p.video_h;
+      const int vw = p.video_hw ? p.video_hw[q.clip * 2 + 1] : p.video_w;
+      // constant indices: the grid table stays in the parameter space
+#pragma unroll
+      for (int i = 0; i < TAPIR_MAX_QUERY_GRIDS; ++i) {
+        if (i >= p.num_grids) break;
+        const tapir_query_grid g = p.grids[i];
+        sample_query_row(g.grid + q.clip * g.clip_stride, 1, g.h, g.w, g.C, q.t, q.y, q.x, 1, vh, vw, 1,
+                         nullptr, g.out + (long long)q.row * g.C);
+      }
+    } else {
+      const int k = blockIdx.y - 1;
+      const int width4 = (k & 1) ? 2 * 2048 / 4 : 2 * 512 / 4;
+      float4* dst = reinterpret_cast<float4*>(p.state[k]) + (long long)q.row * width4;
+      for (int i = threadIdx.x; i < width4; i += blockDim.x) dst[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
   }
 }
 
@@ -582,6 +631,29 @@ int sample_query_features(const float* grid, int T, int gh, int gw, int C, const
                                         frame_slot ? vT : T, frame_slot, out);
   count_launch();
   TAPIR_LAUNCH_CHECK("sample_query_kernel");
+  return kOk;
+}
+
+int sample_query_rows(const tapir_query_grid* grids, int num_grids, int clips, int rows, int video_h,
+                      int video_w, const int32_t* video_hw, const int32_t* count,
+                      const tapir_query_request* requests, float* const* state, int num_state,
+                      cudaStream_t s) {
+  QueryRowsParams p = {};
+  for (int i = 0; i < num_grids; ++i) p.grids[i] = grids[i];
+  p.num_grids = num_grids;
+  p.clips = clips;
+  p.rows = rows;
+  p.video_h = video_h;
+  p.video_w = video_w;
+  p.video_hw = video_hw;
+  p.count = count;
+  p.req = requests;
+  p.state = state;
+  // at most 32 CTAs per table entry: a launch without requests stays a few microseconds
+  const dim3 grid((unsigned)(rows < 32 ? rows : 32), 1u + (unsigned)num_state);
+  sample_query_rows_kernel<<<grid, 128, 0, s>>>(p);
+  count_launch();
+  TAPIR_LAUNCH_CHECK("sample_query_rows_kernel");
   return kOk;
 }
 

@@ -25,6 +25,12 @@ point axis ([1, sum N, ...]) and runs one estimate_trajectories with `points_per
 per-query stages (stage A, local correlation, the mixer, the track update) run over the streams'
 points only.  Each stream's tracks, visibles and logits are slices of its group's packed outputs.
 
+`retarget`, `add_points` and `remove_points` edit a stream's points between steps.  Each edit takes
+effect at the next step, on that step's frame: after a tracker's first edit every group's step
+runs one `tapir_sample_query_rows` launch that samples the requested rows from the step's own
+grids and zeroes their state rows, reading a request table the host uploads before replay.  A
+count change re-packs the group's buffers and re-captures the graph.
+
 With `yuv420=True` the tracker takes `live.YUV420Frames` (NV12 / I420 camera or decoder frames):
 it keeps static Y / U / V buffers of the camera frames, a step copies the 1.5 B/px planes into them
 and replays the graph, and the crop windows and colour matrix are fixed at construction.
@@ -33,6 +39,7 @@ from typing import List, NamedTuple, Optional, Sequence, Tuple, Union
 
 import torch
 
+from tapnet_b200 import _lib
 from tapnet_b200 import live
 from tapnet_b200 import tapir_model
 
@@ -100,6 +107,96 @@ def group_streams(specs: Sequence[StreamSpec], initial_resolution=(256, 256)):
   return list(groups.values())
 
 
+# -- point edits (OnlineTracker.retarget / add_points / remove_points) as pure functions on one
+# stream's pending requests: a dict {point index: (t, y, x)} of the points whose features the next
+# step samples, indices in the stream's current points.
+def edit_indices(idx, count: int, what: str) -> List[int]:
+  """`idx` (an int, a sequence, a 1-D tensor or numpy array) as a list of point indices in
+  [0, count)."""
+  if isinstance(idx, torch.Tensor):
+    if idx.dim() > 1 or idx.dtype.is_floating_point or idx.dtype == torch.bool:
+      raise ValueError(f'{what}: idx must be integers, got a {idx.dtype} {list(idx.shape)} tensor')
+    idx = idx.reshape(-1).tolist()
+  elif hasattr(idx, 'tolist'):  # numpy arrays and scalars (the live demo's np.array([idx]))
+    idx = idx.tolist()
+  if not isinstance(idx, (list, tuple, range)):
+    idx = [idx]
+  out = []
+  for i in idx:
+    if isinstance(i, bool) or not isinstance(i, int):
+      raise ValueError(f'{what}: idx must be integers, got {i!r}')
+    if not 0 <= i < count:
+      raise ValueError(f'{what}: point {i} out of range [0, {count})')
+    out.append(int(i))
+  return out
+
+
+def edit_points(query_points, k: Optional[int], what: str) -> List[Tuple[float, float, float]]:
+  """`query_points` ([k, 3] or [3]: (t, y, x) in the stream's pixels) as host tuples; k = None
+  takes any number."""
+  qp = torch.as_tensor(query_points).detach().to('cpu', torch.float32)
+  if qp.dim() == 1:
+    qp = qp[None]
+  if qp.dim() != 2 or qp.shape[1] != 3 or (k is not None and qp.shape[0] != k):
+    raise ValueError(f'{what}: query_points must be [{"k" if k is None else k}, 3], got '
+                     f'{list(qp.shape)}')
+  return [tuple(p) for p in qp.tolist()]
+
+
+def retarget_requests(pending: dict, count: int, idx, points) -> dict:
+  """Pending requests after re-targeting points `idx` at `points`: the last edit of a point wins."""
+  idx = edit_indices(idx, count, 'retarget')
+  points = edit_points(points, len(idx), 'retarget')
+  out = dict(pending)
+  out.update(zip(idx, points))
+  return out
+
+
+def add_requests(pending: dict, count: int, points) -> Tuple[dict, int, List[int]]:
+  """(pending requests, new count, new indices) after appending `points` to a stream of `count`."""
+  points = edit_points(points, None, 'add_points')
+  new = list(range(count, count + len(points)))
+  out = dict(pending)
+  out.update(zip(new, points))
+  return out, count + len(points), new
+
+
+def remove_requests(pending: dict, count: int, idx) -> Tuple[dict, List[int]]:
+  """(pending requests, kept indices) after removing points `idx`: the kept points keep their
+  order, indices above a removed one shift down, and a removed point's request is dropped.  A
+  stream keeps at least one point."""
+  idx = edit_indices(idx, count, 'remove_points')
+  if len(set(idx)) != len(idx):
+    raise ValueError(f'remove_points: idx {idx} has repeated points')
+  if len(idx) >= count:
+    raise ValueError(f'remove_points: removing {len(idx)} of {count} points; a stream keeps at '
+                     'least one')
+  gone = set(idx)
+  keep = [i for i in range(count) if i not in gone]
+  new_index = {old: new for new, old in enumerate(keep)}
+  return {new_index[i]: p for i, p in pending.items() if i in new_index}, keep
+
+
+def packed_offsets(counts: Sequence[int]) -> List[int]:
+  """Each stream's first row in a point axis packing streams of `counts` points in turn."""
+  return [sum(counts[:i]) for i in range(len(counts))]
+
+
+class _Edits:
+  """A group's request table (tapir_sample_query_rows), sized to its point count: the static
+  device table the graph reads, its pinned staging copy, and the event of the last upload."""
+
+  def __init__(self, g, dev, const):
+    rows = sum(g.counts)
+    self.table = _lib.query_request_table(rows, dev)
+    self.staging = _lib.query_request_table(rows, 'cpu', pin_memory=True)
+    self.uploaded = torch.cuda.Event()
+    self.pending_on_device = False  # the device table holds requests (a nonzero count)
+    self.state = _lib.state_pointer_table(g.state, rows)
+    self.video_hw = (g.video_size if isinstance(g.video_size, tuple)
+                     else const([v for hw in g.video_size for v in hw], dev, torch.int32).view(-1, 2))
+
+
 class _Group:
   """Streams sharing a pass plan: their static inputs, query features and causal state."""
 
@@ -108,7 +205,7 @@ class _Group:
     # stream streams[i]'s points are rows offsets[i] .. offsets[i] + counts[i] - 1 of the group's
     # packed point axis
     self.counts = [counts[s] for s in streams]
-    self.offsets = [sum(self.counts[:i]) for i in range(len(streams))]
+    self.offsets = packed_offsets(self.counts)
     self.uniform = len({(specs[s].frame_hw, specs[s].window) for s in streams}) == 1
     sizes = [specs[s].hw for s in streams]
     # one size: estimate_trajectories' one-size call and launches; else per-clip sizes
@@ -117,6 +214,7 @@ class _Group:
     self.sources = None  # otherwise: one one-frame input per stream, resampled together
     self.query_features = None
     self.state = None
+    self.edits = None  # after the tracker's first point edit: the group's _Edits
 
 
 class OnlineTracker:
@@ -182,9 +280,9 @@ class OnlineTracker:
         order.append(s)
     # row r of the groups' concatenated outputs is stream order[r]: gather them back in the graph
     self._order = torch.tensor([order.index(s) for s in range(self.num_streams)], device=self.dev)
-    # stream s's points in the groups' concatenated point axis
-    packed = [counts[s] for s in order]
-    self._rows = {s: slice(sum(packed[:r]), sum(packed[:r + 1])) for r, s in enumerate(order)}
+    self._stream_order = order
+    self._pack_rows()
+    self._pending = [{} for _ in range(self.num_streams)]  # per stream: point -> (t, y, x)
     # a one-size tracker's input: its group's [S, 1, ...] buffer, into which a step copies the batch
     self._frame = self._groups[0].frames if self._one_size else None
     self._graph = None
@@ -193,6 +291,12 @@ class OnlineTracker:
     self.query_features = None
     self.state = None
     self._out = None
+
+  def _pack_rows(self):
+    # stream s's points in the groups' concatenated point axis
+    packed = [self._counts[s] for s in self._stream_order]
+    offsets = packed_offsets(packed + [0])
+    self._rows = {s: slice(offsets[r], offsets[r + 1]) for r, s in enumerate(self._stream_order)}
 
   def _new_input(self, n, H, W, window):
     if self._yuv is None:
@@ -311,8 +415,13 @@ class OnlineTracker:
   def _step_group(self, g, state):
     """One group's step on its static inputs: its passes and one batched estimate_trajectories
     (B = group size, T = 1) that updates `state` in place; returns (tracks, occ, expd), packed
-    [1, sum N, 1, ...]."""
+    [1, sum N, 1, ...].  After the tracker's first edit it first applies the group's request table,
+    whose state rows are those of g.state."""
     grids = self._group_grids(g)
+    if g.edits is not None:  # the pending point edits, sampled from this frame's grids
+      qf = g.query_features
+      _lib.sample_query_rows(grids.lowres + grids.hires, qf.lowres + qf.hires, g.edits.video_hw,
+                             g.edits.table, g.edits.state)
     r = self.model.estimate_trajectories(g.video_size, False, grids, g.query_features, None, 64,
                                          causal_context=state, get_causal_context=True,
                                          causal_context_out=state, points_per_clip=g.counts)
@@ -375,13 +484,19 @@ class OnlineTracker:
       init = self.model.construct_initial_causal_state(sum(g.counts), len(g.plan) - 1)
       # [1, sum N, 2, 512 | 2048] per block, one tensor per refinement iteration
       g.state = [{k: v.to(self.dev) for k, v in d.items()} for d in init]
+      if g.edits is not None:  # new state buffers: a new pointer table
+        g.edits = _Edits(g, self.dev, self.model._const)
+    self._pending = [{} for _ in range(self.num_streams)]
+    self._publish()
+    return self.query_features
+
+  def _publish(self):
     views = [self._published(g) for g in self._groups]
     if self._one_size:
       self.query_features, self.state = views[0]
     else:
       self.query_features, self.state = [v[0] for v in views], [v[1] for v in views]
     self._graph = None
-    return self.query_features
 
   def _published(self, g):
     """A group's (query features, state) as `query_features` / `state` show them: packed
@@ -472,12 +587,117 @@ class OnlineTracker:
       for g in self._groups:
         for s, dst in zip(g.streams, g.sources):
           self._copy_in(frames[s], dst)
+    self._upload_edits()
     if self._graph is not None and self._graph_sig != self.model._workspace_sig():
       self._graph = None  # stale pointers: the model's buffers or weights changed since capture
     if self._graph is None:
       self._capture()
     self._graph.replay()
     return self._out[0], self._out[1]
+
+  def _upload_edits(self):
+    """Copies the request tables that changed since the last step (the groups with pending edits,
+    and the zero count of those that had some) from their pinned staging to the device."""
+    for g in self._groups:
+      if g.edits is None:
+        continue
+      reqs = [(g.offsets[i] + idx, i) + qp for i, s in enumerate(g.streams)
+              for idx, qp in sorted(self._pending[s].items())]
+      if not reqs and not g.edits.pending_on_device:
+        continue
+      e = g.edits
+      e.uploaded.synchronize()  # the last upload has read the staging buffer
+      _lib.write_query_requests(e.staging, reqs)
+      n = 1 + _lib.REQUEST_WORDS * len(reqs)
+      e.table[:n].copy_(e.staging[:n], non_blocking=True)
+      e.uploaded.record()
+      e.pending_on_device = bool(reqs)
+    self._pending = [{} for _ in range(self.num_streams)]
+
+  # -- point edits: each takes effect at the next step, sampled from that step's frame
+  def _edit_stream(self, stream, what):
+    if self.query_features is None:
+      raise RuntimeError(f'{what}: call init(frame, query_points) first')
+    if isinstance(stream, bool) or not isinstance(stream, int) or not 0 <= stream < self.num_streams:
+      raise ValueError(f'{what}: stream {stream} out of range [0, {self.num_streams})')
+    if what != 'retarget' and isinstance(self.num_points, int) and self.num_streams > 1:
+      raise ValueError(f'{what}: a tracker of one point count for {self.num_streams} streams keeps '
+                       'it; build it with num_points=[...] (one count per stream) to change counts')
+
+  def _start_editing(self):
+    """From the first edit on, every group's step applies its request table."""
+    for g in self._groups:
+      if g.edits is None:
+        g.edits = _Edits(g, self.dev, self.model._const)
+        self._graph = None
+
+  def retarget(self, query_points, idx, stream: int = 0):
+    """Re-targets points `idx` ([k] or an int) of stream `stream` at query_points ([k, 3] as
+    (t, y, x) in that stream's pixels, as update_query takes them; with a one-frame clip t has no
+    effect).  At the next step their features are sampled from that step's frame and their causal
+    state is zeroed, inside the step (pytorch_live_demo.py:180-206 does both with a second
+    backbone pass over the frame).  On a tracker whose step runs several streams through one
+    backbone pass, the features come from that pass, so they can differ in the last bits from
+    update_query's one-frame pass."""
+    self._edit_stream(stream, 'retarget')
+    pending = retarget_requests(self._pending[stream], self._counts[stream], idx, query_points)
+    if pending:
+      self._start_editing()
+    self._pending[stream] = pending
+
+  def add_points(self, query_points, stream: int = 0) -> List[int]:
+    """Appends query_points ([k, 3], (t, y, x) in the stream's pixels) to stream `stream`'s
+    points and returns their indices.  They are tracked from the next step on, their features
+    sampled from that step's frame.  The next step captures the graph again."""
+    self._edit_stream(stream, 'add_points')
+    pending, count, new = add_requests(self._pending[stream], self._counts[stream], query_points)
+    if new:
+      self._resize(stream, list(range(self._counts[stream])), count)
+      self._pending[stream] = pending
+    return new
+
+  def remove_points(self, idx, stream: int = 0):
+    """Removes points `idx` of stream `stream`: the remaining points keep their order, and
+    indices above a removed one shift down.  A stream keeps at least one point.  The next step
+    captures the graph again."""
+    self._edit_stream(stream, 'remove_points')
+    pending, keep = remove_requests(self._pending[stream], self._counts[stream], idx)
+    if len(keep) != self._counts[stream]:
+      self._resize(stream, keep, len(keep))
+      self._pending[stream] = pending
+
+  def _resize(self, stream, keep, count):
+    """Re-packs stream `stream`'s group for the stream's kept points `keep` (old indices, in
+    order) followed by count - len(keep) new points: their query-feature rows hold zeros until
+    the step samples them, their state rows zeros."""
+    gi, slot = self._slot[stream]
+    g = self._groups[gi]
+    total = sum(g.counts)
+    src = []  # each new row's old row, or `total` (a zero row) for a new point
+    for i, (off, n) in enumerate(zip(g.offsets, g.counts)):
+      if i == slot:
+        src += [off + k for k in keep] + [total] * (count - len(keep))
+      else:
+        src += range(off, off + n)
+    src = torch.tensor(src, device=self.dev)
+
+    def repack(x):  # [1, total, ...] -> [1, new total, ...]
+      return torch.cat([x[0], x.new_zeros(1, *x.shape[2:])]).index_select(0, src)[None]
+    qf = g.query_features
+    g.query_features = tapir_model.QueryFeatures(tuple(map(repack, qf.lowres)),
+                                                 tuple(map(repack, qf.hires)), qf.resolutions)
+    g.state = [{k: repack(v) for k, v in d.items()} for d in g.state]
+    g.counts[slot] = count
+    g.offsets = packed_offsets(g.counts)
+    self._counts[stream] = count
+    if isinstance(self.num_points, int):  # one stream: the count stays an int
+      self.num_points = count
+    else:
+      self.num_points = list(self._counts)
+    self._pack_rows()
+    g.edits = None
+    self._start_editing()  # a request table of the new size for this group
+    self._publish()
 
   @property
   def last_logits(self):
@@ -489,7 +709,8 @@ class OnlineTracker:
                    stream: int = 0):
     """Re-targets point `idx` of stream `stream` at (t, y, x) = query_point on `frame` ([H, W, 3],
     that stream's frame; pytorch_live_demo.py:188-200): its features are re-sampled and its causal
-    state zeroed, in place (graph buffers stay valid).  Other streams are not touched."""
+    state zeroed, in place (graph buffers stay valid).  Other streams are not touched.  It applies
+    at once and cancels a pending retarget / add_points request of the point."""
     if self.query_features is None:
       raise RuntimeError('call init(frame, query_points) first')
     if not 0 <= stream < self.num_streams:
@@ -508,3 +729,4 @@ class OnlineTracker:
     for d in g.state:
       for v in d.values():
         v[0, row] = 0
+    self._pending[stream].pop(idx, None)  # applied now: a pending request of the point is void
