@@ -338,14 +338,67 @@ int tapir_yuv420_to_rgb(const tapir_yuv420_frames* src, int32_t frames, uint8_t*
 int tapir_ingest_frames_yuv420(const tapir_yuv420_frames* src, int32_t frames, float* dst,
                                int32_t oH, int32_t oW, void* stream);
 
+/* YUV frames of any common decoder or camera layout: 8- to 16-bit samples, 4:2:0, 4:2:2 or 4:4:4
+ * chroma, planar, semi-planar (NV12, P010 / P016) or packed (YUYV, UYVY).  Luma sample (r, c) of
+ * frame f is the sample at byte y + f * y_frame_stride + r * y_pitch + c * luma_step * sample_bytes;
+ * chroma sample (r, c) is at u + f * u_frame_stride + r * u_pitch + c * chroma_step * sample_bytes
+ * (v likewise), with chroma planes of ceil(H / 2^chroma_shift_y) x ceil(W / 2^chroma_shift_x)
+ * samples.  Each plane pointer gives its first sample, so interleaved layouts are three pointers
+ * into one buffer: NV12 / P010 (chroma_step 2, v = u + sample_bytes), YUYV (luma_step 2,
+ * chroma_step 4, u = y + 1, v = y + 3), UYVY (u = y - 1, v = y + 1).  Strides and pitches are in
+ * bytes; 16-bit samples are little-endian and need 2-byte aligned planes, pitches and strides.
+ *
+ * Conversion contract: pixel (r, c) of the full frame uses chroma sample
+ * (r >> chroma_shift_y, c >> chroma_shift_x) (nearest, absolute coordinates).  Each sample s is
+ * first normalised to 16 bits: 8-bit v16 = s << 8; MSB-aligned 16-bit (P010 / P016) v16 = s;
+ * LSB-aligned (yuv420p10le) v16 = (s & (2^bits - 1)) << (16 - bits).  With C = Y16 - 4096,
+ * k = 298 (limited range) or C = Y16, k = 256 (full range), D = U16 - 32768, E = V16 - 32768:
+ *   R = (k*C + cr*E + 32768) >> 16, G = (k*C - gu*D - gv*E + 32768) >> 16,
+ *   B = (k*C + bu*D + 32768) >> 16
+ * (int32 arithmetic shift, then clamped to [0, 255]) with the (cr, gu, gv, bu) table of
+ * tapir_yuv420_frames plus BT.2020 (non-constant luminance; round(256 x coefficient) like the
+ * other rows): limited (430, 48, 167, 548), full (377, 42, 146, 482).  For 8-bit samples this is
+ * the tapir_yuv420_frames contract exactly ((256 S + 32768) >> 16 == (S + 128) >> 8), so 16-bit
+ * samples holding 8-bit values in their high byte convert to the bytes of the 8-bit frame.  As
+ * there, everything after the conversion is the uint8 RGB path. */
+typedef struct tapir_yuv_frames {
+  const void* y;
+  const void* u;
+  const void* v;
+  int64_t y_frame_stride, u_frame_stride, v_frame_stride;
+  int64_t y_pitch, u_pitch, v_pitch;
+  int32_t H, W;                  /* full frame (luma samples) */
+  int32_t y0, x0, h, w;          /* crop window inside the frame */
+  int32_t matrix;                /* 601, 709 or 2020 */
+  int32_t full_range;            /* 0: limited (16-235 luma at 8 bits), 1: full */
+  int32_t sample_bytes;          /* 1 or 2 */
+  int32_t bits;                  /* 8 (sample_bytes 1) or 8..16 (sample_bytes 2) */
+  int32_t lsb_aligned;           /* 16-bit samples: 0 MSB-aligned (P010), 1 LSB-aligned */
+  int32_t luma_step;             /* samples between luma samples of a row: 1 planar, 2 packed */
+  int32_t chroma_step;           /* >= 1: 1 planar, 2 semi-planar, 4 packed 4:2:2 */
+  int32_t chroma_shift_x;        /* 0 or 1: 1 for 4:2:0 and 4:2:2, 0 for 4:4:4 */
+  int32_t chroma_shift_y;        /* 0 or 1: 1 for 4:2:0, 0 for 4:2:2 and 4:4:4 */
+  int32_t reserved;
+} tapir_yuv_frames;
+
+/* tapir_yuv420_to_rgb, tapir_ingest_frames_yuv420 and tapir_backbone_forward_yuv420 for any
+ * tapir_yuv_frames layout (the 4:2:0 calls run the same kernels).  Every descriptor field is
+ * checked before any launch; a bad one returns 1. */
+int tapir_yuv_to_rgb(const tapir_yuv_frames* src, int32_t frames, uint8_t* dst, void* stream);
+int tapir_ingest_frames_yuv(const tapir_yuv_frames* src, int32_t frames, float* dst, int32_t oH,
+                            int32_t oW, void* stream);
+
 /* One source frame of tapir_ingest_frames_multi: its own format, size, row pitch and crop window.
  * TAPIR_INGEST_U8: pixel (r, c) of the frame is src[r * pitch + c * 3 ...] (bytes; pitch >= 3 W)
  * and the window (y0, x0, h, w) lies inside the H x W frame.  TAPIR_INGEST_YUV420 reads frame 0 of
- * `yuv` inside its own window (src, pitch, H, W and the window fields are then not read).  fp32
+ * `yuv` inside its own window (src, pitch, H, W and the window fields are then not read).
+ * TAPIR_INGEST_YUV reads frame 0 of the tapir_yuv_frames `src` points to, inside its own window;
+ * pitch, H, W and the window fields must then be 0.  fp32
  * frames are not covered: the blend of tapir_bilinear_resize rounds differently (its taps are
  * contracted into FMAs in another order), so they keep one tapir_bilinear_resize call each. */
 #define TAPIR_INGEST_U8 1     /* uint8 RGB [0, 255] (tapir_ingest_frames' input) */
 #define TAPIR_INGEST_YUV420 2 /* 8-bit YUV 4:2:0 (tapir_ingest_frames_yuv420's input) */
+#define TAPIR_INGEST_YUV 3    /* any tapir_yuv_frames layout (tapir_ingest_frames_yuv's input) */
 typedef struct tapir_ingest_desc {
   const void* src;
   int64_t pitch;
@@ -370,6 +423,9 @@ int tapir_ingest_frames_multi(const tapir_ingest_desc* descs, int32_t frames, fl
 int tapir_backbone_forward_yuv420(const tapir_backbone_weights* w, const tapir_yuv420_frames* video,
                                   int32_t frames, float* lowres, float* hires, void* workspace,
                                   size_t workspace_bytes, void* hires_ready_event, void* stream);
+int tapir_backbone_forward_yuv(const tapir_backbone_weights* w, const tapir_yuv_frames* video,
+                               int32_t frames, float* lowres, float* hires, void* workspace,
+                               size_t workspace_bytes, void* hires_ready_event, void* stream);
 
 /* ---- SURVEY 8f row 2: output post-processing (the step after the path) ---------------- */
 /* pytorch_live_demo.py:57-59 / utils/model_utils.py:376-389:

@@ -29,6 +29,7 @@ for t in $TIERS; do
     props)       run props "X=1" tests/test_properties_gpu.py tests/test_batched_gpu.py ;;
     io)          run io "X=1" tests/test_io_gpu.py ;;
     yuv)         run yuv "X=1" tests/test_yuv_gpu.py ;;
+    yuv_formats) run yuv_formats "X=1" tests/test_yuv_formats_gpu.py ;;
     reader)      run reader "X=1" tests/test_windowed_gpu.py tests/test_video_reader_gpu.py ;;
     bulk)        run bulk "X=1" tests/test_bulk_gpu.py ;;
     eval)        run eval "X=1" tests/test_tapvid_gpu.py tests/test_redetection_gpu.py ;;

@@ -17,6 +17,12 @@ for tool in memcheck racecheck; do
       2>&1 | grep -E '^=========|passed|failed' | tail -n 25
   echo "sanitizer yuv $tool rc=${PIPESTATUS[0]}"
 done
+# the general YUV reader (16-bit, packed 4:2:2 and 4:4:4 layouts) through the same three kernels
+timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \
+    python -m pytest -q -m gpu -p no:cacheprovider tests/test_yuv_formats_gpu.py \
+    -k "random_samples or same_bytes or side_stream or feature_grids" \
+    2>&1 | grep -E '^=========|passed|failed' | tail -n 25
+echo "sanitizer yuv_formats memcheck rc=${PIPESTATUS[0]}"
 # then the backbone's memory-bound kernels one at a time, with NaN guards around every output
 # (stem conv, instance norm, im2col, layer norm, L2 norm, resize)
 timeout 1800 compute-sanitizer --tool memcheck --print-limit 20 \

@@ -139,13 +139,24 @@ class Yuv420Frames(Structure):
               ('matrix', c_int32), ('full_range', c_int32), ('reserved', c_int32)]
 
 
+class YuvFrames(Structure):
+  _fields_ = [('y', c_void_p), ('u', c_void_p), ('v', c_void_p),
+              ('y_frame_stride', c_int64), ('u_frame_stride', c_int64), ('v_frame_stride', c_int64),
+              ('y_pitch', c_int64), ('u_pitch', c_int64), ('v_pitch', c_int64),
+              ('H', c_int32), ('W', c_int32), ('y0', c_int32), ('x0', c_int32), ('h', c_int32),
+              ('w', c_int32), ('matrix', c_int32), ('full_range', c_int32),
+              ('sample_bytes', c_int32), ('bits', c_int32), ('lsb_aligned', c_int32),
+              ('luma_step', c_int32), ('chroma_step', c_int32), ('chroma_shift_x', c_int32),
+              ('chroma_shift_y', c_int32), ('reserved', c_int32)]
+
+
 class IngestDesc(Structure):
   _fields_ = [('src', c_void_p), ('pitch', c_int64), ('format', c_int32), ('H', c_int32),
               ('W', c_int32), ('y0', c_int32), ('x0', c_int32), ('h', c_int32), ('w', c_int32),
               ('reserved', c_int32), ('yuv', Yuv420Frames)]
 
 
-INGEST_U8, INGEST_YUV420 = 1, 2
+INGEST_U8, INGEST_YUV420, INGEST_YUV = 1, 2, 3
 INGEST_MAX_FRAMES = 64
 TAPVID_COUNTERS = 18
 
@@ -199,11 +210,17 @@ SIGNATURES = {
     'tapir_yuv420_to_rgb': (ctypes.c_int, [POINTER(Yuv420Frames), c_int32, c_void_p, c_void_p]),
     'tapir_ingest_frames_yuv420': (ctypes.c_int, [POINTER(Yuv420Frames), c_int32, c_void_p,
                                                   c_int32, c_int32, c_void_p]),
+    'tapir_yuv_to_rgb': (ctypes.c_int, [POINTER(YuvFrames), c_int32, c_void_p, c_void_p]),
+    'tapir_ingest_frames_yuv': (ctypes.c_int, [POINTER(YuvFrames), c_int32, c_void_p, c_int32,
+                                               c_int32, c_void_p]),
     'tapir_ingest_frames_multi': (ctypes.c_int, [POINTER(IngestDesc), c_int32, c_void_p, c_int32,
                                                  c_int32, c_void_p]),
     'tapir_backbone_forward_yuv420': (ctypes.c_int, [POINTER(BackboneWeights), POINTER(Yuv420Frames),
                                                      c_int32, c_void_p, c_void_p, c_void_p,
                                                      c_size_t, c_void_p, c_void_p]),
+    'tapir_backbone_forward_yuv': (ctypes.c_int, [POINTER(BackboneWeights), POINTER(YuvFrames),
+                                                  c_int32, c_void_p, c_void_p, c_void_p, c_size_t,
+                                                  c_void_p, c_void_p]),
     'tapir_postprocess_occlusions': (ctypes.c_int, [c_void_p, c_void_p, c_int64, c_void_p,
                                                     c_void_p]),
     'tapir_tapvid_counts': (ctypes.c_int, [POINTER(TapvidArgs), c_void_p]),
@@ -344,7 +361,7 @@ def _nbytes(t):
 
 
 def _is_yuv(x):
-  return hasattr(x, 'c_struct')  # live.YUV420Frames (live imports this module)
+  return hasattr(x, 'yuv_struct')  # live.YUVFrames (live imports this module)
 
 
 def _frames(fn, frames, dtypes=(torch.uint8, torch.float32)):
@@ -452,9 +469,9 @@ def ingest_frames(frames, out, window=None):
   nf, (oh, ow), (H, W) = math.prod(out.shape[:-3]), out.shape[-3:-1], frames.shape[-3:-1]
   if _is_yuv(frames):
     _need(window is None, fn, 'a YUV clip carries its own window')
-    desc = frames.c_struct()
-    return check(load().tapir_ingest_frames_yuv420(byref(desc), nf, ptr(out), oh, ow, stream()),
-                 'tapir_ingest_frames_yuv420')
+    desc = frames.yuv_struct()
+    return check(load().tapir_ingest_frames_yuv(byref(desc), nf, ptr(out), oh, ow, stream()),
+                 'tapir_ingest_frames_yuv')
   y0, x0, h, w = (0, 0, H, W) if window is None else window
   check(load().tapir_ingest_frames(ptr(frames), nf, H, W, y0, x0, h, w, ptr(out), oh, ow,
                                    stream()), 'tapir_ingest_frames')
@@ -479,8 +496,8 @@ def ingest_desc(frame):
   fn = 'ingest_desc'
   if _is_yuv(frame):
     _need(math.prod(frame.shape[:-3]) == 1, fn, f'a YUV clip of one frame, got {tuple(frame.shape)}')
-    yuv = frame.c_struct()
-    return IngestDesc(format=INGEST_YUV420, yuv=yuv), frame._keep
+    yuv = frame.yuv_struct()
+    return IngestDesc(src=ctypes.addressof(yuv), format=INGEST_YUV), (yuv, frame._keep)
   if (frame.dtype != torch.uint8 or frame.dim() != 3 or frame.shape[-1] != 3
       or frame.stride(2) != 1 or frame.stride(1) != 3):
     _bad(fn, 'frame', frame, 'uint8 [H, W, 3] with dense pixels')
@@ -506,12 +523,12 @@ def ingest_frames_multi(frames, out):
                                          stream()), fn)
 
 
-def yuv420_to_rgb(frames, out):
+def yuv_to_rgb(frames, out):
   """A YUV clip's window -> uint8 RGB out [B, T, h, w, 3]."""
-  _check('tapir_yuv420_to_rgb', 'out', out, torch.uint8, frames.shape, device=frames.device)
-  desc = frames.c_struct()
-  check(load().tapir_yuv420_to_rgb(byref(desc), math.prod(out.shape[:-3]), ptr(out), stream()),
-        'tapir_yuv420_to_rgb')
+  _check('tapir_yuv_to_rgb', 'out', out, torch.uint8, frames.shape, device=frames.device)
+  desc = frames.yuv_struct()
+  check(load().tapir_yuv_to_rgb(byref(desc), math.prod(out.shape[:-3]), ptr(out), stream()),
+        'tapir_yuv_to_rgb')
 
 
 # ------------------------------------------------------------------------------ backbone
@@ -544,10 +561,10 @@ def backbone_forward(weights, frames, lowres, hires, workspace, ready_event=None
   _check(fn, 'hires', hires, torch.float32, (n, h // 4, w // 4, schema.HIRES_DIM), device=dev)
   ready = c_void_p(ready_event.cuda_event) if ready_event is not None else None
   if _is_yuv(frames):
-    desc = frames.c_struct(frame0)
-    return check(load().tapir_backbone_forward_yuv420(
+    desc = frames.yuv_struct(frame0)
+    return check(load().tapir_backbone_forward_yuv(
         byref(weights), byref(desc), n, ptr(lowres), ptr(hires), ptr(workspace), _nbytes(workspace),
-        ready, stream()), 'tapir_backbone_forward_yuv420')
+        ready, stream()), 'tapir_backbone_forward_yuv')
   check(load().tapir_backbone_forward_ex(
       byref(weights), None if stem_done else ptr(frames[frame0:]), int(frames.dtype == torch.uint8),
       n, h, w, ptr(lowres), ptr(hires), ptr(workspace), _nbytes(workspace), ready, stream()), fn)

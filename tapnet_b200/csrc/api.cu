@@ -240,19 +240,34 @@ int tapir_ingest_frames(const uint8_t* src, int32_t frames, int32_t H, int32_t W
   return ingest_frames(src, frames, H, W, crop_y, crop_x, crop_h, crop_w, dst, oH, oW, S(stream));
 }
 
+int tapir_yuv_to_rgb(const tapir_yuv_frames* src, int32_t frames, uint8_t* dst, void* stream) {
+  Range nvtx_range("tapir_yuv_to_rgb");
+  TAPIR_RETURN_IF(check_yuv_frames(src, frames, "tapir_yuv_to_rgb"));
+  return yuv_to_rgb(*src, frames, dst, S(stream));
+}
+
 int tapir_yuv420_to_rgb(const tapir_yuv420_frames* src, int32_t frames, uint8_t* dst, void* stream) {
   Range nvtx_range("tapir_yuv420_to_rgb");
-  Yuv420Reader r;
-  TAPIR_RETURN_IF(make_yuv420_reader(src, frames, "tapir_yuv420_to_rgb", &r));
-  return yuv420_to_rgb(r, frames, src->h, src->w, dst, S(stream));
+  tapir_yuv_frames y;
+  TAPIR_RETURN_IF(yuv_from_yuv420(src, "tapir_yuv420_to_rgb", &y));
+  TAPIR_RETURN_IF(check_yuv_frames(&y, frames, "tapir_yuv420_to_rgb"));
+  return yuv_to_rgb(y, frames, dst, S(stream));
+}
+
+int tapir_ingest_frames_yuv(const tapir_yuv_frames* src, int32_t frames, float* dst, int32_t oH,
+                            int32_t oW, void* stream) {
+  Range nvtx_range("tapir_ingest_frames_yuv");
+  TAPIR_RETURN_IF(check_yuv_frames(src, frames, "tapir_ingest_frames_yuv"));
+  return ingest_frames_yuv(*src, frames, dst, oH, oW, S(stream));
 }
 
 int tapir_ingest_frames_yuv420(const tapir_yuv420_frames* src, int32_t frames, float* dst,
                                int32_t oH, int32_t oW, void* stream) {
   Range nvtx_range("tapir_ingest_frames_yuv420");
-  Yuv420Reader r;
-  TAPIR_RETURN_IF(make_yuv420_reader(src, frames, "tapir_ingest_frames_yuv420", &r));
-  return ingest_frames_yuv420(r, frames, src->h, src->w, dst, oH, oW, S(stream));
+  tapir_yuv_frames y;
+  TAPIR_RETURN_IF(yuv_from_yuv420(src, "tapir_ingest_frames_yuv420", &y));
+  TAPIR_RETURN_IF(check_yuv_frames(&y, frames, "tapir_ingest_frames_yuv420"));
+  return ingest_frames_yuv(y, frames, dst, oH, oW, S(stream));
 }
 
 int tapir_ingest_frames_multi(const tapir_ingest_desc* descs, int32_t frames, float* dst,
@@ -261,14 +276,24 @@ int tapir_ingest_frames_multi(const tapir_ingest_desc* descs, int32_t frames, fl
   return ingest_frames_multi(descs, frames, dst, oH, oW, S(stream));
 }
 
+int tapir_backbone_forward_yuv(const tapir_backbone_weights* w, const tapir_yuv_frames* video,
+                               int32_t frames, float* lowres, float* hires, void* workspace,
+                               size_t workspace_bytes, void* hires_ready_event, void* stream) {
+  Range nvtx_range("tapir_backbone_forward_yuv");
+  TAPIR_RETURN_IF(check_yuv_frames(video, frames, "tapir_backbone_forward_yuv"));
+  return backbone_forward(w, nullptr, 0, frames, video->h, video->w, lowres, hires, workspace,
+                          workspace_bytes, S(stream), static_cast<cudaEvent_t>(hires_ready_event), video);
+}
+
 int tapir_backbone_forward_yuv420(const tapir_backbone_weights* w, const tapir_yuv420_frames* video,
                                   int32_t frames, float* lowres, float* hires, void* workspace,
                                   size_t workspace_bytes, void* hires_ready_event, void* stream) {
   Range nvtx_range("tapir_backbone_forward_yuv420");
-  Yuv420Reader r;
-  TAPIR_RETURN_IF(make_yuv420_reader(video, frames, "tapir_backbone_forward_yuv420", &r));
-  return backbone_forward(w, nullptr, 0, frames, video->h, video->w, lowres, hires, workspace,
-                          workspace_bytes, S(stream), static_cast<cudaEvent_t>(hires_ready_event), &r);
+  tapir_yuv_frames y;
+  TAPIR_RETURN_IF(yuv_from_yuv420(video, "tapir_backbone_forward_yuv420", &y));
+  TAPIR_RETURN_IF(check_yuv_frames(&y, frames, "tapir_backbone_forward_yuv420"));
+  return backbone_forward(w, nullptr, 0, frames, y.h, y.w, lowres, hires, workspace,
+                          workspace_bytes, S(stream), static_cast<cudaEvent_t>(hires_ready_event), &y);
 }
 
 int tapir_postprocess_occlusions(const float* occ, const float* expd, int64_t n, uint8_t* visible,

@@ -58,11 +58,13 @@ struct StemRgb {
   }
 };
 
-// YUV 4:2:0: the integer conversion gives the uint8 RGB byte, and a per-CTA table of the 256
-// stem_load values gives exactly the float the uint8 loader computes from that byte.
-struct StemYuv420 {
+// YUV (Reader = YuvReader<uint8_t> or YuvReader<uint16_t>): the integer conversion gives the
+// uint8 RGB byte, and a per-CTA table of the 256 stem_load values gives exactly the float the
+// uint8 loader computes from that byte.
+template <typename Reader>
+struct StemYuv {
   static constexpr int kTableFloats = 256;
-  Yuv420Reader src;
+  Reader src;
   __device__ __forceinline__ void prepare(float* table) const {
     for (int i = threadIdx.x; i < 256; i += blockDim.x) {
       const uint8_t b = (uint8_t)i;
@@ -439,10 +441,13 @@ int stem_conv(const void* video, int video_u8, const float* w_packed, int frames
                           out, in_bytes, s);
 }
 
-int stem_conv_yuv420(const Yuv420Reader& video, const float* w_packed, int frames, int H, int W,
-                     float* out, cudaStream_t s) {
-  return launch_stem_conv(StemYuv420{video}, w_packed, frames, H, W, out,
-                          (double)frames * H * W * 1.5, s);
+int stem_conv_yuv(const tapir_yuv_frames& video, const float* w_packed, int frames, int H, int W,
+                  float* out, cudaStream_t s) {
+  const YuvLayout l = yuv_layout(video);
+  const double in_bytes = frames * yuv_window_bytes(video);
+  if (video.sample_bytes == 1)
+    return launch_stem_conv(StemYuv<YuvReader<uint8_t>>{{l}}, w_packed, frames, H, W, out, in_bytes, s);
+  return launch_stem_conv(StemYuv<YuvReader<uint16_t>>{{l}}, w_packed, frames, H, W, out, in_bytes, s);
 }
 
 int instnorm_stats(const float* x, int frames, long long hw, int C, double* sums, cudaStream_t s) {
@@ -603,10 +608,10 @@ int backbone_stem(const tapir_backbone_weights* w, const void* video_chunk, int 
 
 int backbone_forward(const tapir_backbone_weights* w, const void* video, int video_u8, int frames,
                      int H, int W, float* lowres, float* hires, void* ws, size_t ws_bytes,
-                     cudaStream_t s, cudaEvent_t hires_ready, const Yuv420Reader* yuv) {
+                     cudaStream_t s, cudaEvent_t hires_ready, const tapir_yuv_frames* yuv) {
   // video == nullptr and yuv == nullptr: the stem output of all `frames` frames is already in
   // the workspace (tapir_backbone_stem, called per frame chunk while later chunks are still in
-  // flight on PCIe).  yuv != nullptr: the stem reads the H x W window of YUV 4:2:0 frames.
+  // flight on PCIe).  yuv != nullptr: the stem reads the H x W window of YUV frames.
   TAPIR_CHECK_ARG(w != nullptr && lowres != nullptr && hires != nullptr, "backbone_forward: null pointer");
   TAPIR_CHECK_ARG(frames > 0 && H % 8 == 0 && W % 8 == 0 && H >= 16 && W >= 16,
                   "backbone_forward: image resolution must be a multiple of 8 (H=%d W=%d)", H, W);
@@ -623,7 +628,7 @@ int backbone_forward(const tapir_backbone_weights* w, const void* video, int vid
   int h = H / 2, wd = W / 2;
   float* x = bp.buf[0];
   if (yuv != nullptr)
-    TAPIR_RETURN_IF(stem_conv_yuv420(*yuv, w->stem_w, frames, H, W, x, s));
+    TAPIR_RETURN_IF(stem_conv_yuv(*yuv, w->stem_w, frames, H, W, x, s));
   else if (video != nullptr)
     TAPIR_RETURN_IF(stem_conv(video, video_u8, w->stem_w, frames, H, W, x, s));
   int xi = 0;  // index of the buffer holding x

@@ -59,7 +59,7 @@ struct RgbWindow {
 };
 
 // One ch x cw window of uint8 RGB pixels for every frame of the launch (RgbWindow or
-// Yuv420Reader), as ingest_frames_kernel reads it: each tap normalised through the table.
+// YuvReader<T>), as ingest_frames_kernel reads it: each tap normalised through the table.
 template <typename Reader>
 struct U8Frames {
   Reader r;
@@ -77,10 +77,11 @@ struct U8Frames {
 
 // Device form of one tapir_ingest_desc (checked by the entry point).
 struct IngestFrame {
-  Yuv420Reader yuv;  // TAPIR_INGEST_YUV420: frame 0 of it
+  YuvLayout yuv;       // TAPIR_INGEST_YUV420 / TAPIR_INGEST_YUV: frame 0 of it
   const uint8_t* src;  // TAPIR_INGEST_U8: pixel (y0, x0) of the window
   long long pitch;     // TAPIR_INGEST_U8: row pitch in bytes
-  int format, h, w;  // window size
+  int format, h, w;    // format: TAPIR_INGEST_U8 or TAPIR_INGEST_YUV (both YUV formats); window size
+  int sample_bytes;    // YUV: 1 or 2
 };
 
 // Up to TAPIR_INGEST_MAX_FRAMES frames of their own format and window, one descriptor each.
@@ -98,21 +99,25 @@ struct DescFrames {
       p[0] = q[0];
       p[1] = q[1];
       p[2] = q[2];
+    } else if (d.sample_bytes == 1) {
+      d.yuv.pixel<uint8_t>(0, y, x, p);
     } else {
-      d.yuv.pixel(0, y, x, p);
+      d.yuv.pixel<uint16_t>(0, y, x, p);
     }
     v[0] = lut[p[0]];
     v[1] = lut[p[1]];
     v[2] = lut[p[2]];
   }
 };
+// The launch parameter is the whole table: sm_90 takes up to 32 KB of kernel parameters (CUDA 12.1+).
+static_assert(sizeof(DescFrames) <= 32764 - 64, "DescFrames does not fit the kernel parameter space");
 
 // crop + normalise + resize.  A CTA walks over runs of 256 consecutive output pixels: one thread
 // computes one pixel (3 channels) into shared memory, then the run's 768 floats leave as float4
 // rows (the direct 12-byte-strided stores would touch every sector three times).  The resize is
 // F.interpolate(mode='bilinear', align_corners=False) of the normalised crop, i.e. the same
 // arithmetic as bilinear_resize_kernel (backbone.cu) applied after normalise_u8.  Src gives each
-// frame's window size and its normalised pixels (U8Frames of RgbWindow or Yuv420Reader converting
+// frame's window size and its normalised pixels (U8Frames of RgbWindow or YuvReader<T> converting
 // each tap, or DescFrames with one window and format per frame).  The source is a grid constant:
 // DescFrames' table is indexed by frame without a local copy.
 template <typename Src>
@@ -180,10 +185,10 @@ __global__ void __launch_bounds__(256) ingest_frames_kernel(const __grid_constan
   }
 }
 
-// YUV 4:2:0 crop window -> dense uint8 RGB [frames][h][w][3]; one thread per pixel.
-__global__ void __launch_bounds__(256) yuv420_to_rgb_kernel(const Yuv420Reader src, int h, int w,
-                                                            uint8_t* __restrict__ dst,
-                                                            long long total) {
+// YUV crop window -> dense uint8 RGB [frames][h][w][3]; one thread per pixel.
+template <typename Reader>
+__global__ void __launch_bounds__(256) yuv_to_rgb_kernel(const Reader src, int h, int w,
+                                                         uint8_t* __restrict__ dst, long long total) {
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
        i += (long long)gridDim.x * blockDim.x) {
     const int x = (int)(i % w);
@@ -400,17 +405,39 @@ int ingest_frames(const uint8_t* src, int frames, int H, int W, int crop_y, int 
   return kOk;
 }
 
-int ingest_frames_yuv420(const Yuv420Reader& src, int frames, int h, int w, float* dst, int oH,
-                         int oW, cudaStream_t s) {
-  TAPIR_CHECK_ARG(dst && frames > 0 && h > 0 && w > 0 && oH > 0 && oW > 0,
-                  "ingest_frames_yuv420: bad arguments");
+int ingest_frames_yuv(const tapir_yuv_frames& src, int frames, float* dst, int oH, int oW,
+                      cudaStream_t s) {
+  TAPIR_CHECK_ARG(dst && frames > 0 && oH > 0 && oW > 0, "ingest_frames_yuv: bad arguments");
   const long long total = (long long)frames * oH * oW;
-  ProfileScope ps("ingest_frames_yuv420", s, 0.0, (double)frames * h * w * 1.5 + (double)total * 12);
-  ingest_frames_kernel<<<grid_for(total), 256, 0, s>>>(U8Frames<Yuv420Reader>{src, h, w}, dst, oH, oW,
-                                                       total, (reinterpret_cast<uintptr_t>(dst) & 15) == 0);
+  ProfileScope ps("ingest_frames_yuv", s, 0.0, frames * yuv_window_bytes(src) + (double)total * 12);
+  const YuvLayout l = yuv_layout(src);
+  const bool aligned = (reinterpret_cast<uintptr_t>(dst) & 15) == 0;
+  if (src.sample_bytes == 1)
+    ingest_frames_kernel<<<grid_for(total), 256, 0, s>>>(
+        U8Frames<YuvReader<uint8_t>>{{l}, src.h, src.w}, dst, oH, oW, total, aligned);
+  else
+    ingest_frames_kernel<<<grid_for(total), 256, 0, s>>>(
+        U8Frames<YuvReader<uint16_t>>{{l}, src.h, src.w}, dst, oH, oW, total, aligned);
   count_launch();
   TAPIR_LAUNCH_CHECK("ingest_frames_kernel");
   return kOk;
+}
+
+// The tapir_yuv_frames a TAPIR_INGEST_YUV420 / TAPIR_INGEST_YUV descriptor reads (1 + message if
+// it is no valid one).
+static int ingest_yuv_desc(const tapir_ingest_desc& d, int i, tapir_yuv_frames* out) {
+  if (d.format == TAPIR_INGEST_YUV420) {
+    TAPIR_RETURN_IF(yuv_from_yuv420(&d.yuv, "ingest_frames_multi", out));
+  } else {
+    // format 3 reads nothing but *src: fields set anyway mean a descriptor filled for another format
+    TAPIR_CHECK_ARG(d.pitch == 0 && d.H == 0 && d.W == 0 && d.y0 == 0 && d.x0 == 0 && d.h == 0 &&
+                        d.w == 0,
+                    "ingest_frames_multi: frame %d: format 3 (YUV) takes its size and window from "
+                    "*src; pitch, H, W, y0, x0, h and w must be 0", i);
+    TAPIR_CHECK_ARG(d.src != nullptr, "ingest_frames_multi: frame %d: format 3 (YUV) with src null", i);
+    *out = *static_cast<const tapir_yuv_frames*>(d.src);
+  }
+  return check_yuv_frames(out, 1, "ingest_frames_multi");
 }
 
 int ingest_frames_multi(const tapir_ingest_desc* descs, int frames, float* dst, int oH, int oW,
@@ -423,15 +450,15 @@ int ingest_frames_multi(const tapir_ingest_desc* descs, int frames, float* dst, 
   double in_bytes = 0;
   for (int i = 0; i < frames; ++i) {
     const tapir_ingest_desc& d = descs[i];
-    if (d.format == TAPIR_INGEST_YUV420) {
-      Yuv420Reader r;
-      TAPIR_RETURN_IF(make_yuv420_reader(&d.yuv, 1, "ingest_frames_multi", &r));
-      in_bytes += (double)d.yuv.h * d.yuv.w * 1.5;
+    if (d.format == TAPIR_INGEST_YUV420 || d.format == TAPIR_INGEST_YUV) {
+      tapir_yuv_frames y;
+      TAPIR_RETURN_IF(ingest_yuv_desc(d, i, &y));
+      in_bytes += yuv_window_bytes(y);
       continue;
     }
     TAPIR_CHECK_ARG(d.format == TAPIR_INGEST_U8,
-                    "ingest_frames_multi: frame %d: format %d is not 1 (uint8) or 2 (YUV 4:2:0)", i,
-                    d.format);
+                    "ingest_frames_multi: frame %d: format %d is not 1 (uint8), 2 (YUV 4:2:0) or 3 "
+                    "(YUV)", i, d.format);
     TAPIR_CHECK_ARG(d.src != nullptr && d.H > 0 && d.W > 0 && d.pitch >= 3ll * d.W,
                     "ingest_frames_multi: frame %d: src %p, %dx%d frame, row pitch %lld", i, d.src, d.H,
                     d.W, (long long)d.pitch);
@@ -448,16 +475,20 @@ int ingest_frames_multi(const tapir_ingest_desc* descs, int frames, float* dst, 
       const tapir_ingest_desc& d = descs[f0 + i];
       IngestFrame& fr = src.fr[i];
       fr = IngestFrame{};
-      fr.format = d.format;
-      if (d.format == TAPIR_INGEST_YUV420) {
-        make_yuv420_reader(&d.yuv, 1, "ingest_frames_multi", &fr.yuv);
-        fr.h = d.yuv.h;
-        fr.w = d.yuv.w;
-      } else {
+      if (d.format == TAPIR_INGEST_U8) {
+        fr.format = TAPIR_INGEST_U8;
         fr.src = static_cast<const uint8_t*>(d.src) + (long long)d.y0 * d.pitch + (long long)d.x0 * 3;
         fr.pitch = d.pitch;
         fr.h = d.h;
         fr.w = d.w;
+      } else {
+        tapir_yuv_frames y;
+        ingest_yuv_desc(d, f0 + i, &y);
+        fr.format = TAPIR_INGEST_YUV;
+        fr.yuv = yuv_layout(y);
+        fr.sample_bytes = y.sample_bytes;
+        fr.h = y.h;
+        fr.w = y.w;
       }
     }
     float* out = dst + (long long)f0 * oH * oW * 3;
@@ -471,13 +502,17 @@ int ingest_frames_multi(const tapir_ingest_desc* descs, int frames, float* dst, 
   return kOk;
 }
 
-int yuv420_to_rgb(const Yuv420Reader& src, int frames, int h, int w, uint8_t* dst, cudaStream_t s) {
-  TAPIR_CHECK_ARG(dst && frames > 0 && h > 0 && w > 0, "yuv420_to_rgb: bad arguments");
-  const long long total = (long long)frames * h * w;
-  ProfileScope ps("yuv420_to_rgb", s, 0.0, (double)total * 4.5);
-  yuv420_to_rgb_kernel<<<grid_for(total), 256, 0, s>>>(src, h, w, dst, total);
+int yuv_to_rgb(const tapir_yuv_frames& src, int frames, uint8_t* dst, cudaStream_t s) {
+  TAPIR_CHECK_ARG(dst && frames > 0, "yuv_to_rgb: bad arguments");
+  const long long total = (long long)frames * src.h * src.w;
+  ProfileScope ps("yuv_to_rgb", s, 0.0, frames * yuv_window_bytes(src) + (double)total * 3);
+  const YuvLayout l = yuv_layout(src);
+  if (src.sample_bytes == 1)
+    yuv_to_rgb_kernel<<<grid_for(total), 256, 0, s>>>(YuvReader<uint8_t>{l}, src.h, src.w, dst, total);
+  else
+    yuv_to_rgb_kernel<<<grid_for(total), 256, 0, s>>>(YuvReader<uint16_t>{l}, src.h, src.w, dst, total);
   count_launch();
-  TAPIR_LAUNCH_CHECK("yuv420_to_rgb_kernel");
+  TAPIR_LAUNCH_CHECK("yuv_to_rgb_kernel");
   return kOk;
 }
 

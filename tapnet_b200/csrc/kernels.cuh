@@ -31,9 +31,10 @@ int split_planes(const float* src, long long ld_src, __nv_bfloat16* dst, long lo
                  cudaStream_t s);
 int stem_conv(const void* video, int video_u8, const float* w_packed, int frames, int H, int W,
               float* out, cudaStream_t s);
-// the stem conv on an H x W crop window of YUV 4:2:0 frames (converted inside the patch loads)
-int stem_conv_yuv420(const Yuv420Reader& video, const float* w_packed, int frames, int H, int W,
-                     float* out, cudaStream_t s);
+// the stem conv on the H x W crop window of YUV frames (converted inside the patch loads); the
+// descriptor passed check_yuv_frames
+int stem_conv_yuv(const tapir_yuv_frames& video, const float* w_packed, int frames, int H, int W,
+                  float* out, cudaStream_t s);
 int instnorm_stats(const float* x, int frames, long long hw, int C, double* sums, cudaStream_t s);
 int instnorm_relu_split(const float* x, const double* sums, const float* w, const float* b,
                         int frames, long long hw, int C, __nv_bfloat16* out, long long plane_stride,
@@ -53,14 +54,15 @@ int backbone_stem(const tapir_backbone_weights* w, const void* video_chunk, int 
 int backbone_forward(const tapir_backbone_weights* w, const void* video, int video_u8, int frames,
                      int H, int W, float* lowres, float* hires, void* ws, size_t ws_bytes,
                      cudaStream_t s, cudaEvent_t hires_ready = nullptr,
-                     const Yuv420Reader* yuv = nullptr);
+                     const tapir_yuv_frames* yuv = nullptr);
 
 // ---- callers either side of the path (frames_io.cu; SURVEY 8f rows 1, 2) ----------------
 int ingest_frames(const uint8_t* src, int frames, int H, int W, int crop_y, int crop_x, int crop_h,
                   int crop_w, float* dst, int oH, int oW, cudaStream_t s);
-int ingest_frames_yuv420(const Yuv420Reader& src, int frames, int h, int w, float* dst, int oH,
-                         int oW, cudaStream_t s);
-int yuv420_to_rgb(const Yuv420Reader& src, int frames, int h, int w, uint8_t* dst, cudaStream_t s);
+// YUV descriptors that passed check_yuv_frames
+int ingest_frames_yuv(const tapir_yuv_frames& src, int frames, float* dst, int oH, int oW,
+                      cudaStream_t s);
+int yuv_to_rgb(const tapir_yuv_frames& src, int frames, uint8_t* dst, cudaStream_t s);
 int ingest_frames_multi(const tapir_ingest_desc* descs, int frames, float* dst, int oH, int oW,
                         cudaStream_t s);
 int postprocess_occlusions(const float* occ, const float* expd, long long n, uint8_t* visible,

@@ -31,9 +31,10 @@ runs one `tapir_sample_query_rows` launch that samples the requested rows from t
 grids and zeroes their state rows, reading a request table the host uploads before replay.  A
 count change re-packs the group's buffers and re-captures the graph.
 
-With `yuv420=True` the tracker takes `live.YUV420Frames` (NV12 / I420 camera or decoder frames):
-it keeps static Y / U / V buffers of the camera frames, a step copies the 1.5 B/px planes into them
-and replays the graph, and the crop windows and colour matrix are fixed at construction.
+With `yuv420=True` the tracker takes `live.YUV420Frames` (NV12 / I420 camera or decoder frames),
+with `yuv_layout='p010'` (or another `live.YUVFrames` layout) frames of that layout: it keeps static
+Y / U / V buffers of the camera frames, a step copies the planes into them and replays the graph,
+and the layout, crop windows and colour matrix are fixed at construction.
 """
 from typing import List, NamedTuple, Optional, Sequence, Tuple, Union
 
@@ -225,10 +226,14 @@ class OnlineTracker:
   def __init__(self, model: 'tapir_model.TAPIR', height: Union[int, Sequence[int]],
                width: Union[int, Sequence[int]], num_points: Union[int, Sequence[int]],
                uint8_frames: bool = False, num_streams: int = 1, yuv420: bool = False, window=None,
-               matrix: str = 'bt601', full_range: bool = False):
+               matrix: str = 'bt601', full_range: bool = False, yuv_layout: Optional[str] = None):
     """height x width: the frame size.  With yuv420=True that is the camera frame and `window`
     (y0, x0, h, w; e.g. `live.center_square_window(height, width)`) the crop that is tracked, in
-    whose pixels the tracks are; `matrix` / `full_range` describe the YUV frames.  `height`,
+    whose pixels the tracks are; `matrix` / `full_range` describe the YUV frames.  `yuv_layout`
+    (a `live.YUVFrames.layout` such as 'p010', 'yuv420p10', 'yuv444', 'yuyv') takes the place of
+    yuv420=True for frames of that layout; frames of another layout with the same samples and
+    chroma sampling (nv12 and i420; p010 and p016, whose MSB-aligned samples convert alike) are
+    accepted too.  `height`,
     `width` and `window` may also give one value per stream: init / step then take a list of
     the streams' frames.  `num_points` may give one count per stream (each >= 1): init then takes
     a list of the streams' [N_s, 3] query points, and step / last_logits return lists of the
@@ -245,9 +250,14 @@ class OnlineTracker:
         raise ValueError(f'num_points has {len(counts)} counts for {num_streams} streams')
       if min(counts) < 1:
         raise ValueError(f'num_points: every stream needs at least one point, got {counts}')
-    if yuv420 and uint8_frames:
-      raise ValueError('uint8_frames and yuv420 are exclusive')
-    specs = stream_specs(height, width, num_streams, yuv420, window)
+    if yuv_layout is not None and not live.is_yuv_layout(yuv_layout):
+      raise ValueError(f'yuv_layout: unknown layout {yuv_layout!r}')
+    if yuv420 and yuv_layout is not None:
+      raise ValueError('yuv420 and yuv_layout are exclusive')
+    layout = 'yuv420' if yuv420 else yuv_layout
+    if layout is not None and uint8_frames:
+      raise ValueError('uint8_frames and yuv420 / yuv_layout are exclusive')
+    specs = stream_specs(height, width, num_streams, layout is not None, window)
     self.model = model
     self.specs = specs
     self.num_points = num_points if isinstance(num_points, int) else counts
@@ -259,7 +269,8 @@ class OnlineTracker:
     # uint8_frames: frames are raw [0, 255] camera frames (what pytorch_live_demo.py:139-141 holds
     # before preprocess_frames); the normalisation runs inside the stem conv's loads
     self._frame_dtype = torch.uint8 if uint8_frames else torch.float32
-    self._yuv = (matrix, bool(full_range)) if yuv420 else None
+    self._yuv = (matrix, bool(full_range)) if layout is not None else None
+    self._yuv_layout = layout
     self._groups = [_Group(plan, streams, specs, counts)
                     for plan, streams in group_streams(specs, model.initial_resolution)]
     # streams of one frame size (and window) are one uniform group: init / step take a batch
@@ -301,6 +312,9 @@ class OnlineTracker:
   def _new_input(self, n, H, W, window):
     if self._yuv is None:
       return torch.zeros(n, 1, H, W, 3, dtype=self._frame_dtype, device=self.dev)
+    if self._yuv_layout != 'yuv420':
+      return live.YUVFrames.zeros(self._yuv_layout, n, 1, H, W, self.dev, matrix=self._yuv[0],
+                                  full_range=self._yuv[1], window=window)
     ch, cw = (H + 1) // 2, (W + 1) // 2
     planes = [torch.zeros(n, 1, *hw, dtype=torch.uint8, device=self.dev)
               for hw in ((H, W), (ch, cw), (ch, cw))]
@@ -308,25 +322,22 @@ class OnlineTracker:
 
   @staticmethod
   def _input_slot(frames, i):
-    if isinstance(frames, live.YUV420Frames):
-      return live.YUV420Frames(frames.y[i:i + 1], frames.u[i:i + 1], frames.v[i:i + 1],
-                               frames.matrix, frames.full_range, frames.window)
+    if isinstance(frames, live.YUVFrames):
+      return frames.map_buffers(lambda t: t[i:i + 1])
     return frames[i:i + 1]
 
   def _stream_frames(self, frames, streams):
     """Checks one frame per stream in `streams` (all before any copy): [H, W, 3] tensors (or
-    [1, H, W, 3], [1, 1, H, W, 3]) of the stream's size, or one-frame YUV420Frames of its frame
-    size and window.  Returns them as [1, 1, H, W, 3] tensors / YUV clips."""
-    if isinstance(frames, (torch.Tensor, live.YUV420Frames)) or len(frames) != len(streams):
+    [1, H, W, 3], [1, 1, H, W, 3]) of the stream's size, or one-frame YUVFrames of its frame
+    size, window and samples.  Returns them as [1, 1, H, W, 3] tensors / YUV clips."""
+    if isinstance(frames, (torch.Tensor, live.YUVFrames)) or len(frames) != len(streams):
       got = len(frames) if isinstance(frames, (list, tuple)) else type(frames).__name__
       raise ValueError(f'expected a list of {len(streams)} frames (one per stream), got {got}')
     out = []
     if self._yuv is not None:
       for s, f in zip(streams, frames):
         sp = self.specs[s]
-        if not isinstance(f, live.YUV420Frames):
-          raise ValueError(f'stream {s}: this tracker was built with yuv420=True: pass '
-                           'live.YUV420Frames (one frame format per tracker)')
+        self._check_yuv(f, f'stream {s}: ')
         if f.frame_size != sp.frame_hw or f.window != (sp.window or (0, 0) + sp.frame_hw):
           raise ValueError(f'stream {s}: frame {f.frame_size} window {f.window}, expected '
                            f'{sp.frame_hw} window {sp.window}')
@@ -355,23 +366,22 @@ class OnlineTracker:
     return out
 
   def _copy_in(self, src, dst):
-    if isinstance(dst, live.YUV420Frames):
+    if isinstance(dst, live.YUVFrames):
       for d, p in zip((dst.y, dst.u, dst.v), (src.y, src.u, src.v)):
-        d.copy_(p)
+        d.copy_(p if p.dtype == d.dtype else p.view(d.dtype))  # uint16 / int16: the same bits
     else:
       dst.copy_(src)
 
   def _frames(self, frames):
     """init / step input, all checked before any copy.  A one-size tracker takes one batch:
     [S, H, W, 3], [S, 1, H, W, 3] or, when S = 1, [H, W, 3], returned as [S, 1, H, W, 3] on the
-    device; or YUV420Frames of [S, 1] frames of its frame size, window and matrix, returned as
+    device; or YUVFrames of [S, 1] frames of its frame size, window, samples and matrix, returned as
     they are.  Other trackers take a list of the streams' frames (`_stream_frames`)."""
     if not self._one_size:
       return self._stream_frames(frames, range(self.num_streams))
     S = self.num_streams
     if self._yuv is not None:
-      if not isinstance(frames, live.YUV420Frames):
-        raise ValueError('this tracker was built with yuv420=True: pass live.YUV420Frames')
+      self._check_yuv(frames, '')
       ref = self._frame
       if frames.frame_size != ref.frame_size:
         raise ValueError(f'frame size {frames.frame_size} != {ref.frame_size}')
@@ -383,7 +393,7 @@ class OnlineTracker:
       if frames.device != self.dev:
         raise ValueError(f'frames on {frames.device}, tracker on {self.dev}')
       if tuple(frames.y.shape[:2]) != (S, 1):
-        raise ValueError(f'expected YUV420Frames of [{S}, 1] frames, got '
+        raise ValueError(f'expected YUVFrames of [{S}, 1] frames, got '
                          f'{list(frames.y.shape[:2])}')
       return frames
     frames = frames.to(self.dev, self._frame_dtype, non_blocking=True)
@@ -399,8 +409,18 @@ class OnlineTracker:
       raise ValueError(f'frame size {tuple(frames.shape[2:4])} != {self.hw}')
     return frames
 
+  def _check_yuv(self, f, who):
+    """f is a YUV clip whose samples and chroma sampling are those of the tracker's layout."""
+    ref = self._groups[0].sources[0]
+    if not isinstance(f, live.YUVFrames) or f.sampling != ref.sampling:
+      got = f.layout if isinstance(f, live.YUVFrames) else type(f).__name__
+      built = ('yuv420=True' if self._yuv_layout == 'yuv420'
+               else f'yuv_layout={self._yuv_layout!r}')
+      raise ValueError(f'{who}this tracker was built with {built}: pass live.YUVFrames of that '
+                       f'layout, got {got} (one frame format per tracker)')
+
   def _device_frame(self, f):
-    return f if isinstance(f, live.YUV420Frames) else f.to(self.dev, self._frame_dtype)
+    return f if isinstance(f, live.YUVFrames) else f.to(self.dev, self._frame_dtype)
 
   def _query_features_one(self, frame, qp):
     grids = self.model.get_feature_grids(frame, False)
@@ -410,7 +430,7 @@ class OnlineTracker:
     if g.uniform:
       return self.model.get_feature_grids(g.frames, False)
     return self.model._feature_grids_of_frames(
-        [x if isinstance(x, live.YUV420Frames) else x[0, 0] for x in g.sources], g.plan)
+        [x if isinstance(x, live.YUVFrames) else x[0, 0] for x in g.sources], g.plan)
 
   def _step_group(self, g, state):
     """One group's step on its static inputs: its passes and one batched estimate_trajectories

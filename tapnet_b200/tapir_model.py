@@ -427,7 +427,7 @@ class TAPIR(nn.Module):
       hires_ready_events: Optional[list] = None,
   ) -> FeatureGrids:
     """Reference tapir_model.py:293-392.  video: [B, T, H, W, 3] float in [-1, 1] (or uint8
-    [0, 255], or a device-resident `live.YUV420Frames` clip whose crop window is the video).
+    [0, 255], or a device-resident `live.YUVFrames` clip whose crop window is the video).
 
     `hires_ready_events` (extension, used by tapnet_b200.distributed): a list that receives one
     (hires tensor, torch.cuda.Event) pair per distinct resolution; the event fires as soon as
@@ -444,10 +444,10 @@ class TAPIR(nn.Module):
     # preprocess_frames, pytorch_live_demo.py:30-41): normalised inside the stem conv's loads
     # (or inside the resize), so the 4x larger float video never exists.  Extension of the
     # reference surface; float video behaves exactly as before.
-    # YUV 4:2:0 frames (extension): at the frame's own size the stem conv converts inside its
+    # YUV frames (extension): at the frame's own size the stem conv converts inside its
     # loads; a resized pass converts each bilinear tap in the ingest kernel.  Bit for bit the
     # results of the uint8 RGB frames the conversion produces.
-    if not isinstance(video, live.YUV420Frames):
+    if not isinstance(video, live.YUVFrames):
       video = _backbone_frames(video)
     n, f, vh, vw, _ = video.shape
     host_src = None
@@ -481,7 +481,7 @@ class TAPIR(nn.Module):
     uint8) or one-frame YUV clips.  Each pass resamples uint8 and YUV frames in one ingest launch;
     float32 frames keep one tapir_bilinear_resize launch each (the multi-frame ingest cannot
     reproduce its rounding bit for bit)."""
-    dev = self._device_check(*(None if isinstance(x, live.YUV420Frames) else x for x in frames))
+    dev = self._device_check(*(None if isinstance(x, live.YUVFrames) else x for x in frames))
     pk = self._pack()
     feature_grid, hires_feats, resize_im_shape = [], [], []
     latent = hires = None
@@ -517,7 +517,7 @@ class TAPIR(nn.Module):
           raise ValueError(f'grids_out {name} must be a contiguous float32 {list(shape)} tensor '
                            f'on {dev}, got {t.dtype} {tuple(t.shape)} on {t.device}')
     latent, hires = out
-    src = frames if isinstance(frames, live.YUV420Frames) else frames.view(nf, h, w, 3)
+    src = frames if isinstance(frames, live.YUVFrames) else frames.view(nf, h, w, 3)
     flat_lo, flat_hi = (t.view(nf, *s[2:]) for t, s in zip(out, shapes))
     chunk = _backbone_chunk(h, w, nf)
     ws = self._workspace('backbone', self._backbone_workspace_bytes(nf, h, w), dev)

@@ -277,15 +277,14 @@ def _check_inputs(model, video, query_points):
 
 def _yuv_frames(clip, a, z, repeat=1):
   """Frames a..z-1 of a one-clip YUV clip (each `repeat` times), with its window and matrix."""
-  y, u, v = (t[:, a:z] if repeat == 1 else t[:, a:z].repeat_interleave(repeat, 1)
-             for t in (clip.y, clip.u, clip.v))
-  return live.YUV420Frames(y, u, v, clip.matrix, clip.full_range, clip.window)
+  return clip.map_buffers(lambda t: t[:, a:z] if repeat == 1
+                          else t[:, a:z].repeat_interleave(repeat, 1))
 
 
 def _run_pass(model, pk, video, step, a, z, out, dev):
   """Backbone pass `step` over frames a..z-1 of the one-clip video (or device YUV clip) into out
   (lowres, hires)."""
-  if isinstance(video, live.YUV420Frames):
+  if isinstance(video, live.YUVFrames):
     frames = _yuv_frames(video, a, z)
   else:
     src = tapir_model._backbone_frames(video[:, a:z])
@@ -328,7 +327,7 @@ def _run_frames(model, pk, video, step, out, alone, dev):
     while j < n and not alone[j]:
       j += 1
     if j - i == 1:
-      if isinstance(video, live.YUV420Frames):
+      if isinstance(video, live.YUVFrames):
         pair = _yuv_frames(video, i, i + 1, repeat=2)
       else:
         pair = video[:, i:i + 1].expand(1, 2, *video.shape[2:]).contiguous()
@@ -674,11 +673,11 @@ def choose_reader_window_frames(model, video_shape, num_points, free_bytes,
 
 def _describe(x):
   """(format string, frame count) of what a reader returned; (None, 0) if it is no frame batch."""
-  if isinstance(x, live.YUV420Frames):
+  if isinstance(x, live.YUVFrames):
     if x.y.shape[0] != 1:
       return None, 0
     H, W = x.frame_size
-    return (f'YUV 4:2:0 {H}x{W} frames, window {x.window}, {x.matrix}, '
+    return (f'YUV {x.layout} {x.bits}-bit {H}x{W} frames, window {x.window}, {x.matrix}, '
             f'{"full" if x.full_range else "limited"} range, on {x.device}'), int(x.y.shape[1])
   if (isinstance(x, torch.Tensor) and x.dim() == 4 and x.shape[-1] == 3
       and (x.dtype == torch.uint8 or x.dtype.is_floating_point)):
@@ -699,15 +698,16 @@ class _FrameSource:
     if what is None:
       got = tuple(x.shape) if isinstance(x, torch.Tensor) else type(x).__name__
       raise ValueError(f'read_frames({a}, {z}) returned {got}; expected a uint8 or float '
-                       f'[{z - a}, H, W, 3] tensor or live.YUV420Frames of [1, {z - a}] frames')
+                       f'[{z - a}, H, W, 3] tensor or live.YUVFrames of [1, {z - a}] frames')
     if x.device.type != 'cpu' and x.device != self.dev:
       raise ValueError(f'read_frames({a}, {z}) returned frames on {x.device}; the model is on '
                        f'{self.dev}')
     if self.format is None:
       self.format = what
       self.host = x.device.type == 'cpu'
-      if isinstance(x, live.YUV420Frames):
-        self.yuv = (x.matrix, x.full_range, x.window)
+      if isinstance(x, live.YUVFrames):  # its layout, without its frames
+        self.yuv = x.map_buffers(lambda b: torch.empty((1, 0) + tuple(b.shape[2:]), dtype=b.dtype,
+                                                       device=b.device))
         self.frame_size = x.frame_size
         self.hw = tuple(int(v) for v in x.shape[2:4])
         self.itemsize = 1
@@ -727,20 +727,19 @@ class _FrameSource:
     """Bytes of one frame as the device stores it."""
     H, W = self.frame_size
     if self.yuv is not None:
-      return H * W + 2 * ((H + 1) // 2) * ((W + 1) // 2)
+      return sum(math.prod(b.shape[2:]) * b.element_size() for b in self.yuv.buffers)
     return H * W * 3 * self.itemsize
 
 
 class _FrameStore:
-  """S device frames in a _FrameSource's format: uint8 or float32 RGB [1, S, H, W, 3], or Y, U and
-  V planes [1, S, ...] (the same frames in I420 layout) with the source's window and matrix."""
+  """S device frames in a _FrameSource's format: uint8 or float32 RGB [1, S, H, W, 3], or the
+  source's YUV buffers [1, S, ...] (dense rows) with its layout, window and matrix."""
 
   def __init__(self, src, S, dev):
     self.yuv = src.yuv
     if src.yuv is not None:
-      H, W = src.frame_size
-      self.planes = tuple(torch.empty(1, S, h, w, dtype=torch.uint8, device=dev)
-                          for h, w in ((H, W),) + (((H + 1) // 2, (W + 1) // 2),) * 2)
+      self.planes = tuple(torch.empty((1, S) + tuple(b.shape[2:]), dtype=b.dtype, device=dev)
+                          for b in src.yuv.buffers)
     else:
       dtype = torch.uint8 if src.itemsize == 1 else torch.float32
       self.planes = (torch.empty((1, S) + src.hw + (3,), dtype=dtype, device=dev),)
@@ -749,14 +748,14 @@ class _FrameStore:
     """Slots s..z-1 as a one-clip video or YUV clip."""
     if self.yuv is None:
       return self.planes[0][:, s:z]
-    return live.YUV420Frames(*(t[:, s:z] for t in self.planes), *self.yuv)
+    return self.yuv.with_buffers([t[:, s:z] for t in self.planes])
 
   def put(self, s, x, i, n, non_blocking=True):
     """Frames i..i+n-1 of x (a reader's result or another store) into slots s..s+n-1."""
     if isinstance(x, _FrameStore):
       src = [t[0, i:i + n] for t in x.planes]
-    elif isinstance(x, live.YUV420Frames):
-      src = [t[0, i:i + n] for t in (x.y, x.u, x.v)]
+    elif isinstance(x, live.YUVFrames):
+      src = [t[0, i:i + n] for t in x.buffers]
     else:
       src = [x[i:i + n]]
     for dst, t in zip(self.planes, src):
@@ -918,9 +917,9 @@ def track_video(model, read_frames, num_frames: int, query_points,
   pieces; yields (start, stop, outputs) window by window in frame order.
 
   read_frames(start, stop) returns frames start..stop-1: a uint8 or float [stop - start, H, W, 3]
-  tensor on the host (pinned or pageable) or on the model's device, or a device live.YUV420Frames
+  tensor on the host (pinned or pageable) or on the model's device, or a device live.YUVFrames
   of [1, stop - start] frames whose window is the video.  The first call fixes the frame size and
-  format (for YUV also the window, matrix and range); a later call that returns anything else, or
+  format (for YUV also the layout, window, matrix and range); a later call that returns anything else, or
   a wrong frame count, raises ValueError naming its range.  The query pre-pass asks only for the
   queries' tap frames, each once; the sweep then asks for consecutive ranges that cover
   [0, num_frames) once, in order, one window ahead, so the reader decodes while the GPU works.
