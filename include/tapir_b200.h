@@ -505,6 +505,46 @@ int tapir_paint_point_track(const uint8_t* frames, int32_t T, int32_t H, int32_t
                             int32_t N, const uint8_t* colors, uint8_t* out, void* workspace,
                             size_t workspace_bytes, void* stream);
 
+/* ---- f8: camera homographies from point tracks (the step after the path) --------------- */
+/* viz_utils.py:301-648 get_homographies_wrt_frame in float64: one homography per frame that maps
+ * background points into the reference frame, each track's squared distance to its canonical
+ * point per frame, and the canonical points.  tracks [N][T][2] (x, y pixels) float
+ * (tracks_fp64 = 0) or double (1); occluded [N][T] uint8 (non-zero = occluded).  stop_thresholds
+ * is a device copy of tapir_ransac_stop_thresholds(N, targ_inlier_frac).  Outputs: homogs
+ * [T][3][3], err [N][T], canonical [N][2] (double); ransac_stats [T][2] int32 (hypotheses
+ * evaluated, best inlier count per frame of the initial sweep; 0 / 0 for the reference frame and
+ * frames with <= 4 usable points) or NULL.  RANSAC draws come from a fixed SplitMix64 stream, so
+ * the result is a function of the inputs.  Workspace: tapir_homographies_workspace_bytes(T, N),
+ * 256-byte aligned.  Launches per frame step: 4 in the initial sweep, 2 per refinement step (3 for
+ * the reference frame of a pass before the last), plus 2; no allocation, no host sync.  Every
+ * argument is checked first; a bad one returns 1 before any CUDA call. */
+typedef struct {
+  const void* tracks;            /* [N][T][2] */
+  int32_t tracks_fp64;           /* 0: float, 1: double */
+  int32_t N, T;
+  int32_t reference_frame;       /* 0 .. T-1 */
+  const uint8_t* occluded;       /* [N][T] */
+  double width, height;          /* image size in pixels, > 0 */
+  double thresh;                 /* outlier threshold in normalised coordinates, > 0 */
+  double outlier_point_threshold;/* required inlier fraction of a canonical point, > 0 */
+  int32_t num_refinement_passes; /* >= 0 */
+  int32_t reserved;
+  const double* stop_thresholds; /* [N] device */
+  double* homogs;                /* [T][3][3] */
+  double* err;                   /* [N][T] */
+  double* canonical;             /* [N][2] */
+  int32_t* ransac_stats;         /* [T][2] or NULL */
+  void* workspace;
+  size_t workspace_bytes;
+} tapir_homography_args;
+/* Host only: thr[it] = min(1 - (it + 1) / N, targ_inlier_frac * pow(0.99, it)) * N for it in
+ * 0 .. N-1 into the host array out (libm pow).  RANSAC stops after hypothesis k once its best
+ * count is >= thr[k + 1].  Bad arguments return 1. */
+int tapir_ransac_stop_thresholds(int32_t N, double targ_inlier_frac, double* out);
+/* 0 for T < 1 or N < 1. */
+size_t tapir_homographies_workspace_bytes(int32_t T, int32_t N);
+int tapir_homographies_wrt_frame(const tapir_homography_args* args, void* stream);
+
 /* ---- f6: evaluation (the step before the path) -------------------------------------- */
 /* tapvid/evaluation_datasets.py:41-45 resize_video on uint8 RGB frames, bit for bit as PIL's
  * Image.resize(..., LANCZOS) (what mediapy.resize_video runs per uint8 frame).  Per axis

@@ -14,7 +14,7 @@ CUDA graph.  Outputs and workspaces are tensors the caller passes in.
 import ctypes
 import math
 import os
-from ctypes import POINTER, Structure, byref, c_char_p, c_float, c_int32, c_int64, c_size_t, c_ulonglong, c_void_p
+from ctypes import POINTER, Structure, byref, c_char_p, c_double, c_float, c_int32, c_int64, c_size_t, c_ulonglong, c_void_p
 
 import torch
 
@@ -128,6 +128,16 @@ class RedetectionArgs(Structure):
               ('B', c_int32), ('N', c_int32), ('T', c_int32), ('capacity', c_int64),
               ('event_t', c_void_p), ('event_duration', c_void_p), ('event_values', c_void_p),
               ('event_count', c_void_p)]
+
+
+class HomographyArgs(Structure):
+  _fields_ = [('tracks', c_void_p), ('tracks_fp64', c_int32), ('N', c_int32), ('T', c_int32),
+              ('reference_frame', c_int32), ('occluded', c_void_p), ('width', c_double),
+              ('height', c_double), ('thresh', c_double), ('outlier_point_threshold', c_double),
+              ('num_refinement_passes', c_int32), ('reserved', c_int32),
+              ('stop_thresholds', c_void_p), ('homogs', c_void_p), ('err', c_void_p),
+              ('canonical', c_void_p), ('ransac_stats', c_void_p), ('workspace', c_void_p),
+              ('workspace_bytes', c_size_t)]
 
 
 class Yuv420Frames(Structure):
@@ -272,6 +282,9 @@ SIGNATURES = {
     'tapir_paint_point_track': (ctypes.c_int, [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int32,
                                                c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_size_t,
                                                c_void_p]),
+    'tapir_ransac_stop_thresholds': (ctypes.c_int, [c_int32, c_double, c_void_p]),
+    'tapir_homographies_workspace_bytes': (c_size_t, [c_int32, c_int32]),
+    'tapir_homographies_wrt_frame': (ctypes.c_int, [POINTER(HomographyArgs), c_void_p]),
     'tapir_lanczos_weights': (c_int32, [c_int32, c_int32, c_void_p, c_void_p]),
     'tapir_resize_lanczos_u8_workspace_bytes': (c_size_t, [c_int32, c_int32, c_int32, c_int32, c_int32]),
     'tapir_resize_lanczos_u8': (ctypes.c_int, [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32,
@@ -1001,6 +1014,46 @@ def paint_point_track(frames, tracks, visibles, colors, out, workspace):
   check(load().tapir_paint_point_track(
       ptr(frames), T, H, W, ptr(tracks), int(fp64), ptr(visibles), N, ptr(colors), ptr(out),
       ptr(workspace), _nbytes(workspace), stream()), fn)
+
+
+def ransac_stop_thresholds(N, targ_inlier_frac):
+  """Host only: the RANSAC stop table thr [N] float64 (numpy)."""
+  import numpy as np  # pylint: disable=g-import-not-at-top
+  out = np.empty(max(int(N), 1), np.float64)
+  check(load().tapir_ransac_stop_thresholds(int(N), float(targ_inlier_frac), out.ctypes.data),
+        'tapir_ransac_stop_thresholds')
+  return out
+
+
+def homographies_workspace_bytes(T, N):
+  return int(load().tapir_homographies_workspace_bytes(int(T), int(N)))
+
+
+def homographies_wrt_frame(tracks, occluded, width, height, reference_frame, thresh,
+                           outlier_point_threshold, num_refinement_passes, stop_thresholds, homogs,
+                           err, canonical, ransac_stats, workspace):
+  """Camera homographies of tracks [N, T, 2] (x, y pixels; float32 or float64) with occluded
+  [N, T] (bool / uint8): homogs float64 [T, 3, 3], err float64 [N, T], canonical float64 [N, 2],
+  ransac_stats int32 [T, 2] or None.  stop_thresholds: float64 [N] on the device
+  (ransac_stop_thresholds); workspace: uint8, at least homographies_workspace_bytes(T, N)."""
+  fn = 'tapir_homographies_wrt_frame'
+  (N, T, _), dev = tracks.shape, tracks.device
+  fp64 = tracks.dtype == torch.float64
+  _check(fn, 'tracks', tracks, torch.float64 if fp64 else torch.float32, (N, T, 2))
+  _need(occluded.dtype in (torch.bool, torch.uint8), fn, f'occluded must be bool or uint8, got {occluded.dtype}')
+  _check(fn, 'occluded', occluded, occluded.dtype, (N, T), device=dev)
+  _check(fn, 'stop_thresholds', stop_thresholds, torch.float64, (N,), device=dev)
+  _check(fn, 'homogs', homogs, torch.float64, (T, 3, 3), device=dev)
+  _check(fn, 'err', err, torch.float64, (N, T), device=dev)
+  _check(fn, 'canonical', canonical, torch.float64, (N, 2), device=dev)
+  if ransac_stats is not None:
+    _check(fn, 'ransac_stats', ransac_stats, torch.int32, (T, 2), device=dev)
+  _check(fn, 'workspace', workspace, torch.uint8, device=dev)
+  args = HomographyArgs(ptr(tracks), int(fp64), N, T, int(reference_frame), ptr(occluded), float(width),
+                        float(height), float(thresh), float(outlier_point_threshold),
+                        int(num_refinement_passes), 0, ptr(stop_thresholds), ptr(homogs), ptr(err),
+                        ptr(canonical), ptr(ransac_stats), ptr(workspace), _nbytes(workspace))
+  check(load().tapir_homographies_wrt_frame(byref(args), stream(dev)), fn)
 
 
 # ------------------------------------------------------------------------------ evaluation

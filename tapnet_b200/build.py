@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libtapir_b200.so')
 SOURCES = ['common.cu', 'gemm_tc.cu', 'gemm_simt.cu', 'backbone.cu', 'stage_a.cu', 'refine.cu',
-           'frames_io.cu', 'paint.cu', 'resample.cu', 'api.cu']
+           'frames_io.cu', 'paint.cu', 'resample.cu', 'homography.cu', 'api.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '-Xcompiler', '-fPIC']
 

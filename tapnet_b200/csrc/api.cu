@@ -1,6 +1,8 @@
 // extern "C" surface of libtapir_b200.so (include/tapir_b200.h).
 #include <nvtx3/nvToolsExt.h>
 
+#include <cmath>
+
 #include "kernels.cuh"
 
 namespace tapir {
@@ -620,6 +622,47 @@ int tapir_paint_point_track(const uint8_t* frames, int32_t T, int32_t H, int32_t
   }
   return paint_point_track(frames, T, H, W, tracks, tracks_fp64, visibles, N, colors, out, workspace,
                            S(stream));
+}
+
+int tapir_ransac_stop_thresholds(int32_t N, double targ_inlier_frac, double* out) {
+  TAPIR_CHECK_ARG(N >= 1 && out != nullptr, "tapir_ransac_stop_thresholds: N=%d, out %p", N, (void*)out);
+  TAPIR_CHECK_ARG(std::isfinite(targ_inlier_frac) && targ_inlier_frac > 0.0,
+                  "tapir_ransac_stop_thresholds: targ_inlier_frac=%g must be positive", targ_inlier_frac);
+  ransac_stop_thresholds(N, targ_inlier_frac, out);
+  return kOk;
+}
+
+size_t tapir_homographies_workspace_bytes(int32_t T, int32_t N) {
+  return homographies_workspace_bytes(T, N);
+}
+
+int tapir_homographies_wrt_frame(const tapir_homography_args* a, void* stream) {
+  Range nvtx_range("tapir_homographies_wrt_frame");
+  const char* fn = "tapir_homographies_wrt_frame";
+  TAPIR_CHECK_ARG(a != nullptr, "%s: null args", fn);
+  TAPIR_CHECK_ARG(a->N >= 1 && a->T >= 1 && (long long)a->N * a->T <= (1ll << 30),
+                  "%s: bad shape N=%d T=%d (N, T >= 1, N T <= 2^30)", fn, a->N, a->T);
+  TAPIR_CHECK_ARG(a->tracks_fp64 == 0 || a->tracks_fp64 == 1, "%s: tracks_fp64=%d", fn, a->tracks_fp64);
+  TAPIR_CHECK_ARG(a->reference_frame >= 0 && a->reference_frame < a->T,
+                  "%s: reference_frame=%d outside 0..%d", fn, a->reference_frame, a->T - 1);
+  TAPIR_CHECK_ARG(std::isfinite(a->width) && std::isfinite(a->height) && a->width > 0 && a->height > 0,
+                  "%s: image size %g x %g must be positive", fn, a->width, a->height);
+  TAPIR_CHECK_ARG(std::isfinite(a->thresh) && a->thresh > 0 && std::isfinite(a->outlier_point_threshold) &&
+                      a->outlier_point_threshold > 0,
+                  "%s: thresh=%g and outlier_point_threshold=%g must be positive", fn, a->thresh,
+                  a->outlier_point_threshold);
+  TAPIR_CHECK_ARG(a->num_refinement_passes >= 0 && a->num_refinement_passes <= 1000,
+                  "%s: num_refinement_passes=%d outside 0..1000", fn, a->num_refinement_passes);
+  TAPIR_CHECK_ARG(a->tracks && a->occluded && a->stop_thresholds && a->homogs && a->err && a->canonical &&
+                      a->workspace,
+                  "%s: null pointer", fn);
+  TAPIR_CHECK_ARG(aligned(a->tracks, a->tracks_fp64 ? 8 : 4) && aligned(a->stop_thresholds, 8) &&
+                      aligned(a->homogs, 8) && aligned(a->err, 8) && aligned(a->canonical, 8) &&
+                      aligned(a->ransac_stats, 4) && aligned(a->workspace, 256),
+                  "%s: tracks and outputs must be aligned to their dtype, workspace to 256 bytes", fn);
+  const size_t need = homographies_workspace_bytes(a->T, a->N);
+  TAPIR_CHECK_ARG(a->workspace_bytes >= need, "%s: workspace %zu bytes < %zu", fn, a->workspace_bytes, need);
+  return homographies_wrt_frame(a, S(stream));
 }
 
 namespace {

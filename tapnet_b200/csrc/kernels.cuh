@@ -71,6 +71,13 @@ int tapvid_counts(const tapir_tapvid_args* a, cudaStream_t s);
 int redetection_max_events(int T);
 int redetection_events(const tapir_redetection_args* a, cudaStream_t s);
 
+// ---- camera homographies from point tracks (homography.cu; viz_utils.py:301-648) -----------
+size_t homographies_workspace_bytes(int T, int N);
+// Host only: the RANSAC stop table thr[it] = min(1 - (it + 1) / N, frac * pow(0.99, it)) * N.
+void ransac_stop_thresholds(int N, double frac, double* out);
+// Arguments checked by tapir_homographies_wrt_frame.
+int homographies_wrt_frame(const tapir_homography_args* a, cudaStream_t s);
+
 // ---- Lanczos resize of uint8 RGB clips (resample.cu; PIL's 8-bit LANCZOS) -------------------
 // Host only: the per-axis kernel width, and the (xmin, n) bounds [out][2] and 22-bit fixed-point
 // taps [out][ksize] of one axis.
